@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- tracker.update() frames/sec (BASELINE.json metric), B200 arm and CPU reference arm.
+"""bench.py -- tracker.update() frames/sec (BASELINE.json metric), GPU arm and CPU reference arm.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--config 2|3|4|5]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--config 2|3|4|5] [--dump-outputs DIR]
 
 Default workload (config.workload) = BASELINE.json configs[1]: BoT-SORT + OSNet_x0_25 ReID inside update(), one
 1280x720 stream of 256 detections per frame per GPU, reference bench generator (benchmark_fps.py:60-94), YAML-default
@@ -20,12 +20,15 @@ Kalman predict/update, assignment rounds, lifecycle, output rows).
           BaseTracker-shaped `BotSort.update(dets, img)` of the reference seam -- every step copies the frame(s) +
           detections host->device and reads the result rows back (`e2e_pinned` = the same call with page-locked frames).
   roofline : SURVEY 8(d): ReID algorithmic FLOP per step (crops x FLOP/crop of the backbone) / step time, against the
-          measured dense BF16 tensor peak; `hbm` carries the measured DRAM traffic of the ReID kernels (ncu) beside it.
+          dense BF16 tensor peak (MEASURED_PEAKS.json when present, else the H100 SXM data sheet figure).
   parity : the first frames of the TIMED workload through the device path and through the oracle (outside the timed
           region): ids / det_ind / conf / cls equal, boxes within 1e-4.
   cpu_baseline : the oracle port of the reference path (numpy/scipy/torch-CPU restatement pinned to the reference by
           tests/golden) on this box's host cores, on a bounded sample of the same workload.
 `--impl reference` runs that CPU arm alone and prints the same line shape.
+`--dump-outputs DIR` writes the rows the timed path returned for its last step, one DIR/rows_stream<s>.npy (float32,
+[rows][8]: x1 y1 x2 y2 id conf cls det_ind) per stream; inputs and ReID weights are seeded, so two builds run with the same
+arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -54,7 +57,7 @@ if WORLD > 1 and "BENCH_KEEP_VISIBLE" not in os.environ:
 
 import numpy as np  # noqa: E402
 
-RING = 64  # distinct frames in the input ring of config 2: 64 x 2.76 MB = 177 MB > 126 MB of L2
+RING = 64  # distinct frames in the input ring of config 2: 64 x 2.76 MB = 177 MB > 50 MB of L2
 BOTSORT = dict(
     track_high_thresh=0.6296854875023994, track_low_thresh=0.1014392537025336,
     new_track_thresh=0.6246494191492591, track_buffer=40, match_thresh=0.7722224024589055,
@@ -95,7 +98,7 @@ def measured_peaks():
     if p.exists():
         d = json.loads(p.read_text())
         return dict(hbm_gbs=float(d["hbm_gbs"]), tensor_tflops=float(d["bf16_tflops_sustained"]), source="measured")
-    return dict(hbm_gbs=6650.0, tensor_tflops=1400.0, source="fallback")
+    return dict(hbm_gbs=3350.0, tensor_tflops=989.0, source="H100 SXM data sheet (dense BF16, 700 W), not measured")
 
 
 class ClockSampler:
@@ -103,7 +106,7 @@ class ClockSampler:
 
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
-         "clocks_event_reasons.sw_power_cap")
+         "clocks_event_reasons.sw_power_cap,power.limit")
 
     def __init__(self):
         self.rows = []
@@ -131,8 +134,9 @@ class ClockSampler:
         mx = [float(r[1]) for r in self.rows if len(r) > 1 and r[1].replace(".", "").isdigit()]
         names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
         reasons = [n for i, n in enumerate(names) if any(len(r) > 3 + i and r[3 + i].lower().startswith("active") for r in self.rows)]
+        pl = [float(r[7]) for r in self.rows if len(r) > 7 and r[7].replace(".", "").isdigit()]
         return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": max(mx) if mx else None,
-                "reasons": reasons, "samples": len(sm)}
+                "power_limit_w": max(pl) if pl else None, "reasons": reasons, "samples": len(sm)}
 
 
 
@@ -250,7 +254,7 @@ def _cpu_stream_worker(job):
 
 
 def run_reference(args):
-    """The reference path on the host cores for the SAME workload as the B200 arm at this --gpus: `streams` streams per
+    """The reference path on the host cores for the SAME workload as the GPU arm at this --gpus: `streams` streams per
     GPU, i.e. N x streams independent streams.  One stream: one tracker with the fastest thread count of a bounded probe.
     More: concurrent tracker processes (the reference's own replay parallelism is one process per sequence,
     engine/eval/replay.py:27-115), each with an equal share of the usable cores; value = sum of the streams' rates.
@@ -292,7 +296,7 @@ def run_reference(args):
 
 
 # ------------------------------------------------------------------------------------------------------
-# B200 arm
+# GPU arm
 # ------------------------------------------------------------------------------------------------------
 def device_run(cfg, blob, K, Wm, dist, profile=True):
     """value (device-resident inputs, CUDA events) + the per-class profile of one configuration on this rank's GPU."""
@@ -348,9 +352,7 @@ def device_run(cfg, blob, K, Wm, dist, profile=True):
     if not lib.boxmot_b200_tracker_elapsed_ms(trk.handle, ctypes.byref(ms)):
         raise RuntimeError(_lib.last_error(lib))
     torch.cuda.synchronize()
-    out_rows = (ctypes.c_int * S)()
-    if not lib.boxmot_b200_tracker_fetch(trk.handle, None, None, out_rows):   # surfaces device-side errors
-        raise RuntimeError(_lib.last_error(lib))
+    last_rows = [np.asarray(r, np.float32).reshape(-1, 8) for r in trk.fetch()]   # surfaces device-side errors
     value_ms = ms.value
     prof, assoc_phases = None, None
     if profile:
@@ -374,7 +376,7 @@ def device_run(cfg, blob, K, Wm, dist, profile=True):
     del d_imgs, d_dets
     torch.cuda.empty_cache()
     return dict(value_ms=value_ms, crops=crops, launches_per_step=launches_per_step, prof=prof, assoc_phases=assoc_phases,
-                clocks=clock_info, per_stream=per_stream, new_tracker=new_tracker)
+                clocks=clock_info, per_stream=per_stream, new_tracker=new_tracker, last_rows=last_rows)
 
 
 def e2e_run(cfg, blob, per_stream, K, Wm, dist, pinned):
@@ -437,18 +439,12 @@ def parity_check(cfg, blob, oracle_rows, per_stream):
             "what": "ids, det_ind, conf, cls of every output row of the first frames of the timed stream, device vs oracle"}
 
 
-def traffic_record(cfg, crops):
-    """Measured DRAM bytes per step of the ReID kernels (ncu --set full captures, profiles/traffic.json)."""
-    try:
-        tj = json.loads((ROOT / "profiles" / "traffic.json").read_text())
-    except Exception:
-        return None
-    rec = tj.get(f"config{cfg['id']}")
-    if not rec:
-        return None
-    scale = crops / max(1.0, rec.get("crops_per_step", crops))
-    return {"dram_bytes_per_step": rec["dram_bytes_per_step"] * scale, "per_class": rec.get("per_class"),
-            "source": rec.get("source"), "scaled_from_crops": rec.get("crops_per_step")}
+def dump_outputs(out_dir, rows):
+    """Rows of the last timed step, one float32 file per stream (a few hundred rows each: far below 64 MB)."""
+    d = Path(out_dir)
+    d.mkdir(parents=True, exist_ok=True)
+    for s, r in enumerate(rows):
+        np.save(d / f"rows_stream{RANK * len(rows) + s}.npy", np.asarray(r, np.float32))
 
 
 def run_b200(args):
@@ -464,8 +460,6 @@ def run_b200(args):
         dist.init_process_group("nccl", device_id=torch.device("cuda:0"))
     cfg = dict(CONFIGS[args.config], id=args.config)
     K, Wm = args.steps, max(3, args.warmup)
-    if args.config == 3:
-        K, Wm = min(K, 24), min(Wm, 8)      # association at 2000 live tracks is tens of ms per frame: keep the run short
     tmp = Path(tempfile.mkdtemp(prefix="b200bench_"))
     blob = make_blob(tmp, cfg["arch"])
     S = cfg["streams"]
@@ -474,15 +468,17 @@ def run_b200(args):
 
     dev = device_run(cfg, blob, K, Wm, dist)
     value_ms, crops, prof = dev["value_ms"], dev["crops"], dev["prof"]
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, dev["last_rows"])
     e2e_ms, n_out, api = e2e_run(cfg, blob, dev["per_stream"], K, Wm, dist, pinned=False)
     e2e_pin_ms, _, _ = e2e_run(cfg, blob, dev["per_stream"], K, Wm, dist, pinned=True)
 
     extra5 = None
     if args.config == 2 and not args.no_extra:
-        # BASELINE config 5 shape on the same GPUs (16 streams x 256 dets per GPU), short: the scaling run then carries
+        # BASELINE config 5 shape on the same GPUs (16 streams x 256 dets per GPU), same steps: the scaling run then carries
         # the 128-stream figure at N = 8 beside the one-stream-per-GPU headline
         c5 = dict(CONFIGS[5], id=5)
-        d5 = device_run(c5, blob, 12, 3, dist, profile=False)
+        d5 = device_run(c5, blob, K, Wm, dist, profile=False)
         extra5 = (d5["value_ms"], d5["crops"])
 
     from boxmot_b200 import sharding
@@ -505,8 +501,6 @@ def run_b200(args):
     achieved = gflop_step / step_s / 1e3                              # TFLOP/s per GPU
     reid_ms = sum(prof[c]["ms_per_step"] for c in CLASSES if c != "association")
     dom = max((c for c in CLASSES if c != "association"), key=lambda c: prof[c]["ms_per_step"])
-    tr = traffic_record(cfg, crops)
-    compulsory = crops * (29e3 + 4 * cfg["feat"])                     # source patch + embedding row per crop (SURVEY 8d)
     tc_path = cfg["arch"] == "osnet_x0_25"
     line = {
         "metric": METRIC, "value": fps, "unit": "frames/s", "n_gpus": WORLD, "steps": K, "warmup": Wm,
@@ -515,8 +509,8 @@ def run_b200(args):
         "config": {"workload": cfg["workload"], "baseline_config": args.config, "streams_per_gpu": S, "dets_per_frame": cfg["dets"],
                    "crops_per_step_per_gpu": crops,
                    "reid": f"{cfg['arch']} random-init (seed 0); " + (
-                       "tensor-core path: tcgen05 kind::f16 on split-BF16 operands (hi*hi + lo*hi + hi*lo, FP32 accumulate, "
-                       "embedding error 2e-6 of the row scale), depthwise / pooling / gates in float32" if tc_path else "float32 CUDA-core kernels"),
+                       "tensor-core path: wgmma on split-BF16 operands (hi*hi + lo*hi + hi*lo, FP32 accumulate), depthwise / "
+                       "pooling / gates in float32" if tc_path else "float32 CUDA-core kernels"),
                    "l2": f"input ring of {cfg['ring']} distinct frames per stream ({cfg['ring'] * S * img_bytes / 1e6:.0f} MB) and a "
                          f"per-chunk activation workspace larger than L2; no explicit flush",
                    "parallelism": f"streams x{WORLD * S} ({S} per GPU)",
@@ -530,35 +524,30 @@ def run_b200(args):
                 "host_memory": "pageable"},
         "e2e_pinned": {"value": total_frames / (e2e_pin_ms * 1e-3), "unit": "frames/s", "ms_per_step": e2e_pin_ms / K,
                        "host_memory": "page-locked frames (copied straight from the caller's buffer)"},
+        "device": torch.cuda.get_device_name(0),
         "gpu_launches": dev["launches_per_step"] * K,
         "launches_per_step": dev["launches_per_step"],
         "clocks": dev["clocks"],
         # SURVEY 8(d): achieved = crops/s x FLOP/crop of the backbone, per GPU, over the measured step time
         "roofline": {"kernel": "ReID backbone (all conv / fc kernels of a step)", "bound": "tensor", "achieved": achieved,
                      "peak": peaks["tensor_tflops"], "unit": "TFLOP/s", "frac": achieved / peaks["tensor_tflops"],
-                     "traffic": None if tr is None else tr["dram_bytes_per_step"], "peak_source": peaks["source"],
+                     "peak_source": peaks["source"],
                      "algorithmic_gflop_per_step": gflop_step, "gflop_per_crop": GFLOP_PER_CROP[cfg["arch"]],
                      "step_ms": value_ms / K,
-                     "note": "peak = measured dense BF16 cuBLAS (sustained); the tensor-core path issues 3 BF16 products per "
-                             "algorithmic MAC (split operands, 2 instructions), so 1/3 of the tensor work is algorithmic",
+                     "note": "the tensor-core path issues 3 BF16 products per algorithmic MAC (split operands), so 1/3 of the "
+                             "tensor work is algorithmic",
                      "serialised_reid_ms_per_step": reid_ms,
                      "frac_serialised": gflop_step / (reid_ms * 1e-3) / 1e3 / peaks["tensor_tflops"],
-                     "hbm": None if tr is None else {
-                         "achieved": tr["dram_bytes_per_step"] / (reid_ms * 1e-3) / 1e9, "peak": peaks["hbm_gbs"], "unit": "GB/s",
-                         "frac": tr["dram_bytes_per_step"] / (reid_ms * 1e-3) / 1e9 / peaks["hbm_gbs"],
-                         "measured_dram_bytes_per_step": tr["dram_bytes_per_step"], "compulsory_bytes_per_step": compulsory,
-                         "traffic_over_compulsory": tr["dram_bytes_per_step"] / compulsory, "per_class": tr["per_class"],
-                         "source": tr["source"]},
                      "dominant_class": dom, "dominant_class_ms": prof[dom]["ms_per_step"]},
         "kernel_classes": prof,
         "association_phase_sm_clocks_per_step": dev["assoc_phases"],
     }
     if extra5:
-        fps5 = WORLD * CONFIGS[5]["streams"] * 12 / (red[3] * 1e-3)
+        fps5 = WORLD * CONFIGS[5]["streams"] * K / (red[3] * 1e-3)
         line["config5"] = {"workload": CONFIGS[5]["workload"], "value": fps5, "unit": "frames/s", "streams": WORLD * CONFIGS[5]["streams"],
-                           "ms_per_step": red[3] / 12, "steps": 12,
-                           "reid_tflops_per_gpu": extra5[1] * GFLOP_PER_CROP["osnet_x0_25"] / (red[3] * 1e-3 / 12) / 1e3,
-                           "frac_of_tensor_peak": extra5[1] * GFLOP_PER_CROP["osnet_x0_25"] / (red[3] * 1e-3 / 12) / 1e3 / peaks["tensor_tflops"]}
+                           "ms_per_step": red[3] / K, "steps": K,
+                           "reid_tflops_per_gpu": extra5[1] * GFLOP_PER_CROP["osnet_x0_25"] / (red[3] * 1e-3 / K) / 1e3,
+                           "frac_of_tensor_peak": extra5[1] * GFLOP_PER_CROP["osnet_x0_25"] / (red[3] * 1e-3 / K) / 1e3 / peaks["tensor_tflops"]}
     if WORLD == 1 and not args.skip_cpu:
         cb = cpu_arm(cfg, args.cpu_frames, 1, keep_rows=True)
         rows = cb.pop("_rows")
@@ -574,13 +563,16 @@ def run_b200(args):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=200)
+    ap.add_argument("--steps", type=int, default=200,
+                    help="timed steps of the GPU arm (headline, e2e and config-5 legs); the CPU reference arm (--impl reference) "
+                         "times at most 12 frames within ~40 s, the cpu_baseline leg --cpu-frames within ~25 s")
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--config", type=int, default=2, choices=[2, 3, 4, 5], help="BASELINE.json configuration (default: the headline)")
     ap.add_argument("--cpu-frames", type=int, default=8)
     ap.add_argument("--skip-cpu", action="store_true", help="kernel A/B experiments only: omit the cpu_baseline / parity legs")
     ap.add_argument("--no-extra", action="store_true", help="omit the short config-5 (16 streams per GPU) measurement")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the rows of the last timed step as DIR/rows_stream<s>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

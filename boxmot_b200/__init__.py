@@ -1,4 +1,4 @@
-"""boxmot_b200 -- B200-native (sm_100a CUDA) drop-in for BoxMOT's per-frame track-update hot path.
+"""boxmot_b200 -- H100-native (sm_90a CUDA) drop-in for BoxMOT's per-frame track-update hot path.
 
 Public surface mirrors the reference seams for this path only (SURVEY.md section 8b):
   * ``ByteTrack`` / ``BotSort`` / ``DeepOcSort`` / ``OcSort`` / ``StrongSort``: ``update(dets, img, embs=None) -> TrackResults`` like

@@ -129,7 +129,7 @@ def load_library():
     if _LIB is None:
         if not LIB_PATH.exists():
             raise B200Error(
-                f"{LIB_PATH} is missing: build it with `python -m boxmot_b200.build` (nvcc, sm_100a). "
+                f"{LIB_PATH} is missing: build it with `python -m boxmot_b200.build` (nvcc, sm_90a). "
                 "boxmot_b200 has no CPU fallback.")
         lib = ctypes.CDLL(str(LIB_PATH))
         for name, (res, args) in SYMBOLS.items():

@@ -1,14 +1,14 @@
 // host_stage.h -- parallel staging copies of pageable frames into the engine's page-locked buffer.
 //
-// A 1280x720 BGR frame is 2.76 MB; one thread moves it in 0.17 ms on the B200 host (0.33 ms in the build container), which
-// is ~10 % of an end-to-end BotSort.update(dets, img) at 256 detections.  StagePool splits the copy into cache-line
+// A 1280x720 BGR frame is 2.76 MB; one host thread needs a noticeable share of an end-to-end BotSort.update(dets, img) at
+// 256 detections to copy it.  StagePool splits the copy into cache-line
 // aligned pieces over a few persistent worker threads plus the caller; the caller is told when each piece lands (in
 // order) so that it can queue that piece's host-to-device DMA while the rest is still being copied.
 //
-// MEASURED (round 2, scripts/sweep_stage.sh on the B200 box): the isolated copy drops to 0.06 ms with 3 helpers
-// (scripts/microbench/stage_pool_test.cpp), but the whole update() gets SLOWER -- 1.72 ms with the caller alone, 1.84 ms with
-// one helper, 2.00 ms with three (helpers woken from a condition variable once per frame, four small DMAs instead of
-// one).  Helpers are therefore opt-in: BOXMOT_B200_STAGE_THREADS=N (caller included), default 1.
+// Helpers make the isolated copy faster (scripts/microbench/stage_pool_test.cpp) but can make the whole update() slower:
+// they are woken from a condition variable once per frame and the frame goes as several small DMAs instead of one
+// (scripts/sweep_stage.sh compares the settings).  Helpers are therefore opt-in: BOXMOT_B200_STAGE_THREADS=N (caller
+// included), default 1.
 //
 // Host-only C++ (no CUDA types).  The pool is created lazily, re-created after a fork (worker threads do not survive
 // one), and joined when the process-wide instance is destroyed.

@@ -218,7 +218,7 @@ BMB_FN void jv_augment_wide(S& s, int n, int ld, int zrow, int n_free, int* mbx)
 
 // ---- column-owned CTA-wide augmentation (wide == 2) --------------------------------------------------------------
 // jv_augment_wide walks the open part of the column LIST, so every relaxed entry costs a chain of shared-memory reads
-// (cols[k] -> v[jj], d[jj]); measured 1 200 cycles per band column at n = 1 500.  Here every thread OWNS the columns
+// (cols[k] -> v[jj], d[jj]) per band column.  Here every thread OWNS the columns
 // tid, tid + NT, ... and keeps their distance d and the negated price (0.0 - v) in registers; "open" (position >= hi)
 // is a bit per owned column refreshed from the inverse permutation pos[] whenever the band changes.  A band column
 // then costs one pass of register arithmetic and one barrier.  The band-minimum hits are recovered in POSITION order
@@ -628,8 +628,8 @@ BMB_FN void jv_augment_owned(S& s, int n, int ld, int zrow, int n_free, int* mbx
                 const double* ci = c + (size_t)i * ld;
                 const double h = (zr ? 0.0 : ci[j]) - v[j] - mind;
                 // look ahead to the next band column that needs a relaxation: its cost row is prefetched while this one
-                // is relaxed (with the no-op columns skipped the next list entry is usually not the next row to load;
-                // measured 3.7 k cycles per relaxed column without this).  [lo, la) stays no-op whatever this step
+                // is relaxed (with the no-op columns skipped the next list entry is usually not the next row to load,
+                // so without this every relaxed column waits for its row).  [lo, la) stays no-op whatever this step
                 // appends to the band: hits only write list positions >= hi.
                 const int la = walking ? walk(lo, hi) : lo;
                 known = walking && la != hi;
@@ -656,7 +656,7 @@ BMB_FN void jv_augment_owned(S& s, int n, int ld, int zrow, int n_free, int* mbx
                     }
                 } else {
                     // the row entries first, all loads in flight together (inside the branchy loop below each load waited
-                    // for the previous column: ~3.7 k cycles per relaxed band column on the config-3 frames), then the
+                    // for the previous column), then the
                     // prefetch of the next row, then the arithmetic
                     double cq[JV_OWN];
 #pragma unroll
@@ -813,7 +813,7 @@ BMB_FN void jv_augment_owned(S& s, int n, int ld, int zrow, int n_free, int* mbx
 
 // CTA-wide augmenting row reduction (feature JV_F_ARRWIDE): the same sequential rounds as the one-warp loop in
 // jv_dense_solve, but the lexicographic two-smallest search of a round runs on every thread (the one-warp loop waits for
-// one dependent global load per 32 columns: 13 k cycles per round on the config-3 frames), per-warp results are merged
+// one dependent global load per 32 columns), per-warp results are merged
 // through shared memory by every thread alike (top-2 under the strict order (value, index) is associative), and thread 0
 // applies the round's writes between two barriers.
 struct JvTop2 { double a1, a2; int i1, i2; };

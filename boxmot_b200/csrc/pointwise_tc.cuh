@@ -1,30 +1,32 @@
-// pointwise_tc.cuh -- 1x1 convolution (GEMM) on the 5th-generation tensor cores: tcgen05.mma kind::tf32 with a
-// three-term split so that the result keeps float32 accuracy (the path's embedding bound is 1e-4):
+// pointwise_tc.cuh -- 1x1 convolution (GEMM) on the Hopper tensor cores: wgmma kind tf32 with a three-term split so
+// that the result keeps float32 accuracy (the path's embedding bound is 1e-4):
 //
 //     a = a_hi + a_lo,  w = w_hi + w_lo   (hi = top 19 bits, lo = exact remainder)
 //     D += A_hi*W_hi + A_hi*W_lo + A_lo*W_hi          (the dropped A_lo*W_lo term is ~2^-22 relative)
 //
-// One persistent CTA = 128 threads: tiles of 128 output rows x all N output channels.
-//   * weights (both halves, pre-arranged in the UMMA canonical K-major layout at model load) are pulled into
-//     shared memory once per CTA by a bulk async copy (cp.async.bulk, completes on an mbarrier);
-//   * per tile the 128 x K activation block is loaded by all threads (float4, coalesced), optionally built on
-//     the fly as the gated sum of the four OSBlock branches, split into hi / lo and written in the canonical
-//     no-swizzle K-major layout (8-row x 16-byte core matrices);
-//   * one thread issues the tcgen05.mma chain (3 per 8-wide K step) accumulating in TMEM and commits to an
-//     mbarrier; the four warps then read their 32 TMEM lanes back (tcgen05.ld), add bias / residual, apply ReLU
-//     and store float4 rows.
-// Layout reference: cute/atom/mma_traits_sm100.hpp (INTERLEAVE K-major canonical layout
-// ((8,m),(T,2)):((1T,SBO),(1,LBO))) and cute/arch/mma_sm100_desc.hpp (descriptor bit fields).
+// One persistent CTA = 256 threads (two warpgroups): tiles of 128 output rows x all N output channels.
+//   * weights (both halves, pre-arranged in the canonical K-major layout at model load) are pulled into shared memory
+//     once per CTA by a bulk async copy (cp.async.bulk, completes on an mbarrier);
+//   * per tile the 128 x K activation block is loaded by all threads (float4, coalesced), optionally built on the fly
+//     as the gated sum of the four OSBlock branches, split into hi / lo and written in the canonical no-swizzle K-major
+//     layout (8-row x 16-byte core matrices);
+//   * warpgroup g issues the wgmma chain (3 per 8-wide K step) for rows 64 g .. 64 g + 63 into register accumulators;
+//     its epilogue adds bias / residual, applies ReLU and stores float2 pairs.
+// Layout reference: cute/atom/mma_traits_sm90_gmma.hpp (INTERLEAVE K-major canonical layout
+// ((8,m),(T,2)):((1T,SBO),(1,LBO))) and cute/arch/mma_sm90_desc.hpp (descriptor bit fields).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include "wgmma.cuh"
 
 namespace bmb {
 namespace tc {
 
 constexpr int TILE_M = 128;
 constexpr int KC = 64;        // K chunk staged in shared memory per MMA batch (floats)
-constexpr int THREADS = 128;
+constexpr int THREADS = 256;
+constexpr int NPAD_MAX = 128;   // widest accumulator (64 registers per thread)
 
 struct Args {
     const float* in;          // PLAIN: [M][K]; GATED: x [M][K - mid] (null when K == mid)
@@ -37,60 +39,7 @@ struct Args {
     int K, N, Kpad, Npad, mid, HW, relu;
 };
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-// bounded wait: a protocol bug must trap instead of hanging the GPU
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-    const uint32_t addr = smem_u32(bar);
-    for (uint32_t spin = 0; spin < (1u << 28); ++spin) {
-        uint32_t done;
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-            "selp.u32 %0, 1, 0, p;\n\t}"
-            : "=r"(done) : "r"(addr), "r"(parity) : "memory");
-        if (done) return;
-    }
-    __trap();
-}
-__device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-    // SmemDescriptor: start[0,14) | LBO[16,30) | SBO[32,46) | version=1 [46,48) | layout_type=0 (no swizzle) [61,64)
-    uint64_t d = 0;
-    d |= (uint64_t)((saddr >> 4) & 0x3fff);
-    d |= (uint64_t)((lbo_bytes >> 4) & 0x3fff) << 16;
-    d |= (uint64_t)((sbo_bytes >> 4) & 0x3fff) << 32;
-    d |= (uint64_t)1 << 46;
-    return d;
-}
-__device__ __forceinline__ void mma_tf32(uint32_t tmem_d, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void mma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, float* v) {
-    uint32_t r[8];
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-                 : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 8; ++i) v[i] = __uint_as_float(r[i]);
-}
+using um::smem_u32;
 
 // canonical (no swizzle, K-major) offset in floats of element (row, k) in a block whose K extent is `kext`
 __device__ __host__ __forceinline__ size_t canon_off(int row, int k, int kext) {
@@ -100,8 +49,7 @@ __device__ __host__ __forceinline__ size_t canon_off(int row, int k, int kext) {
 template <bool GATED>
 __global__ void __launch_bounds__(THREADS) k_pointwise_tc(const Args a, const int* __restrict__ d_n, int off, int cap) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
-    __shared__ __align__(8) uint64_t bar_w, bar_mma;
-    __shared__ uint32_t tmem_base_s;
+    __shared__ __align__(8) uint64_t bar_w;
     int n_crops = *d_n - off;
     n_crops = n_crops < 0 ? 0 : (n_crops > cap ? cap : n_crops);
     const int M = n_crops * a.HW;
@@ -113,32 +61,22 @@ __global__ void __launch_bounds__(THREADS) k_pointwise_tc(const Args a, const in
     float* sB = reinterpret_cast<float*>(smem_raw);                 // [2][Npad x Kpad] canonical
     float* sA_hi = sB + 2 * (size_t)Npad * Kpad;                    // [128 x kc] canonical
     float* sA_lo = sA_hi + (size_t)TILE_M * kc_max;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t tmem_cols = Npad <= 32 ? 32u : (Npad <= 64 ? 64u : (Npad <= 128 ? 128u : 256u));
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2;
+    const int row = wg * 64 + (warp & 3) * 16 + (lane >> 2), cq = 2 * (lane & 3);
 
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_s)), "r"(tmem_cols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
     if (threadIdx.x == 0) {
-        mbar_init(&bar_w, 1);
-        mbar_init(&bar_mma, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        um::mbar_init(&bar_w, 1);
+        um::fence_mbar_init();
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = tmem_base_s;
     if (threadIdx.x == 0) {
         const uint32_t wbytes = (uint32_t)(2 * (size_t)Npad * Kpad * sizeof(float));
-        mbar_expect_tx(&bar_w, wbytes);
-        bulk_g2s(sB, a.w_tc, wbytes, &bar_w);
+        um::mbar_expect_tx(&bar_w, wbytes);
+        um::bulk_g2s(sB, a.w_tc, wbytes, &bar_w);
     }
-    // instruction descriptor: D=f32, A=B=tf32, both K-major, N = Npad, M = 128
-    const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(Npad >> 3) << 17) | ((uint32_t)(TILE_M >> 4) << 24);
     const int KX = GATED ? K - a.mid : 0;
-    uint32_t mma_phase = 0;
     bool weights_ready = false;
+    float acc[2 * NPAD_MAX / 4];
 
     for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
         const int m0 = tile * TILE_M;
@@ -175,59 +113,48 @@ __global__ void __launch_bounds__(THREADS) k_pointwise_tc(const Args a, const in
                 *reinterpret_cast<float4*>(sA_hi + o) = hi;
                 *reinterpret_cast<float4*>(sA_lo + o) = lo;
             }
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+            um::fence_async_smem();
             __syncthreads();
-            // ---- MMA chain for this chunk ----
-            if (threadIdx.x == 0) {
-                if (!weights_ready) { mbar_wait(&bar_w, 0); weights_ready = true; }
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint32_t a_hi = smem_u32(sA_hi), a_lo = smem_u32(sA_lo);
-                const uint32_t b_hi = smem_u32(sB), b_lo = smem_u32(sB + (size_t)Npad * Kpad);
+            // ---- MMA chain for this chunk: warpgroup wg owns rows 64 wg .. 64 wg + 63 (8 row groups of kc * 32 bytes) ----
+            if (!weights_ready) { um::mbar_wait(&bar_w, 0); weights_ready = true; }
+            {
                 const uint32_t sbo_a = (uint32_t)kc * 32, sbo_b = (uint32_t)Kpad * 32;  // bytes between 8-row groups
+                const uint32_t a_hi = smem_u32(sA_hi) + (uint32_t)wg * 8u * sbo_a, a_lo = smem_u32(sA_lo) + (uint32_t)wg * 8u * sbo_a;
+                const uint32_t b_hi = smem_u32(sB), b_lo = smem_u32(sB + (size_t)Npad * Kpad);
+                um::wg_fence();
                 for (int ks = 0; ks < kc; ks += 8) {
                     const uint32_t ao = (uint32_t)(ks >> 2) * 128, bo = (uint32_t)((k0 + ks) >> 2) * 128;
-                    const uint64_t dah = make_desc(a_hi + ao, 128, sbo_a), dal = make_desc(a_lo + ao, 128, sbo_a);
-                    const uint64_t dbh = make_desc(b_hi + bo, 128, sbo_b), dbl = make_desc(b_lo + bo, 128, sbo_b);
-                    mma_tf32(tmem_base, dah, dbh, idesc, (k0 + ks) > 0 ? 1u : 0u);
-                    mma_tf32(tmem_base, dah, dbl, idesc, 1u);
-                    mma_tf32(tmem_base, dal, dbh, idesc, 1u);
+                    const uint64_t dah = um::make_desc(a_hi + ao, 128, sbo_a), dal = um::make_desc(a_lo + ao, 128, sbo_a);
+                    um::mma_rt<true>(Npad, acc, dah, b_hi + bo, 128, sbo_b, (k0 + ks) > 0 ? 1u : 0u);
+                    um::mma_rt<true>(Npad, acc, dah, b_lo + bo, 128, sbo_b, 1u);
+                    um::mma_rt<true>(Npad, acc, dal, b_hi + bo, 128, sbo_b, 1u);
                 }
-                mma_commit(&bar_mma);
+                um::wg_commit();
+                um::wg_wait_all();
+                um::wg_fence_acc<2 * NPAD_MAX / 4>(acc);
             }
-            mbar_wait(&bar_mma, mma_phase);
-            mma_phase ^= 1u;
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+            __syncthreads();  // both warpgroups have read the A chunk before it is restaged
         }
-        // ---- epilogue: TMEM -> registers -> bias / residual / ReLU -> global (thread = output row) ----
-        const int m = m0 + warp * 32 + lane;
-        float* orow = a.out + (size_t)m * N;
-        const float* rrow = a.residual ? a.residual + (size_t)m * N : nullptr;
-        for (int c0 = 0; c0 < N; c0 += 8) {
-            float v[8];
-            tmem_ld8(tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)c0, v);
+        // ---- epilogue: registers -> bias / residual / ReLU -> global (two rows x 2 columns per 8-column group) ----
 #pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const int c = c0 + h * 4;
-                if (c < N) {
-                    const float4 b = *reinterpret_cast<const float4*>(a.bias + c);
-                    float4 o = make_float4(v[h * 4] + b.x, v[h * 4 + 1] + b.y, v[h * 4 + 2] + b.z, v[h * 4 + 3] + b.w);
-                    if (rrow) {
-                        const float4 r = *reinterpret_cast<const float4*>(rrow + c);
-                        o.x += r.x; o.y += r.y; o.z += r.z; o.w += r.w;
+        for (int i = 0; i < NPAD_MAX / 8; ++i) {
+            const int c = 8 * i + cq;
+            if (c < N) {
+                const float2 b = *reinterpret_cast<const float2*>(a.bias + c);
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int m = m0 + row + 8 * h;
+                    float2 o = make_float2(acc[4 * i + 2 * h] + b.x, acc[4 * i + 2 * h + 1] + b.y);
+                    if (a.residual) {
+                        const float2 r = *reinterpret_cast<const float2*>(a.residual + (size_t)m * N + c);
+                        o.x += r.x; o.y += r.y;
                     }
-                    if (a.relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f); }
-                    if (a.relu == 2) { o.x = fminf(o.x, 6.f); o.y = fminf(o.y, 6.f); o.z = fminf(o.z, 6.f); o.w = fminf(o.w, 6.f); }
-                    *reinterpret_cast<float4*>(orow + c) = o;
+                    if (a.relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); }
+                    if (a.relu == 2) { o.x = fminf(o.x, 6.f); o.y = fminf(o.y, 6.f); }
+                    *reinterpret_cast<float2*>(a.out + (size_t)m * N + c) = o;
                 }
             }
         }
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        __syncthreads();  // all TMEM reads of this tile are done before the next tile's first MMA overwrites D
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    }
-    if (warp == 0) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(tmem_cols) : "memory");
     }
 }
 

@@ -7,9 +7,8 @@
 //                                           OSBlock / OSNet.forward (eval mode, BatchNorm folded offline)
 //   native/cpp/trackers/base/src/reid_onnx.cpp:51-383  (per-crop batch-1 ORT forward of the native path)
 //
-// Data layout: activations are NHWC float32 in HBM, one chunk of crops at a time (256 by default: measured on B200,
-// one full-width chunk beats two L2-resident half chunks -- 415 vs 351 frames/s at 208 crops -- because the small
-// tile kernels are latency-bound and want full waves); weights are a BN-folded float32 blob
+// Data layout: activations are NHWC float32 in HBM, one chunk of crops at a time (256 by default: one
+// full-width chunk keeps the small, latency-bound tile kernels in full waves); weights are a BN-folded float32 blob
 // (boxmot_b200/weights.py) uploaded once.  Round-1 kernels are float32 CUDA-core kernels with shared-memory
 // tiling; every 1x1 convolution goes through one GEMM-shaped kernel (k_pointwise) whose prologue can build
 // the gated branch sum on the fly and whose epilogue fuses bias / residual / ReLU.
@@ -37,6 +36,13 @@ namespace bmb {
 
 constexpr int IN_H = 256, IN_W = 128;
 constexpr uint32_t BLOB_MAGIC = 0x45523242u;
+
+// streaming multiprocessors of the current device: grid-stride kernels launch a few CTAs per SM
+static int sm_count() {
+    int dev = 0, n = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) n = 0;
+    return n > 0 ? n : 132;
+}
 
 __device__ __forceinline__ int chunk_count(const int* d_n, int off, int cap) {
     int n = *d_n - off;
@@ -155,7 +161,7 @@ __global__ void __launch_bounds__(256) k_stem(const float* __restrict__ blob, co
             sw[e] = w[(size_t)k * C0 + co0 + c];
         }
         __syncthreads();
-        // packed FP32x2 FMAs (FFMA2, sm_100): two output channels per instruction, IEEE per lane (= fmaf bit for bit)
+        // two output channels per float2, IEEE fmaf per lane
         float2 acc0[8], acc1[8];
 #pragma unroll
         for (int c = 0; c < 8; ++c) { acc0[c] = make_float2(0.f, 0.f); acc1[c] = make_float2(0.f, 0.f); }
@@ -172,10 +178,10 @@ __global__ void __launch_bounds__(256) k_stem(const float* __restrict__ blob, co
                     for (int q = 0; q < 4; ++q) {
                         const float4 wv = wp[q];
                         const float2 w01 = make_float2(wv.x, wv.y), w23 = make_float2(wv.z, wv.w);
-                        acc0[q * 2 + 0] = __ffma2_rn(a0p, w01, acc0[q * 2 + 0]);
-                        acc0[q * 2 + 1] = __ffma2_rn(a0p, w23, acc0[q * 2 + 1]);
-                        acc1[q * 2 + 0] = __ffma2_rn(a1p, w01, acc1[q * 2 + 0]);
-                        acc1[q * 2 + 1] = __ffma2_rn(a1p, w23, acc1[q * 2 + 1]);
+                        acc0[q * 2 + 0] = um::ffma2(a0p, w01, acc0[q * 2 + 0]);
+                        acc0[q * 2 + 1] = um::ffma2(a0p, w23, acc0[q * 2 + 1]);
+                        acc1[q * 2 + 0] = um::ffma2(a1p, w01, acc1[q * 2 + 0]);
+                        acc1[q * 2 + 1] = um::ffma2(a1p, w23, acc1[q * 2 + 1]);
                     }
                 }
             }
@@ -263,7 +269,7 @@ struct PwArgs {
     const float* residual;    // [M][N] or null
     float* out;               // [M][N]
     int K, N, mid, HW, relu;
-    const float* w_tc;        // canonical hi/lo weight blocks for the tcgen05 path (null: CUDA-core kernel)
+    const float* w_tc;        // canonical hi/lo weight blocks for the tensor-core path (null: CUDA-core kernel)
     int Kpad, Npad;
 };
 
@@ -362,7 +368,7 @@ struct LightArgs {
     const float* bias[4];
     float* sums[4];   // [crops][tiles][C] or null
     int H, W, C, R;   // R = tile rows
-    const float* wtc[4];   // 1x1 weights as canonical K-major hi / lo blocks (tc::pack_weights) for the tcgen05 stage
+    const float* wtc[4];   // 1x1 weights as canonical K-major hi / lo blocks (tc::pack_weights) for the tensor-core stage
 };
 
 __global__ void k_lightconv(const LightArgs a, const int* __restrict__ d_n, int off, int cap) {
@@ -522,27 +528,16 @@ __global__ void __launch_bounds__(NTHREADS, MINB) k_lightconv2(const LightArgs a
     asm volatile("cp.async.commit_group;");
     asm volatile("cp.async.wait_group 0;");
     if constexpr (TC) {
-        // ---- phase A on the tensor cores: T = X * Wpw as tcgen05.mma kind::tf32 with the 3-term hi/lo split
-        // (float32-class accuracy).  The staged tile IS the canonical no-swizzle K-major operand: a core matrix is 8
-        // consecutive pixels x 16 bytes of one K-chunk plane (contiguous 128 B), the next K chunk is one plane further
+        // ---- phase A on the tensor cores: T = X * Wpw as wgmma tf32 with the 3-term hi/lo split (float32-class
+        // accuracy).  The staged tile IS the canonical no-swizzle K-major operand: a core matrix is 8 consecutive
+        // pixels x 16 bytes of one K-chunk plane (contiguous 128 B), the next K chunk is one plane further
         // (LBO = n_pxp * 16 B), the next 8 pixels 128 B further (SBO).  X is split in place (hi) and into the T buffer
-        // (lo); the accumulators of all 128-pixel tiles live in TMEM at once, one commit, then T overwrites lo.
-        static_assert(!TC || (C % 16 == 0 && C <= 64), "tcgen05 stage: N must be a multiple of 16");
-        __shared__ __align__(8) uint64_t bar_mma;
-        __shared__ uint32_t tmem_base_s;
-        constexpr int n_mt = (n_px + 127) / 128;
-        constexpr uint32_t tmem_cols = n_mt * C <= 32 ? 32u : (n_mt * C <= 64 ? 64u : (n_mt * C <= 128 ? 128u : (n_mt * C <= 256 ? 256u : 512u)));
-        static_assert(!TC || n_mt * 128 <= n_pxp, "tile rows must stay inside the padded planes");
-        static_assert(!TC || n_mt * C <= 512, "accumulators must fit TMEM");
+        // (lo); each warpgroup takes every other 64-pixel slice and overwrites the lo rows of its slice with T once its
+        // own MMAs on them have completed (no other slice reads those rows).
+        static_assert(!TC || (C % 16 == 0 && C <= 64), "tensor-core stage: N must be a multiple of 16");
+        constexpr int n_ms = (n_px + 63) / 64;
+        static_assert(!TC || n_ms * 64 <= n_pxp, "tile rows must stay inside the padded planes");
         const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-        if (warp == 0) {
-            asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tc::smem_u32(&tmem_base_s)), "r"(tmem_cols) : "memory");
-            asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-        }
-        if (threadIdx.x == 0) {
-            tc::mbar_init(&bar_mma, 1);
-            asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        }
         // packed weights (hi block then lo block, canonical [n][k]) over the plain copy in sW: 2 * C * C floats fit
         // because sW + sD + sP follow each other (C*C + 9C + 64C >= 2*C*C for C <= 64)
         __syncthreads();   // cp.async data + the plain sW copy are complete: sW may be overwritten
@@ -563,50 +558,43 @@ __global__ void __launch_bounds__(NTHREADS, MINB) k_lightconv2(const LightArgs a
             sX[e] = hi;
             sT[e] = lo;
         }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+        um::fence_async_smem();
         __syncthreads();
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t tmem_base = tmem_base_s;
-        if (threadIdx.x == 0) {
-            const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(C >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-            const uint32_t a_hi = tc::smem_u32(sX), a_lo = tc::smem_u32(sT);
-            const uint32_t b_hi = tc::smem_u32(sWtc), b_lo = tc::smem_u32(sWtc + C * C);
+        {
+            const uint32_t a_hi = um::smem_u32(sX), a_lo = um::smem_u32(sT);
+            const uint32_t b_hi = um::smem_u32(sWtc), b_lo = um::smem_u32(sWtc + C * C);
             const uint32_t lbo_a = (uint32_t)n_pxp * 16u, sbo_a = 128u, lbo_b = 128u, sbo_b = (uint32_t)C * 32u;
-#pragma unroll 1
-            for (int t = 0; t < n_mt; ++t) {
+            const int wg = warp >> 2, row = (warp & 3) * 16 + (lane >> 2), cq = 2 * (lane & 3);
+            float* sTf = reinterpret_cast<float*>(sT);
+            for (int u = wg; u < n_ms; u += NT / 128) {
+                float acc[TC ? C / 2 : 1];
+                um::wg_fence();
 #pragma unroll
                 for (int ks = 0; ks < C; ks += 8) {
-                    const uint32_t ao = (uint32_t)t * 2048u + (uint32_t)(ks >> 2) * lbo_a, bo = (uint32_t)(ks >> 2) * 128u;
-                    const uint64_t dah = tc::make_desc(a_hi + ao, lbo_a, sbo_a), dal = tc::make_desc(a_lo + ao, lbo_a, sbo_a);
-                    const uint64_t dbh = tc::make_desc(b_hi + bo, lbo_b, sbo_b), dbl = tc::make_desc(b_lo + bo, lbo_b, sbo_b);
-                    const uint32_t d = tmem_base + (uint32_t)(t * C);
-                    tc::mma_tf32(d, dah, dbh, idesc, ks > 0 ? 1u : 0u);
-                    tc::mma_tf32(d, dah, dbl, idesc, 1u);
-                    tc::mma_tf32(d, dal, dbh, idesc, 1u);
+                    const uint32_t ao = (uint32_t)u * 1024u + (uint32_t)(ks >> 2) * lbo_a, bo = (uint32_t)(ks >> 2) * 128u;
+                    const uint64_t dah = um::make_desc(a_hi + ao, lbo_a, sbo_a), dal = um::make_desc(a_lo + ao, lbo_a, sbo_a);
+                    um::mma<C, true>(acc, dah, b_hi + bo, lbo_b, sbo_b, ks > 0 ? 1u : 0u);
+                    um::mma<C, true>(acc, dah, b_lo + bo, lbo_b, sbo_b, 1u);
+                    um::mma<C, true>(acc, dal, b_hi + bo, lbo_b, sbo_b, 1u);
                 }
-            }
-            tc::mma_commit(&bar_mma);
-        }
-        tc::mbar_wait(&bar_mma, 0);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        // TMEM -> T (planar): warp w reads lanes 32*(w%4).. of the tiles t = w/4, w/4 + 2, ...
-        for (int t = warp >> 2; t < n_mt; t += 2) {
-            const int p = t * 128 + (warp & 3) * 32 + lane;
+                um::wg_commit();
+                um::wg_wait_all();
+                um::wg_fence_acc<C / 2>(acc);
 #pragma unroll
-            for (int c0 = 0; c0 < C; c0 += 8) {
-                float v[8];
-                tc::tmem_ld8(tmem_base + ((uint32_t)((warp & 3) * 32) << 16) + (uint32_t)(t * C + c0), v);
-                if (p < n_px) {
-                    sT[(c0 / 4) * n_pxp + p] = make_float4(v[0], v[1], v[2], v[3]);
-                    sT[(c0 / 4 + 1) * n_pxp + p] = make_float4(v[4], v[5], v[6], v[7]);
+                for (int h = 0; h < 2; ++h) {
+                    const int p = u * 64 + row + 8 * h;
+                    if (p < n_px) {
+#pragma unroll
+                        for (int i = 0; i < C / 8; ++i) {
+                            const int c = 8 * i + cq;
+                            *reinterpret_cast<float2*>(sTf + ((size_t)(c >> 2) * n_pxp + p) * 4 + (c & 3)) =
+                                make_float2(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
+                        }
+                    }
                 }
             }
         }
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
         __syncthreads();
-        if (warp == 0)
-            asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(tmem_cols) : "memory");
         sD = sD2;
         sP = sD2 + 9 * C;
     } else {
@@ -1205,7 +1193,7 @@ struct BlockW {
     size_t g1w, g1b, g2w, g2b;
     size_t cw, cb;
     TcW tc_c1, tc_c;
-    TcW light_tc[10];   // LightConv 1x1 weights packed for the tcgen05 stage (mid % 16 == 0)
+    TcW light_tc[10];   // LightConv 1x1 weights packed for the tensor-core stage (mid % 16 == 0)
 };
 
 namespace tcx { struct Plan; }
@@ -1230,13 +1218,14 @@ struct ReidModel {
     TcW tc_trans[2], tc_c5;
     float* d_wtc = nullptr;    // all packed tensor-core weights
     bool use_tc = false;
-    bool pw_small = true;   // 128-thread pointwise CTAs (measured 3 % faster than 256); BOXMOT_B200_PW_SMALL=0 for the 256-thread shape
+    int sms = sm_count();   // streaming multiprocessors of the device the model was loaded on (grid sizes)
+    bool pw_small = true;   // 128-thread pointwise CTAs; BOXMOT_B200_PW_SMALL=0 for the 256-thread shape
     bool pw_v2 = true;      // BOXMOT_B200_PW_V1=1 selects the first-generation pointwise GEMM (A/B runs)
     bool light_small = false;  // BOXMOT_B200_LIGHT_SMALL=1: stage-2 LightConv as 8-row tiles, 128 threads, 4 CTAs / SM
-    bool light_tc = false;     // BOXMOT_B200_LIGHT_TC=1: the stage-2 LightConv 1x1 stage on tcgen05 (tf32 x3)
+    bool light_tc = false;     // BOXMOT_B200_LIGHT_TC=1: the stage-2 LightConv 1x1 stage on the tensor cores (tf32 x3)
     bool light_chain = true;   // BOXMOT_B200_LIGHT_CHAIN=0: per-level LightConv launches instead of whole-branch CTAs
-    int chain_var = 2;         // BOXMOT_B200_CHAIN_VAR: 2 (default) stage 2 per level + stages 3-4 chained (measured best:
-                               // 8-row stage-2 chain tiles recompute 25 % halo rows); 0 all chained; 1 stage-2 chain
+    int chain_var = 2;         // BOXMOT_B200_CHAIN_VAR: 2 (default) stage 2 per level + stages 3-4 chained (8-row
+                               // stage-2 chain tiles recompute 25 % halo rows); 0 all chained; 1 stage-2 chain
                                // tiles of 16 rows with 512 threads (1 CTA / SM)
     bool light_v2 = true;   // BOXMOT_B200_LIGHT_V1=1 selects the first-generation LightConv kernel (A/B runs)
     // workspace for one chunk of crops
@@ -1255,7 +1244,7 @@ struct ReidModel {
     double prof_ms[REID_N_CLASSES] = {0};
     int prof_launches[REID_N_CLASSES] = {0};
     int preprocess = 0;        // 0 resize, 1 resize_pad
-    tcx::Plan* tc = nullptr;   // tensor-core path (tcgen05 + TMA, reid_tc.cuh): the default for the widths it covers
+    tcx::Plan* tc = nullptr;   // tensor-core path (wgmma + TMA, reid_tc.cuh): the default for the widths it covers
     int debug_stop = -1;       // stop after this stage index and leave the tensor in debug_ptr
     const float* debug_ptr = nullptr;
     size_t debug_floats_per_crop = 0;
@@ -1389,11 +1378,11 @@ ReidModel* reid_load(const char* path) {
         if (o != n_floats) throw std::runtime_error("ReID blob size does not match its header");
         RCUDA_OK(cudaMalloc(&m->d_w, sizeof(float) * n_floats));
         RCUDA_OK(cudaMemcpy(m->d_w, host.data(), sizeof(float) * n_floats, cudaMemcpyHostToDevice));
-        {   // tensor-core copies of every 1x1 weight that fits the tcgen05 kernel's shared-memory budget
+        {   // tensor-core copies of every 1x1 weight that fits the tensor-core kernel's accumulators and shared memory
             const char* env = getenv("BOXMOT_B200_REID_TC");
-            // Measured in round 1 (profiles/r1_tcgen05_pointwise.md): at OSNet_x0_25's K,N <= 128 every 1x1 layer is
-            // bandwidth-bound and the float32 CUDA-core GEMM is 1.2-1.8x faster than this first (unpipelined)
-            // tcgen05 kernel, so the tensor-core path is opt-in until it is pipelined / fused.
+            // At OSNet_x0_25's K,N <= 128 every 1x1 layer is bandwidth-bound, and on an H100 this unpipelined kernel is
+            // 1.1-2.4x slower than the float32 CUDA-core GEMM (tests/test_gpu_pointwise_tc.py prints both), so the
+            // standalone tensor-core GEMM is opt-in.
             m->use_tc = env && env[0] == '1';
             const char* lv = getenv("BOXMOT_B200_LIGHT_V1");
             m->light_v2 = !(lv && lv[0] == '1');
@@ -1409,7 +1398,7 @@ ReidModel* reid_load(const char* path) {
             std::vector<Todo> todo;
             auto add = [&](TcW* dst, size_t w, int K, int N) {
                 const int Kpad = (K + 7) / 8 * 8, Npad = (N + 15) / 16 * 16;
-                if (Npad > 256 || tc::smem_bytes(Kpad, Npad) > 200 * 1024) return;
+                if (Npad > tc::NPAD_MAX || tc::smem_bytes(Kpad, Npad) > 200 * 1024) return;
                 dst->Kpad = Kpad; dst->Npad = Npad;
                 todo.push_back({dst, w, K, N, packed.size()});
                 packed.resize(packed.size() + 2 * (size_t)Npad * Kpad);
@@ -1527,12 +1516,10 @@ struct Launcher {
         t.gates = a.gates; t.w_tc = a.w_tc; t.bias = a.bias; t.residual = a.residual; t.out = a.out;
         t.K = a.K; t.N = a.N; t.Kpad = a.Kpad; t.Npad = a.Npad; t.mid = a.mid; t.HW = a.HW; t.relu = a.relu;
         const size_t smem = tc::smem_bytes(a.Kpad, a.Npad);
-        const int tmem_cols = a.Npad <= 32 ? 32 : (a.Npad <= 64 ? 64 : (a.Npad <= 128 ? 128 : 256));
         int per_sm = (int)((220 * 1024) / (smem + 1024));
-        per_sm = per_sm < 1 ? 1 : (per_sm > 512 / tmem_cols ? 512 / tmem_cols : per_sm);
-        per_sm = per_sm > 8 ? 8 : per_sm;
+        per_sm = per_sm < 1 ? 1 : (per_sm > 8 ? 8 : per_sm);
         const int tiles = (int)(((size_t)upper * a.HW) / tc::TILE_M);
-        const int grid = tiles < 148 * per_sm ? tiles : 148 * per_sm;
+        const int grid = tiles < m->sms * per_sm ? tiles : m->sms * per_sm;
         begin(CLS_POINTWISE);
         if (a.gates) {
             RCUDA_OK(cudaFuncSetAttribute(tc::k_pointwise_tc<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -1629,7 +1616,7 @@ struct Launcher {
             launch_light2<16, 32, 8, 2, 4, false, 128>(a, n_branches);
             return true;
         }
-        if (m->light_tc && a.C == 16 && a.W == 32 && a.R == 16 && a.wtc[0]) {   // tcgen05 1x1 stage (opt-in)
+        if (m->light_tc && a.C == 16 && a.W == 32 && a.R == 16 && a.wtc[0]) {   // tensor-core 1x1 stage (opt-in)
             launch_light2<16, 32, 16, 4, 2, true>(a, n_branches);
             return true;
         }
@@ -1699,7 +1686,7 @@ int reid_forward(ReidModel* m, const uint8_t* d_images, size_t image_stride, int
             float* X = m->bufA;
             float* Xo = m->bufB;
             L.begin(CLS_STEM);
-            k_stem3<<<148 * 8, 256, 0, st>>>(m->blob, W + m->mb_stem_w, W + m->mb_stem_b, m->mb_stemp, d_ncrops, off,
+            k_stem3<<<m->sms * 8, 256, 0, st>>>(m->blob, W + m->mb_stem_w, W + m->mb_stem_b, m->mb_stemp, d_ncrops, off,
                                               upper, X);
             L.end();
             ++L.launches;
@@ -1710,7 +1697,7 @@ int reid_forward(ReidModel* m, const uint8_t* d_images, size_t image_stride, int
                 e.K = b.cinp; e.N = b.midp; e.HW = H * Wd; e.relu = 2;
                 L.pointwise(e);
                 L.begin(CLS_LIGHTCONV);
-                k_dwconv3<<<148 * 8, 256, 0, st>>>(m->x1, H, Wd, b.midp, b.stride, W + b.wd, W + b.bd, d_ncrops, off,
+                k_dwconv3<<<m->sms * 8, 256, 0, st>>>(m->x1, H, Wd, b.midp, b.stride, W + b.wd, W + b.bd, d_ncrops, off,
                                                     upper, m->Y[0][0]);
                 L.end();
                 ++L.launches;
@@ -1779,7 +1766,7 @@ int reid_forward(ReidModel* m, const uint8_t* d_images, size_t image_stride, int
         }
         if (stop_here(m->bufA, (size_t)8192 * m->c[0])) { launches += L.launches; continue; }
         L.begin(CLS_MAXPOOL);
-        k_maxpool3s2<<<148 * 8, 256, 0, st>>>(m->bufA, 128, 64, m->c[0], d_ncrops, off, upper, m->bufB);
+        k_maxpool3s2<<<m->sms * 8, 256, 0, st>>>(m->bufA, 128, 64, m->c[0], d_ncrops, off, upper, m->bufB);
         L.end();
         ++L.launches;
         if (stop_here(m->bufB, (size_t)2048 * m->c[0])) { launches += L.launches; continue; }
@@ -1858,7 +1845,7 @@ int reid_forward(ReidModel* m, const uint8_t* d_images, size_t image_stride, int
                 p.w_tc = m->tc_trans[s].w; p.Kpad = m->tc_trans[s].Kpad; p.Npad = m->tc_trans[s].Npad;
                 L.pointwise(p);
                 L.begin(CLS_AVGPOOL);
-                k_avgpool2<<<148 * 4, 256, 0, st>>>(Xo, H, Wd, C, d_ncrops, off, upper, X);
+                k_avgpool2<<<m->sms * 4, 256, 0, st>>>(Xo, H, Wd, C, d_ncrops, off, upper, X);
                 L.end();
                 ++L.launches;
                 H /= 2; Wd /= 2;
@@ -1916,7 +1903,7 @@ void standalone_pointwise(const float* A, int M, int K, const float* W, int N, c
         if (use_tc) {
             if (M % tc::TILE_M) throw std::runtime_error("tensor-core path needs M % 128 == 0");
             const int Kpad = (K + 7) / 8 * 8, Npad = (N + 15) / 16 * 16;
-            if (Npad > 256 || tc::smem_bytes(Kpad, Npad) > 200 * 1024) throw std::runtime_error("shape exceeds the tcgen05 kernel's shared-memory budget");
+            if (Npad > tc::NPAD_MAX || tc::smem_bytes(Kpad, Npad) > 200 * 1024) throw std::runtime_error("shape exceeds the tensor-core kernel's accumulators or shared memory");
             std::vector<float> packed(2 * (size_t)Npad * Kpad);
             tc::pack_weights(W, K, N, Kpad, Npad, packed.data());
             RCUDA_OK(cudaMalloc(&dWtc, sizeof(float) * packed.size()));

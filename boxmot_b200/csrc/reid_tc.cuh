@@ -1,29 +1,27 @@
-// reid_tc.cuh -- the Blackwell-native OSNet path: every 1x1 convolution of the network runs on the 5th-generation tensor
-// cores (tcgen05.mma kind::f16 on split-BF16 operands, FP32 accumulators in TMEM), activations travel between kernels as
+// reid_tc.cuh -- the tensor-core OSNet path for Hopper: every 1x1 convolution of the network runs as wgmma (BF16 split
+// operands read from shared memory, FP32 accumulators in registers), activations travel between kernels as
 // channel-blocked BF16 "hi + lo" planes that TMA boxes (cp.async.bulk.tensor, zero fill = convolution padding) drop
-// straight into the UMMA canonical layout, the depthwise 3x3 / bias / ReLU / gate / pooling epilogues run on the CUDA
-// cores between the MMAs.
+// straight into the canonical no-swizzle K-major operand layout, the depthwise 3x3 / bias / ReLU / gate / pooling
+// epilogues run on the CUDA cores between the MMAs.
 //
-// Replaces (relative to /root/reference/boxmot):  reid/backbones/osnet.py:63-155 (Conv1x1, Conv1x1Linear,
-// LightConv3x3), :161-210 (ChannelGate), :212-260 (OSBlock), :380-405 (featuremaps after the stem) in eval mode.
+// Replaces (relative to boxmot):  reid/backbones/osnet.py:63-155 (Conv1x1, Conv1x1Linear, LightConv3x3), :161-210
+// (ChannelGate), :212-260 (OSBlock), :380-405 (featuremaps after the stem) in eval mode.
 //
 // Numerics: a float32 value x is carried as hi = bf16(x), lo = bf16(x - hi) (|x - hi - lo| <= 2^-17 |x|); a product
 // A*W is evaluated as  A_hi*W_hi + A_lo*W_hi + A_hi*W_lo  with FP32 accumulation (the dropped lo*lo term is 2^-16
-// relative).  Measured on B200 (profiles/r2_tc_probe.jsonl): 4-6e-6 of the output scale per GEMM, and a
-// tcgen05.mma with M = 128 costs ~75 cycles whatever N <= 128 is -- so the three products are issued as TWO
-// instructions per K step: A_hi x [W_hi | W_lo] (N' = 2N columns) and A_lo x W_hi (first N columns), and the
-// epilogue adds the two column groups.
+// relative).  Where the weights are stored as [W_hi | W_lo] along the output channel, A_hi x [W_hi | W_lo] is one
+// wgmma of 2N columns and A_lo x W_hi accumulates into its first N columns; the epilogue adds the two column groups.
 //
 // Kernels:
 //   k_chain_tc   one OSBlock branch (1-4 LightConv3x3 = 1x1 -> depthwise 3x3 -> BN -> ReLU) per CTA on a haloed row
-//                tile: TMA box of conv1's output -> [MMA 1x1 -> TMEM -> T (smem, fp32) -> depthwise on CUDA cores ->
-//                split planes in place] x depth -> branch output planes + channel sums for the gate.
-//   k_gemm_tc    warp-specialised pointwise GEMM (TMA producer warp / MMA issuer warp / 8 epilogue warps) over 128-pixel
-//                tiles: A = up to two plane tensors streamed through an mbarrier ring, B resident in shared memory
-//                (optionally  gate (x) conv3  folded per crop), epilogue bias + ReLU -> planes, optional 2x2 average
-//                pool, optional float32 NHWC copy, optional second GEMM on the fresh tile (next block's conv1).
+//                tile: TMA box of conv1's output -> [wgmma 1x1 -> T (smem, fp32) -> depthwise on CUDA cores -> split
+//                planes in place] x depth -> branch output planes + channel sums for the gate.
+//   k_gemm_tc    warp-specialised pointwise GEMM (TMA producer warp / two consumer warpgroups, 64 pixels each) over
+//                128-pixel tiles: A = up to two plane tensors streamed through an mbarrier ring, B resident in shared
+//                memory (optionally  gate (x) conv3  folded per crop), epilogue bias + ReLU -> planes, optional 2x2
+//                average pool, optional float32 NHWC copy, optional second GEMM on the fresh tile (next block's conv1).
 #pragma once
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace bmb {
 namespace tcx {
@@ -35,9 +33,7 @@ __device__ __forceinline__ int tc_chunk_count(const int* d_n, int off, int cap) 
     n = n < 0 ? 0 : n;
     return n > cap ? cap : n;
 }
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(um::smem_u32(bar)) : "memory");
-}
+using um::mbar_arrive;
 
 // ------------------------------------------------------------------------------------------------------------------
 // maxpool 3x3 stride 2 pad 1 on the stem output (float32 NHWC) -> split planes  [crops][C/8][H/2][W/2][8]
@@ -178,8 +174,8 @@ __device__ void gates_fold(const GatesTcArgs& a, const int n, float* mean /*128*
 // k_chain_tc: one branch of an OSBlock per CTA.  grid = (row tiles, 4 branches (deepest first), crops), 256 threads.
 // Shared memory: X hi / lo planes [CP/8][NPX][8] (NPX = (R + 8) padded rows of W + 2 pixels; the TMA box of conv1's
 // output lands here with zero fill outside the image = every layer's zero padding), T [CP/4][NPXT] float4 (1x1 result),
-// two weight slots.  Per level: one thread issues 2 MMAs per 128-pixel tile and K step, all warps move the TMEM
-// accumulators into T, then column walkers (3x3 register window, as in the float32 kernels of round 1) apply the
+// two weight slots.  Per level: each warpgroup takes every other 64-pixel slice of the rows the level reads, runs two
+// wgmma chains per slice (A_hi x [W_hi | W_lo], A_lo x W_hi) and adds the column groups into T, then column walkers (3x3 register window, as in the float32 kernels of round 1) apply the
 // depthwise taps + bias + ReLU and write the next level's X as hi / lo planes in place; the last level goes to the
 // branch-output planes in HBM and leaves per-tile channel sums for the ChannelGate.
 // ------------------------------------------------------------------------------------------------------------------
@@ -203,9 +199,10 @@ struct ChainGeom {
     static constexpr int X_BYTES = (CP / 8) * NPX * 16;               // one of hi / lo
     static constexpr int T_BYTES = (CR / 4) * NPXT * 16;               // only the real channels pass through T
     static constexpr int WSLOT_BYTES = (CP / 8) * 2 * CP * 16 + 9 * CP * 4 + CP * 4;
-    static constexpr int TMEM_COLS = NT_MAX * 2 * CP;
-    // the last M tile may read past the planes: keep one tile of slack after X so those reads stay inside the allocation
-    static constexpr size_t SMEM = 2 * (size_t)X_BYTES + T_BYTES + 2 * WSLOT_BYTES + 128;
+    // the slices of a level end on a 128-pixel boundary, up to 127 pixels past the planes: hi runs into lo (not written
+    // while MMAs run), lo into a slack of 128 pixels, so no MMA reads shared memory that another warpgroup writes
+    static constexpr int X_SLACK = 128 * 16;
+    static constexpr size_t SMEM = 2 * (size_t)X_BYTES + X_SLACK + T_BYTES + 2 * WSLOT_BYTES + 128;
 };
 
 template <int CP, int CR, int W, int R, int NSPLIT>
@@ -218,14 +215,13 @@ __global__ void __launch_bounds__(256) k_chain_tc(const __grid_constant__ ChainT
     const int H = a.H;
     constexpr int TW = G::TW, NPX = G::NPX, NPXT = G::NPXT, C8 = CP / 8, C4 = CR / 4, KS = CP / 16;
     extern __shared__ __align__(128) unsigned char smem[];
-    __shared__ __align__(8) uint64_t bar_tma, bar_mma, bar_w[2];
-    __shared__ uint32_t tmem_slot;
+    __shared__ __align__(8) uint64_t bar_tma, bar_w[2];
     unsigned char* sXh = smem;
     unsigned char* sXl = sXh + G::X_BYTES;
-    float4* sT = reinterpret_cast<float4*>(sXl + G::X_BYTES);
+    float4* sT = reinterpret_cast<float4*>(sXl + G::X_BYTES + G::X_SLACK);
     unsigned char* sWs = reinterpret_cast<unsigned char*>(sT) + G::T_BYTES;
     float* sP = reinterpret_cast<float*>(sT);                     // [256 / C4][CR] channel-sum slots (after the last level)
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int lane = threadIdx.x & 31;
     const int y0 = tile * R, g0 = y0 - 4;
 #ifdef BMB_TC_CLOCKS
     long long ck[24];
@@ -238,8 +234,8 @@ __global__ void __launch_bounds__(256) k_chain_tc(const __grid_constant__ ChainT
 
     // weights of level lv (1-based) -> slot (lv & 1): two bulk copies by thread 0 (the packed [W_hi | W_lo] block, and the
     // depthwise taps + bias, which the plan stores back to back), completing on the slot's barrier.  The copy for level
-    // lv + 1 is issued while level lv's MMAs run; nobody waits on global memory (plain loads by all threads stalled
-    // every level for 800 - 2 800 cycles).
+    // lv + 1 is issued while level lv's MMAs run; nobody waits on global memory (plain loads by all threads would stall
+    // every level).
     constexpr uint32_t PW_BYTES = C8 * 2 * CP * 16, DW_BYTES = 10 * CP * 4;
     auto fetch_weights = [&](int lv) {
         unsigned char* dst = sWs + (size_t)(lv & 1) * G::WSLOT_BYTES;
@@ -248,11 +244,10 @@ __global__ void __launch_bounds__(256) k_chain_tc(const __grid_constant__ ChainT
         um::bulk_g2s(dst + PW_BYTES, a.wdw[l0 + lv - 1], DW_BYTES, &bar_w[lv & 1]);
     };
 
-    // the input box first (its latency overlaps the TMEM allocation and the weight staging): thread 0 initialises the
-    // barriers, publishes them to the async proxy and issues the two TMA loads by itself
+    // the input box first (its latency overlaps the weight staging): thread 0 initialises the barriers, publishes them
+    // to the async proxy and issues the two TMA loads by itself
     if (threadIdx.x == 0) {
         um::mbar_init(&bar_tma, 1);
-        um::mbar_init(&bar_mma, 1);
         um::mbar_init(&bar_w[0], 1);
         um::mbar_init(&bar_w[1], 1);
         um::fence_mbar_init();
@@ -261,11 +256,7 @@ __global__ void __launch_bounds__(256) k_chain_tc(const __grid_constant__ ChainT
         um::tma_load_4d(sXl, &a.map_lo, -4, g0, 0, n, &bar_tma);
         fetch_weights(1);
     }
-    if (warp == 1) um::tmem_alloc(&tmem_slot, um::tmem_cols_pow2(G::TMEM_COLS));
-    um::tc_fence_before();
     __syncthreads();
-    um::tc_fence_after();
-    const uint32_t tmem = tmem_slot;
     TCK();
     um::mbar_wait(&bar_tma, 0);
     TCK();
@@ -278,7 +269,6 @@ __global__ void __launch_bounds__(256) k_chain_tc(const __grid_constant__ ChainT
     constexpr int n_split_max = (act / walkers) < 1 ? 1 : (act / walkers);
     constexpr int n_split = NSPLIT > 0 && NSPLIT < n_split_max ? NSPLIT : n_split_max;
     float4 psum = make_float4(0.f, 0.f, 0.f, 0.f);
-    uint32_t mma_phase = 0;
 
     for (int lv = 1; lv <= depth; ++lv) {
         const int ext = depth - lv;
@@ -287,55 +277,44 @@ __global__ void __launch_bounds__(256) k_chain_tc(const __grid_constant__ ChainT
         const int pa = (la - 1) * TW, pb = (lb + 1) * TW;      // pixels whose 1x1 result it reads
         const int t0 = pa >> 7, t1 = (pb + 127) >> 7;
         um::mbar_wait(&bar_w[lv & 1], (uint32_t)((lv - 1) >> 1) & 1u);     // this level's weights (k-th use of the slot)
-        if (threadIdx.x == 0) {
-            // the other slot was last read by level lv - 1 (its MMAs were waited for, its walkers passed the barrier)
-            if (lv < depth) fetch_weights(lv + 1);
-            const uint32_t id2 = um::idesc_bf16(128, 2 * CP), id1 = um::idesc_bf16(128, CP);
+        // the other slot was last read by level lv - 1 (its MMAs were waited for, its walkers passed the barrier)
+        if (threadIdx.x == 0 && lv < depth) fetch_weights(lv + 1);
+        TCK();
+        {   // ---- 1x1 on the tensor cores, T = (A_hi W_hi + A_lo W_hi) + A_hi W_lo, one 64-pixel slice at a time ----
             const uint32_t lbo_a = (uint32_t)NPX * 16u, lbo_b = 2u * CP * 16u;
             const uint32_t xh = um::smem_u32(sXh), xl = um::smem_u32(sXl), wb = um::smem_u32(wslot);
-            for (int t = t0; t < t1; ++t)
+            const int wg = threadIdx.x >> 7, row = ((threadIdx.x >> 5) & 3) * 16 + (lane >> 2), cq = 2 * (lane & 3);
+            float* sTf = reinterpret_cast<float*>(sT);
+            for (int u = 2 * t0 + wg; u < 2 * t1; u += 2) {
+                float acc[CP];
+                um::wg_fence();
 #pragma unroll
                 for (int ks = 0; ks < KS; ++ks)
-                    um::mma_bf16(tmem + (uint32_t)((t - t0) * 2 * CP), um::make_desc(xh + (uint32_t)t * 2048u + ks * 2 * lbo_a, lbo_a, 128),
-                                 um::make_desc(wb + ks * 2 * lbo_b, lbo_b, 128), id2, ks > 0);
-            for (int t = t0; t < t1; ++t)
+                    um::mma<2 * CP, false>(acc, um::make_desc(xh + (uint32_t)u * 1024u + ks * 2 * lbo_a, lbo_a, 128), wb + ks * 2 * lbo_b,
+                                           lbo_b, 128, ks > 0);
 #pragma unroll
                 for (int ks = 0; ks < KS; ++ks)
-                    um::mma_bf16(tmem + (uint32_t)((t - t0) * 2 * CP), um::make_desc(xl + (uint32_t)t * 2048u + ks * 2 * lbo_a, lbo_a, 128),
-                                 um::make_desc(wb + ks * 2 * lbo_b, lbo_b, 128), id1, 1);
-            um::mma_commit(&bar_mma);
-        }
-        TCK();
-        um::mbar_wait(&bar_mma, mma_phase);
-        mma_phase ^= 1u;
-        um::tc_fence_after();
-        TCK();
-        // ---- TMEM -> T: warp = (lane quadrant, tile parity); T = (A_hi W_hi + A_lo W_hi) + A_hi W_lo ----
-        {
-            const int q = warp & 3;
-            for (int slot = warp >> 2; slot < t1 - t0; slot += 2) {
-                const int p = (t0 + slot) * 128 + q * 32 + lane;
+                    um::mma<CP, false>(acc, um::make_desc(xl + (uint32_t)u * 1024u + ks * 2 * lbo_a, lbo_a, 128), wb + ks * 2 * lbo_b,
+                                       lbo_b, 128, 1);
+                um::wg_commit();
+                um::wg_wait_all();
+                um::wg_fence_acc<CP>(acc);
 #pragma unroll
-                for (int c0 = 0; c0 < CP; c0 += 16) {
-                    uint32_t v1[16], v2[16];
-                    const uint32_t ta = tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(slot * 2 * CP + c0);
-                    um::tmem_ld16(ta, v1);
-                    um::tmem_ld16(ta + CP, v2);
-                    um::tmem_ld_wait();
+                for (int h = 0; h < 2; ++h) {
+                    const int p = u * 64 + row + 8 * h;
                     if (p < NPX) {
 #pragma unroll
-                        for (int j = 0; j < 4; ++j) {
-                            const float2 lo2 = __fadd2_rn(make_float2(__uint_as_float(v1[4 * j]), __uint_as_float(v1[4 * j + 1])),
-                                                          make_float2(__uint_as_float(v2[4 * j]), __uint_as_float(v2[4 * j + 1])));
-                            const float2 hi2 = __fadd2_rn(make_float2(__uint_as_float(v1[4 * j + 2]), __uint_as_float(v1[4 * j + 3])),
-                                                          make_float2(__uint_as_float(v2[4 * j + 2]), __uint_as_float(v2[4 * j + 3])));
-                            if (c0 / 4 + j < C4) sT[(c0 / 4 + j) * NPXT + p] = make_float4(lo2.x, lo2.y, hi2.x, hi2.y);
+                        for (int i = 0; i < CP / 8; ++i) {
+                            const int c = 8 * i + cq;
+                            if (c / 4 < C4)
+                                *reinterpret_cast<float2*>(sTf + ((size_t)(c >> 2) * NPXT + p) * 4 + (c & 3)) =
+                                    um::fadd2(make_float2(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]),
+                                              make_float2(acc[CP / 2 + 4 * i + 2 * h], acc[CP / 2 + 4 * i + 2 * h + 1]));
                         }
                     }
                 }
             }
         }
-        um::tc_fence_before();
         __syncthreads();
         TCK();
         // ---- depthwise 3x3 + bias + ReLU on image rows [ya, yb): next level's X (planes, in place) or the branch output ----
@@ -350,7 +329,7 @@ __global__ void __launch_bounds__(256) k_chain_tc(const __grid_constant__ ChainT
                 const int c4 = wk % C4, x = (wk / C4) % W, sp = wk / walkers;
                 const int ra = ya + sp * rows_per, rb = min(ra + rows_per, yb);
                 if (ra >= rb) continue;
-                // packed FP32x2 arithmetic (FFMA2, sm_100): two channels per instruction, IEEE per lane
+                // channel pairs: two independent IEEE chains per pair, never contracted
                 float2 wv[9][2];
 #pragma unroll
                 for (int t = 0; t < 9; ++t) {
@@ -389,20 +368,20 @@ __global__ void __launch_bounds__(256) k_chain_tc(const __grid_constant__ ChainT
                     tp += TW;                                                                                          \
                     /* three independent partial sums per channel pair (one per window row): 6 chains of 3 FFMA2 */   \
                     float2 a0 = bv0, a1 = bv1;                                                                         \
-                    float2 b0 = __fmul2_rn(win[i1][0][0], wv[3][0]), b1 = __fmul2_rn(win[i1][0][1], wv[3][1]);          \
-                    float2 c0 = __fmul2_rn(win[i2][0][0], wv[6][0]), c1 = __fmul2_rn(win[i2][0][1], wv[6][1]);          \
-                    a0 = __ffma2_rn(win[i0][0][0], wv[0][0], a0);                                                      \
-                    a1 = __ffma2_rn(win[i0][0][1], wv[0][1], a1);                                                      \
+                    float2 b0 = um::fmul2(win[i1][0][0], wv[3][0]), b1 = um::fmul2(win[i1][0][1], wv[3][1]);          \
+                    float2 c0 = um::fmul2(win[i2][0][0], wv[6][0]), c1 = um::fmul2(win[i2][0][1], wv[6][1]);          \
+                    a0 = um::ffma2(win[i0][0][0], wv[0][0], a0);                                                      \
+                    a1 = um::ffma2(win[i0][0][1], wv[0][1], a1);                                                      \
                     _Pragma("unroll") for (int kx = 1; kx < 3; ++kx) {                                                 \
-                        a0 = __ffma2_rn(win[i0][kx][0], wv[kx][0], a0);                                                \
-                        a1 = __ffma2_rn(win[i0][kx][1], wv[kx][1], a1);                                                \
-                        b0 = __ffma2_rn(win[i1][kx][0], wv[3 + kx][0], b0);                                            \
-                        b1 = __ffma2_rn(win[i1][kx][1], wv[3 + kx][1], b1);                                            \
-                        c0 = __ffma2_rn(win[i2][kx][0], wv[6 + kx][0], c0);                                            \
-                        c1 = __ffma2_rn(win[i2][kx][1], wv[6 + kx][1], c1);                                            \
+                        a0 = um::ffma2(win[i0][kx][0], wv[kx][0], a0);                                                \
+                        a1 = um::ffma2(win[i0][kx][1], wv[kx][1], a1);                                                \
+                        b0 = um::ffma2(win[i1][kx][0], wv[3 + kx][0], b0);                                            \
+                        b1 = um::ffma2(win[i1][kx][1], wv[3 + kx][1], b1);                                            \
+                        c0 = um::ffma2(win[i2][kx][0], wv[6 + kx][0], c0);                                            \
+                        c1 = um::ffma2(win[i2][kx][1], wv[6 + kx][1], c1);                                            \
                     }                                                                                                  \
-                    a0 = __fadd2_rn(__fadd2_rn(a0, b0), c0);                                                           \
-                    a1 = __fadd2_rn(__fadd2_rn(a1, b1), c1);                                                           \
+                    a0 = um::fadd2(um::fadd2(a0, b0), c0);                                                           \
+                    a1 = um::fadd2(um::fadd2(a1, b1), c1);                                                           \
                     a0.x = fmaxf(a0.x, 0.f); a0.y = fmaxf(a0.y, 0.f);                                                  \
                     a1.x = fmaxf(a1.x, 0.f); a1.y = fmaxf(a1.y, 0.f);                                                  \
                     uint32_t h0, h1, e0, e1;                                                                           \
@@ -412,8 +391,8 @@ __global__ void __launch_bounds__(256) k_chain_tc(const __grid_constant__ ChainT
                         *reinterpret_cast<uint2*>(a.y_hi + go) = make_uint2(h0, h1);                                   \
                         *reinterpret_cast<uint2*>(a.y_lo + go) = make_uint2(e0, e1);                                   \
                         go += (size_t)W * 8;                                                                           \
-                        ps0 = __fadd2_rn(ps0, a0);                                                                     \
-                        ps1 = __fadd2_rn(ps1, a1);                                                                     \
+                        ps0 = um::fadd2(ps0, a0);                                                                     \
+                        ps1 = um::fadd2(ps1, a1);                                                                     \
                     } else {                                                                                           \
                         *reinterpret_cast<uint2*>(xh) = make_uint2(h0, h1);                                            \
                         *reinterpret_cast<uint2*>(xl) = make_uint2(e0, e1);                                            \
@@ -446,16 +425,14 @@ __global__ void __launch_bounds__(256) k_chain_tc(const __grid_constant__ ChainT
             }
         }
         um::fence_async_smem();
-        um::tc_fence_before();
         __syncthreads();
-        um::tc_fence_after();
         TCK();
     }
 #ifdef BMB_TC_CLOCKS
     if (threadIdx.x == 0 && blockIdx.x == 1 && n == 5) {
         printf("chain CP%d W%d br%d: setup %lld tma %lld |", CP, W, br, ck[1] - ck[0], ck[2] - ck[1]);
-        for (int i = 2; i + 4 < nck + 1 && i + 4 <= 23; i += 4)
-            printf(" issue %lld mma %lld epi %lld dw %lld |", ck[i + 1] - ck[i], ck[i + 2] - ck[i + 1], ck[i + 3] - ck[i + 2], ck[i + 4] - ck[i + 3]);
+        for (int i = 2; i + 3 < nck + 1 && i + 3 <= 23; i += 3)
+            printf(" wait %lld mma %lld dw %lld |", ck[i + 1] - ck[i], ck[i + 2] - ck[i + 1], ck[i + 3] - ck[i + 2]);
         printf(" total %lld\n", ck[nck - 1] - ck[0]);
     }
 #endif
@@ -469,10 +446,8 @@ __global__ void __launch_bounds__(256) k_chain_tc(const __grid_constant__ ChainT
             for (int g = 0; g < n_grp; ++g) s += sP[g * CR + c];
         a.sums[br][((size_t)n * gridDim.x + tile) * CP + c] = s;
     }
-    um::tc_fence_before();
     __threadfence();                                   // publish the sums before counting this CTA in
     __syncthreads();
-    if (warp == 1) um::tmem_dealloc(tmem, um::tmem_cols_pow2(G::TMEM_COLS));
     // the last CTA of the crop (tiles x 4 branches) turns the sums into gates and folds them into conv3
     __shared__ int s_last;
     __shared__ float s_mean[128], s_hid[16], s_gate[128];
@@ -520,10 +495,10 @@ constexpr int chain_rows() { return R; }
 
 // ------------------------------------------------------------------------------------------------------------------
 // k_gemm_tc: out[p][n] = act( sum_src sum_k A_src[p][k] * B[k][n] + bias[n] ) over 128-pixel tiles of a crop.
-// grid = (tile groups, crops), 320 threads: warp 0 = TMA producer, warp 1 = MMA issuer (+ TMEM owner),
-// warps 2..9 = epilogue (lane quadrant = warp % 4, column half = (warp - 2) / 4).
+// grid = (tile groups, crops), 288 threads: warps 0-7 = two consumer warpgroups (warpgroup g owns pixels 64 g .. 64 g + 63
+// of every tile: wgmma into registers, then the epilogue on its own rows), warp 8 = TMA producer.
 // ------------------------------------------------------------------------------------------------------------------
-constexpr int GEMM_THREADS = 320;
+constexpr int GEMM_THREADS = 288;
 
 struct GemmTcArgs {
     CUtensorMap map_hi[2], map_lo[2];   // A sources: box (64 pixels, 2, kc planes, 1 crop)
@@ -533,7 +508,6 @@ struct GemmTcArgs {
     int rows_per_tile;                  // 128 / W
     int tiles_per_crop, tiles_per_cta;
     int n_stage;                        // ring depth
-    int acc_bufs;                       // accumulators of the first GEMM in TMEM (2: the next tile's MMAs overlap this tile's epilogue)
     // B: rows [0, gate_rows) are built in the kernel as  gate[b][c] * w3[c][n]  (row = b * midp + c), the rest is copied
     const bf16* b_packed;               // [K8][2*NP][8] packed [hi | lo]; rows below gate_rows are ignored
     int K8;                             // total planes of K
@@ -591,13 +565,12 @@ inline GemmSmem gemm_smem_layout(int K8, int NP, int NP2, int n_stage, bool tail
     return s;
 }
 
-__global__ void __launch_bounds__(GEMM_THREADS, 2) k_gemm_tc(const __grid_constant__ GemmTcArgs a, const int* __restrict__ d_n, int off, int cap,
+__global__ void __launch_bounds__(GEMM_THREADS, 1) k_gemm_tc(const __grid_constant__ GemmTcArgs a, const int* __restrict__ d_n, int off, int cap,
                                                             const GemmSmem L, const GemmHeadIO hio) {
     const int n = blockIdx.y;
     if (n >= tc_chunk_count(d_n, off, cap)) return;
     extern __shared__ __align__(128) unsigned char smem[];
-    __shared__ __align__(8) uint64_t bar_full[4], bar_empty[4], bar_acc_full[2], bar_acc_empty[2], bar_acc2_full, bar_b_ready, bar_w;
-    __shared__ uint32_t tmem_slot;
+    __shared__ __align__(8) uint64_t bar_full[4], bar_empty[4], bar_w;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int NP = a.NP, NP2 = a.NP2;
     const bool tail = a.b2_packed != nullptr;
@@ -608,43 +581,15 @@ __global__ void __launch_bounds__(GEMM_THREADS, 2) k_gemm_tc(const __grid_consta
     unsigned char* sRing = smem + L.ring;
     unsigned char* sA2 = smem + L.a2;
     float* sF = reinterpret_cast<float*>(smem + L.f);
-    float* sGate = reinterpret_cast<float*>(smem + L.gate);      // [4][32] gates, then [4][32] means
-    // TMEM: acc_bufs accumulators of NP columns (the three split products of a K step land on the same columns), then
-    // the tail's NP2 columns
-    const uint32_t nbuf = (uint32_t)a.acc_bufs;
-    const uint32_t acc_cols = nbuf * NP, acc2_cols = tail ? (uint32_t)NP2 : 0u;
-    const uint32_t tmem_cols = um::tmem_cols_pow2(acc_cols + acc2_cols);
 
     if (threadIdx.x == 0) {
-        for (int i = 0; i < a.n_stage; ++i) { um::mbar_init(&bar_full[i], 1); um::mbar_init(&bar_empty[i], 1); }
-        for (int i = 0; i < 2; ++i) { um::mbar_init(&bar_acc_full[i], 1); um::mbar_init(&bar_acc_empty[i], 256); }
-        um::mbar_init(&bar_acc2_full, 1);
-        um::mbar_init(&bar_b_ready, 256);
+        for (int i = 0; i < a.n_stage; ++i) { um::mbar_init(&bar_full[i], 1); um::mbar_init(&bar_empty[i], 2); }
         um::mbar_init(&bar_w, 1);
         um::fence_mbar_init();
     }
-    if (warp == 1) um::tmem_alloc(&tmem_slot, tmem_cols);
-    um::tc_fence_before();
     __syncthreads();
-    um::tc_fence_after();
-    const uint32_t tmem = tmem_slot;
-#ifdef BMB_TC_CLOCKS
-    const long long gk0 = clock64();
-    long long gk[40];
-    int ngk = 0;
-    const bool gprint = blockIdx.x == 0 && n == 5;
-    __shared__ long long s_gk[2][40];
-    __shared__ int s_ngk[2];
-#define GCK() do { if (ngk < 40) gk[ngk++] = clock64() - gk0; } while (0)
-#else
-#define GCK() do { } while (0)
-#endif
 
-    // chunk table of one tile: (source, first plane, planes)
-    int n_chunks = 0;
-    for (int s = 0; s < a.n_src; ++s) n_chunks += a.src_planes[s] / a.src_kc[s];
-
-    if (warp == 0) {
+    if (warp == 8) {
         // ================= TMA producer =================
         if (lane == 0) {
             {   // packed weights (everything below the gate-folded rows, and the tail's B) by bulk async copies
@@ -657,15 +602,6 @@ __global__ void __launch_bounds__(GEMM_THREADS, 2) k_gemm_tc(const __grid_consta
             }
             uint32_t it = 0;
             for (int tile = tile0; tile < tile1; ++tile) {
-#ifdef BMB_GEMM_L2PF
-                // the ring holds a fraction of a tile: pull the next tile's boxes into L2 while this one streams
-                if (tile + 1 < tile1)
-                    for (int s = 0; s < a.n_src; ++s)
-                        for (int p0 = 0; p0 < a.src_planes[s]; p0 += a.src_kc[s]) {
-                            um::tma_prefetch_4d(&a.map_hi[s], 0, (tile + 1) * 2, p0, n);
-                            um::tma_prefetch_4d(&a.map_lo[s], 0, (tile + 1) * 2, p0, n);
-                        }
-#endif
                 for (int s = 0; s < a.n_src; ++s) {
                     const int kc = a.src_kc[s];
                     for (int p0 = 0; p0 < a.src_planes[s]; p0 += kc, ++it) {
@@ -679,285 +615,204 @@ __global__ void __launch_bounds__(GEMM_THREADS, 2) k_gemm_tc(const __grid_consta
                 }
             }
         }
-    } else if (warp == 1) {
-        // ================= MMA issuer =================
-        if (lane == 0) {
-            const uint32_t id1 = um::idesc_bf16(128, NP);
-            const uint32_t lbo_b = 2u * NP * 16u, lo_off = (uint32_t)NP * 16u;       // a K plane of B = NP rows W_hi, then NP rows W_lo
-            um::mbar_wait(&bar_b_ready, 0);
-            um::mbar_wait(&bar_w, 0);
-            um::tc_fence_after();
-            GCK();
-            uint32_t it = 0, ti = 0;
-            for (int tile = tile0; tile < tile1; ++tile, ++ti) {
-                const uint32_t buf = ti % nbuf, use = ti / nbuf;
-                um::mbar_wait(&bar_acc_empty[buf], (use & 1u) ^ 1u);
-                um::tc_fence_after();
-                GCK();
-                const uint32_t acc = tmem + buf * (uint32_t)NP;
-                uint32_t kplane = 0, first = 1;
-                for (int s = 0; s < a.n_src; ++s) {
-                    const int kc = a.src_kc[s];
-                    for (int p0 = 0; p0 < a.src_planes[s]; p0 += kc, ++it) {
-                        const uint32_t slot = it % (uint32_t)a.n_stage, ph = (it / (uint32_t)a.n_stage) & 1u;
-                        um::mbar_wait(&bar_full[slot], ph);
-                        um::tc_fence_after();
-                        const uint32_t ah = um::smem_u32(sRing + (size_t)slot * a.slot_bytes), al = ah + a.slot_bytes / 2;
-                        for (int ks = 0; ks < kc / 2; ++ks) {
-                            const uint32_t bb = um::smem_u32(sB) + (kplane + 2 * ks) * lbo_b;
-                            const uint64_t dh = um::make_desc(bb, lbo_b, 128), dl = um::make_desc(bb + lo_off, lbo_b, 128);
-                            const uint64_t xh = um::make_desc(ah + ks * 2 * 2048u, 2048u, 128), xl = um::make_desc(al + ks * 2 * 2048u, 2048u, 128);
-                            um::mma_bf16(acc, xh, dh, id1, first ? 0u : 1u);      // A_hi W_hi
-                            um::mma_bf16(acc, xl, dh, id1, 1u);                   // A_lo W_hi
-                            um::mma_bf16(acc, xh, dl, id1, 1u);                   // A_hi W_lo
-                            first = 0;
-                        }
-                        kplane += kc;
-                        um::mma_commit(&bar_empty[slot]);
-                    }
-                }
-                um::mma_commit(&bar_acc_full[buf]);
-                GCK();
-            }
-#ifdef BMB_TC_CLOCKS
-            if (gprint) { for (int i = 0; i < ngk; ++i) s_gk[0][i] = gk[i]; s_ngk[0] = ngk; }
-#endif
-        }
-    } else {
-        // ================= epilogue warps =================
-        const int et = threadIdx.x - 64;                       // 0..255
-        const int q = warp & 3, half = (warp - 2) >> 2;
-        const int m = q * 32 + lane;                           // pixel of the tile = TMEM lane
-        // B arrives by bulk copies (producer warp): the packed rows and, for the combine GEMM, this crop's gate-folded rows
-        um::fence_async_smem();
-        mbar_arrive(&bar_b_ready);
-        GCK();
+        return;
+    }
 
-        const int cw = NP / 2;                                  // columns this warp owns: [half * cw, half * cw + cw)
-        uint32_t ti = 0;
-        for (int tile = tile0; tile < tile1; ++tile, ++ti) {
-            const uint32_t buf = ti % nbuf, use = ti / nbuf;
-            um::mbar_wait(&bar_acc_full[buf], use & 1u);
-            um::tc_fence_after();
-            GCK();
-            const int px = tile * 128 + m;                      // pixel of the crop
-            if (a.head_w) {
-                // ---- conv5 + head: the tile is the whole 16 x 8 map.  Column sums over the 128 TMEM lanes (= pixels):
-                // butterfly over the 32 lanes of a warp, the four lane quadrants through shared memory (the ring is idle:
-                // every slot was consumed before the accumulator was committed) ----
-                float* part = reinterpret_cast<float*>(sRing);          // [4][NP]
-                float* pooled = part + 4 * NP;                          // [NP]
-                float* red = pooled + NP;                               // [8]
-                float* feat = red + 8;                                  // [head_feat]
-                const uint32_t tq = tmem + ((uint32_t)(q * 32) << 16) + buf * (uint32_t)NP;
-                for (int c0 = half * cw; c0 < half * cw + cw; c0 += 8) {
-                    uint32_t v[8];
-                    um::tmem_ld8(tq + c0, v);
-                    um::tmem_ld_wait();
-                    const float4 b0 = *reinterpret_cast<const float4*>(a.bias + c0), b1 = *reinterpret_cast<const float4*>(a.bias + c0 + 4);
-                    const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-                    float o[8];
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        o[j] = fmaxf(__uint_as_float(v[j]) + bb[j], 0.f);
-#pragma unroll
-                        for (int sh = 16; sh > 0; sh >>= 1) o[j] += __shfl_xor_sync(0xffffffffu, o[j], sh);
-                    }
-                    if (lane == 0) {
-                        *reinterpret_cast<float4*>(part + q * NP + c0) = make_float4(o[0], o[1], o[2], o[3]);
-                        *reinterpret_cast<float4*>(part + q * NP + c0 + 4) = make_float4(o[4], o[5], o[6], o[7]);
-                    }
+    // ================= consumer warpgroups =================
+    const int et = threadIdx.x;                                 // 0..255
+    const int wg = warp >> 2;
+    const int row = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // pixel of the tile of accumulator rows h = 0; h = 1 is row + 8
+    const int cq = 2 * (lane & 3);                              // first of the two columns of an 8-column group
+    const uint32_t lbo_b = 2u * NP * 16u, lo_off = (uint32_t)NP * 16u;   // a K plane of B = NP rows W_hi, then NP rows W_lo
+    um::mbar_wait(&bar_w, 0);
+    float acc[64];
+    uint32_t it = 0;
+    for (int tile = tile0; tile < tile1; ++tile) {
+        uint32_t kplane = 0, first = 1;
+        for (int s = 0; s < a.n_src; ++s) {
+            const int kc = a.src_kc[s];
+            for (int p0 = 0; p0 < a.src_planes[s]; p0 += kc, ++it) {
+                const uint32_t slot = it % (uint32_t)a.n_stage, ph = (it / (uint32_t)a.n_stage) & 1u;
+                um::mbar_wait(&bar_full[slot], ph);
+                const uint32_t ah = um::smem_u32(sRing + (size_t)slot * a.slot_bytes) + (uint32_t)wg * 1024u, al = ah + a.slot_bytes / 2;
+                um::wg_fence();
+                for (int ks = 0; ks < kc / 2; ++ks) {
+                    const uint32_t bb = um::smem_u32(sB) + (kplane + 2 * ks) * lbo_b;
+                    const uint64_t xh = um::make_desc(ah + ks * 2 * 2048u, 2048u, 128), xl = um::make_desc(al + ks * 2 * 2048u, 2048u, 128);
+                    um::mma_rt<false>(NP, acc, xh, bb, lbo_b, 128, first ? 0u : 1u);      // A_hi W_hi
+                    um::mma_rt<false>(NP, acc, xl, bb, lbo_b, 128, 1u);                   // A_lo W_hi
+                    um::mma_rt<false>(NP, acc, xh, bb + lo_off, lbo_b, 128, 1u);          // A_hi W_lo
+                    first = 0;
                 }
-                um::tc_fence_before();
-                mbar_arrive(&bar_acc_empty[buf]);
-                asm volatile("bar.sync 1, 256;" ::: "memory");
-                for (int c = et; c < NP; c += 256) pooled[c] = ((part[c] + part[NP + c]) + (part[2 * NP + c] + part[3 * NP + c])) / 128.f;
-                asm volatile("bar.sync 1, 256;" ::: "memory");
-                const int FEAT = a.head_feat, C = a.N;
-                float sq = 0.f;
-                for (int f = et; f < FEAT; f += 256) {
-                    float t[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-                    int c = 0;
-                    for (; c + 8 <= C; c += 8) {
-#pragma unroll
-                        for (int u = 0; u < 8; ++u) t[u] = fmaf(pooled[c + u], a.head_w[(size_t)(c + u) * FEAT + f], t[u]);
-                    }
-                    for (; c < C; ++c) t[0] = fmaf(pooled[c], a.head_w[(size_t)c * FEAT + f], t[0]);
-                    float sv = a.head_b[f] + (((t[0] + t[1]) + (t[2] + t[3])) + ((t[4] + t[5]) + (t[6] + t[7])));
-                    sv = fmaxf(sv, 0.f);
-                    feat[f] = sv;
-                    sq = fmaf(sv, sv, sq);
-                }
-#pragma unroll
-                for (int sh = 16; sh > 0; sh >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, sh);
-                if (lane == 0) red[warp - 2] = sq;
-                asm volatile("bar.sync 1, 256;" ::: "memory");
-                float tot = 0.f;
-                for (int w = 0; w < 8; ++w) tot += red[w];
-                const float nrm = sqrtf(tot);
-                float* dst = hio.out + (size_t)hio.crops[off + n].out_row * hio.out_ld;
-                for (int f = et; f < FEAT; f += 256) dst[f] = feat[f] / nrm;
-                continue;
-            }
-            auto emit = [&](const uint32_t* v1, const int c0) {
-                const float4 b0 = *reinterpret_cast<const float4*>(a.bias + c0), b1 = *reinterpret_cast<const float4*>(a.bias + c0 + 4);
-                float o[8];
-                o[0] = __uint_as_float(v1[0]) + b0.x; o[1] = __uint_as_float(v1[1]) + b0.y;
-                o[2] = __uint_as_float(v1[2]) + b0.z; o[3] = __uint_as_float(v1[3]) + b0.w;
-                o[4] = __uint_as_float(v1[4]) + b1.x; o[5] = __uint_as_float(v1[5]) + b1.y;
-                o[6] = __uint_as_float(v1[6]) + b1.z; o[7] = __uint_as_float(v1[7]) + b1.w;
-                if (a.relu) {
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) o[j] = fmaxf(o[j], 0.f);
-                }
-                if (a.out_f32) {
-                    float* dst = a.out_f32 + ((size_t)n * a.HW + px) * a.N + c0;
-                    if (c0 + 8 <= a.N) {
-                        *reinterpret_cast<float4*>(dst) = make_float4(o[0], o[1], o[2], o[3]);
-                        *reinterpret_cast<float4*>(dst + 4) = make_float4(o[4], o[5], o[6], o[7]);
-                    } else {
-                        for (int j = 0; j < 8; ++j)
-                            if (c0 + j < a.N) dst[j] = o[j];
-                    }
-                }
-                if (a.pool) {
-                    float* f = sF + (size_t)m * (NP + 4) + c0;
-                    *reinterpret_cast<float4*>(f) = make_float4(o[0], o[1], o[2], o[3]);
-                    *reinterpret_cast<float4*>(f + 4) = make_float4(o[4], o[5], o[6], o[7]);
-                } else if (a.out_hi || tail) {
-                    uint32_t h[4], l[4];
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) um::split2(o[2 * j], o[2 * j + 1], h[j], l[j]);
-                    const uint4 hv = make_uint4(h[0], h[1], h[2], h[3]), lv = make_uint4(l[0], l[1], l[2], l[3]);
-                    if (a.out_hi) {
-                        const size_t e = ((size_t)n * (NP / 8) + c0 / 8) * a.HW + px;
-                        reinterpret_cast<uint4*>(a.out_hi)[e] = hv;
-                        reinterpret_cast<uint4*>(a.out_lo)[e] = lv;
-                    }
-                    if (tail) {
-                        *reinterpret_cast<uint4*>(sA2 + ((size_t)(c0 / 8) * 128 + m) * 16) = hv;
-                        *reinterpret_cast<uint4*>(sA2 + ((size_t)(NP / 8 + c0 / 8) * 128 + m) * 16) = lv;
-                    }
-                }
-            };
-            {   // TMEM -> registers two 8-column groups deep: the loads of the next group fly while this one is processed
-                const int cb = half * cw, ce = cb + cw;
-                const uint32_t tq = tmem + ((uint32_t)(q * 32) << 16) + buf * (uint32_t)NP;
-                uint32_t pa[8], qa[8];
-                um::tmem_ld8(tq + cb, pa);
-                for (int c0 = cb; c0 < ce; c0 += 16) {
-                    um::tmem_ld_wait();
-                    if (c0 + 8 < ce) um::tmem_ld8(tq + c0 + 8, qa);
-                    emit(pa, c0);
-                    if (c0 + 8 < ce) {
-                        um::tmem_ld_wait();
-                        if (c0 + 16 < ce) um::tmem_ld8(tq + c0 + 16, pa);
-                        emit(qa, c0 + 8);
-                    }
-                }
-            }
-            um::tc_fence_before();
-            mbar_arrive(&bar_acc_empty[buf]);
-            GCK();
-            // 2x2 average pool of the tile in sF (rows_per_tile x W, row stride NPx + 4) -> (rows/2 x W/2) planes; same
-            // operation order as the float32 kernel of round 1: (a + b + c + d) * 0.25, a=(y,x) b=(y,x+1) c=(y+1,x) d=(y+1,x+1)
-            auto pool_store = [&](const int NPx, bf16* o_hi, bf16* o_lo) {
-                asm volatile("bar.sync 1, 256;" ::: "memory");
-                const int Wt = a.W, OW = Wt / 2, OHt = a.rows_per_tile / 2;
-                const int items = OHt * OW * (NPx / 8);
-                const int OHW = a.HW / 4;
-                for (int e = et; e < items; e += 256) {
-                    const int pp = e % (OHt * OW), c8 = e / (OHt * OW);
-                    const int oy = pp / OW, ox = pp - oy * OW;
-                    const float* f0 = sF + (size_t)((2 * oy) * Wt + 2 * ox) * (NPx + 4) + c8 * 8;
-                    const float* f1 = f0 + (NPx + 4);
-                    const float* f2 = f0 + (size_t)Wt * (NPx + 4);
-                    const float* f3 = f2 + (NPx + 4);
-                    uint32_t h[4], l[4];
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        const float x0 = (f0[2 * j] + f1[2 * j] + f2[2 * j] + f3[2 * j]) * 0.25f;
-                        const float x1 = (f0[2 * j + 1] + f1[2 * j + 1] + f2[2 * j + 1] + f3[2 * j + 1]) * 0.25f;
-                        um::split2(x0, x1, h[j], l[j]);
-                    }
-                    const int opx = (tile * OHt + oy) * OW + ox;
-                    const size_t o = ((size_t)n * (NPx / 8) + c8) * OHW + opx;
-                    reinterpret_cast<uint4*>(o_hi)[o] = make_uint4(h[0], h[1], h[2], h[3]);
-                    reinterpret_cast<uint4*>(o_lo)[o] = make_uint4(l[0], l[1], l[2], l[3]);
-                }
-                asm volatile("bar.sync 1, 256;" ::: "memory");   // sF is rewritten by the next tile
-            };
-            if (a.pool) pool_store(NP, a.out_hi, a.out_lo);
-            if (tail) {
-                // the fresh tile (hi | lo planes in sA2) is the A operand of the second GEMM: every epilogue thread publishes
-                // its rows to the async proxy, one of them issues the MMAs (the MMA warp is already on the next tile)
-                um::fence_async_smem();
-                asm volatile("bar.sync 1, 256;" ::: "memory");
-                if (et == 0) {
-                    um::tc_fence_after();
-                    const uint32_t jd1 = um::idesc_bf16(128, NP2);
-                    const uint32_t lbo_b2 = 2u * NP2 * 16u, lo2 = (uint32_t)NP2 * 16u;
-                    const uint32_t ah = um::smem_u32(sA2), al = ah + (uint32_t)(NP / 8) * 2048u;
-                    for (int ks = 0; ks < NP / 16; ++ks) {
-                        const uint32_t bb = um::smem_u32(sB2) + ks * 2 * lbo_b2;
-                        const uint64_t dh = um::make_desc(bb, lbo_b2, 128), dl = um::make_desc(bb + lo2, lbo_b2, 128);
-                        const uint64_t xh = um::make_desc(ah + ks * 2 * 2048u, 2048u, 128), xl = um::make_desc(al + ks * 2 * 2048u, 2048u, 128);
-                        um::mma_bf16(tmem + acc_cols, xh, dh, jd1, ks > 0);
-                        um::mma_bf16(tmem + acc_cols, xl, dh, jd1, 1u);
-                        um::mma_bf16(tmem + acc_cols, xh, dl, jd1, 1u);
-                    }
-                    um::mma_commit(&bar_acc2_full);
-                }
-                um::mbar_wait(&bar_acc2_full, ti & 1u);
-                um::tc_fence_after();
-                GCK();
-                const int cw2 = NP2 / 2;
-                for (int c0 = half * cw2; c0 < half * cw2 + cw2; c0 += 8) {
-                    uint32_t v1[8];
-                    const uint32_t ta = tmem + ((uint32_t)(q * 32) << 16) + acc_cols + (uint32_t)c0;
-                    um::tmem_ld8(ta, v1);
-                    um::tmem_ld_wait();
-                    const float4 b0 = *reinterpret_cast<const float4*>(a.bias2 + c0), b1 = *reinterpret_cast<const float4*>(a.bias2 + c0 + 4);
-                    const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-                    float o[8];
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) o[j] = fmaxf(__uint_as_float(v1[j]) + bb[j], 0.f);
-                    if (a.pool2) {
-                        float* f = sF + (size_t)m * (NP2 + 4) + c0;     // aliases the tail's A tile: its MMAs have completed
-                        *reinterpret_cast<float4*>(f) = make_float4(o[0], o[1], o[2], o[3]);
-                        *reinterpret_cast<float4*>(f + 4) = make_float4(o[4], o[5], o[6], o[7]);
-                    } else {
-                        uint32_t h[4], l[4];
-#pragma unroll
-                        for (int j = 0; j < 4; ++j) um::split2(o[2 * j], o[2 * j + 1], h[j], l[j]);
-                        const size_t e = ((size_t)n * (NP2 / 8) + c0 / 8) * a.HW + px;
-                        reinterpret_cast<uint4*>(a.out2_hi)[e] = make_uint4(h[0], h[1], h[2], h[3]);
-                        reinterpret_cast<uint4*>(a.out2_lo)[e] = make_uint4(l[0], l[1], l[2], l[3]);
-                    }
-                }
-                um::tc_fence_before();
-                if (a.pool2) pool_store(NP2, a.out2_hi, a.out2_lo);
-                GCK();
+                um::wg_commit();
+                um::wg_wait_all();
+                um::wg_fence_acc<64>(acc);
+                if ((et & 127) == 0) mbar_arrive(&bar_empty[slot]);     // this warpgroup is done with the slot
+                kplane += kc;
             }
         }
-#ifdef BMB_TC_CLOCKS
-        if (gprint && et == 0) { for (int i = 0; i < ngk; ++i) s_gk[1][i] = gk[i]; s_ngk[1] = ngk; }
-#endif
-    }
-    um::tc_fence_before();
-    __syncthreads();
-    if (warp == 1) um::tmem_dealloc(tmem, tmem_cols);
-#ifdef BMB_TC_CLOCKS
-    if (gprint && threadIdx.x == 0) {
-        // MMA thread: B ready | per tile: accumulator free, MMAs issued (, tail MMAs issued)
-        // epilogue thread 0: | per tile: accumulator full, epilogue 1 done (, tail accumulator full, epilogue 2 done)
-        for (int w = 0; w < 2; ++w) {
-            printf("gemm K8 %d NP %d tail %d groups %d stages %d %s:", a.K8, NP, (int)tail, (int)gridDim.x, a.n_stage, w ? "EPI" : "MMA");
-            for (int i = 0; i < s_ngk[w]; ++i) printf(" %lld", s_gk[w][i]);
-            printf("\n");
+        if (a.head_w) {
+            // ---- conv5 + head: the tile is the whole 16 x 8 map.  Column sums over the 128 pixels: the two rows of a
+            // thread, a butterfly over the 8 row groups of a warp, the 8 warps through shared memory (the ring, once
+            // both warpgroups' MMAs have read their last slot; the producer has no further chunk to load) ----
+            um::bar_sync(1, 256);
+            float* part = reinterpret_cast<float*>(sRing);          // [8][NP]
+            float* pooled = part + 8 * NP;                          // [NP]
+            float* red = pooled + NP;                               // [8]
+            float* feat = red + 8;                                  // [head_feat]
+#pragma unroll
+            for (int i = 0; i < 16; ++i) {
+                const int c = 8 * i + cq;
+                if (c < NP) {
+                    const float2 b = *reinterpret_cast<const float2*>(a.bias + c);
+                    float o0 = fmaxf(acc[4 * i] + b.x, 0.f) + fmaxf(acc[4 * i + 2] + b.x, 0.f);
+                    float o1 = fmaxf(acc[4 * i + 1] + b.y, 0.f) + fmaxf(acc[4 * i + 3] + b.y, 0.f);
+#pragma unroll
+                    for (int sh = 4; sh < 32; sh <<= 1) {
+                        o0 += __shfl_xor_sync(0xffffffffu, o0, sh);
+                        o1 += __shfl_xor_sync(0xffffffffu, o1, sh);
+                    }
+                    if (lane < 4) *reinterpret_cast<float2*>(part + warp * NP + c) = make_float2(o0, o1);
+                }
+            }
+            um::bar_sync(1, 256);
+            for (int c = et; c < NP; c += 256)
+                pooled[c] = (((part[c] + part[NP + c]) + (part[2 * NP + c] + part[3 * NP + c])) +
+                             ((part[4 * NP + c] + part[5 * NP + c]) + (part[6 * NP + c] + part[7 * NP + c]))) / 128.f;
+            um::bar_sync(1, 256);
+            const int FEAT = a.head_feat, C = a.N;
+            float sq = 0.f;
+            for (int f = et; f < FEAT; f += 256) {
+                float t[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+                int c = 0;
+                for (; c + 8 <= C; c += 8) {
+#pragma unroll
+                    for (int u = 0; u < 8; ++u) t[u] = fmaf(pooled[c + u], a.head_w[(size_t)(c + u) * FEAT + f], t[u]);
+                }
+                for (; c < C; ++c) t[0] = fmaf(pooled[c], a.head_w[(size_t)c * FEAT + f], t[0]);
+                float sv = a.head_b[f] + (((t[0] + t[1]) + (t[2] + t[3])) + ((t[4] + t[5]) + (t[6] + t[7])));
+                sv = fmaxf(sv, 0.f);
+                feat[f] = sv;
+                sq = fmaf(sv, sv, sq);
+            }
+#pragma unroll
+            for (int sh = 16; sh > 0; sh >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, sh);
+            if (lane == 0) red[warp] = sq;
+            um::bar_sync(1, 256);
+            float tot = 0.f;
+            for (int w = 0; w < 8; ++w) tot += red[w];
+            const float nrm = sqrtf(tot);
+            float* dst = hio.out + (size_t)hio.crops[off + n].out_row * hio.out_ld;
+            for (int f = et; f < FEAT; f += 256) dst[f] = feat[f] / nrm;
+            um::bar_sync(1, 256);                                  // part / pooled are rewritten by the next tile
+            continue;
+        }
+        // ---- epilogue: bias (+ ReLU) on the thread's two rows x (2 columns per 8-column group) ----
+#pragma unroll
+        for (int i = 0; i < 16; ++i) {
+            const int c = 8 * i + cq;
+            if (c < NP) {
+                const float2 b = *reinterpret_cast<const float2*>(a.bias + c);
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int m = row + 8 * h, px = tile * 128 + m;
+                    float o0 = acc[4 * i + 2 * h] + b.x, o1 = acc[4 * i + 2 * h + 1] + b.y;
+                    if (a.relu) { o0 = fmaxf(o0, 0.f); o1 = fmaxf(o1, 0.f); }
+                    if (a.out_f32) {
+                        float* dst = a.out_f32 + ((size_t)n * a.HW + px) * a.N + c;
+                        if (c + 1 < a.N) *reinterpret_cast<float2*>(dst) = make_float2(o0, o1);
+                        else if (c < a.N) dst[0] = o0;
+                    }
+                    if (a.pool) {
+                        *reinterpret_cast<float2*>(sF + (size_t)m * (NP + 4) + c) = make_float2(o0, o1);
+                    } else if (a.out_hi || tail) {
+                        uint32_t hv, lv;
+                        um::split2(o0, o1, hv, lv);
+                        if (a.out_hi) {
+                            const size_t e = (((size_t)n * (NP / 8) + i) * a.HW + px) * 4 + (lane & 3);
+                            reinterpret_cast<uint32_t*>(a.out_hi)[e] = hv;
+                            reinterpret_cast<uint32_t*>(a.out_lo)[e] = lv;
+                        }
+                        if (tail) {
+                            *reinterpret_cast<uint32_t*>(sA2 + ((size_t)i * 128 + m) * 16 + (lane & 3) * 4) = hv;
+                            *reinterpret_cast<uint32_t*>(sA2 + ((size_t)(NP / 8 + i) * 128 + m) * 16 + (lane & 3) * 4) = lv;
+                        }
+                    }
+                }
+            }
+        }
+        // 2x2 average pool of the tile in sF (rows_per_tile x W, row stride NPx + 4) -> (rows/2 x W/2) planes;
+        // (a + b + c + d) * 0.25, a=(y,x) b=(y,x+1) c=(y+1,x) d=(y+1,x+1)
+        auto pool_store = [&](const int NPx, bf16* o_hi, bf16* o_lo) {
+            um::bar_sync(1, 256);
+            const int Wt = a.W, OW = Wt / 2, OHt = a.rows_per_tile / 2;
+            const int items = OHt * OW * (NPx / 8);
+            const int OHW = a.HW / 4;
+            for (int e = et; e < items; e += 256) {
+                const int pp = e % (OHt * OW), c8 = e / (OHt * OW);
+                const int oy = pp / OW, ox = pp - oy * OW;
+                const float* f0 = sF + (size_t)((2 * oy) * Wt + 2 * ox) * (NPx + 4) + c8 * 8;
+                const float* f1 = f0 + (NPx + 4);
+                const float* f2 = f0 + (size_t)Wt * (NPx + 4);
+                const float* f3 = f2 + (NPx + 4);
+                uint32_t h[4], l[4];
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    const float x0 = (f0[2 * j] + f1[2 * j] + f2[2 * j] + f3[2 * j]) * 0.25f;
+                    const float x1 = (f0[2 * j + 1] + f1[2 * j + 1] + f2[2 * j + 1] + f3[2 * j + 1]) * 0.25f;
+                    um::split2(x0, x1, h[j], l[j]);
+                }
+                const int opx = (tile * OHt + oy) * OW + ox;
+                const size_t o = ((size_t)n * (NPx / 8) + c8) * OHW + opx;
+                reinterpret_cast<uint4*>(o_hi)[o] = make_uint4(h[0], h[1], h[2], h[3]);
+                reinterpret_cast<uint4*>(o_lo)[o] = make_uint4(l[0], l[1], l[2], l[3]);
+            }
+            um::bar_sync(1, 256);   // sF is rewritten by the next tile
+        };
+        if (a.pool) pool_store(NP, a.out_hi, a.out_lo);
+        if (tail) {
+            // the fresh tile (hi | lo planes in sA2) is the A operand of the second GEMM: a warpgroup's MMAs read only the
+            // 64 rows it wrote itself
+            um::fence_async_smem();
+            um::bar_sync(2 + wg, 128);
+            const uint32_t lbo_b2 = 2u * NP2 * 16u, lo2 = (uint32_t)NP2 * 16u;
+            const uint32_t ah = um::smem_u32(sA2) + (uint32_t)wg * 1024u, al = ah + (uint32_t)(NP / 8) * 2048u;
+            um::wg_fence();
+            for (int ks = 0; ks < NP / 16; ++ks) {
+                const uint32_t bb = um::smem_u32(sB2) + ks * 2 * lbo_b2;
+                const uint64_t xh = um::make_desc(ah + ks * 2 * 2048u, 2048u, 128), xl = um::make_desc(al + ks * 2 * 2048u, 2048u, 128);
+                um::mma_rt<false>(NP2, acc, xh, bb, lbo_b2, 128, ks > 0);
+                um::mma_rt<false>(NP2, acc, xl, bb, lbo_b2, 128, 1u);
+                um::mma_rt<false>(NP2, acc, xh, bb + lo2, lbo_b2, 128, 1u);
+            }
+            um::wg_commit();
+            um::wg_wait_all();
+            um::wg_fence_acc<64>(acc);
+            if (a.pool2) um::bar_sync(1, 256);                     // sF aliases sA2: both warpgroups' MMAs have read it
+#pragma unroll
+            for (int i = 0; i < 16; ++i) {
+                const int c = 8 * i + cq;
+                if (c < NP2) {
+                    const float2 b = *reinterpret_cast<const float2*>(a.bias2 + c);
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        const int m = row + 8 * h, px = tile * 128 + m;
+                        const float o0 = fmaxf(acc[4 * i + 2 * h] + b.x, 0.f), o1 = fmaxf(acc[4 * i + 2 * h + 1] + b.y, 0.f);
+                        if (a.pool2) {
+                            *reinterpret_cast<float2*>(sF + (size_t)m * (NP2 + 4) + c) = make_float2(o0, o1);
+                        } else {
+                            uint32_t hv, lv;
+                            um::split2(o0, o1, hv, lv);
+                            const size_t e = (((size_t)n * (NP2 / 8) + i) * a.HW + px) * 4 + (lane & 3);
+                            reinterpret_cast<uint32_t*>(a.out2_hi)[e] = hv;
+                            reinterpret_cast<uint32_t*>(a.out2_lo)[e] = lv;
+                        }
+                    }
+                }
+            }
+            if (a.pool2) pool_store(NP2, a.out2_hi, a.out2_lo);
         }
     }
-#endif
 }
 
 
@@ -974,11 +829,12 @@ __global__ void __launch_bounds__(GEMM_THREADS, 2) k_gemm_tc(const __grid_consta
 // * A CTA = (crop, strip of 8 pooled columns): the 39 input columns it needs are staged column-major with 4 channels
 //   per pixel, [col][padded row][R G B 0] BF16 (8 B per pixel, 2112 B per column).  The 7 vertical taps x 4 channels of
 //   output row oy of one input column are then the 64 contiguous bytes at 16 * oy: a "Toeplitz" A operand with
-//   LBO = 16 B, SBO = 128 B (overlapping rows; validated on hardware, profiles/r2_tc_probe.jsonl).  One M tile = the
+//   LBO = 16 B, SBO = 128 B (overlapping rows; the stem parity tests of tests/test_gpu_reid.py pin it).  One M tile = the
 //   128 output rows of one stem column; K = 7 kx x (8 taps x 4 channels) = 14 K steps of 16; B = [W'_hi | W'_lo].
-// * TMEM lanes = output rows: the pool's horizontal maximum runs over consecutive accumulators in the same thread, the
-//   vertical one over neighbouring lanes (shuffles; the three warp boundaries go through 3 KB of shared memory).
-// grid = (4 strips, crops), 256 threads, 2 CTAs / SM (108 KB shared memory, 256 TMEM columns each).
+// * Warpgroup g owns output rows 64 g .. 64 g + 63 of every stem column (one m64n32 accumulator): the pool's horizontal
+//   maximum runs over consecutive stem columns in the same thread's registers, the vertical one over rows staged in
+//   shared memory (up to 4 pooled columns x 128 rows x 16 channels per batch of 8 stem columns).
+// grid = (4 strips, crops), 256 threads (two warpgroups), 130 KB shared memory.
 // ------------------------------------------------------------------------------------------------------------------
 struct FrontTcArgs {
     const uint8_t* images;
@@ -997,7 +853,8 @@ struct FrontCrop { float x1, y1, x2, y2; int image, out_row; };
 constexpr int FR_COLS = 39, FR_ROWS = 264, FR_CS = FR_ROWS * 8 + 16;     // staged columns, padded rows, bytes per column (+16: bank spread)
 constexpr int FR_A_BYTES = FR_COLS * FR_CS;
 constexpr int FR_W_BYTES = 7 * 4 * 32 * 16;
-constexpr size_t FR_SMEM = FR_A_BYTES + FR_W_BYTES + 128;
+constexpr int FR_H_BYTES = 4 * 128 * 16 * 4;                                // horizontally pooled rows of one batch
+constexpr size_t FR_SMEM = FR_A_BYTES + FR_W_BYTES + FR_H_BYTES + 128;
 
 __device__ __forceinline__ void fr_coeff(int d, int src_n, double scale, bool clamp, int& idx, int& a0, int& a1) {
     float f = (float)(((double)d + 0.5) * scale - 0.5);
@@ -1012,18 +869,16 @@ __device__ __forceinline__ void fr_coeff(int d, int src_n, double scale, bool cl
     a1 = (int)rintf(f * 2048.0f);
 }
 
-__global__ void __launch_bounds__(256, 2) k_front_tc(const FrontTcArgs a, const int* __restrict__ d_n, int off, int cap) {
+__global__ void __launch_bounds__(256, 1) k_front_tc(const FrontTcArgs a, const int* __restrict__ d_n, int off, int cap) {
     const int n = blockIdx.y;
     if (n >= tc_chunk_count(d_n, off, cap)) return;
     const int strip = blockIdx.x;
     extern __shared__ __align__(128) unsigned char smem[];
-    __shared__ __align__(8) uint64_t bar_mma;
-    __shared__ uint32_t tmem_slot;
     __shared__ int xi[128], xa0[128], xa1[128], yi[256], ya0[256], ya1[256];
     __shared__ __align__(16) float sBias[4 * 4 * 16];
-    __shared__ __align__(16) float sEx[3][4][16];                 // boundary rows oy = 31, 63, 95 of the 4 pooled columns of a batch
     unsigned char* sA = smem;
     unsigned char* sW = smem + FR_A_BYTES;
+    float* sH = reinterpret_cast<float*>(smem + FR_A_BYTES + FR_W_BYTES);   // [4 pooled columns][128 rows][16 channels]
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const FrontCrop cd = reinterpret_cast<const FrontCrop*>(a.crops)[off + n];
 #ifdef BMB_TC_CLOCKS
@@ -1035,8 +890,6 @@ __global__ void __launch_bounds__(256, 2) k_front_tc(const FrontTcArgs a, const 
 #endif
     FCK();
 
-    if (warp == 1) um::tmem_alloc(&tmem_slot, 256);
-    if (threadIdx.x == 0) { um::mbar_init(&bar_mma, 1); um::fence_mbar_init(); }
     // box.round().astype(int): round half to even; clip to the frame (base_backend.py:160-175)
     const int x1 = (int)rintf(cd.x1), y1 = (int)rintf(cd.y1), x2 = (int)rintf(cd.x2), y2 = (int)rintf(cd.y2);
     const int cx1 = max(0, x1), cy1 = max(0, y1), cx2 = min(a.cols, x2), cy2 = min(a.rows, y2);
@@ -1127,129 +980,108 @@ __global__ void __launch_bounds__(256, 2) k_front_tc(const FrontTcArgs a, const 
         }
     }
     um::fence_async_smem();
-    um::tc_fence_before();
     __syncthreads();
-    um::tc_fence_after();
-    const uint32_t tmem = tmem_slot;
     FCK();
 
     // stem columns of this strip: j = 0..16  <->  ox = 16 * strip - 1 + j  (ox = -1 does not exist: zero)
-    const int q = warp & 3, half = warp >> 2;                      // TMEM lane quadrant, channel half (8 channels)
-    const int oy = q * 32 + lane;
-    const int rc = oy == 0 ? 0 : (oy == 1 ? 1 : (oy == 127 ? 3 : 2));
-    float prev1[8], prev2[8];
+    const int wg = warp >> 2;
+    const int row = wg * 64 + (warp & 3) * 16 + (lane >> 2);      // output rows oy = row (h = 0) and row + 8 (h = 1)
+    const int cq = 2 * (lane & 3);                                 // channels 8 i + cq + e, i, e in {0, 1}
+    int rcl[2];
 #pragma unroll
-    for (int c = 0; c < 8; ++c) { prev1[c] = 0.f; prev2[c] = 0.f; }
-    uint32_t mma_phase = 0;
+    for (int h = 0; h < 2; ++h) {
+        const int oy = row + 8 * h;
+        rcl[h] = oy == 0 ? 0 : (oy == 1 ? 1 : (oy == 127 ? 3 : 2));
+    }
+    float prev1[2][4], prev2[2][4];
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int c = 0; c < 4; ++c) { prev1[h][c] = 0.f; prev2[h][c] = 0.f; }
+    const uint32_t sa = um::smem_u32(sA) + (uint32_t)wg * 1024u, sw_ = um::smem_u32(sW);
     for (int j0 = 0; j0 < 17; j0 += 8) {
         const int j1 = min(j0 + 8, 17);
-        if (threadIdx.x == 0) {
-            const uint32_t id2 = um::idesc_bf16(128, 32);
-            const uint32_t sa = um::smem_u32(sA), sw_ = um::smem_u32(sW);
-            for (int j = j0; j < j1; ++j) {
-                if (16 * strip - 1 + j < 0) continue;
-                const uint32_t d = tmem + (uint32_t)((j - j0) * 32);
+        // ---- per stem column: MMAs, bias + ReLU, horizontal 3-max over consecutive stem columns (registers) ----
+        for (int j = j0; j < j1; ++j) {
+            const int ox = 16 * strip - 1 + j;
+            float v[2][4];
+            if (ox >= 0) {
+                float acc[16];
+                um::wg_fence();
 #pragma unroll
                 for (int kx = 0; kx < 7; ++kx)
 #pragma unroll
                     for (int ks = 0; ks < 2; ++ks)
-                        um::mma_bf16(d, um::make_desc(sa + (uint32_t)(2 * j + kx) * FR_CS + ks * 32, 16, 128),
-                                     um::make_desc(sw_ + (uint32_t)(kx * 4 + 2 * ks) * 512u, 512u, 128), id2, (kx | ks) != 0);
+                        um::mma<32, false>(acc, um::make_desc(sa + (uint32_t)(2 * j + kx) * FR_CS + ks * 32, 16, 128),
+                                           sw_ + (uint32_t)(kx * 4 + 2 * ks) * 512u, 512u, 128, (kx | ks) != 0);
+                um::wg_commit();
+                um::wg_wait_all();
+                um::wg_fence_acc<16>(acc);
+                const int cc = ox == 0 ? 0 : (ox == 1 ? 1 : (ox == 63 ? 3 : 2));
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const float* bb = sBias + (rcl[h] * 4 + cc) * 16;
+#pragma unroll
+                    for (int i = 0; i < 2; ++i)
+#pragma unroll
+                        for (int e = 0; e < 2; ++e)   // [W_hi | W_lo]: channel c is column c plus column c + 16
+                            v[h][2 * i + e] = fmaxf(acc[4 * i + 2 * h + e] + acc[4 * (i + 2) + 2 * h + e] + bb[8 * i + cq + e], 0.f);
+                }
+            } else {
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+#pragma unroll
+                    for (int c = 0; c < 4; ++c) v[h][c] = 0.f;
             }
-            um::mma_commit(&bar_mma);
-        }
-        FCK();
-        um::mbar_wait(&bar_mma, mma_phase);
-        mma_phase ^= 1u;
-        um::tc_fence_after();
-        FCK();
-        // ---- epilogue: bias + ReLU, horizontal 3-max over consecutive stem columns (registers) ----
-        float hreg[4][8];
-        int n_h = 0;
-        uint32_t ra[2][8], rb[2][8];                               // double-buffered TMEM reads: the next column's loads fly
-        const uint32_t tq = tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(half * 8);
-        {
-            const int ox0 = 16 * strip - 1 + j0;
-            if (ox0 >= 0) { um::tmem_ld8(tq, ra[0]); um::tmem_ld8(tq + 16, rb[0]); }
-        }
+            if ((j & 1) == 0 && j >= 2) {                          // ox = 2 px + 1: third column of pooled px = 8 strip + j / 2 - 1
+                float* hs = sH + (size_t)(((j - j0) >> 1) & 3) * 128 * 16;
 #pragma unroll
-        for (int jj = 0; jj < 8; ++jj) {
-            const int j = j0 + jj;
-            if (j < j1) {
-                const int ox = 16 * strip - 1 + j;
-                um::tmem_ld_wait();
-                if (jj + 1 < 8 && j + 1 < j1) { um::tmem_ld8(tq + (jj + 1) * 32, ra[(jj + 1) & 1]); um::tmem_ld8(tq + (jj + 1) * 32 + 16, rb[(jj + 1) & 1]); }
-                float v[8];
-                if (ox >= 0) {
-                    const int cc = ox == 0 ? 0 : (ox == 1 ? 1 : (ox == 63 ? 3 : 2));
-                    const float* bb = sBias + (rc * 4 + cc) * 16 + half * 8;
+                for (int h = 0; h < 2; ++h)
 #pragma unroll
-                    for (int c = 0; c < 8; ++c) v[c] = fmaxf(__uint_as_float(ra[jj & 1][c]) + __uint_as_float(rb[jj & 1][c]) + bb[c], 0.f);
-                } else {
-#pragma unroll
-                    for (int c = 0; c < 8; ++c) v[c] = 0.f;
-                }
-                if ((j & 1) == 0 && j >= 2) {                      // ox = 2 px + 1: third column of pooled px = 8 strip + j / 2 - 1
-#pragma unroll
-                    for (int c = 0; c < 8; ++c) hreg[(jj >> 1) & 3][c] = fmaxf(fmaxf(prev2[c], prev1[c]), v[c]);
-                    ++n_h;
-                }
-#pragma unroll
-                for (int c = 0; c < 8; ++c) { prev2[c] = prev1[c]; prev1[c] = v[c]; }
+                    for (int i = 0; i < 2; ++i)
+                        *reinterpret_cast<float2*>(hs + (row + 8 * h) * 16 + 8 * i + cq) =
+                            make_float2(fmaxf(fmaxf(prev2[h][2 * i], prev1[h][2 * i]), v[h][2 * i]),
+                                        fmaxf(fmaxf(prev2[h][2 * i + 1], prev1[h][2 * i + 1]), v[h][2 * i + 1]));
             }
-        }
-        um::tmem_ld_wait();
-        // pooled columns finished in this batch: j = 2, 4, 6 (batch 0: also ... ) -> slots by (jj >> 1)
-        // batch 0 (j0 = 0): j = 2, 4, 6 -> slots 1, 2, 3;  batch 1 (j0 = 8): j = 8, 10, 12, 14 -> slots 0..3;  batch 2: j = 16 -> slot 0
-        const int s_first = j0 == 0 ? 1 : 0, s_last = j0 == 0 ? 3 : (j0 == 8 ? 3 : 0);
-        // ---- vertical 3-max over lanes (oy - 1, oy, oy + 1); warp boundaries through shared memory ----
-        if (lane == 31 && q < 3) {
 #pragma unroll
-            for (int s = 0; s < 4; ++s)
-                if (s >= s_first && s <= s_last) {
+            for (int h = 0; h < 2; ++h)
 #pragma unroll
-                    for (int c = 0; c < 8; ++c) sEx[q][s][half * 8 + c] = hreg[s][c];
-                }
+                for (int c = 0; c < 4; ++c) { prev2[h][c] = prev1[h][c]; prev1[h][c] = v[h][c]; }
         }
         __syncthreads();
-#pragma unroll
-        for (int s = 0; s < 4; ++s) {
-            if (s < s_first || s > s_last) continue;
+        // pooled columns finished in this batch: j = 2, 4, 6 (batch 0) -> slots 1, 2, 3;  batch 1 (j0 = 8): j = 8, 10, 12,
+        // 14 -> slots 0..3;  batch 2: j = 16 -> slot 0
+        const int s_first = j0 == 0 ? 1 : 0, s_last = j0 == 0 ? 3 : (j0 == 8 ? 3 : 0);
+        // ---- vertical 3-max over rows (oy - 1, oy, oy + 1), oy = 2 py; one item = (slot, py, 8 channels) ----
+        const int items = (s_last - s_first + 1) * 64 * 2;
+        for (int e = threadIdx.x; e < items; e += 256) {
+            const int s = s_first + (e >> 7), py = (e >> 1) & 63, half = e & 1;
+            const float* hs = sH + (size_t)s * 128 * 16 + half * 8;
+            const int oy = 2 * py;
             float m[8];
 #pragma unroll
             for (int c = 0; c < 8; ++c) {
-                const float h = hreg[s][c];
-                float up = __shfl_up_sync(0xffffffffu, h, 1);
-                const float dn = __shfl_down_sync(0xffffffffu, h, 1);
-                if (lane == 0) up = q > 0 ? sEx[q - 1][s][half * 8 + c] : 0.f;
-                m[c] = fmaxf(fmaxf(up, h), dn);
+                const float up = oy > 0 ? hs[(oy - 1) * 16 + c] : 0.f;
+                m[c] = fmaxf(fmaxf(up, hs[oy * 16 + c]), hs[(oy + 1) * 16 + c]);
             }
-            if ((lane & 1) == 0) {
-                // pooled pixel (py, px): j of the slot = j0 + 2 s (+ 0), px = 8 strip + (j0 + 2 s) / 2 - 1
-                const int px = 8 * strip + (j0 + 2 * s) / 2 - 1;
-                const int py = oy >> 1;
-                uint32_t h4[4], l4[4];
+            const int px = 8 * strip + (j0 + 2 * s) / 2 - 1;
+            uint32_t h4[4], l4[4];
 #pragma unroll
-                for (int c = 0; c < 4; ++c) um::split2(m[2 * c], m[2 * c + 1], h4[c], l4[c]);
-                const size_t e = (((size_t)n * 2 + half) * 64 + py) * 32 + px;
-                reinterpret_cast<uint4*>(a.p_hi)[e] = make_uint4(h4[0], h4[1], h4[2], h4[3]);
-                reinterpret_cast<uint4*>(a.p_lo)[e] = make_uint4(l4[0], l4[1], l4[2], l4[3]);
-            }
+            for (int c = 0; c < 4; ++c) um::split2(m[2 * c], m[2 * c + 1], h4[c], l4[c]);
+            const size_t o = (((size_t)n * 2 + half) * 64 + py) * 32 + px;
+            reinterpret_cast<uint4*>(a.p_hi)[o] = make_uint4(h4[0], h4[1], h4[2], h4[3]);
+            reinterpret_cast<uint4*>(a.p_lo)[o] = make_uint4(l4[0], l4[1], l4[2], l4[3]);
         }
-        um::tc_fence_before();
-        __syncthreads();                                            // TMEM and sEx are reused by the next batch
-        um::tc_fence_after();
-        (void)n_h;
+        __syncthreads();                                            // sH is reused by the next batch
         FCK();
     }
 #ifdef BMB_TC_CLOCKS
     if (threadIdx.x == 0 && n == 5) {
         printf("front strip %d: setup %lld resize %lld |", strip, fk[1] - fk[0], fk[2] - fk[1]);
-        for (int i = 2; i + 3 < nfk + 1; i += 3) printf(" issue %lld mma %lld epi %lld |", fk[i + 1] - fk[i], fk[i + 2] - fk[i + 1], fk[i + 3] - fk[i + 2]);
+        for (int i = 3; i < nfk; ++i) printf(" batch %lld |", fk[i] - fk[i - 1]);
         printf(" total %lld\n", fk[nfk - 1] - fk[0]);
     }
 #endif
-    if (warp == 1) um::tmem_dealloc(tmem, 256);
 }
 
 }  // namespace tcx

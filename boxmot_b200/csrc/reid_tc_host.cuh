@@ -20,8 +20,7 @@ PFN_encodeTiled tensor_map_encoder() {
 
 // Tensor maps over a plane tensor [crops][C8][H][W][8] of BF16.  The same bytes are described as 32-bit elements with
 // long inner rows: a 16-byte inner box (one pixel of one plane) makes the TMA unit issue one request per pixel
-// (3 264 per chain tile, measured latency-bound in profiles/r2a); a whole padded image row / 64 pixels per request
-// brings that to ~100.  Out-of-bounds elements read as zero (= the convolution's zero padding).
+// (3 264 per chain tile); a whole padded image row / 64 pixels per request brings that to ~100.  Out-of-bounds elements read as zero (= the convolution's zero padding).
 static void encode_u32_map(CUtensorMap* out, const void* base, int rank, const cuuint64_t* dims, const cuuint64_t* strides,
                            const cuuint32_t* box) {
     cuuint32_t es[5] = {1, 1, 1, 1, 1};

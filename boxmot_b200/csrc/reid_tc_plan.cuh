@@ -183,12 +183,7 @@ Plan* plan_build(ReidModel* m, const float* hw) {
                     if ((int)layout(cand).total <= P->smem_limit) ns = cand;
             }
             if (!ns) throw std::runtime_error("tensor-core GEMM does not fit shared memory");
-            if (g.NP + (tail ? g.NP2 : 0) > 512) throw std::runtime_error("tensor-core GEMM does not fit TMEM");
-            {   // a second accumulator when the CTA has more than one tile and the columns fit next to a co-resident CTA's
-                const bool two_ctas = (int)layout(ns).total <= half_limit;
-                const int cols = 2 * g.NP + (tail ? g.NP2 : 0);
-                g.acc_bufs = (g.tiles_per_cta > 1 && cols <= (two_ctas ? 256 : 512)) ? 2 : 1;
-            }
+            if (g.NP > 128 || (tail && g.NP2 > 128)) throw std::runtime_error("tensor-core GEMM: more than 128 output channels");
             for (int s = 0; s < g.n_src; ++s) {   // the boxes follow the chunk size
                 make_tile_map(&g.map_hi[s], L.src_hi[s], P->chunk, g.src_planes[s], g.HW, g.src_kc[s]);
                 make_tile_map(&g.map_lo[s], L.src_lo[s], P->chunk, g.src_planes[s], g.HW, g.src_kc[s]);
@@ -379,7 +374,7 @@ int plan_run(ReidModel* m, const FrontInput& fi, const int* d_n, int off, int up
                 break;
             }
             case LK_MAXPOOL_PLANES:
-                k_maxpool_planes<<<148 * 4, 256, 0, st>>>(m->bufA, 128, 64, m->c[0], d_n, off, upper, P->P.hi, P->P.lo);
+                k_maxpool_planes<<<m->sms * 4, 256, 0, st>>>(m->bufA, 128, 64, m->c[0], d_n, off, upper, P->P.hi, P->P.lo);
                 break;
             case LK_CHAIN_S2:
                 chain_launch<BMB_CHAIN_S2>(L.chain, L.chain_tiles, upper, d_n, off, st);
@@ -407,7 +402,7 @@ int plan_run(ReidModel* m, const FrontInput& fi, const int* d_n, int off, int up
                 m->debug_ptr = P->c5;
                 m->debug_floats_per_crop = (size_t)128 * m->c[3];
             } else {
-                k_planes_to_nhwc<<<148 * 4, 256, 0, st>>>(L.dbg_hi, L.dbg_lo, L.dbg_C8, L.dbg_HW, L.dbg_C, d_n, off, upper, P->dbg);
+                k_planes_to_nhwc<<<m->sms * 4, 256, 0, st>>>(L.dbg_hi, L.dbg_lo, L.dbg_C8, L.dbg_HW, L.dbg_C, d_n, off, upper, P->dbg);
                 m->debug_ptr = P->dbg;
                 m->debug_floats_per_crop = (size_t)L.dbg_HW * L.dbg_C;
             }

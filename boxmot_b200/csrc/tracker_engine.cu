@@ -170,10 +170,9 @@ __global__ void __launch_bounds__(256) k_docs_embcost(const DocsCfg cfg, DocsStr
     if (slot >= 0 && d0 + td < D) s.embq[(size_t)(d0 + td) * cfg.cap_tracks + slot] = dot;
 }
 
-// CTA-wide augmentation of the dense JV solver (jv_dense.cuh::jv_augment_wide): measured 4.2 s -> 0.65 s per frame
-// on the BASELINE config-3 shape (512 detections, 1 500 live tracks), identical results; the column-owned variant
-// (jv_augment_owned, mode 2) 0.53 s and is the default since its tracker-level GPU run (goldens + config-3 ids) went
-// green in round 2.  Mode 3 (the default) is mode 2 plus the two exact shortcuts described at jv_augment_owned
+// CTA-wide augmentation of the dense JV solver (jv_dense.cuh::jv_augment_wide) replaces the one-warp walk on the
+// BASELINE config-3 shape (512 detections, 1 500 live tracks) with identical results; the column-owned variant
+// (jv_augment_owned, mode 2) goes further.  Mode 3 (the default) is mode 2 plus the two exact shortcuts described at jv_augment_owned
 // (no-op band columns walked over, parallel tail of _find_dense).  BOXMOT_B200_JV_WIDE=0/1/2/3 sets the initial
 // value, boxmot_b200_jv_dense_mode() changes it (parity tests run every variant).
 // 0..2: the older variants; 3: mode 3 with every shortcut; >= 4: raw `mode | feature bits << 2` (bisecting on hardware)
@@ -469,7 +468,9 @@ void Engine::construct(const BoxMOTB200TrackerConfig& p) {
         CUDA_OK(cudaHostAlloc(&h_crops_hint, sizeof(int), cudaHostAllocMapped));
         *h_crops_hint = 0;
         CUDA_OK(cudaHostGetDevicePointer(&d_crops_hint, h_crops_hint, 0));
-        n_split = 3;   // measured at 208 crops: 1 slice 518 / 407 frames/s (value / e2e), 2: 560 / 432, 3: 570 / 443, 4: 579 / 434
+        // one H100 80GB HBM3, bench.py default workload (value / e2e frames/s, two runs each): 1 slice 454 / 307-315,
+        // 2: 503 / 347, 3: 496 / 334-338, 4: 498-500 / 339-351
+        n_split = 2;
         if (const char* sp = getenv("BOXMOT_B200_REID_SPLIT")) n_split = atoi(sp);
         n_split = n_split < 1 ? 1 : (n_split > MAX_SPLIT ? MAX_SPLIT : n_split);
         if (n_split > 1) CUDA_OK(cudaEventCreateWithFlags(&ev_crops, cudaEventDisableTiming));

@@ -1,7 +1,7 @@
 /*
- * boxmot_b200.h -- C ABI of libboxmot_b200.so: the B200-native drop-in for BoxMOT's per-frame track-update
+ * boxmot_b200.h -- C ABI of libboxmot_b200.so: the H100-native drop-in for BoxMOT's per-frame track-update
  * hot path (ReID embedding CNN over detection crops, batched Kalman predict/update, IoU + cosine cost build and
- * linear assignment), sm_100a CUDA behind plain-C entry points (pointers and sizes only; no torch types).
+ * linear assignment), sm_90a CUDA behind plain-C entry points (pointers and sizes only; no torch types).
  *
  * Part 1 re-exports, symbol for symbol, the C ABI the reference's ctypes loaders bind
  * (paths relative to /root/reference/boxmot/native/cpp/trackers):
@@ -270,7 +270,7 @@ BOXMOT_B200_API int boxmot_b200_iou_cost(const double* track_xyxy, int rows, con
 /* max(0, cosine distance) of float32 rows a (T,F) x b (D,F) -> (T,D) float64. */
 BOXMOT_B200_API int boxmot_b200_cosine_cost(const float* a, int rows, const float* b, int cols, int dim, double* out);
 /* 1x1 convolution as a GEMM on host arrays: out (M,N) = act(A (M,K) * W (K,N) + bias (+ residual)); K, N multiples
- * of 4.  use_tensor_cores = 1 runs the tcgen05 tf32x3 kernel (M % 128 == 0), 0 the CUDA-core kernel.  elapsed_ms
+ * of 4.  use_tensor_cores = 1 runs the wgmma tf32x3 kernel (M % 128 == 0), 0 the CUDA-core kernel.  elapsed_ms
  * (optional) receives the average device time of 10 back-to-back launches. */
 BOXMOT_B200_API int boxmot_b200_pointwise_gemm(const float* a, int m, int k, const float* w, int n, const float* bias,
                                                const float* residual, int relu, int use_tensor_cores, float* out,

@@ -1,7 +1,7 @@
 import sys, ctypes, tempfile, json
 from pathlib import Path
 import numpy as np
-sys.path.insert(0,'/root/repo')
+sys.path.insert(0, str(__import__('pathlib').Path(__file__).resolve().parents[1]))
 import boxmot_b200 as bb
 from boxmot_b200 import _lib
 from boxmot_b200.synthetic import bench_stream

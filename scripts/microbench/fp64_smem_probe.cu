@@ -1,7 +1,7 @@
 // Probe of the primitives the one-CTA-per-stream float64 kernels are made of (dense JV solver, Kalman update):
 // FP64 add latency / throughput, shared-memory pointer-chase latency through a typed (LDS) and a generic (LD.E)
 // pointer, and the cost of __syncthreads_or, all for ONE CTA of 256 threads on one SM -- the launch shape of
-// k_docs_frame.  Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o fp64_smem_probe fp64_smem_probe.cu
+// k_docs_frame.  Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o fp64_smem_probe fp64_smem_probe.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 

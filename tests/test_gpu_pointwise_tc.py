@@ -1,4 +1,4 @@
-"""tcgen05 (tf32 x3) pointwise GEMM against float64 numpy and against the CUDA-core kernel, at the layer shapes
+"""Tensor-core (wgmma tf32 x3) pointwise GEMM against float64 numpy and against the CUDA-core kernel, at the layer shapes
 of OSNet_x0_25 (and padding cases N=24, K=88)."""
 import ctypes
 
@@ -40,7 +40,7 @@ def test_tcgen05_pointwise_matches_fp64(m, k, n, relu, use_res):
     scale = np.abs(want).max()
     err_tc = np.abs(got_tc - want).max() / scale
     err_cc = np.abs(got_cc - want).max() / scale
-    print(f"M={m} K={k} N={n}: tcgen05 {ms_tc * 1e3:.1f} us err {err_tc:.2e} | cuda-core {ms_cc * 1e3:.1f} us err {err_cc:.2e}")
+    print(f"M={m} K={k} N={n}: tensor cores {ms_tc * 1e3:.1f} us err {err_tc:.2e} | cuda-core {ms_cc * 1e3:.1f} us err {err_cc:.2e}")
     assert err_cc < 2e-6
     assert err_tc < 2e-6, "tf32 x3 split must keep float32-class accuracy"
 
@@ -55,6 +55,6 @@ def test_tcgen05_pointwise_large_timing(m, k, n):
     got_tc, ms_tc = _gemm(a, w, bias, None, 1, 1)
     got_cc, ms_cc = _gemm(a, w, bias, None, 1, 0)
     gb = (m * k + m * n) * 4 / 1e9
-    print(f"M={m} K={k} N={n}: tcgen05 {ms_tc * 1e3:.1f} us ({gb / ms_tc * 1e3:.0f} GB/s) | cuda-core {ms_cc * 1e3:.1f} us "
+    print(f"M={m} K={k} N={n}: tensor cores {ms_tc * 1e3:.1f} us ({gb / ms_tc * 1e3:.0f} GB/s) | cuda-core {ms_cc * 1e3:.1f} us "
           f"({gb / ms_cc * 1e3:.0f} GB/s)")
     np.testing.assert_allclose(got_tc, got_cc, rtol=0, atol=2e-5 * np.abs(got_cc).max())

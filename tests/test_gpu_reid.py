@@ -65,8 +65,8 @@ def test_every_stage_matches_oracle(tmp_path):
         w = want[name].permute(0, 2, 3, 1).contiguous().numpy().reshape(len(boxes), -1)
         g = reid.debug_stage(boxes, img, idx)
         assert g.shape == w.shape, (name, g.shape, w.shape)
-        # the stem tap (1) is the float32 kernel; pool (2, fused front kernel) and the blocks run on the tensor cores with split-BF16 operands (4-6e-6 of the
-        # output scale per GEMM, measured): 5e-5 of the stage's scale, the embedding bound itself stays 1e-4
+        # the stem tap (1) is the float32 kernel; pool (2, fused front kernel) and the blocks run on the tensor cores with split-BF16 operands (a few 1e-6 of the
+        # output scale per GEMM): 5e-5 of the stage's scale, the embedding bound itself stays 1e-4
         tol = (2e-5 if idx < 2 else 5e-5) * max(1.0, float(np.abs(w).max()))
         assert np.abs(g - w).max() < tol, f"stage {name}: max err {np.abs(g - w).max():.3e}"
 
@@ -135,9 +135,9 @@ def test_reid_abi_errors(tmp_path):
                                  {"BOXMOT_B200_LIGHT_TC": "1"}, {"BOXMOT_B200_LIGHT_SMALL": "1"},
                                  {"BOXMOT_B200_PW_SMALL": "0"}])
 def test_alternative_kernel_paths_keep_parity(tmp_path, monkeypatch, env):
-    """Every selectable kernel generation / configuration keeps the embeddings within the bound: tcgen05 (tf32 x3)
+    """Every selectable kernel generation / configuration keeps the embeddings within the bound: tensor-core (tf32 x3)
     pointwise path, other chunk sizes, per-level vs whole-branch LightConv, first-generation kernels."""
-    # the tensor-core path (tcgen05 + TMA) is the default; every other switch selects among the float32 kernels
+    # the tensor-core path (wgmma + TMA) is the default; every other switch selects among the float32 kernels
     monkeypatch.setenv("BOXMOT_B200_REID_FP32", "1")
     for k, v in env.items():
         monkeypatch.setenv(k, v)
