@@ -35,6 +35,7 @@ namespace bmb {
     } while (0)
 
 constexpr int IN_H = 256, IN_W = 128;
+constexpr int IN_H_MAX = 384;   // LMBN_n crops are 384x128 (the width of every model is 128)
 constexpr uint32_t BLOB_MAGIC = 0x45523242u;
 
 // streaming multiprocessors of the current device: grid-stride kernels launch a few CTAs per SM
@@ -51,7 +52,7 @@ __device__ __forceinline__ int chunk_count(const int* d_n, int off, int cap) {
 }
 
 // ---------------------------------------------------------------------------------------------------
-// K1: crop + OpenCV-exact bilinear resize + BGR->RGB + /255 + mean/std  ->  (N,256,128,3) float32
+// K1: crop + OpenCV-exact bilinear resize + BGR->RGB + /255 + mean/std  ->  (N,in_h,128,3) float32
 // One CTA per crop.  cv2.resize(INTER_LINEAR) on uint8 is integer arithmetic: 11-bit coefficients derived from a
 // float32 phase, horizontal pass in int32, vertical (((b0*(S0>>4))>>16)+((b1*(S1>>4))>>16)+2)>>2.  x phases are
 // clamped at the borders, y rows are clipped at fetch (pinned against cv2 in tests/test_oracle_reid.py).
@@ -72,25 +73,25 @@ __device__ __forceinline__ void linear_coeff(int d, int src_n, double scale, boo
 __global__ void __launch_bounds__(256) k_crop_resize_norm(const uint8_t* __restrict__ images, size_t image_stride,
                                                           int rows, int cols, const CropDesc* __restrict__ crops,
                                                           const int* __restrict__ d_n, int off, int cap,
-                                                          float* __restrict__ blob, int pad_mode) {
+                                                          float* __restrict__ blob, int pad_mode, int in_h) {
     const int n = blockIdx.x;
     if (n >= chunk_count(d_n, off, cap)) return;
     const CropDesc cd = crops[off + n];
     __shared__ int xi[IN_W], xa0[IN_W], xa1[IN_W];
-    __shared__ int yi[IN_H], ya0[IN_H], ya1[IN_H];
+    __shared__ int yi[IN_H_MAX], ya0[IN_H_MAX], ya1[IN_H_MAX];
     // box.round().astype(int): round half to even
     const int x1 = (int)rintf(cd.x1), y1 = (int)rintf(cd.y1), x2 = (int)rintf(cd.x2), y2 = (int)rintf(cd.y2);
     const int cx1 = max(0, x1), cy1 = max(0, y1), cx2 = min(cols, x2), cy2 = min(rows, y2);
     const bool valid = cx2 > cx1 && cy2 > cy1;
     const int sw = cx2 - cx1, sh = cy2 - cy1;
     // resize_pad (preprocessing.py:21-45): scale = min(W / w, H / h); new = int(size * scale); centred, ImageNet-mean border
-    int nw = IN_W, nh = IN_H, pl = 0, pt = 0;
+    int nw = IN_W, nh = in_h, pl = 0, pt = 0;
     if (valid && pad_mode) {
-        const double sc = fmin((double)IN_W / (double)sw, (double)IN_H / (double)sh);
+        const double sc = fmin((double)IN_W / (double)sw, (double)in_h / (double)sh);
         nw = max(1, (int)((double)sw * sc));
         nh = max(1, (int)((double)sh * sc));
         pl = (IN_W - nw) / 2;
-        pt = (IN_H - nh) / 2;
+        pt = (in_h - nh) / 2;
     }
     if (valid) {
         const double sx = 1.0 / ((double)nw / (double)sw), sy = 1.0 / ((double)nh / (double)sh);
@@ -99,10 +100,10 @@ __global__ void __launch_bounds__(256) k_crop_resize_norm(const uint8_t* __restr
     }
     __syncthreads();
     const uint8_t* img = images + (size_t)cd.image * image_stride;
-    float* out = blob + (size_t)n * IN_H * IN_W * 3;
+    float* out = blob + (size_t)n * in_h * IN_W * 3;
     const float mean[3] = {0.485f, 0.456f, 0.406f};
     const float stdv[3] = {0.229f, 0.224f, 0.225f};
-    for (int p = threadIdx.x; p < IN_H * IN_W; p += blockDim.x) {
+    for (int p = threadIdx.x; p < in_h * IN_W; p += blockDim.x) {
         const int py = p / IN_W, px = p - py * IN_W;
         const int dy = py - pt, dx = px - pl;
         int v[3] = {0, 0, 0};
@@ -131,14 +132,14 @@ __global__ void __launch_bounds__(256) k_crop_resize_norm(const uint8_t* __restr
 }
 
 // ---------------------------------------------------------------------------------------------------
-// K2: stem 7x7 stride-2 conv (3 -> C0) + folded BN + ReLU : (N,256,128,3) -> (N,128,64,C0)
+// K2: stem 7x7 stride-2 conv (3 -> C0) + folded BN + ReLU : (N,in_h,128,3) -> (N,in_h/2,64,C0)
 // CTA = 8 output rows x 64 columns of one crop; the 21 x 134 x 3 input window and the weight chunk live in
 // shared memory; a thread owns two output pixels (x, x+32) x 16 output channels.
 // ---------------------------------------------------------------------------------------------------
 constexpr int ST_R = 8, ST_IR = 2 * ST_R + 5, ST_IC = IN_W + 6;
 __global__ void __launch_bounds__(256) k_stem(const float* __restrict__ blob, const float* __restrict__ w,
                                               const float* __restrict__ bias, int C0, const int* __restrict__ d_n,
-                                              int off, int cap, float* __restrict__ out) {
+                                              int off, int cap, float* __restrict__ out, int in_h) {
     const int n = blockIdx.y;
     if (n >= chunk_count(d_n, off, cap)) return;
     extern __shared__ __align__(16) float smem[];
@@ -146,12 +147,12 @@ __global__ void __launch_bounds__(256) k_stem(const float* __restrict__ blob, co
     float* sw = smem + ((ST_IR * ST_IC * 3 + 3) & ~3);  // [147][16], 16-byte aligned for float4 reads
     const int oy0 = blockIdx.x * ST_R;
     const int iy0 = oy0 * 2 - 3;
-    const float* src = blob + (size_t)n * IN_H * IN_W * 3;
+    const float* src = blob + (size_t)n * in_h * IN_W * 3;
     for (int e = threadIdx.x; e < ST_IR * ST_IC * 3; e += blockDim.x) {
         const int r = e / (ST_IC * 3), rem = e - r * (ST_IC * 3);
         const int cidx = rem / 3, ch = rem - cidx * 3;
         const int iy = iy0 + r, ix = cidx - 3;
-        sin[e] = (iy >= 0 && iy < IN_H && ix >= 0 && ix < IN_W) ? src[((size_t)iy * IN_W + ix) * 3 + ch] : 0.f;
+        sin[e] = (iy >= 0 && iy < in_h && ix >= 0 && ix < IN_W) ? src[((size_t)iy * IN_W + ix) * 3 + ch] : 0.f;
     }
     const int ty = threadIdx.x >> 5, tx = threadIdx.x & 31;
     for (int co0 = 0; co0 < C0; co0 += 16) {
@@ -186,7 +187,7 @@ __global__ void __launch_bounds__(256) k_stem(const float* __restrict__ blob, co
                 }
             }
         }
-        float* o0 = out + (((size_t)n * 128 + oy0 + ty) * 64 + tx) * C0 + co0;
+        float* o0 = out + (((size_t)n * (in_h / 2) + oy0 + ty) * 64 + tx) * C0 + co0;
         float* o1 = o0 + (size_t)32 * C0;
 #pragma unroll
         for (int q = 0; q < 4; ++q) {
@@ -1180,6 +1181,10 @@ __global__ void k_head(const float* __restrict__ x, int HW, int C, const float* 
     for (int f = threadIdx.x; f < FEAT; f += blockDim.x) dst[f] = dst[f] / nrm;
 }
 
+}  // namespace bmb
+#include "lmbn_head.cuh"
+namespace bmb {
+
 // ---------------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------------
@@ -1203,8 +1208,21 @@ struct MbBlock {
     size_t we, be, wd, bd, wp, bp;
 };
 
+// LMBN_n (arch 3): OSNet_x1_0 trunk up to conv3[0], three branches (global, partial, channel) of conv3[1:] + conv4 +
+// conv5 with their own weights, the bottleneck OSBlock of the global branch, and the neck weights of the head
+struct LmbnW {
+    BlockW trunk[3];                      // backone.2.0, backone.2.1, backone.3
+    size_t trunk_tw = 0, trunk_tb = 0;    // backone.2.2 transition
+    BlockW br[3][3];                      // per branch: .0.1, .1.0, .1.1
+    size_t br_tw[3] = {0, 0, 0}, br_tb[3] = {0, 0, 0}, br_c5w[3] = {0, 0, 0}, br_c5b[3] = {0, 0, 0};
+    BlockW bottleneck;
+    size_t neck_w[5] = {0, 0, 0, 0, 0}, neck_b[5] = {0, 0, 0, 0, 0}, sh_w = 0, sh_b = 0, ch_st = 0;
+};
+
 struct ReidModel {
-    int arch = 1;                 // 1 OSNet, 2 MobileNetV2
+    int arch = 1;                 // 1 OSNet, 2 MobileNetV2, 3 LMBN_n
+    int in_h = IN_H;              // crop height (the width is IN_W for every model)
+    LmbnW lm;
     std::vector<MbBlock> mb;      // MobileNetV2 bottlenecks
     int mb_stem = 0, mb_stemp = 0, mb_last = 0;
     size_t mb_stem_w = 0, mb_stem_b = 0, mb_c9w = 0, mb_c9b = 0;
@@ -1237,6 +1255,8 @@ struct ReidModel {
     float* Y[4][2] = {{nullptr, nullptr}, {nullptr, nullptr}, {nullptr, nullptr}, {nullptr, nullptr}};
     float* sums[4] = {nullptr, nullptr, nullptr, nullptr};
     float* gates = nullptr;
+    float* trunk = nullptr;    // LMBN_n: trunk output, read by all three branches
+    float* pooled = nullptr;   // LMBN_n: [crops][6][512] head poolings
     // per-kernel-class device timing (bench / profiles): events around every launch when enabled
     bool profile = false;
     std::vector<cudaEvent_t> prof_ev;
@@ -1267,7 +1287,7 @@ ReidModel* reid_load(const char* path) {
     if (!f) throw std::runtime_error(std::string("cannot open ReID blob: ") + path);
     int32_t hdr[16];
     f.read(reinterpret_cast<char*>(hdr), sizeof(hdr));
-    if (!f || (uint32_t)hdr[0] != BLOB_MAGIC || hdr[1] != 1 || (hdr[2] != 1 && hdr[2] != 2))
+    if (!f || (uint32_t)hdr[0] != BLOB_MAGIC || hdr[1] != 1 || hdr[2] < 1 || hdr[2] > 3)
         throw std::runtime_error("not a version-1 .b200reid blob (export it with boxmot_b200.weights.export_blob)");
     ReidModel* m = new ReidModel();
     if (hdr[2] == 2) {
@@ -1334,47 +1354,80 @@ ReidModel* reid_load(const char* path) {
     try {
         for (int i = 0; i < 4; ++i) m->c[i] = hdr[3 + i];
         m->feat = hdr[7];
+        m->arch = hdr[2];
         const size_t n_floats = (size_t)hdr[8];
         if (m->c[0] % 16 != 0 || m->feat < 1) throw std::runtime_error("unsupported OSNet width (stem channels)");
+        if (m->arch == 3) {
+            if (hdr[9] != 384 || m->c[0] != 64 || m->c[1] != 256 || m->c[2] != 384 || m->c[3] != LMBN_C ||
+                m->feat != LMBN_VECS * LMBN_C)
+                throw std::runtime_error("unsupported LMBN_n blob header (expected 384x128 input, widths 64/256/384/512, 3584-d)");
+            m->in_h = hdr[9];
+        }
         std::vector<float> host(n_floats);
         f.read(reinterpret_cast<char*>(host.data()), sizeof(float) * n_floats);
         if (!f) throw std::runtime_error("truncated ReID blob");
         size_t o = 0;
         auto take = [&](size_t n) { size_t r = o; o += (n + 3) / 4 * 4; return r; };  // 16-byte aligned tensors
+        auto take_block = [&](BlockW& b, int cin, int cout) {
+            b.cin = cin;
+            b.cout = cout;
+            b.mid = b.cout / 4;
+            b.hid = b.mid / 16;
+            b.has_ds = b.cin != b.cout;
+            if (b.mid % 8 != 0 || b.hid < 1) throw std::runtime_error("unsupported OSNet width (mid channels)");
+            b.c1w = take((size_t)b.cin * b.mid);
+            b.c1b = take(b.mid);
+            for (int l = 0; l < 10; ++l) {
+                b.light[l].pw = take((size_t)b.mid * b.mid);
+                b.light[l].dw = take((size_t)9 * b.mid);
+                b.light[l].b = take(b.mid);
+            }
+            b.g1w = take((size_t)b.mid * b.hid);
+            b.g1b = take(b.hid);
+            b.g2w = take((size_t)b.hid * b.mid);
+            b.g2b = take(b.mid);
+            b.cw = take((size_t)(b.mid + (b.has_ds ? b.cin : 0)) * b.cout);
+            b.cb = take(b.cout);
+        };
         m->stem_w = take((size_t)147 * m->c[0]);
         m->stem_b = take(m->c[0]);
-        for (int s = 0; s < 3; ++s) {
-            for (int j = 0; j < 2; ++j) {
-                BlockW& b = m->blocks[s * 2 + j];
-                b.cin = j == 0 ? m->c[s] : m->c[s + 1];
-                b.cout = m->c[s + 1];
-                b.mid = b.cout / 4;
-                b.hid = b.mid / 16;
-                b.has_ds = b.cin != b.cout;
-                if (b.mid % 8 != 0 || b.hid < 1) throw std::runtime_error("unsupported OSNet width (mid channels)");
-                b.c1w = take((size_t)b.cin * b.mid);
-                b.c1b = take(b.mid);
-                for (int l = 0; l < 10; ++l) {
-                    b.light[l].pw = take((size_t)b.mid * b.mid);
-                    b.light[l].dw = take((size_t)9 * b.mid);
-                    b.light[l].b = take(b.mid);
+        if (m->arch == 3) {   // weights.fold_lmbn_n walk order
+            LmbnW& lm = m->lm;
+            take_block(lm.trunk[0], 64, 256);
+            take_block(lm.trunk[1], 256, 256);
+            lm.trunk_tw = take((size_t)256 * 256);
+            lm.trunk_tb = take(256);
+            take_block(lm.trunk[2], 256, 384);
+            for (int br = 0; br < 3; ++br) {
+                take_block(lm.br[br][0], 384, 384);
+                lm.br_tw[br] = take((size_t)384 * 384);
+                lm.br_tb[br] = take(384);
+                take_block(lm.br[br][1], 384, 512);
+                take_block(lm.br[br][2], 512, 512);
+                lm.br_c5w[br] = take((size_t)512 * 512);
+                lm.br_c5b[br] = take(512);
+            }
+            take_block(lm.bottleneck, 512, 512);
+            for (int k = 0; k < 5; ++k) {
+                lm.neck_w[k] = take((size_t)LMBN_C * LMBN_C);
+                lm.neck_b[k] = take(LMBN_C);
+            }
+            lm.sh_w = take((size_t)(LMBN_C / 2) * LMBN_C);
+            lm.sh_b = take(LMBN_C);
+            lm.ch_st = take((size_t)4 * LMBN_C);
+        } else {
+            for (int s = 0; s < 3; ++s) {
+                for (int j = 0; j < 2; ++j) take_block(m->blocks[s * 2 + j], j == 0 ? m->c[s] : m->c[s + 1], m->c[s + 1]);
+                if (s < 2) {
+                    m->trans_w[s] = take((size_t)m->c[s + 1] * m->c[s + 1]);
+                    m->trans_b[s] = take(m->c[s + 1]);
                 }
-                b.g1w = take((size_t)b.mid * b.hid);
-                b.g1b = take(b.hid);
-                b.g2w = take((size_t)b.hid * b.mid);
-                b.g2b = take(b.mid);
-                b.cw = take((size_t)(b.mid + (b.has_ds ? b.cin : 0)) * b.cout);
-                b.cb = take(b.cout);
             }
-            if (s < 2) {
-                m->trans_w[s] = take((size_t)m->c[s + 1] * m->c[s + 1]);
-                m->trans_b[s] = take(m->c[s + 1]);
-            }
+            m->c5w = take((size_t)m->c[3] * m->c[3]);
+            m->c5b = take(m->c[3]);
+            m->fcw = take((size_t)m->c[3] * m->feat);
+            m->fcb = take(m->feat);
         }
-        m->c5w = take((size_t)m->c[3] * m->c[3]);
-        m->c5b = take(m->c[3]);
-        m->fcw = take((size_t)m->c[3] * m->feat);
-        m->fcb = take(m->feat);
         if (o != n_floats) throw std::runtime_error("ReID blob size does not match its header");
         RCUDA_OK(cudaMalloc(&m->d_w, sizeof(float) * n_floats));
         RCUDA_OK(cudaMemcpy(m->d_w, host.data(), sizeof(float) * n_floats, cudaMemcpyHostToDevice));
@@ -1383,7 +1436,7 @@ ReidModel* reid_load(const char* path) {
             // At OSNet_x0_25's K,N <= 128 every 1x1 layer is bandwidth-bound, and on an H100 this unpipelined kernel is
             // 1.1-2.4x slower than the float32 CUDA-core GEMM (tests/test_gpu_pointwise_tc.py prints both), so the
             // standalone tensor-core GEMM is opt-in.
-            m->use_tc = env && env[0] == '1';
+            m->use_tc = env && env[0] == '1' && m->arch == 1;   // LMBN_n runs the float32 CUDA-core kernels only
             const char* lv = getenv("BOXMOT_B200_LIGHT_V1");
             m->light_v2 = !(lv && lv[0] == '1');
             if (const char* cv = getenv("BOXMOT_B200_LIGHT_CHAIN")) m->light_chain = !(cv[0] == '0');
@@ -1403,15 +1456,17 @@ ReidModel* reid_load(const char* path) {
                 todo.push_back({dst, w, K, N, packed.size()});
                 packed.resize(packed.size() + 2 * (size_t)Npad * Kpad);
             };
-            for (int bi = 0; bi < 6; ++bi) {
+            for (int bi = 0; bi < (m->arch == 1 ? 6 : 0); ++bi) {
                 BlockW& b = m->blocks[bi];
                 add(&b.tc_c1, b.c1w, b.cin, b.mid);
                 add(&b.tc_c, b.cw, b.mid + (b.has_ds ? b.cin : 0), b.cout);
                 if (b.mid % 16 == 0)
                     for (int l = 0; l < 10; ++l) add(&b.light_tc[l], b.light[l].pw, b.mid, b.mid);
             }
-            for (int s = 0; s < 2; ++s) add(&m->tc_trans[s], m->trans_w[s], m->c[s + 1], m->c[s + 1]);
-            add(&m->tc_c5, m->c5w, m->c[3], m->c[3]);
+            if (m->arch == 1) {
+                for (int s = 0; s < 2; ++s) add(&m->tc_trans[s], m->trans_w[s], m->c[s + 1], m->c[s + 1]);
+                add(&m->tc_c5, m->c5w, m->c[3], m->c[3]);
+            }
             for (auto& t : todo) tc::pack_weights(host.data() + t.w, t.K, t.N, t.dst->Kpad, t.dst->Npad, packed.data() + t.at);
             if (!packed.empty()) {
                 RCUDA_OK(cudaMalloc(&m->d_wtc, sizeof(float) * packed.size()));
@@ -1424,10 +1479,21 @@ ReidModel* reid_load(const char* path) {
             const int v = atoi(ce);
             if (v >= 8 && v <= 1024) m->chunk = v;
         }
+        // per-crop activations: the stem output (in_h/2 x 64 x c0) or the stage-2 maps (in_h/4 x 32 x c1), whichever is larger
+        auto big_of = [&](int in_h) { return std::max((size_t)(in_h / 2) * 64 * m->c[0], (size_t)(in_h / 4) * 32 * m->c[1]); };
+        auto mid_of = [&](int in_h) { return (size_t)(in_h / 4) * 32 * (m->c[1] / 4); };
+        auto workspace_floats = [&](int in_h, bool lmbn) {   // per crop, every buffer allocated below
+            return (size_t)in_h * IN_W * 3 + 2 * big_of(in_h) + 9 * mid_of(in_h) + 4 * 64 * (size_t)(m->c[3] / 4) +
+                   4 * (size_t)(m->c[3] / 4) + (lmbn ? (size_t)(in_h / 8) * 16 * m->c[2] + (size_t)LMBN_POOLS * LMBN_C : 0);
+        };
+        // LMBN_n's maps are 1.5x taller and it keeps the trunk output: fewer crops per chunk, so that a chunk's
+        // workspace stays within what an OSNet of the same widths at 256x128 takes for the configured chunk
+        if (m->arch == 3)
+            m->chunk = std::max(8, (int)((size_t)m->chunk * workspace_floats(IN_H, false) / workspace_floats(m->in_h, true)));
         const size_t CH = m->chunk;
-        const size_t big = (size_t)8192 * m->c[0] > (size_t)2048 * m->c[1] ? (size_t)8192 * m->c[0] : (size_t)2048 * m->c[1];
-        const size_t mid_max = (size_t)2048 * (m->c[1] / 4);
-        RCUDA_OK(cudaMalloc(&m->blob, sizeof(float) * CH * IN_H * IN_W * 3));
+        const size_t big = big_of(m->in_h);
+        const size_t mid_max = mid_of(m->in_h);
+        RCUDA_OK(cudaMalloc(&m->blob, sizeof(float) * CH * m->in_h * IN_W * 3));
         RCUDA_OK(cudaMalloc(&m->bufA, sizeof(float) * CH * big));
         RCUDA_OK(cudaMalloc(&m->bufB, sizeof(float) * CH * big));
         RCUDA_OK(cudaMalloc(&m->x1, sizeof(float) * CH * mid_max));
@@ -1436,6 +1502,10 @@ ReidModel* reid_load(const char* path) {
             RCUDA_OK(cudaMalloc(&m->sums[b], sizeof(float) * CH * 64 * (m->c[3] / 4)));
         }
         RCUDA_OK(cudaMalloc(&m->gates, sizeof(float) * CH * 4 * (m->c[3] / 4)));
+        if (m->arch == 3) {
+            RCUDA_OK(cudaMalloc(&m->trunk, sizeof(float) * CH * (m->in_h / 8) * 16 * m->c[2]));
+            RCUDA_OK(cudaMalloc(&m->pooled, sizeof(float) * CH * LMBN_POOLS * LMBN_C));
+        }
         {   // tensor-core path: the default wherever its kernel instances cover the widths (BOXMOT_B200_REID_FP32=1
             // keeps the float32 CUDA-core kernels of round 1, e.g. for A/B runs)
             const char* fe = getenv("BOXMOT_B200_REID_FP32");
@@ -1452,7 +1522,7 @@ void reid_free(ReidModel* m) {
     if (!m) return;
     cudaFree(m->d_w); cudaFree(m->d_wtc); cudaFree(m->blob); cudaFree(m->bufA); cudaFree(m->bufB); cudaFree(m->x1);
     for (int b = 0; b < 4; ++b) { cudaFree(m->Y[b][0]); cudaFree(m->Y[b][1]); cudaFree(m->sums[b]); }
-    cudaFree(m->gates);
+    cudaFree(m->gates); cudaFree(m->trunk); cudaFree(m->pooled);
     tcx::plan_free(m->tc);
     delete m;
 }
@@ -1659,6 +1729,192 @@ int pick_tile_rows(int H, int W, int C) {
     }
     return 1;
 }
+
+// Debug taps: stage index i stops the chunk after the i-th tapped tensor and leaves it in m->debug_ptr.
+struct StageTaps {
+    ReidModel* m;
+    int idx = 0;
+    bool operator()(const float* ptr, size_t per_crop) {
+        if (m->debug_stop == idx++) { m->debug_ptr = ptr; m->debug_floats_per_crop = per_crop; return true; }
+        return false;
+    }
+};
+
+struct FrameIn {
+    const uint8_t* images;
+    size_t image_stride;
+    int rows, cols;
+    const CropDesc* crops;
+};
+
+// Crop staging, 7x7 stem and 3x3 max pool of one chunk (taps 0-2): the pooled map (in_h/4 x 32 x c0) ends in m->bufB.
+// Returns true when a debug tap stopped the chunk.
+bool run_front(Launcher& L, const FrameIn& fi, StageTaps& stop_here) {
+    ReidModel* m = L.m;
+    const float* W = m->d_w;
+    L.begin(CLS_CROP);
+    k_crop_resize_norm<<<L.upper, 256, 0, L.st>>>(fi.images, fi.image_stride, fi.rows, fi.cols, fi.crops, L.d_n, L.off,
+                                                  L.cap, m->blob, m->preprocess, m->in_h);
+    L.end();
+    ++L.launches;
+    if (stop_here(m->blob, (size_t)m->in_h * IN_W * 3)) return true;
+    {
+        const size_t smem = sizeof(float) * ((size_t)((ST_IR * ST_IC * 3 + 3) & ~3) + 147 * 16);
+        RCUDA_OK(cudaFuncSetAttribute(k_stem, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        L.begin(CLS_STEM);
+        k_stem<<<dim3(m->in_h / 2 / ST_R, L.upper), 256, smem, L.st>>>(m->blob, W + m->stem_w, W + m->stem_b, m->c[0],
+                                                                       L.d_n, L.off, L.cap, m->bufA, m->in_h);
+        L.end();
+        ++L.launches;
+    }
+    if (stop_here(m->bufA, (size_t)(m->in_h / 2) * 64 * m->c[0])) return true;
+    L.begin(CLS_MAXPOOL);
+    k_maxpool3s2<<<m->sms * 8, 256, 0, L.st>>>(m->bufA, m->in_h / 2, 64, m->c[0], L.d_n, L.off, L.cap, m->bufB);
+    L.end();
+    ++L.launches;
+    return stop_here(m->bufB, (size_t)(m->in_h / 4) * 32 * m->c[0]);
+}
+
+// One OSBlock (osnet.py:213-260): conv1 -> the four LightConv3x3 branches -> shared ChannelGate -> conv3 (+ downsample,
+// or the identity) + ReLU.  X [crops][H][Wd][cin] -> Xo [crops][H][Wd][cout] (Xo != X); scratch m->x1, m->Y, m->sums,
+// m->gates.
+void run_osblock(Launcher& L, const BlockW& b, const float* X, float* Xo, int H, int Wd) {
+    ReidModel* m = L.m;
+    const float* W = m->d_w;
+    const int HW = H * Wd;
+    PwArgs p{};
+    p.in = X; p.w = W + b.c1w; p.bias = W + b.c1b; p.out = m->x1;
+    p.K = b.cin; p.N = b.mid; p.HW = HW; p.relu = 1;
+    p.w_tc = b.tc_c1.w; p.Kpad = b.tc_c1.Kpad; p.Npad = b.tc_c1.Npad;
+    L.pointwise(p);
+    int R = 0;
+    if (m->light_chain && m->light_v2) {
+        ChainArgs ca{};
+        ca.in = m->x1; ca.H = H;
+        for (int br = 0; br < 4; ++br) { ca.out[br] = m->Y[br][kDepth[br] & 1]; ca.sums[br] = m->sums[br]; }
+        for (int l = 0; l < 10; ++l) {
+            ca.wpw[l] = W + b.light[l].pw; ca.wdw[l] = W + b.light[l].dw; ca.bias[l] = W + b.light[l].b;
+        }
+        R = L.light_chain(ca, b.mid, Wd);
+    }
+    const bool chained = R > 0;
+    if (!chained) R = m->light_v2 ? pick_tile_rows2(H, Wd, b.mid) : pick_tile_rows(H, Wd, b.mid);
+    if (!chained && m->light_small && m->light_v2 && b.mid == 16 && Wd == 32) R = 8;
+    const int tiles = H / R;
+    const int threads = (256 / (b.mid / 4)) * (b.mid / 4);  // a multiple of the channel groups
+    for (int level = 1; level <= 4 && !chained; ++level) {
+        LightArgs la{};
+        la.H = H; la.W = Wd; la.C = b.mid; la.R = R;
+        int nb = 0;
+        for (int l = 0; l < 10; ++l) {
+            if (kLevelOfLight[l] != level) continue;
+            const int br = kBranchOfLight[l];
+            la.in[nb] = level == 1 ? m->x1 : m->Y[br][(level - 1) & 1];
+            la.out[nb] = m->Y[br][level & 1];
+            la.wpw[nb] = W + b.light[l].pw;
+            la.wdw[nb] = W + b.light[l].dw;
+            la.bias[nb] = W + b.light[l].b;
+            la.wtc[nb] = b.light_tc[l].w;
+            la.sums[nb] = kDepth[br] == level ? m->sums[br] : nullptr;
+            ++nb;
+        }
+        L.light(la, nb, threads);
+    }
+    GateArgs ga{};
+    for (int br = 0; br < 4; ++br) ga.sums[br] = m->sums[br];
+    ga.w1 = W + b.g1w; ga.b1 = W + b.g1b; ga.w2 = W + b.g2w; ga.b2 = W + b.g2b;
+    ga.gates = m->gates; ga.C = b.mid; ga.hid = b.hid; ga.tiles = tiles; ga.HW = HW;
+    L.begin(CLS_GATES);
+    k_gates<<<L.upper, 128, sizeof(float) * (4 * b.mid + 4 * b.hid), L.st>>>(ga, L.d_n, L.off, L.cap);
+    L.end();
+    ++L.launches;
+    PwArgs c{};
+    for (int br = 0; br < 4; ++br) c.branch[br] = m->Y[br][kDepth[br] & 1];
+    c.gates = m->gates; c.mid = b.mid;
+    c.in = b.has_ds ? X : nullptr;
+    c.residual = b.has_ds ? nullptr : X;
+    c.w = W + b.cw; c.bias = W + b.cb; c.out = Xo;
+    c.K = b.mid + (b.has_ds ? b.cin : 0); c.N = b.cout; c.HW = HW; c.relu = 1;
+    c.w_tc = b.tc_c.w; c.Kpad = b.tc_c.Kpad; c.Npad = b.tc_c.Npad;
+    L.pointwise(c);
+}
+
+// Transition (osnet.py conv2[2], conv3[2]): 1x1 + folded BN + ReLU of X [crops][H][Wd][C] into tmp, then 2x2 average
+// pool into out [crops][H/2][Wd/2][C] (out may be X).
+void run_transition(Launcher& L, const float* X, float* tmp, float* out, int H, int Wd, int C, size_t w, size_t bias,
+                    const TcW& tc) {
+    ReidModel* m = L.m;
+    PwArgs p{};
+    p.in = X; p.w = m->d_w + w; p.bias = m->d_w + bias; p.out = tmp;
+    p.K = C; p.N = C; p.HW = H * Wd; p.relu = 1;
+    p.w_tc = tc.w; p.Kpad = tc.Kpad; p.Npad = tc.Npad;
+    L.pointwise(p);
+    L.begin(CLS_AVGPOOL);
+    k_avgpool2<<<m->sms * 4, 256, 0, L.st>>>(tmp, H, Wd, C, L.d_n, L.off, L.cap, out);
+    L.end();
+    ++L.launches;
+}
+
+// LMBN_n, one chunk (lmbn_n.py:83-146 in eval).  Taps: 0 crop, 1 stem, 2 pool, 3 backone.2.0, 4 backone.2.1,
+// 5 backone.2.2, 6 trunk end (backone.3), then per branch in the order global, bottleneck, partial, channel:
+// 7-11 global .0.1, .0.2, .1.0, .1.1, .2 (branch end), 12 bottleneck, 13-17 partial, 18-22 channel.
+void run_lmbn_chunk(Launcher& L, const FrameIn& fi, float* d_out, int out_ld) {
+    ReidModel* m = L.m;
+    const LmbnW& lm = m->lm;
+    StageTaps stop_here{m};
+    if (run_front(L, fi, stop_here)) return;
+    float* A = m->bufA;
+    float* B = m->bufB;
+    int H = m->in_h / 4, Wd = 32;
+    run_osblock(L, lm.trunk[0], B, A, H, Wd);
+    if (stop_here(A, (size_t)H * Wd * 256)) return;
+    run_osblock(L, lm.trunk[1], A, B, H, Wd);
+    if (stop_here(B, (size_t)H * Wd * 256)) return;
+    run_transition(L, B, A, B, H, Wd, 256, lm.trunk_tw, lm.trunk_tb, TcW{});
+    H /= 2; Wd /= 2;
+    if (stop_here(B, (size_t)H * Wd * 256)) return;
+    run_osblock(L, lm.trunk[2], B, m->trunk, H, Wd);
+    if (stop_here(m->trunk, (size_t)H * Wd * 384)) return;
+    const int bh = H / 2, bw = Wd / 2;   // branch maps after their transition: 24 x 8
+    for (int br = 0; br < 3; ++br) {
+        run_osblock(L, lm.br[br][0], m->trunk, A, H, Wd);
+        if (stop_here(A, (size_t)H * Wd * 384)) return;
+        run_transition(L, A, B, A, H, Wd, 384, lm.br_tw[br], lm.br_tb[br], TcW{});
+        if (stop_here(A, (size_t)bh * bw * 384)) return;
+        run_osblock(L, lm.br[br][1], A, B, bh, bw);
+        if (stop_here(B, (size_t)bh * bw * LMBN_C)) return;
+        run_osblock(L, lm.br[br][2], B, A, bh, bw);
+        if (stop_here(A, (size_t)bh * bw * LMBN_C)) return;
+        PwArgs p{};   // conv5
+        p.in = A; p.w = m->d_w + lm.br_c5w[br]; p.bias = m->d_w + lm.br_c5b[br]; p.out = B;
+        p.K = LMBN_C; p.N = LMBN_C; p.HW = bh * bw; p.relu = 1;
+        L.pointwise(p);
+        if (stop_here(B, (size_t)bh * bw * LMBN_C)) return;
+        const float* pool_src = B;
+        if (br == 0) {   // BatchFeatureErase_Top in eval: the bottleneck OSBlock; glo and glo_drop are its output
+            run_osblock(L, lm.bottleneck, B, A, bh, bw);
+            if (stop_here(A, (size_t)bh * bw * LMBN_C)) return;
+            pool_src = A;
+        }
+        L.begin(CLS_HEAD);
+        k_lmbn_pool<<<L.upper, 256, 0, L.st>>>(pool_src, bh, bw, LMBN_C, br, m->pooled, L.d_n, L.off, L.cap);
+        L.end();
+        ++L.launches;
+    }
+    NeckArgs na{};
+    for (int k = 0; k < 5; ++k) { na.w[k] = m->d_w + lm.neck_w[k]; na.b[k] = m->d_w + lm.neck_b[k]; }
+    na.wsh = m->d_w + lm.sh_w; na.bsh = m->d_w + lm.sh_b; na.chst = m->d_w + lm.ch_st;
+    RCUDA_OK(cudaFuncSetAttribute(k_lmbn_neck, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)NECK_SMEM));
+    L.begin(CLS_HEAD);
+    k_lmbn_neck<<<dim3(LMBN_C / NECK_COLS, 6), 256, NECK_SMEM, L.st>>>(na, m->pooled, fi.crops, L.d_n, L.off, L.cap,
+                                                                         d_out, out_ld);
+    L.end();
+    ++L.launches;
+    L.begin(CLS_HEAD);
+    k_l2_normalise<<<L.upper, 256, 0, L.st>>>(fi.crops, L.d_n, L.off, L.cap, d_out, out_ld, m->feat);
+    L.end();
+    ++L.launches;
+}
 }  // namespace
 
 }  // namespace bmb
@@ -1680,7 +1936,7 @@ int reid_forward(ReidModel* m, const uint8_t* d_images, size_t image_stride, int
             Launcher L{m, d_ncrops, off, upper, upper, st};
             L.begin(CLS_CROP);
             k_crop_resize_norm<<<upper, 256, 0, st>>>(d_images, image_stride, rows, cols, d_crops, d_ncrops, off, upper,
-                                                      m->blob, m->preprocess);
+                                                      m->blob, m->preprocess, IN_H);
             L.end();
             ++L.launches;
             float* X = m->bufA;
@@ -1723,21 +1979,27 @@ int reid_forward(ReidModel* m, const uint8_t* d_images, size_t image_stride, int
         RCUDA_OK(cudaGetLastError());
         return launches;
     }
+    const FrameIn fi{d_images, image_stride, rows, cols, d_crops};
+    if (m->arch == 3) {
+        for (int off = first_crop; off < last_crop; off += m->chunk) {
+            const int upper = (last_crop - off) < m->chunk ? (last_crop - off) : m->chunk;
+            Launcher L{m, d_ncrops, off, upper, upper, st};
+            run_lmbn_chunk(L, fi, d_out, out_ld);
+            launches += L.launches;
+        }
+        RCUDA_OK(cudaGetLastError());
+        return launches;
+    }
     for (int off = first_crop; off < last_crop; off += m->chunk) {
         const int upper = (last_crop - off) < m->chunk ? (last_crop - off) : m->chunk;
         Launcher L{m, d_ncrops, off, upper, upper, st};
-        int stage_idx = 0;
-        auto stop_here = [&](const float* ptr, size_t per_crop) {
-            if (m->debug_stop == stage_idx) { m->debug_ptr = ptr; m->debug_floats_per_crop = per_crop; ++stage_idx; return true; }
-            ++stage_idx;
-            return false;
-        };
+        StageTaps stop_here{m};
         if (m->tc && m->debug_stop != 0 && m->debug_stop != 1) {
             // tensor-core path: crop staging, stem and max pool are one fused kernel (k_front_tc); diagnostic stops at the
             // blob / stem tensors (0, 1) run the float32 kernels below instead
             bool tc_stopped = false;
-            const tcx::FrontInput fi{d_images, image_stride, rows, cols, d_crops, d_out, out_ld};
-            L.launches += tcx::plan_run(m, fi, d_ncrops, off, upper, st, &tc_stopped, L);
+            const tcx::FrontInput tfi{d_images, image_stride, rows, cols, d_crops, d_out, out_ld};
+            L.launches += tcx::plan_run(m, tfi, d_ncrops, off, upper, st, &tc_stopped, L);
             if (!tc_stopped && !(m->tc->head_fused && m->debug_stop < 0)) {
                 const int C = m->c[3];
                 L.begin(CLS_HEAD);
@@ -1749,27 +2011,7 @@ int reid_forward(ReidModel* m, const uint8_t* d_images, size_t image_stride, int
             launches += L.launches;
             continue;
         }
-        L.begin(CLS_CROP);
-        k_crop_resize_norm<<<upper, 256, 0, st>>>(d_images, image_stride, rows, cols, d_crops, d_ncrops, off, upper,
-                                                  m->blob, m->preprocess);
-        L.end();
-        ++L.launches;
-        if (stop_here(m->blob, (size_t)IN_H * IN_W * 3)) { launches += L.launches; continue; }
-        {
-            const size_t smem = sizeof(float) * ((size_t)((ST_IR * ST_IC * 3 + 3) & ~3) + 147 * 16);
-            RCUDA_OK(cudaFuncSetAttribute(k_stem, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            L.begin(CLS_STEM);
-            k_stem<<<dim3(128 / ST_R, upper), 256, smem, st>>>(m->blob, W + m->stem_w, W + m->stem_b, m->c[0], d_ncrops,
-                                                                off, upper, m->bufA);
-            L.end();
-            ++L.launches;
-        }
-        if (stop_here(m->bufA, (size_t)8192 * m->c[0])) { launches += L.launches; continue; }
-        L.begin(CLS_MAXPOOL);
-        k_maxpool3s2<<<m->sms * 8, 256, 0, st>>>(m->bufA, 128, 64, m->c[0], d_ncrops, off, upper, m->bufB);
-        L.end();
-        ++L.launches;
-        if (stop_here(m->bufB, (size_t)2048 * m->c[0])) { launches += L.launches; continue; }
+        if (run_front(L, fi, stop_here)) { launches += L.launches; continue; }
         float* X = m->bufB;
         float* Xo = m->bufA;
         int H = 64, Wd = 32;
@@ -1777,77 +2019,14 @@ int reid_forward(ReidModel* m, const uint8_t* d_images, size_t image_stride, int
         for (int s = 0; s < 3 && !stopped; ++s) {
             for (int j = 0; j < 2 && !stopped; ++j) {
                 const BlockW& b = m->blocks[s * 2 + j];
-                const int HW = H * Wd;
-                PwArgs p{};
-                p.in = X; p.w = W + b.c1w; p.bias = W + b.c1b; p.out = m->x1;
-                p.K = b.cin; p.N = b.mid; p.HW = HW; p.relu = 1;
-                p.w_tc = b.tc_c1.w; p.Kpad = b.tc_c1.Kpad; p.Npad = b.tc_c1.Npad;
-                L.pointwise(p);
-                int R = 0;
-                if (m->light_chain && m->light_v2) {
-                    ChainArgs ca{};
-                    ca.in = m->x1; ca.H = H;
-                    for (int br = 0; br < 4; ++br) { ca.out[br] = m->Y[br][kDepth[br] & 1]; ca.sums[br] = m->sums[br]; }
-                    for (int l = 0; l < 10; ++l) {
-                        ca.wpw[l] = W + b.light[l].pw; ca.wdw[l] = W + b.light[l].dw; ca.bias[l] = W + b.light[l].b;
-                    }
-                    R = L.light_chain(ca, b.mid, Wd);
-                }
-                const bool chained = R > 0;
-                if (!chained) R = m->light_v2 ? pick_tile_rows2(H, Wd, b.mid) : pick_tile_rows(H, Wd, b.mid);
-                if (!chained && m->light_small && m->light_v2 && b.mid == 16 && Wd == 32) R = 8;
-                const int tiles = H / R;
-                const int threads = (256 / (b.mid / 4)) * (b.mid / 4);  // a multiple of the channel groups
-                for (int level = 1; level <= 4 && !chained; ++level) {
-                    LightArgs la{};
-                    la.H = H; la.W = Wd; la.C = b.mid; la.R = R;
-                    int nb = 0;
-                    for (int l = 0; l < 10; ++l) {
-                        if (kLevelOfLight[l] != level) continue;
-                        const int br = kBranchOfLight[l];
-                        la.in[nb] = level == 1 ? m->x1 : m->Y[br][(level - 1) & 1];
-                        la.out[nb] = m->Y[br][level & 1];
-                        la.wpw[nb] = W + b.light[l].pw;
-                        la.wdw[nb] = W + b.light[l].dw;
-                        la.bias[nb] = W + b.light[l].b;
-                        la.wtc[nb] = b.light_tc[l].w;
-                        la.sums[nb] = kDepth[br] == level ? m->sums[br] : nullptr;
-                        ++nb;
-                    }
-                    L.light(la, nb, threads);
-                }
-                GateArgs ga{};
-                for (int br = 0; br < 4; ++br) ga.sums[br] = m->sums[br];
-                ga.w1 = W + b.g1w; ga.b1 = W + b.g1b; ga.w2 = W + b.g2w; ga.b2 = W + b.g2b;
-                ga.gates = m->gates; ga.C = b.mid; ga.hid = b.hid; ga.tiles = tiles; ga.HW = HW;
-                L.begin(CLS_GATES);
-                k_gates<<<upper, 128, sizeof(float) * (4 * b.mid + 4 * b.hid), st>>>(ga, d_ncrops, off, upper);
-                L.end();
-                ++L.launches;
-                PwArgs c{};
-                for (int br = 0; br < 4; ++br) c.branch[br] = m->Y[br][kDepth[br] & 1];
-                c.gates = m->gates; c.mid = b.mid;
-                c.in = b.has_ds ? X : nullptr;
-                c.residual = b.has_ds ? nullptr : X;
-                c.w = W + b.cw; c.bias = W + b.cb; c.out = Xo;
-                c.K = b.mid + (b.has_ds ? b.cin : 0); c.N = b.cout; c.HW = HW; c.relu = 1;
-                c.w_tc = b.tc_c.w; c.Kpad = b.tc_c.Kpad; c.Npad = b.tc_c.Npad;
-                L.pointwise(c);
+                run_osblock(L, b, X, Xo, H, Wd);
                 float* t = X; X = Xo; Xo = t;
-                if (stop_here(X, (size_t)HW * b.cout)) { stopped = true; break; }
+                if (stop_here(X, (size_t)H * Wd * b.cout)) { stopped = true; break; }
             }
             if (stopped) break;
             if (s < 2) {
                 const int C = m->c[s + 1];
-                PwArgs p{};
-                p.in = X; p.w = W + m->trans_w[s]; p.bias = W + m->trans_b[s]; p.out = Xo;
-                p.K = C; p.N = C; p.HW = H * Wd; p.relu = 1;
-                p.w_tc = m->tc_trans[s].w; p.Kpad = m->tc_trans[s].Kpad; p.Npad = m->tc_trans[s].Npad;
-                L.pointwise(p);
-                L.begin(CLS_AVGPOOL);
-                k_avgpool2<<<m->sms * 4, 256, 0, st>>>(Xo, H, Wd, C, d_ncrops, off, upper, X);
-                L.end();
-                ++L.launches;
+                run_transition(L, X, Xo, X, H, Wd, C, m->trans_w[s], m->trans_b[s], m->tc_trans[s]);
                 H /= 2; Wd /= 2;
                 if (stop_here(X, (size_t)H * Wd * C)) { stopped = true; break; }
             }

@@ -16,7 +16,7 @@ import numpy as np
 
 from . import _lib
 from ._lib import B200Error
-from .weights import export_blob, read_blob
+from .weights import ARCH_LMBN_N, export_blob, read_blob
 
 
 class _StagedCrops:
@@ -49,6 +49,8 @@ class B200ReID:
             raise TypeError("weights must be a path to a .pt checkpoint or a .b200reid blob")
         header, _ = read_blob(self.blob_path)
         self.feature_dim = int(header[7])
+        if header[2] == ARCH_LMBN_N:
+            self.input_shape = (int(header[9]), 128)   # LMBN_n runs on 384x128 crops (base_backend.py:59-60)
         self.half = bool(half)
         self.device = "cuda:0"
         self.handle = ctypes.c_void_p()
@@ -125,8 +127,8 @@ class B200ReID:
             raise B200Error(self._err())
         return out.astype(np.float16) if self.half else out
 
-    def warmup(self, imgsz=((256, 128, 3),)):
-        im = np.zeros(imgsz[0], dtype=np.uint8)
+    def warmup(self, imgsz=None):
+        im = np.zeros(imgsz[0] if imgsz else (*self.input_shape, 3), dtype=np.uint8)
         self.get_features(np.array([[0, 0, 64, 64], [0, 0, 128, 128]], np.float32), im)
 
     # ---- diagnostics --------------------------------------------------------------------------------------
@@ -135,7 +137,7 @@ class B200ReID:
         boxes = self._boxes(xyxys)
         img = np.ascontiguousarray(img, dtype=np.uint8)
         per = ctypes.c_int(0)
-        cap = len(boxes) * 8192 * 64
+        cap = len(boxes) * (self.input_shape[0] // 2) * 64 * 64   # the largest tap: the stem output
         out = np.empty(cap, np.float32)
         ok = self.lib.boxmot_b200_reid_debug_stage(self.handle, boxes.ctypes.data, len(boxes), img.ctypes.data,
                                                    img.shape[0], img.shape[1], stage, out.ctypes.data, cap,

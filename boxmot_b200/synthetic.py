@@ -55,12 +55,9 @@ def bench_stream(n_dets: int, n_frames: int, hw=(720, 1280), stream: int = 0):
 
 
 
-def make_osnet_state(arch: str = "osnet_x0_25", seed: int = 0, feature_dim: int = 512, num_classes: int = 1041):
+def _osnet_makers(g, sd):
+    """conv / bn / osblock generators writing seeded tensors with the reference's parameter names into `sd`."""
     import torch
-
-    ch = OSNET_ARCHS[arch]
-    g = torch.Generator().manual_seed(seed)
-    sd = {}
 
     def conv(name, co, ci, k, groups=1, gain=1.0):
         fan_in = (ci // groups) * k * k
@@ -97,6 +94,16 @@ def make_osnet_state(arch: str = "osnet_x0_25", seed: int = 0, feature_dim: int 
             conv(name + ".downsample.conv", cout, cin, 1)
             bn(name + ".downsample.bn", cout)
 
+    return conv, bn, osblock
+
+
+def make_osnet_state(arch: str = "osnet_x0_25", seed: int = 0, feature_dim: int = 512, num_classes: int = 1041):
+    import torch
+
+    ch = OSNET_ARCHS[arch]
+    g = torch.Generator().manual_seed(seed)
+    sd = {}
+    conv, bn, osblock = _osnet_makers(g, sd)
     conv("conv1.conv", ch[0], 3, 7)
     bn("conv1.bn", ch[0])
     for s, (cin, cout) in enumerate(((ch[0], ch[1]), (ch[1], ch[2]), (ch[2], ch[3]))):
@@ -113,6 +120,47 @@ def make_osnet_state(arch: str = "osnet_x0_25", seed: int = 0, feature_dim: int 
     bn("fc.1", feature_dim)
     sd["classifier.weight"] = 0.01 * torch.randn(num_classes, feature_dim, generator=g)
     sd["classifier.bias"] = torch.zeros(num_classes)
+    return sd
+
+
+LMBN_BRANCHES = ("global_branch", "partial_branch", "channel_branch")
+
+
+def make_lmbn_n_state(seed: int = 0, num_classes: int = 702):
+    """Seeded state dict with the parameter names of the reference's LMBN_n (reid/backbones/lmbn/lmbn_n.py): the
+    OSNet_x1_0 trunk up to conv3[0] (`backone`), three branches of conv3[1:] + conv4 + conv5 (nn.Sequential slicing
+    keeps the indices: `*_branch.0.1`, `*_branch.0.2.0`), the BatchFeatureErase_Top bottleneck OSBlock, five BNNeck3
+    necks, `shared` and two BNNeck.  Every BatchNorm has randomised running statistics so folding is exercised."""
+    import torch
+
+    g = torch.Generator().manual_seed(seed)
+    sd = {}
+    conv, bn, osblock = _osnet_makers(g, sd)
+    conv("backone.0.conv", 64, 3, 7)
+    bn("backone.0.bn", 64)
+    osblock("backone.2.0", 64, 256)
+    osblock("backone.2.1", 256, 256)
+    conv("backone.2.2.0.conv", 256, 256, 1)
+    bn("backone.2.2.0.bn", 256)
+    osblock("backone.3", 256, 384)
+    for br in LMBN_BRANCHES:
+        osblock(f"{br}.0.1", 384, 384)
+        conv(f"{br}.0.2.0.conv", 384, 384, 1)
+        bn(f"{br}.0.2.0.bn", 384)
+        osblock(f"{br}.1.0", 384, 512)
+        osblock(f"{br}.1.1", 512, 512)
+        conv(f"{br}.2.conv", 512, 512, 1)
+        bn(f"{br}.2.bn", 512)
+    for i in range(5):
+        conv(f"reduction_{i}.reduction", 512, 512, 1)
+        bn(f"reduction_{i}.bn", 512)
+        sd[f"reduction_{i}.classifier.weight"] = 0.001 * torch.randn(num_classes, 512, generator=g)
+    conv("shared.0", 512, 256, 1, gain=2.0)
+    bn("shared.1", 512)
+    for j in range(2):
+        bn(f"reduction_ch_{j}.bn", 512)
+        sd[f"reduction_ch_{j}.classifier.weight"] = 0.001 * torch.randn(num_classes, 512, generator=g)
+    osblock("batch_drop_block.drop_batch_bottleneck", 512, 512)
     return sd
 
 

@@ -16,6 +16,8 @@ followed by float32 parameters in the exact order csrc/reid_model.cu walks them:
       transition (s < 2)  W[cout][cout], b[cout]
     conv5     W[c3][c3], b[c3]
     fc        W[c3][feat] (BatchNorm1d folded), b[feat]
+Arch 3 (LMBN_n, `fold_lmbn_n`) keeps the OSNet header dims (64, 256, 384, 512, feat 3584) and records the input
+height (384) in header word 9; its tensors reuse the OSBlock / transition layouts above.
 All 1x1 weights are stored K-major ([cin][cout]) so a thread owning consecutive output channels loads
 consecutive floats; every tensor is zero-padded to a multiple of 4 floats (16-byte aligned float4 loads).
 """
@@ -32,6 +34,7 @@ MAGIC = 0x45523242  # 'B2RE'
 VERSION = 1
 ARCH_OSNET = 1
 ARCH_MOBILENETV2 = 2
+ARCH_LMBN_N = 3
 BRANCHES = (("conv2a", 1), ("conv2b", 2), ("conv2c", 3), ("conv2d", 4))
 EPS = 1e-5
 
@@ -70,42 +73,46 @@ def _pw(sd, name, bn=None):
     return w.T.copy(), b
 
 
+def _fold_osblock(sd, name, cin, cout) -> List[np.ndarray]:
+    mid = cout // 4
+    assert sd[name + ".conv1.conv.weight"].shape[:2] == (mid, cin)
+    out = list(_pw(sd, name + ".conv1.conv", name + ".conv1.bn"))
+    for br, depth in BRANCHES:
+        for k in range(depth):
+            lname = f"{name}.{br}" if br == "conv2a" else f"{name}.{br}.{k}"
+            wpw, _ = _pw(sd, lname + ".conv1")
+            sc, sh = _bn_fold(sd, lname + ".bn")
+            wdw = _np(sd[lname + ".conv2.weight"])[:, 0] * sc[:, None, None]  # [c][3][3]
+            out += [wpw, wdw.reshape(mid, 9).T.copy(), sh]
+    w1, b1 = _pw(sd, name + ".gate.fc1")
+    w2, b2 = _pw(sd, name + ".gate.fc2")
+    out += [w1, b1, w2, b2]
+    w3, b3 = _pw(sd, name + ".conv3.conv", name + ".conv3.bn")
+    if (name + ".downsample.conv.weight") in sd:
+        wd, bd = _pw(sd, name + ".downsample.conv", name + ".downsample.bn")
+        out += [np.concatenate([w3, wd], 0), b3 + bd]
+    else:
+        assert cin == cout
+        out += [w3, b3]
+    return out
+
+
+def _fold_stem(sd, conv, bn) -> List[np.ndarray]:
+    w = _np(sd[conv + ".weight"])  # [c0][3][7][7]
+    scale, shift = _bn_fold(sd, bn)
+    w = w * scale[:, None, None, None]
+    return [w.transpose(2, 3, 1, 0).reshape(147, w.shape[0]), shift]
+
+
 def fold_osnet(sd) -> Tuple[List[int], List[np.ndarray]]:
     c0 = sd["conv1.conv.weight"].shape[0]
     chans = [c0] + [sd[f"conv{s + 2}.1.conv3.conv.weight"].shape[0] for s in range(3)]
     feat = sd["fc.0.weight"].shape[0]
-    out: List[np.ndarray] = []
-    # stem
-    w = _np(sd["conv1.conv.weight"])  # [c0][3][7][7]
-    scale, shift = _bn_fold(sd, "conv1.bn")
-    w = w * scale[:, None, None, None]
-    out += [w.transpose(2, 3, 1, 0).reshape(147, c0), shift]
+    out: List[np.ndarray] = _fold_stem(sd, "conv1.conv", "conv1.bn")
     for s in range(3):
         stage = f"conv{s + 2}"
         for j in range(2):
-            name = f"{stage}.{j}"
-            cin = chans[s] if j == 0 else chans[s + 1]
-            cout = chans[s + 1]
-            mid = cout // 4
-            assert sd[name + ".conv1.conv.weight"].shape[:2] == (mid, cin)
-            out += list(_pw(sd, name + ".conv1.conv", name + ".conv1.bn"))
-            for br, depth in BRANCHES:
-                for k in range(depth):
-                    lname = f"{name}.{br}" if br == "conv2a" else f"{name}.{br}.{k}"
-                    wpw, _ = _pw(sd, lname + ".conv1")
-                    sc, sh = _bn_fold(sd, lname + ".bn")
-                    wdw = _np(sd[lname + ".conv2.weight"])[:, 0] * sc[:, None, None]  # [c][3][3]
-                    out += [wpw, wdw.reshape(mid, 9).T.copy(), sh]
-            w1, b1 = _pw(sd, name + ".gate.fc1")
-            w2, b2 = _pw(sd, name + ".gate.fc2")
-            out += [w1, b1, w2, b2]
-            w3, b3 = _pw(sd, name + ".conv3.conv", name + ".conv3.bn")
-            if (name + ".downsample.conv.weight") in sd:
-                wd, bd = _pw(sd, name + ".downsample.conv", name + ".downsample.bn")
-                out += [np.concatenate([w3, wd], 0), b3 + bd]
-            else:
-                assert cin == cout
-                out += [w3, b3]
+            out += _fold_osblock(sd, f"{stage}.{j}", chans[s] if j == 0 else chans[s + 1], chans[s + 1])
         if s < 2:
             out += list(_pw(sd, f"{stage}.2.0.conv", f"{stage}.2.0.bn"))
     out += list(_pw(sd, "conv5.conv", "conv5.bn"))
@@ -114,6 +121,61 @@ def fold_osnet(sd) -> Tuple[List[int], List[np.ndarray]]:
     scale, shift = _bn_fold(sd, "fc.1")
     out += [(wf * scale[:, None]).T.copy(), bf * scale + shift]
     return chans + [feat], out
+
+
+# LMBN_n (reid/backbones/lmbn/lmbn_n.py): the output row interleaves seven 512-d vectors, element c*7 + k being channel
+# c of vector k.  LMBN_NECKS lists, per vector k < 5, the BNNeck3 that produces it (reduction_0 on the average-pooled
+# bottleneck output, reduction_4 on its max pool, reduction_1 on the max-pooled partial branch, reduction_2 / _3 on
+# the averages of its top / bottom halves); vectors 5 and 6 are the channel halves through `shared` + reduction_ch_*.
+LMBN_NECKS = (0, 4, 1, 2, 3)
+LMBN_INPUT_H = 384
+LMBN_FEAT = 3584
+
+
+def _lmbn_n_keys():
+    from .synthetic import make_lmbn_n_state
+
+    return {k for k in make_lmbn_n_state(0, num_classes=1) if not k.endswith("num_batches_tracked")}
+
+
+def is_lmbn(sd) -> bool:
+    return "backone.0.conv.weight" in sd
+
+
+def fold_lmbn_n(sd) -> List[np.ndarray]:
+    """LMBN_n state dict -> arrays of the arch-3 blob in the order csrc/reid_model.cu walks them:
+        stem | trunk: backone.2.0, backone.2.1, transition backone.2.2.0, backone.3 (OSBlocks laid out as in OSNet)
+        per branch (global, partial, channel): OSBlock .0.1, transition .0.2.0, OSBlocks .1.0 and .1.1, conv5 .2
+        bottleneck OSBlock (batch_drop_block.drop_batch_bottleneck; BatchDropTop is the identity in eval)
+        necks: for k in LMBN_NECKS: reduction_k 1x1 with its BatchNorm1d folded, W[512][512], b[512]
+        shared: 1x1 256 -> 512 with shared.1 folded, W[256][512], b[512]
+        reduction_ch_0, reduction_ch_1: BatchNorm1d as scale[512], shift[512] (it follows a ReLU: not foldable)
+    Refuses (ValueError) any state dict whose key set is not exactly LMBN_n's, e.g. lmbn_ain_n's instance norms."""
+    keys = {k for k in sd if not k.endswith("num_batches_tracked")}
+    want = _lmbn_n_keys()
+    if keys != want:
+        extra, missing = sorted(keys - want)[:3], sorted(want - keys)[:3]
+        raise ValueError(f"not an LMBN_n state dict (unexpected keys {extra}, missing keys {missing})")
+    out: List[np.ndarray] = _fold_stem(sd, "backone.0.conv", "backone.0.bn")
+    out += _fold_osblock(sd, "backone.2.0", 64, 256)
+    out += _fold_osblock(sd, "backone.2.1", 256, 256)
+    out += list(_pw(sd, "backone.2.2.0.conv", "backone.2.2.0.bn"))
+    out += _fold_osblock(sd, "backone.3", 256, 384)
+    from .synthetic import LMBN_BRANCHES
+
+    for br in LMBN_BRANCHES:
+        out += _fold_osblock(sd, f"{br}.0.1", 384, 384)
+        out += list(_pw(sd, f"{br}.0.2.0.conv", f"{br}.0.2.0.bn"))
+        out += _fold_osblock(sd, f"{br}.1.0", 384, 512)
+        out += _fold_osblock(sd, f"{br}.1.1", 512, 512)
+        out += list(_pw(sd, f"{br}.2.conv", f"{br}.2.bn"))
+    out += _fold_osblock(sd, "batch_drop_block.drop_batch_bottleneck", 512, 512)
+    for k in LMBN_NECKS:
+        out += list(_pw(sd, f"reduction_{k}.reduction", f"reduction_{k}.bn"))
+    out += list(_pw(sd, "shared.0", "shared.1"))
+    for j in range(2):
+        out += list(_bn_fold(sd, f"reduction_ch_{j}.bn"))
+    return out
 
 
 def _pad4(n: int) -> int:
@@ -192,8 +254,11 @@ def export_blob(weights, out_path=None) -> Path:
     elif "conv1.conv.weight" in sd and "conv5.conv.weight" in sd and "fc.0.weight" in sd:
         dims, arrays = fold_osnet(sd)
         arch = ARCH_OSNET
+    elif is_lmbn(sd):
+        arrays = fold_lmbn_n(sd)
+        arch, dims = ARCH_LMBN_N, [64, 256, 384, 512, LMBN_FEAT]
     else:
-        raise ValueError("only OSNet and MobileNetV2 state dicts are implemented on the B200 ReID path")
+        raise ValueError("only OSNet, MobileNetV2 and LMBN_n state dicts are implemented on the B200 ReID path")
     # every tensor starts on a 16-byte boundary (the kernels read weights as float4)
     padded = []
     for a in arrays:
@@ -201,6 +266,8 @@ def export_blob(weights, out_path=None) -> Path:
         padded.append(np.pad(flat, (0, (-flat.size) % 4)))
     payload = np.concatenate(padded)
     header = [MAGIC, VERSION, arch, *dims, int(payload.size)] + [0] * (16 - 9)
+    if arch == ARCH_LMBN_N:
+        header[9] = LMBN_INPUT_H
     out_path = Path(out_path)
     tmp = out_path.with_suffix(out_path.suffix + ".tmp")
     with open(tmp, "wb") as f:
