@@ -94,6 +94,9 @@ SYMBOLS = {
     "boxmot_b200_tracker_set_cmc": (c_int, [c_void_p, c_char_p]),
     "boxmot_b200_cmc_ecc": (c_int, [c_void_p, c_void_p, c_int, c_int, c_double, c_double, c_int, c_void_p, POINTER(c_int),
                                     c_void_p]),
+    "boxmot_b200_cmc_sof_create": (c_void_p, [c_double, c_int, c_double, c_double]),
+    "boxmot_b200_cmc_sof_apply": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_int, c_void_p, POINTER(c_int)]),
+    "boxmot_b200_cmc_sof_destroy": (None, [c_void_p]),
     "boxmot_b200_tracker_mark": (c_int, [c_void_p, c_int]),
     "boxmot_b200_tracker_elapsed_ms": (c_int, [c_void_p, POINTER(c_double)]),
     "boxmot_b200_tracker_phase_clocks": (c_int, [c_void_p, c_int, c_void_p, c_int]),

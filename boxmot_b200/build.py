@@ -12,7 +12,7 @@ LIB = PKG / "libboxmot_b200.so"
 
 # -fmad=false for the float64 tracker translation units: the reference's numpy arithmetic never contracts
 # a*b+c, and the Kalman / IoU / cost expressions are reproduced operation by operation.
-TRACKER_SOURCES = ["tracker_engine.cu", "ss_kernels.cu", "cmc_kernels.cu", "capi.cu"]
+TRACKER_SOURCES = ["tracker_engine.cu", "ss_kernels.cu", "cmc_kernels.cu", "cmc_sof_kernels.cu", "capi.cu"]
 REID_SOURCES = ["reid_model.cu"]
 COMMON = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
           "-Xcompiler", "-fPIC,-fvisibility=hidden"]

@@ -280,6 +280,22 @@ int boxmot_b200_cmc_ecc(const uint8_t* prev_bgr, const uint8_t* cur_bgr, int row
         standalone_ecc(prev_bgr, cur_bgr, rows, cols, scale, eps, max_iter, warp2x3, status, prepared);
     });
 }
+BoxMOTB200CmcSof* boxmot_b200_cmc_sof_create(double scale, int min_inliers, double min_inlier_ratio,
+                                             double ransac_reproj_threshold) {
+    void* h = nullptr;
+    guard([&] { h = sof_create(scale, min_inliers, min_inlier_ratio, ransac_reproj_threshold); });
+    return reinterpret_cast<BoxMOTB200CmcSof*>(h);
+}
+int boxmot_b200_cmc_sof_apply(BoxMOTB200CmcSof* handle, const uint8_t* bgr, int rows, int cols, const float* dets_xyxy,
+                              int n_dets, float* warp2x3, int* status) {
+    return guard([&] {
+        if (!handle || !bgr || !warp2x3) throw std::runtime_error("NULL argument");
+        sof_apply(handle, bgr, rows, cols, dets_xyxy, n_dets, warp2x3, status);
+    });
+}
+void boxmot_b200_cmc_sof_destroy(BoxMOTB200CmcSof* handle) {
+    guard([&] { sof_destroy(handle); });
+}
 int boxmot_b200_jv_dense_mode(int cta_wide) {
     return guard([&] { set_jv_wide(cta_wide); });
 }

@@ -60,13 +60,20 @@ __global__ void __launch_bounds__(512) k_cmc_ecc(uint8_t* prev, const uint8_t* c
     if (threadIdx.x == 0) has_prev[s] = 1;
 }
 
+void cmc_enqueue_prepare(const uint8_t* images, size_t image_stride, int rows, int cols, int S, double scale, uint8_t* out,
+                         cudaStream_t st) {
+    int h, w;
+    cmc_scaled_size(rows, cols, scale, &h, &w);
+    dim3 g((h * w + 255) / 256, S);
+    k_cmc_prepare<<<g, 256, 0, st>>>(images, image_stride, rows, cols, 1.0 / scale, out, h, w);
+}
+
 void cmc_enqueue_ecc(const uint8_t* images, size_t image_stride, int rows, int cols, int S, double scale, double eps,
                      int max_iter, uint8_t* prev, uint8_t* cur, int* has_prev, const int* const* gate, double* warp,
                      cudaStream_t st) {
     int h, w;
     cmc_scaled_size(rows, cols, scale, &h, &w);
-    dim3 g((h * w + 255) / 256, S);
-    k_cmc_prepare<<<g, 256, 0, st>>>(images, image_stride, rows, cols, 1.0 / scale, cur, h, w);
+    cmc_enqueue_prepare(images, image_stride, rows, cols, S, scale, cur, st);
     k_cmc_ecc<<<S, 512, 0, st>>>(prev, cur, has_prev, gate, h, w, eps, max_iter, (float)scale, warp);
     CMC_CUDA_OK(cudaGetLastError());
 }

@@ -46,6 +46,8 @@ void reid_profile_collect(ReidModel* m, double* ms, int* launches);
 void reid_set_debug_stop(ReidModel* m, int stage);
 const float* reid_debug_tensor(const ReidModel* m, size_t* floats_per_crop);
 
+struct SofState;   // cmc_sof_kernels.cu
+
 // ---- tracker engine (tracker_engine.cu) -----------------------------------------------------------------
 struct Engine {
     TrkCfg cfg{};
@@ -72,7 +74,8 @@ struct Engine {
     float* d_embs = nullptr;
     double* d_warp = nullptr;      // [S][8] pending camera-motion warps (slot 6 = pending flag)
     bool warp_dirty = false;
-    // on-device camera-motion estimation (cmc_ecc.cuh): 0 = off (warps are supplied), 1 = the reference's ECC defaults
+    // on-device camera-motion estimation: 0 = off (warps are supplied), 1 = the reference's ECC defaults (cmc_ecc.cuh),
+    // 2 = the reference's SOF defaults (cmc_sof.cuh)
     int cmc_mode = 0;
     double cmc_scale = 0.15, cmc_eps = 1e-5;
     int cmc_iters = 100;
@@ -81,6 +84,7 @@ struct Engine {
     uint8_t* d_cmc_cur = nullptr;
     int* d_cmc_has_prev = nullptr;       // [S]
     const int** d_cmc_gate = nullptr;    // [S] device pointers to the live-track count (StrongSORT) or null
+    SofState* sof = nullptr;             // cmc_mode 2: the reference's SOF estimator (BoT-SORT, DeepOCSORT)
     float* d_out = nullptr;
     int* d_scalars_out = nullptr;
     CropDesc* d_crops = nullptr;
@@ -143,7 +147,7 @@ struct Engine {
     int snapshot(int stream_index, int* ids, double* means, double* covs, int cap);
     int track_ids(int stream_index, int which, int* ids, int cap);
     void set_warp(int stream_index, const double* warp6);
-    void set_cmc(const char* method);   // "ecc" | "none" / "" / NULL
+    void set_cmc(const char* method);   // "ecc" | "sof" | "none" / "" / NULL
     void read_timers(int stream_index, long long* out16, bool reset);
     void set_profile(bool on);
     void profile_read(double* ms, int* launch_counts);  // REID_N_CLASSES + 1 entries (last = association)
@@ -178,11 +182,31 @@ inline void cmc_scaled_size(int rows, int cols, double scale, int* h, int* w) {
     *h = (int)nearbyint(rows * scale);
     *w = (int)nearbyint(cols * scale);
 }
+// BaseCMC.preprocess of S frames (image_stride bytes apart) into out [S][h * w]
+void cmc_enqueue_prepare(const uint8_t* images, size_t image_stride, int rows, int cols, int S, double scale, uint8_t* out,
+                         cudaStream_t st);
 void cmc_enqueue_ecc(const uint8_t* images, size_t image_stride, int rows, int cols, int S, double scale, double eps,
                      int max_iter, uint8_t* prev, uint8_t* cur, int* has_prev, const int* const* gate, double* warp,
                      cudaStream_t st);
 void standalone_ecc(const uint8_t* prev_bgr, const uint8_t* cur_bgr, int rows, int cols, double scale, double eps,
                     int max_iter, float* warp6, int* status, uint8_t* prepared_out);
+
+// ---- SOF camera-motion estimator (cmc_sof_kernels.cu) ---------------------------------------------------------------
+// SofState: per-stream estimator state of S streams (pyramids, keypoints, workspace sized from the registration image)
+SofState* sof_state_create(int S, double scale, int min_inliers, double min_ratio, double ransac_thresh);
+void sof_state_free(SofState* st);
+void sof_state_reset(SofState* st, cudaStream_t cs);   // every stream initialises again on its next frame
+// SOF.apply for S frames (device, image_stride bytes apart); the boxes of the detection rows dets [S][det_cap][det_stride]
+// (n: ndets[S]; with conf_col >= 0 only rows with row[conf_col] > conf_thr) leave the corner mask.  Accepted warps land
+// in warp8 [S][8] with the pending flag set.  Returns the number of launches.
+int sof_state_enqueue(SofState* st, const uint8_t* images, size_t image_stride, int rows, int cols, const float* dets,
+                      const int* ndets, int det_cap, int det_stride, int conf_col, float conf_thr, double* warp8,
+                      cudaStream_t cs);
+// standalone handle (boxmot_b200_cmc_sof_*)
+void* sof_create(double scale, int min_inliers, double min_ratio, double ransac_thresh);
+void sof_apply(void* handle, const uint8_t* bgr, int rows, int cols, const float* dets_xyxy, int n_dets, float* warp6,
+               int* status);
+void sof_destroy(void* handle);
 
 void standalone_jv(const double* cost, int R, int C, int* x, int* y);
 void set_jv_wide(int mode);   // dense-JV augmentation variant used by every later launch of this process

@@ -514,6 +514,7 @@ void Engine::release() {
     }
     if (reid) reid_free(reid);
     cudaFree(d_cmc_prev); cudaFree(d_cmc_cur); cudaFree(d_cmc_has_prev); cudaFree(d_cmc_gate);
+    if (sof) sof_state_free(sof);
     cudaFree(d_warp); cudaFree(d_mem); cudaFree(d_dets); cudaFree(d_ndets); cudaFree(d_embs); cudaFree(d_out);
     cudaFree(d_scalars_out); cudaFree(d_streams); cudaFree(d_docs); cudaFree(d_ss); cudaFree(d_crops); cudaFree(d_ncrops); cudaFree(d_images);
     cudaFreeHost(h_dets); cudaFreeHost(h_ndets); cudaFreeHost(h_out); cudaFreeHost(h_scalars);
@@ -528,6 +529,7 @@ void Engine::release() {
 void Engine::reset() {
     if (reid_stream) CUDA_OK(cudaStreamSynchronize(reid_stream));
     if (d_cmc_has_prev) CUDA_OK(cudaMemsetAsync(d_cmc_has_prev, 0, sizeof(int) * S, stream));   // ECC.prev_img = None
+    if (sof) sof_state_reset(sof, stream);   // a fresh SOF: the next frame initialises
     if (is_docs || is_ss) {
         CUDA_OK(cudaStreamSynchronize(stream));
         for (int i = 0; i < S; ++i) CUDA_OK(cudaMemsetAsync(d_mem + stream_bytes * i, 0, persistent_bytes, stream));
@@ -749,9 +751,19 @@ void Engine::enqueue_association(TrkStream* streams_dev, const float* embs_src) 
 void Engine::set_cmc(const char* method) {
     const bool off = !method || !method[0] || strcmp(method, "none") == 0 || strcmp(method, "None") == 0;
     if (off) { cmc_mode = 0; return; }
+    if (strcmp(method, "sof") == 0) {
+        // botsort.py:142,301 (every frame, every detection row) and deepocsort.py:330-349 (every frame, the rows with
+        // conf > det_thresh); StrongSORT's estimator is ECC
+        if (is_ss || (!is_docs && cfg.kind != KIND_XYWH))
+            throw std::runtime_error("on-device SOF applies to BoT-SORT and DeepOCSORT (StrongSORT's estimator is ecc)");
+        if (!sof) sof = sof_state_create(S, 0.15, 8, 0.2, 3.0);
+        else if (cmc_mode != 2) sof_state_reset(sof, stream);
+        cmc_mode = 2;
+        return;
+    }
     if (strcmp(method, "ecc") != 0)
-        throw std::runtime_error(std::string("camera-motion method '") + method + "' is not built on the device (ecc, none); "
-                                 "sof / orb / sift warps can be supplied through set_warp");
+        throw std::runtime_error(std::string("camera-motion method '") + method + "' is not built on the device (ecc, sof, "
+                                 "none); orb / sift warps can be supplied through set_warp");
     if ((!is_ss && !is_docs && cfg.kind != KIND_XYWH) || is_docs)
         throw std::runtime_error("on-device ECC applies to BoT-SORT and StrongSORT (ByteTrack has no CMC, DeepOCSORT's is sof)");
     if (is_ss && !d_cmc_gate) {   // StrongSORT estimates only while tracks exist
@@ -768,6 +780,12 @@ void Engine::enqueue_cmc(const uint8_t* images_dev, int rows, int cols) {
     int h, w;
     cmc_scaled_size(rows, cols, cmc_scale, &h, &w);
     if (h < 3 || w < 3) throw std::runtime_error("camera-motion estimation: frame too small for the registration scale");
+    if (cmc_mode == 2) {
+        launches += sof_state_enqueue(sof, images_dev, (size_t)rows * cols * 3, rows, cols, d_dets, d_ndets, (int)cfg.cap_dets,
+                                      6, is_docs ? 4 : -1, is_docs ? dcfg.det_thresh_f32 : 0.f, d_warp, stream);
+        warp_dirty = true;   // the estimate applies to this frame only
+        return;
+    }
     if (h != cmc_h || w != cmc_w) {
         CUDA_OK(cudaStreamSynchronize(stream));
         cudaFree(d_cmc_prev); cudaFree(d_cmc_cur); d_cmc_prev = d_cmc_cur = nullptr;

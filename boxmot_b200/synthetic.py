@@ -299,3 +299,70 @@ def camera_pan_sequence(n_frames: int = 16, hw=(360, 640), n_objects: int = 24, 
             e = np.maximum(protos[vis] + 0.3 * rng.normal(size=(int(vis.sum()), dim)).astype(np.float32), 0.0)
             embs.append((e / np.linalg.norm(e, axis=1, keepdims=True)).astype(np.float32))
     return frames, dets, np.asarray(offs), (embs if dim else None)
+
+
+def camera_similarity_sequence(n_frames: int = 12, hw=(360, 640), n_objects: int = 24, seed: int = 5,
+                               max_step: float = 4.0, max_rot_deg: float = 1.0, max_zoom: float = 0.01):
+    """Moving-camera input for the partial-affine (similarity) estimators: a smooth textured canvas, like
+    `camera_pan_sequence`'s, seen through a window that per frame pans by up to `max_step` pixels (sub-pixel), rotates by
+    up to `max_rot_deg` degrees and zooms by up to `max_zoom`, sampled bilinearly, plus sensor noise.  Detections are
+    the boxes of objects that stand still on the canvas, carried into the image by the window's similarity.  Pure numpy,
+    seeded.  Returns (frames [H,W,3] uint8 BGR, dets (n,6) float32 per frame, windows (n_frames, 4) float64 =
+    (centre x, centre y, angle rad, zoom) of each frame's window on the canvas)."""
+    h, w = hw
+    rng = np.random.default_rng(seed)
+    margin = int(max_step * n_frames + 0.05 * max(h, w) * (1 + max_rot_deg * n_frames / 10.0)) + 16
+    H, W = h + 2 * margin, w + 2 * margin
+    yy, xx = np.mgrid[0:H, 0:W].astype(np.float32)
+    canvas = np.zeros((H, W, 3), np.float32)
+
+    def smooth_field(cell):
+        gh, gw = H // cell + 3, W // cell + 3
+        g = rng.random((gh, gw)).astype(np.float32)
+        fy, fx = yy / cell, xx / cell
+        y0, x0 = fy.astype(np.int64), fx.astype(np.int64)
+        ay, ax = fy - y0, fx - x0
+        return (g[y0, x0] * (1 - ay) * (1 - ax) + g[y0, x0 + 1] * (1 - ay) * ax
+                + g[y0 + 1, x0] * ay * (1 - ax) + g[y0 + 1, x0 + 1] * ay * ax)
+
+    for c in range(3):
+        canvas[..., c] = smooth_field(56) + 0.5 * smooth_field(28) + 0.08 * rng.random((H, W)).astype(np.float32)
+    canvas -= canvas.min()
+    canvas = canvas / canvas.max() * 215.0 + 20.0
+    cx = rng.uniform(margin + 40, margin + w - 40, n_objects)
+    cy = rng.uniform(margin + 40, margin + h - 40, n_objects)
+    bw = rng.uniform(18, 46, n_objects)
+    bh = rng.uniform(36, 90, n_objects)
+    px, py, ang, zoom = W / 2.0, H / 2.0, 0.0, 1.0
+    gy, gx = np.mgrid[0:h, 0:w].astype(np.float64)
+    gx -= (w - 1) / 2.0
+    gy -= (h - 1) / 2.0
+    frames, dets, wins = [], [], []
+    for f in range(n_frames):
+        if f:
+            px += rng.uniform(-max_step, max_step)
+            py += rng.uniform(-max_step, max_step)
+            ang += np.deg2rad(rng.uniform(-max_rot_deg, max_rot_deg))
+            zoom *= 1.0 + rng.uniform(-max_zoom, max_zoom)
+        wins.append((px, py, ang, zoom))
+        ca, sa = np.cos(ang) / zoom, np.sin(ang) / zoom   # image pixel -> canvas point
+        sx = px + ca * gx - sa * gy
+        sy = py + sa * gx + ca * gy
+        x0 = np.clip(np.floor(sx).astype(np.int64), 0, W - 2)
+        y0 = np.clip(np.floor(sy).astype(np.int64), 0, H - 2)
+        ax = (sx - x0)[..., None]
+        ay = (sy - y0)[..., None]
+        win = (canvas[y0, x0] * (1 - ay) * (1 - ax) + canvas[y0, x0 + 1] * (1 - ay) * ax
+               + canvas[y0 + 1, x0] * ay * (1 - ax) + canvas[y0 + 1, x0 + 1] * ay * ax)
+        win = win + rng.normal(0.0, 1.5, (h, w, 3))
+        frames.append(np.clip(np.rint(win), 0, 255).astype(np.uint8))
+        # canvas point -> image pixel (inverse similarity) for the object centres
+        dx, dy = cx - px, cy - py
+        ix = (np.cos(ang) * dx + np.sin(ang) * dy) * zoom + (w - 1) / 2.0
+        iy = (-np.sin(ang) * dx + np.cos(ang) * dy) * zoom + (h - 1) / 2.0
+        x1, y1 = ix - bw * zoom / 2, iy - bh * zoom / 2
+        d = np.stack([x1, y1, x1 + bw * zoom, y1 + bh * zoom, rng.uniform(0.55, 0.95, n_objects),
+                      np.zeros(n_objects)], 1)
+        vis = (rng.random(n_objects) > 0.1) & (d[:, 0] > 0) & (d[:, 1] > 0) & (d[:, 2] < w) & (d[:, 3] < h)
+        dets.append(d[vis].astype(np.float32))
+    return frames, dets, np.asarray(wins)

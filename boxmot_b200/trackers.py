@@ -289,10 +289,12 @@ class MultiStreamTracker:
         self.cmc = None
 
     def set_cmc(self, method: Optional[str]) -> None:
-        """Camera-motion ESTIMATION on the device from the frames passed to `update` (BoT-SORT, StrongSORT): "ecc" = the
+        """Camera-motion ESTIMATION on the device from the frames passed to `update`: "ecc" (BoT-SORT, StrongSORT) = the
         reference's ECC estimator with its defaults (motion/cmc/ecc.py:23-108: translation model, eps 1e-5, 100 iterations,
-        gray image at scale 0.15), run where the reference runs it (botsort.py:142, strongsort.py:83-86); None / "none"
-        turns it off (warps are then supplied through `set_warp`)."""
+        gray image at scale 0.15), run where the reference runs it (botsort.py:142, strongsort.py:83-86); "sof" (BoT-SORT,
+        DeepOCSORT) = the reference's SOF estimator with its defaults (motion/cmc/sof.py; `boxmot_b200.SOF`), run on every
+        frame with the detection boxes the reference masks (BoT-SORT: every row, DeepOCSORT: conf > det_thresh); None /
+        "none" turns it off (warps are then supplied through `set_warp`).  `reset()` restarts the estimator."""
         m = None if method in (None, "", "none", "None") else str(method)
         if not self.lib.boxmot_b200_tracker_set_cmc(self.handle, m.encode() if m else None):
             raise B200Error(_lib.last_error(self.lib))
@@ -507,6 +509,11 @@ class _SingleStreamTracker:
         self._engine.reset()
         self.frame_count = 0
 
+    def set_cmc(self, method: Optional[str]) -> None:
+        """Turn on-device camera-motion estimation on or off after construction (`MultiStreamTracker.set_cmc`):
+        "sof" for BoT-SORT and DeepOCSORT, "ecc" for BoT-SORT and StrongSORT, None to turn it off."""
+        self._engine.set_cmc(method)
+
     def update(self, dets, img=None, embs=None, masks=None, warp=None) -> TrackResults:
         """`warp`: optional 2x3 camera-motion matrix for this frame (BoT-SORT, DeepOCSORT, StrongSORT); the reference
         estimates it with OpenCV inside update() (botsort.py:142-144, deepocsort.py:345-348, strongsort.py:83-86), here the
@@ -589,9 +596,9 @@ class BotSort(_SingleStreamTracker):
     """BoT-SORT on the GPU; arguments as boxmot/trackers/bbox/botsort/botsort.py:66-118.
 
     `use_cmc=True` with `cmc_method="ecc"` (the reference constructor's method) estimates the camera warp on the device
-    every frame from `img` (SURVEY 8f-3, `MultiStreamTracker.set_cmc`); the other estimators (sof, orb, sift) are OpenCV
-    feature pipelines outside this path: pass `use_cmc=False` and, if you have their warp, `update(..., warp=)`.
-    `use_cmc` defaults to False here (the reference: True)."""
+    every frame from `img` (SURVEY 8f-3, `MultiStreamTracker.set_cmc`).  SOF (botsort.yaml's method) also runs on the
+    device: build with `use_cmc=False` and call `set_cmc("sof")`.  ORB and SIFT are outside this path: pass their warp
+    through `update(..., warp=)`.  `use_cmc` defaults to False here (the reference: True)."""
 
     _kind = "botsort"
 
@@ -619,10 +626,11 @@ class BotSort(_SingleStreamTracker):
 
 
 class DeepOcSort(_SingleStreamTracker):
-    """DeepOCSORT on the GPU; arguments as boxmot/trackers/bbox/deepocsort/deepocsort.py:263-300.  `cmc_off` must be
-    True: camera-motion ESTIMATION is outside this hot path (SURVEY N6); a warp obtained elsewhere is applied exactly
-    as the reference applies its own (`apply_affine_correction` on every track before the predict step) when passed
-    as `update(dets, img, embs, warp=warp_2x3)`."""
+    """DeepOCSORT on the GPU; arguments as boxmot/trackers/bbox/deepocsort/deepocsort.py:263-300.  `cmc_off=False` runs
+    the reference's SOF estimator on the device on every frame, from `img` and the detections with conf > det_thresh
+    (deepocsort.py:330-349).  With the default `cmc_off=True` (the reference: False) a warp obtained elsewhere is
+    applied exactly as the reference applies its own (`apply_affine_correction` on every track before the predict
+    step) when passed as `update(dets, img, embs, warp=warp_2x3)`."""
 
     _kind = "deepocsort"
 
@@ -631,13 +639,13 @@ class DeepOcSort(_SingleStreamTracker):
                  cmc_off: bool = True, aw_off: bool = False, Q_xy_scaling: float = 0.01, Q_s_scaling: float = 0.0001,
                  det_thresh: float = 0.3, max_age: int = 30, min_hits: int = 3, iou_threshold: float = 0.3,
                  **kwargs: Any):
-        if not cmc_off:
-            raise NotImplementedError("cmc_off=False: camera-motion compensation is out of scope (pass cmc_off=True)")
         super().__init__(reid_model=None if embedding_off else reid_model, delta_t=delta_t, inertia=inertia,
                          w_association_emb=w_association_emb, alpha_fixed_emb=alpha_fixed_emb, aw_param=aw_param,
                          embedding_off=embedding_off, aw_off=aw_off, Q_xy_scaling=Q_xy_scaling,
                          Q_s_scaling=Q_s_scaling, det_thresh=det_thresh, max_age=max_age, min_hits=min_hits,
                          iou_threshold=iou_threshold, **kwargs)
+        if not cmc_off:
+            self._engine.set_cmc("sof")
 
 
 class OcSort(_SingleStreamTracker):
@@ -742,8 +750,9 @@ def resolve_tracker_args(tracker_type, tracker_config=None, evolve_param_dict=No
 
         _CMC_WARNED[kind] = True
         warnings.warn(f"boxmot_b200.create_tracker('{kind}'): the reference configuration runs camera-motion compensation "
-                      f"({method if kind == 'botsort' else 'sof'}); only 'ecc' is estimated on the device -- this tracker applies "
-                      "a warp supplied through update(..., warp=), without one it behaves as with CMC off", stacklevel=3)
+                      f"({method if kind == 'botsort' else 'sof'}); this tracker is built with it off and applies a warp supplied "
+                      "through update(..., warp=), without one it behaves as with CMC off -- call tracker.set_cmc('sof') "
+                      "(BoT-SORT, DeepOCSORT) to estimate SOF on the device like the reference", stacklevel=3)
     args.pop("cmc_method", None)
     if kind == "botsort":
         args["use_cmc"] = bot_ecc

@@ -218,8 +218,11 @@ BOXMOT_B200_API int boxmot_b200_tracker_set_warp(BoxMOTB200Tracker* handle, int 
  * the reference's ECC estimator with its defaults -- cv2.findTransformECC translation model, eps 1e-5, 100 iterations,
  * gray registration image at scale 0.15 (boxmot/motion/cmc/ecc.py:23-108, base_cmc.py:29-60) -- as StrongSORT runs it on
  * every frame that starts with tracks (trackers/bbox/strongsort/strongsort.py:67,83-86) and BoT-SORT with
- * cmc_method="ecc" (trackers/bbox/botsort/botsort.py:78,116-117,142).  "none" / "" / NULL turns it off again.  The
- * estimate replaces a warp supplied for the same frame.  BoT-SORT and StrongSORT handles only. */
+ * cmc_method="ecc" (trackers/bbox/botsort/botsort.py:78,116-117,142) -- BoT-SORT and StrongSORT handles.  Method "sof"
+ * is the reference's SOF estimator with its defaults (boxmot/motion/cmc/sof.py; as boxmot_b200_cmc_sof_*) on every
+ * frame, with the detection boxes the reference masks: every row for BoT-SORT (botsort.py:301), the rows with
+ * conf > det_thresh for DeepOCSORT (deepocsort.py:330-349) -- BoT-SORT and DeepOCSORT handles.  "none" / "" / NULL
+ * turns it off again.  The estimate replaces a warp supplied for the same frame; reset restarts the estimator. */
 BOXMOT_B200_API int boxmot_b200_tracker_set_cmc(BoxMOTB200Tracker* handle, const char* method);
 /* Device timing on the handle's own CUDA stream: record mark 0 / mark 1 around a region, then read the elapsed
  * milliseconds (synchronises on mark 1). */
@@ -249,6 +252,19 @@ BOXMOT_B200_API int boxmot_b200_jv_dense(const double* cost, int rows, int cols,
  * image of `cur` (BaseCMC.preprocess). */
 BOXMOT_B200_API int boxmot_b200_cmc_ecc(const uint8_t* prev_bgr, const uint8_t* cur_bgr, int rows, int cols, double scale,
                                         double eps, int max_iter, float* warp2x3, int* status, uint8_t* prepared);
+/* Standalone SOF estimator: the reference's SOF(scale, min_inliers, min_inlier_ratio, ransac_reproj_threshold) camera-
+ * motion estimator (boxmot/motion/cmc/sof.py: corners, cornerSubPix on the initialising frame, pyramidal LK, RANSAC
+ * partial affine) running on the device.  One handle is one video: it keeps the previous pyramid and keypoints.
+ * apply() takes a BGR frame (rows x cols x 3 uint8, host) and the frame's detection boxes (n_dets x 4 float32 xyxy in
+ * frame pixels, host; NULL when n_dets is 0, cleared from the corner mask) and writes the float32 2x3 warp SOF.apply
+ * returns (row major).  status: 0 = initialising frame (identity), 1 = estimated, 2 = rejected (identity: too few
+ * tracks or inliers).  A new frame size starts the estimator afresh. */
+typedef struct BoxMOTB200CmcSof BoxMOTB200CmcSof;
+BOXMOT_B200_API BoxMOTB200CmcSof* boxmot_b200_cmc_sof_create(double scale, int min_inliers, double min_inlier_ratio,
+                                                             double ransac_reproj_threshold);
+BOXMOT_B200_API int boxmot_b200_cmc_sof_apply(BoxMOTB200CmcSof* handle, const uint8_t* bgr, int rows, int cols,
+                                              const float* dets_xyxy, int n_dets, float* warp2x3, int* status);
+BOXMOT_B200_API void boxmot_b200_cmc_sof_destroy(BoxMOTB200CmcSof* handle);
 /* Augmentation variant of the dense solver for this process: 3 = column-owned CTA-wide search with the exact shortcuts
  * (no-op band columns, parallel _find_dense tail, hit list, CTA-wide row reduction; the default), 2 = column-owned
  * (distances in registers), 1 = CTA-wide search over list positions, 0 = one-warp search; values >= 4 are
