@@ -17,7 +17,8 @@
 //                tile: TMA box of conv1's output -> [wgmma 1x1 -> T (smem, fp32) -> depthwise on CUDA cores -> split
 //                planes in place] x depth -> branch output planes + channel sums for the gate.
 //   k_gemm_tc    warp-specialised pointwise GEMM (TMA producer warp / two consumer warpgroups, 64 pixels each) over
-//                128-pixel tiles: A = up to two plane tensors streamed through an mbarrier ring, B resident in shared
+//                128-pixel tiles, one instance per output width and epilogue mode: A = up to two plane tensors streamed
+//                through an mbarrier ring (MMAs pipelined one k-step deep), B resident in shared
 //                memory (optionally  gate (x) conv3  folded per crop), epilogue bias + ReLU -> planes, optional 2x2
 //                average pool, optional float32 NHWC copy, optional second GEMM on the fresh tile (next block's conv1).
 #pragma once
@@ -565,15 +566,31 @@ inline GemmSmem gemm_smem_layout(int K8, int NP, int NP2, int n_stage, bool tail
     return s;
 }
 
-__global__ void __launch_bounds__(GEMM_THREADS, 1) k_gemm_tc(const __grid_constant__ GemmTcArgs a, const int* __restrict__ d_n, int off, int cap,
-                                                            const GemmSmem L, const GemmHeadIO hio) {
+// Epilogue modes of k_gemm_tc (compile time, with the output widths NP and NP2): bias (+ ReLU) -> planes / float32 NHWC;
+// the same with a 2x2 average pool; a second GEMM on the fresh tile (tail) -> planes; the tail with its output pooled
+// (a transition fused behind a block); conv5 + the fused head.
+enum GemmMode { GM_PLAIN, GM_POOL, GM_TAIL, GM_TAIL_POOL2, GM_HEAD };
+
+// CTAs per SM an instance is compiled for: two (<= 112 registers per thread) where the B operand and a >= 2-deep ring of
+// the plan's launches fit half of the SM's shared memory.  One for the combine GEMMs of stages 3 and 4 (B alone is
+// 72-128 KB) and for conv5 + head (at 112 registers it spills).  The plan asks the occupancy calculator either way.
+template <int NP, int NP2, int MODE>
+constexpr int gemm_min_ctas() {
+    return NP == 128 || ((MODE == GM_TAIL || MODE == GM_TAIL_POOL2) && NP >= 96) ? 1 : 2;
+}
+
+template <int NP, int NP2, int MODE>
+__global__ void __launch_bounds__(GEMM_THREADS, (gemm_min_ctas<NP, NP2, MODE>()))
+    k_gemm_tc(const __grid_constant__ GemmTcArgs a, const int* __restrict__ d_n, int off, int cap, const GemmSmem L, const GemmHeadIO hio) {
+    constexpr bool tail = MODE == GM_TAIL || MODE == GM_TAIL_POOL2, pool = MODE == GM_POOL, pool2 = MODE == GM_TAIL_POOL2;
+    static_assert(NP % 16 == 0 && NP >= 16 && NP <= 128, "NP: 16 .. 128 output channels");
+    static_assert(tail ? (NP2 % 16 == 0 && NP2 >= 16 && NP2 <= 128) : NP2 == 0, "NP2: the tail's output channels");
+    constexpr int NACC = (NP2 > NP ? NP2 : NP) / 2;              // accumulator registers per thread (m64nN: N / 2)
     const int n = blockIdx.y;
     if (n >= tc_chunk_count(d_n, off, cap)) return;
     extern __shared__ __align__(128) unsigned char smem[];
     __shared__ __align__(8) uint64_t bar_full[4], bar_empty[4], bar_w;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int NP = a.NP, NP2 = a.NP2;
-    const bool tail = a.b2_packed != nullptr;
     const int tile0 = blockIdx.x * a.tiles_per_cta;
     const int tile1 = min(tile0 + a.tiles_per_cta, a.tiles_per_crop);
     unsigned char* sB = smem + L.b;
@@ -625,33 +642,42 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) k_gemm_tc(const __grid_consta
     const int cq = 2 * (lane & 3);                              // first of the two columns of an 8-column group
     const uint32_t lbo_b = 2u * NP * 16u, lo_off = (uint32_t)NP * 16u;   // a K plane of B = NP rows W_hi, then NP rows W_lo
     um::mbar_wait(&bar_w, 0);
-    float acc[64];
+    float acc[NACC];
     uint32_t it = 0;
     for (int tile = tile0; tile < tile1; ++tile) {
         uint32_t kplane = 0, first = 1;
+        uint32_t held = 0;                                      // slot of the previous chunk, whose MMAs may still run
+        // one commit group per k-step (two planes, three MMAs): the next k-step is issued before the previous one has
+        // drained, and a ring slot goes back to the producer once the last group that reads it has completed.  Every
+        // group accumulates into the same registers in issue order, which wgmma orders by itself; nothing else touches
+        // acc until the final wait.  (The MMAs sit unconditionally in the loop body: a conditional wgmma with groups in
+        // flight makes ptxas serialise them.)
         for (int s = 0; s < a.n_src; ++s) {
             const int kc = a.src_kc[s];
             for (int p0 = 0; p0 < a.src_planes[s]; p0 += kc, ++it) {
                 const uint32_t slot = it % (uint32_t)a.n_stage, ph = (it / (uint32_t)a.n_stage) & 1u;
                 um::mbar_wait(&bar_full[slot], ph);
                 const uint32_t ah = um::smem_u32(sRing + (size_t)slot * a.slot_bytes) + (uint32_t)wg * 1024u, al = ah + a.slot_bytes / 2;
-                um::wg_fence();
                 for (int ks = 0; ks < kc / 2; ++ks) {
                     const uint32_t bb = um::smem_u32(sB) + (kplane + 2 * ks) * lbo_b;
                     const uint64_t xh = um::make_desc(ah + ks * 2 * 2048u, 2048u, 128), xl = um::make_desc(al + ks * 2 * 2048u, 2048u, 128);
-                    um::mma_rt<false>(NP, acc, xh, bb, lbo_b, 128, first ? 0u : 1u);      // A_hi W_hi
-                    um::mma_rt<false>(NP, acc, xl, bb, lbo_b, 128, 1u);                   // A_lo W_hi
-                    um::mma_rt<false>(NP, acc, xh, bb + lo_off, lbo_b, 128, 1u);          // A_hi W_lo
+                    um::wg_fence();
+                    um::mma<NP, false>(acc, xh, bb, lbo_b, 128, first ? 0u : 1u);      // A_hi W_hi
+                    um::mma<NP, false>(acc, xl, bb, lbo_b, 128, 1u);                   // A_lo W_hi
+                    um::mma<NP, false>(acc, xh, bb + lo_off, lbo_b, 128, 1u);          // A_hi W_lo
                     first = 0;
+                    um::wg_commit();
+                    um::wg_wait<1>();                           // the previous k-step's group has completed
+                    if (ks == 0 && kplane > 0 && (et & 127) == 0) mbar_arrive(&bar_empty[held]);   // so has the previous chunk
                 }
-                um::wg_commit();
-                um::wg_wait_all();
-                um::wg_fence_acc<64>(acc);
-                if ((et & 127) == 0) mbar_arrive(&bar_empty[slot]);     // this warpgroup is done with the slot
+                held = slot;
                 kplane += kc;
             }
         }
-        if (a.head_w) {
+        um::wg_wait<0>();
+        um::wg_fence_acc<NACC>(acc);
+        if ((et & 127) == 0) mbar_arrive(&bar_empty[held]);
+        if constexpr (MODE == GM_HEAD) {
             // ---- conv5 + head: the tile is the whole 16 x 8 map.  Column sums over the 128 pixels: the two rows of a
             // thread, a butterfly over the 8 row groups of a warp, the 8 warps through shared memory (the ring, once
             // both warpgroups' MMAs have read their last slot; the producer has no further chunk to load) ----
@@ -661,19 +687,17 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) k_gemm_tc(const __grid_consta
             float* red = pooled + NP;                               // [8]
             float* feat = red + 8;                                  // [head_feat]
 #pragma unroll
-            for (int i = 0; i < 16; ++i) {
+            for (int i = 0; i < NP / 8; ++i) {
                 const int c = 8 * i + cq;
-                if (c < NP) {
-                    const float2 b = *reinterpret_cast<const float2*>(a.bias + c);
-                    float o0 = fmaxf(acc[4 * i] + b.x, 0.f) + fmaxf(acc[4 * i + 2] + b.x, 0.f);
-                    float o1 = fmaxf(acc[4 * i + 1] + b.y, 0.f) + fmaxf(acc[4 * i + 3] + b.y, 0.f);
+                const float2 b = *reinterpret_cast<const float2*>(a.bias + c);
+                float o0 = fmaxf(acc[4 * i] + b.x, 0.f) + fmaxf(acc[4 * i + 2] + b.x, 0.f);
+                float o1 = fmaxf(acc[4 * i + 1] + b.y, 0.f) + fmaxf(acc[4 * i + 3] + b.y, 0.f);
 #pragma unroll
-                    for (int sh = 4; sh < 32; sh <<= 1) {
-                        o0 += __shfl_xor_sync(0xffffffffu, o0, sh);
-                        o1 += __shfl_xor_sync(0xffffffffu, o1, sh);
-                    }
-                    if (lane < 4) *reinterpret_cast<float2*>(part + warp * NP + c) = make_float2(o0, o1);
+                for (int sh = 4; sh < 32; sh <<= 1) {
+                    o0 += __shfl_xor_sync(0xffffffffu, o0, sh);
+                    o1 += __shfl_xor_sync(0xffffffffu, o1, sh);
                 }
+                if (lane < 4) *reinterpret_cast<float2*>(part + warp * NP + c) = make_float2(o0, o1);
             }
             um::bar_sync(1, 256);
             for (int c = et; c < NP; c += 256)
@@ -705,13 +729,11 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) k_gemm_tc(const __grid_consta
             float* dst = hio.out + (size_t)hio.crops[off + n].out_row * hio.out_ld;
             for (int f = et; f < FEAT; f += 256) dst[f] = feat[f] / nrm;
             um::bar_sync(1, 256);                                  // part / pooled are rewritten by the next tile
-            continue;
-        }
-        // ---- epilogue: bias (+ ReLU) on the thread's two rows x (2 columns per 8-column group) ----
+        } else {
+            // ---- epilogue: bias (+ ReLU) on the thread's two rows x (2 columns per 8-column group) ----
 #pragma unroll
-        for (int i = 0; i < 16; ++i) {
-            const int c = 8 * i + cq;
-            if (c < NP) {
+            for (int i = 0; i < NP / 8; ++i) {
+                const int c = 8 * i + cq;
                 const float2 b = *reinterpret_cast<const float2*>(a.bias + c);
 #pragma unroll
                 for (int h = 0; h < 2; ++h) {
@@ -723,7 +745,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) k_gemm_tc(const __grid_consta
                         if (c + 1 < a.N) *reinterpret_cast<float2*>(dst) = make_float2(o0, o1);
                         else if (c < a.N) dst[0] = o0;
                     }
-                    if (a.pool) {
+                    if constexpr (pool) {
                         *reinterpret_cast<float2*>(sF + (size_t)m * (NP + 4) + c) = make_float2(o0, o1);
                     } else if (a.out_hi || tail) {
                         uint32_t hv, lv;
@@ -733,72 +755,70 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) k_gemm_tc(const __grid_consta
                             reinterpret_cast<uint32_t*>(a.out_hi)[e] = hv;
                             reinterpret_cast<uint32_t*>(a.out_lo)[e] = lv;
                         }
-                        if (tail) {
+                        if constexpr (tail) {
                             *reinterpret_cast<uint32_t*>(sA2 + ((size_t)i * 128 + m) * 16 + (lane & 3) * 4) = hv;
                             *reinterpret_cast<uint32_t*>(sA2 + ((size_t)(NP / 8 + i) * 128 + m) * 16 + (lane & 3) * 4) = lv;
                         }
                     }
                 }
             }
-        }
-        // 2x2 average pool of the tile in sF (rows_per_tile x W, row stride NPx + 4) -> (rows/2 x W/2) planes;
-        // (a + b + c + d) * 0.25, a=(y,x) b=(y,x+1) c=(y+1,x) d=(y+1,x+1)
-        auto pool_store = [&](const int NPx, bf16* o_hi, bf16* o_lo) {
-            um::bar_sync(1, 256);
-            const int Wt = a.W, OW = Wt / 2, OHt = a.rows_per_tile / 2;
-            const int items = OHt * OW * (NPx / 8);
-            const int OHW = a.HW / 4;
-            for (int e = et; e < items; e += 256) {
-                const int pp = e % (OHt * OW), c8 = e / (OHt * OW);
-                const int oy = pp / OW, ox = pp - oy * OW;
-                const float* f0 = sF + (size_t)((2 * oy) * Wt + 2 * ox) * (NPx + 4) + c8 * 8;
-                const float* f1 = f0 + (NPx + 4);
-                const float* f2 = f0 + (size_t)Wt * (NPx + 4);
-                const float* f3 = f2 + (NPx + 4);
-                uint32_t h[4], l[4];
+            // 2x2 average pool of the tile in sF (rows_per_tile x W, row stride NPx + 4) -> (rows/2 x W/2) planes;
+            // (a + b + c + d) * 0.25, a=(y,x) b=(y,x+1) c=(y+1,x) d=(y+1,x+1)
+            auto pool_store = [&](const int NPx, bf16* o_hi, bf16* o_lo) {
+                um::bar_sync(1, 256);
+                const int Wt = a.W, OW = Wt / 2, OHt = a.rows_per_tile / 2;
+                const int items = OHt * OW * (NPx / 8);
+                const int OHW = a.HW / 4;
+                for (int e = et; e < items; e += 256) {
+                    const int pp = e % (OHt * OW), c8 = e / (OHt * OW);
+                    const int oy = pp / OW, ox = pp - oy * OW;
+                    const float* f0 = sF + (size_t)((2 * oy) * Wt + 2 * ox) * (NPx + 4) + c8 * 8;
+                    const float* f1 = f0 + (NPx + 4);
+                    const float* f2 = f0 + (size_t)Wt * (NPx + 4);
+                    const float* f3 = f2 + (NPx + 4);
+                    uint32_t h[4], l[4];
 #pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                    const float x0 = (f0[2 * j] + f1[2 * j] + f2[2 * j] + f3[2 * j]) * 0.25f;
-                    const float x1 = (f0[2 * j + 1] + f1[2 * j + 1] + f2[2 * j + 1] + f3[2 * j + 1]) * 0.25f;
-                    um::split2(x0, x1, h[j], l[j]);
+                    for (int j = 0; j < 4; ++j) {
+                        const float x0 = (f0[2 * j] + f1[2 * j] + f2[2 * j] + f3[2 * j]) * 0.25f;
+                        const float x1 = (f0[2 * j + 1] + f1[2 * j + 1] + f2[2 * j + 1] + f3[2 * j + 1]) * 0.25f;
+                        um::split2(x0, x1, h[j], l[j]);
+                    }
+                    const int opx = (tile * OHt + oy) * OW + ox;
+                    const size_t o = ((size_t)n * (NPx / 8) + c8) * OHW + opx;
+                    reinterpret_cast<uint4*>(o_hi)[o] = make_uint4(h[0], h[1], h[2], h[3]);
+                    reinterpret_cast<uint4*>(o_lo)[o] = make_uint4(l[0], l[1], l[2], l[3]);
                 }
-                const int opx = (tile * OHt + oy) * OW + ox;
-                const size_t o = ((size_t)n * (NPx / 8) + c8) * OHW + opx;
-                reinterpret_cast<uint4*>(o_hi)[o] = make_uint4(h[0], h[1], h[2], h[3]);
-                reinterpret_cast<uint4*>(o_lo)[o] = make_uint4(l[0], l[1], l[2], l[3]);
-            }
-            um::bar_sync(1, 256);   // sF is rewritten by the next tile
-        };
-        if (a.pool) pool_store(NP, a.out_hi, a.out_lo);
-        if (tail) {
-            // the fresh tile (hi | lo planes in sA2) is the A operand of the second GEMM: a warpgroup's MMAs read only the
-            // 64 rows it wrote itself
-            um::fence_async_smem();
-            um::bar_sync(2 + wg, 128);
-            const uint32_t lbo_b2 = 2u * NP2 * 16u, lo2 = (uint32_t)NP2 * 16u;
-            const uint32_t ah = um::smem_u32(sA2) + (uint32_t)wg * 1024u, al = ah + (uint32_t)(NP / 8) * 2048u;
-            um::wg_fence();
-            for (int ks = 0; ks < NP / 16; ++ks) {
-                const uint32_t bb = um::smem_u32(sB2) + ks * 2 * lbo_b2;
-                const uint64_t xh = um::make_desc(ah + ks * 2 * 2048u, 2048u, 128), xl = um::make_desc(al + ks * 2 * 2048u, 2048u, 128);
-                um::mma_rt<false>(NP2, acc, xh, bb, lbo_b2, 128, ks > 0);
-                um::mma_rt<false>(NP2, acc, xl, bb, lbo_b2, 128, 1u);
-                um::mma_rt<false>(NP2, acc, xh, bb + lo2, lbo_b2, 128, 1u);
-            }
-            um::wg_commit();
-            um::wg_wait_all();
-            um::wg_fence_acc<64>(acc);
-            if (a.pool2) um::bar_sync(1, 256);                     // sF aliases sA2: both warpgroups' MMAs have read it
+                um::bar_sync(1, 256);   // sF is rewritten by the next tile
+            };
+            if constexpr (pool) pool_store(NP, a.out_hi, a.out_lo);
+            if constexpr (tail) {
+                // the fresh tile (hi | lo planes in sA2) is the A operand of the second GEMM: a warpgroup's MMAs read only the
+                // 64 rows it wrote itself
+                um::fence_async_smem();
+                um::bar_sync(2 + wg, 128);
+                const uint32_t lbo_b2 = 2u * NP2 * 16u, lo2 = (uint32_t)NP2 * 16u;
+                const uint32_t ah = um::smem_u32(sA2) + (uint32_t)wg * 1024u, al = ah + (uint32_t)(NP / 8) * 2048u;
+                um::wg_fence();
+                for (int ks = 0; ks < NP / 16; ++ks) {
+                    const uint32_t bb = um::smem_u32(sB2) + ks * 2 * lbo_b2;
+                    const uint64_t xh = um::make_desc(ah + ks * 2 * 2048u, 2048u, 128), xl = um::make_desc(al + ks * 2 * 2048u, 2048u, 128);
+                    um::mma<NP2, false>(acc, xh, bb, lbo_b2, 128, ks > 0);
+                    um::mma<NP2, false>(acc, xl, bb, lbo_b2, 128, 1u);
+                    um::mma<NP2, false>(acc, xh, bb + lo2, lbo_b2, 128, 1u);
+                }
+                um::wg_commit();
+                um::wg_wait<0>();
+                um::wg_fence_acc<NACC>(acc);
+                if constexpr (pool2) um::bar_sync(1, 256);             // sF aliases sA2: both warpgroups' MMAs have read it
 #pragma unroll
-            for (int i = 0; i < 16; ++i) {
-                const int c = 8 * i + cq;
-                if (c < NP2) {
+                for (int i = 0; i < NP2 / 8; ++i) {
+                    const int c = 8 * i + cq;
                     const float2 b = *reinterpret_cast<const float2*>(a.bias2 + c);
 #pragma unroll
                     for (int h = 0; h < 2; ++h) {
                         const int m = row + 8 * h, px = tile * 128 + m;
                         const float o0 = fmaxf(acc[4 * i + 2 * h] + b.x, 0.f), o1 = fmaxf(acc[4 * i + 2 * h + 1] + b.y, 0.f);
-                        if (a.pool2) {
+                        if constexpr (pool2) {
                             *reinterpret_cast<float2*>(sF + (size_t)m * (NP2 + 4) + c) = make_float2(o0, o1);
                         } else {
                             uint32_t hv, lv;
@@ -809,10 +829,30 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) k_gemm_tc(const __grid_consta
                         }
                     }
                 }
+                if constexpr (pool2) pool_store(NP2, a.out2_hi, a.out2_lo);
             }
-            if (a.pool2) pool_store(NP2, a.out2_hi, a.out2_lo);
         }
     }
+}
+
+// the instances the plan of OSNet_x0_25 launches (both launch lists); a layout without one is refused at plan build
+typedef void (*GemmKernel)(GemmTcArgs, const int*, int, int, GemmSmem, GemmHeadIO);
+struct GemmInstance { int NP, NP2, mode; GemmKernel fn; };
+#define BMB_GEMM(np, np2, mode) {np, np2, mode, k_gemm_tc<np, np2, mode>}
+static const GemmInstance kGemmInstances[] = {
+    BMB_GEMM(16, 0, GM_PLAIN), BMB_GEMM(32, 0, GM_PLAIN),     // conv1 of every block
+    BMB_GEMM(64, 0, GM_PLAIN), BMB_GEMM(96, 0, GM_PLAIN),     // combine without a tail (diagnostic list)
+    BMB_GEMM(128, 0, GM_PLAIN),                               // combine of the last block; conv5 (diagnostic list)
+    BMB_GEMM(64, 0, GM_POOL), BMB_GEMM(96, 0, GM_POOL),       // unfused transitions (diagnostic list)
+    BMB_GEMM(64, 16, GM_TAIL), BMB_GEMM(96, 32, GM_TAIL), BMB_GEMM(128, 32, GM_TAIL),   // combine + next conv1
+    BMB_GEMM(64, 64, GM_TAIL_POOL2), BMB_GEMM(96, 96, GM_TAIL_POOL2),                   // combine + transition
+    BMB_GEMM(128, 0, GM_HEAD),                                // conv5 + head
+};
+#undef BMB_GEMM
+inline GemmKernel gemm_instance(int NP, int NP2, int mode) {
+    for (const GemmInstance& g : kGemmInstances)
+        if (g.NP == NP && g.NP2 == NP2 && g.mode == mode) return g.fn;
+    return nullptr;
 }
 
 

@@ -101,6 +101,8 @@ struct Launch {
     const bf16* src_lo[2] = {nullptr, nullptr};
     FrontTcArgs front{};
     GemmSmem gl{};
+    GemmKernel gemm_fn = nullptr;   // the k_gemm_tc instance of (NP, NP2, epilogue mode)
+    int gemm_ctas = 0;              // its CTAs per SM at layout gl, as the occupancy calculator reports them
     int gemm_groups = 0;
     int stage_after = -1;       // debug stage index whose tensor exists after this launch
     // the tensor to expose when a debug stop hits here

@@ -120,7 +120,8 @@ Plan* plan_build(ReidModel* m, const float* hw) {
         RCUDA_OK(chain_prepare<BMB_CHAIN_S2>());
         RCUDA_OK(chain_prepare<BMB_CHAIN_S3>());
         RCUDA_OK(chain_prepare<BMB_CHAIN_S4>());
-        RCUDA_OK(cudaFuncSetAttribute(k_gemm_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, P->smem_limit));
+        for (const GemmInstance& gi : kGemmInstances)
+            RCUDA_OK(cudaFuncSetAttribute(gi.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, P->smem_limit));
         RCUDA_OK(cudaFuncSetAttribute(k_front_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FR_SMEM));
 
         // ---- launches ----
@@ -156,11 +157,23 @@ Plan* plan_build(ReidModel* m, const float* hw) {
         auto finish_into = [&](Launch& L, std::vector<Launch>* out) {
             GemmTcArgs& g = L.gemm;
             const bool tail = g.b2_packed != nullptr;
-            // two CTAs per SM (they overlap each other's MMA / epilogue / load latencies) when a >= 2-deep ring fits half
-            // the shared memory -- with smaller ring chunks (2 planes) if that is what it takes; otherwise one CTA with
-            // the deepest ring that fits
-            const int half_limit = (P->smem_limit + 1024) / 2 - 1024 - 512;
+            if (g.NP > 128 || (tail && g.NP2 > 128)) throw std::runtime_error("tensor-core GEMM: more than 128 output channels");
+            const int mode = g.head_w ? GM_HEAD : g.pool ? GM_POOL : !tail ? GM_PLAIN : g.pool2 ? GM_TAIL_POOL2 : GM_TAIL;
+            L.gemm_fn = gemm_instance(g.NP, tail ? g.NP2 : 0, mode);
+            if (!L.gemm_fn)
+                throw std::runtime_error("tensor-core GEMM: no kernel instance for NP = " + std::to_string(g.NP) + ", NP2 = " +
+                                         std::to_string(tail ? g.NP2 : 0) + ", epilogue mode " + std::to_string(mode));
             auto layout = [&](int ns) { return gemm_smem_layout(g.K8, g.NP, g.NP2, ns, tail, g.pool != 0, g.slot_bytes, g.pool2 != 0); };
+            auto ctas = [&](int ns) {     // CTAs per SM of the instance at this layout (registers, shared memory, threads)
+                const size_t bytes = layout(ns).total;
+                int c = 0;
+                if ((int)bytes <= P->smem_limit)
+                    RCUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&c, L.gemm_fn, GEMM_THREADS, bytes));
+                return c;
+            };
+            // two CTAs per SM (they overlap each other's MMA / epilogue / load latencies) when the occupancy calculator
+            // places two with a >= 2-deep ring -- with smaller ring chunks (2 planes) if that is what it takes; otherwise
+            // one CTA with the deepest ring that fits
             int ns = 0;
             for (int pass = 0; pass < 2 && !ns; ++pass) {
                 int kc_max = 2;
@@ -170,7 +183,7 @@ Plan* plan_build(ReidModel* m, const float* hw) {
                 }
                 g.slot_bytes = kc_max * 128 * 16 * 2;
                 for (int cand = 4; cand >= 2 && !ns; --cand)
-                    if ((int)layout(cand).total <= half_limit) ns = cand;
+                    if (ctas(cand) >= 2) ns = cand;
             }
             if (!ns) {
                 int kc_max = 2;
@@ -180,10 +193,10 @@ Plan* plan_build(ReidModel* m, const float* hw) {
                 }
                 g.slot_bytes = kc_max * 128 * 16 * 2;
                 for (int cand = 4; cand >= 2 && !ns; --cand)
-                    if ((int)layout(cand).total <= P->smem_limit) ns = cand;
+                    if (ctas(cand) >= 1) ns = cand;
             }
             if (!ns) throw std::runtime_error("tensor-core GEMM does not fit shared memory");
-            if (g.NP > 128 || (tail && g.NP2 > 128)) throw std::runtime_error("tensor-core GEMM: more than 128 output channels");
+            L.gemm_ctas = ctas(ns);
             for (int s = 0; s < g.n_src; ++s) {   // the boxes follow the chunk size
                 make_tile_map(&g.map_hi[s], L.src_hi[s], P->chunk, g.src_planes[s], g.HW, g.src_kc[s]);
                 make_tile_map(&g.map_lo[s], L.src_lo[s], P->chunk, g.src_planes[s], g.HW, g.src_kc[s]);
@@ -386,7 +399,7 @@ int plan_run(ReidModel* m, const FrontInput& fi, const int* d_n, int off, int up
                 chain_launch<BMB_CHAIN_S4>(L.chain, L.chain_tiles, upper, d_n, off, st);
                 break;
             case LK_GEMM:
-                k_gemm_tc<<<dim3(L.gemm_groups, upper), GEMM_THREADS, L.gl.total, st>>>(L.gemm, d_n, off, upper, L.gl, GemmHeadIO{fi.crops, fi.out, fi.out_ld});
+                L.gemm_fn<<<dim3(L.gemm_groups, upper), GEMM_THREADS, L.gl.total, st>>>(L.gemm, d_n, off, upper, L.gl, GemmHeadIO{fi.crops, fi.out, fi.out_ld});
                 break;
         }
         prof.end();

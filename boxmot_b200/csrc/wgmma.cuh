@@ -52,6 +52,9 @@ __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.a
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// waits until at most N committed groups of this warpgroup are still in flight
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 // keeps the compiler from touching accumulator registers across an asynchronous wgmma
 template <int NREG>
 __device__ __forceinline__ void wg_fence_acc(float* d) {
@@ -148,7 +151,8 @@ __device__ __forceinline__ void mma(float* d, uint64_t a, uint32_t b_addr, uint3
         else wg_bf16_n16(d, a, make_desc(b_addr, b_lbo, b_sbo), acc);
     }
 }
-// the same with N known at run time (N in 16 .. 128, multiple of 16); d holds 64 registers
+// the same with N known at run time (N in 16 .. 128, multiple of 16); d holds 64 registers.  The switch around every
+// MMA makes ptxas serialise the wgmma of the caller; only the opt-in tf32 pointwise kernel uses it.
 template <bool TF32>
 __device__ __forceinline__ void mma_rt(int N, float* d, uint64_t a, uint32_t b_addr, uint32_t b_lbo, uint32_t b_sbo, uint32_t acc) {
     switch (N) {
