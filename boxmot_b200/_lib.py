@@ -16,6 +16,7 @@ TRACKER_BYTETRACK = 0
 TRACKER_BOTSORT = 1
 TRACKER_DEEPOCSORT = 2
 TRACKER_STRONGSORT = 3
+TRACKER_BOOSTTRACK = 4
 
 
 class BoxMOTByteTrackConfig(ctypes.Structure):
@@ -46,7 +47,11 @@ class BoxMOTB200TrackerConfig(ctypes.Structure):
                 ("q_xy_scaling", c_double), ("q_s_scaling", c_double),
                 ("n_init", c_int), ("nn_budget", c_int), ("min_conf", c_double), ("max_cos_dist", c_double),
                 ("max_iou_dist", c_double), ("mc_lambda", c_double), ("ema_alpha", c_double),
-                ("reid_preprocess", c_int)]
+                ("reid_preprocess", c_int),
+                ("use_dlo_boost", c_int), ("use_duo_boost", c_int), ("use_rich_s", c_int), ("use_sb", c_int),
+                ("use_vt", c_int), ("s_sim_corr", c_int), ("dlo_boost_coef", c_double), ("lambda_iou", c_double),
+                ("lambda_mhd", c_double), ("lambda_shape", c_double), ("min_box_area", c_double),
+                ("aspect_ratio_thresh", c_double)]
 
 
 # every symbol include/boxmot_b200.h declares: name -> (restype, argtypes)

@@ -12,6 +12,7 @@
 #include "tracker_core.cuh"
 #include "docs_core.cuh"
 #include "ss_core.cuh"
+#include "bt_core.cuh"
 
 namespace bmb {
 
@@ -66,6 +67,11 @@ struct Engine {
     SsCfg scfg{};
     SsStream* d_ss = nullptr;
     std::vector<SsStream> h_ss;
+    bool is_bt = false;                // BoostTrack engine (bt_core.cuh)
+    BtCfg btcfg{};
+    BtStream* d_bt = nullptr;
+    std::vector<BtStream> h_bt;
+    double* d_conf_pow = nullptr;      // 0.9 ** k, k = 0 .. max_age + 1 (KalmanBoxTracker.get_confidence)
     std::vector<float*> out_ptr;       // per-stream output rows / scalars / timers (either family)
     std::vector<int*> scalars_ptr;
     std::vector<long long*> timers_ptr;
@@ -124,6 +130,7 @@ struct Engine {
     std::vector<TrkStream> h_streams_alt;
     DocsStream* d_docs_alt = nullptr;
     SsStream* d_ss_alt = nullptr;
+    BtStream* d_bt_alt = nullptr;
     cudaEvent_t ev_reid_done[2]{};
     cudaEvent_t ev_assoc_done[2]{};
     int pipe_parity = 0;
@@ -164,6 +171,7 @@ struct Engine {
     void enqueue_association(TrkStream* streams_dev, const float* embs_src);
     void enqueue_crops(int parity, cudaStream_t st);            // crop list of the family, from input set `parity`
     void enqueue_family_association(int parity);                // association launches of the family on `stream`
+    void enqueue_bt(BtStream* streams_dev);                      // BoostTrack: embedding cost + frame kernel
     int run_reid(cudaStream_t main_stream, const uint8_t* images_dev, int rows, int cols, int total, float* embs_out);
     void enqueue_fetch();
     void finish_fetch(float* const* out, const int* out_cap, int* out_rows);

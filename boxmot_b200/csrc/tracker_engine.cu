@@ -211,6 +211,63 @@ __global__ void __launch_bounds__(256) k_docs_frame(const DocsCfg cfg, DocsStrea
     docs_frame(cfg, s);
 }
 
+// BoostTrack appearance similarity dets_embs @ trk_embs.T (boosttrack.py:353-358) for every (detection row, live slot):
+// float32 rows x float64 track embeddings, float64 accumulate in feature order (k_docs_embcost's arithmetic).  The
+// reference multiplies in float32 while every live track still holds its birth embedding and with BLAS otherwise; both
+// differ from this sum in the last bits only.
+__global__ void __launch_bounds__(256) k_bt_embcost(const BtCfg cfg, BtStream* streams) {
+    const BtStream& s = streams[blockIdx.z];
+    const int D = min(*s.n_dets, cfg.cap_dets);
+    const int T = s.scalars[SC_N_ACTIVE];
+    const int r0 = blockIdx.y * EMB_TR, d0 = blockIdx.x * EMB_TD;
+    if (r0 >= T || d0 >= D) return;
+    __shared__ double sa[EMB_TR][EMB_TK + 1];
+    __shared__ float sb[EMB_TD][EMB_TK + 1];
+    __shared__ int slot_of[EMB_TR];
+    const int F = cfg.feat_dim;
+    const int tr = threadIdx.x / EMB_TD, td = threadIdx.x % EMB_TD;
+    if (threadIdx.x < EMB_TR) slot_of[threadIdx.x] = r0 + threadIdx.x < T ? s.tracks[r0 + threadIdx.x] : -1;
+    __syncthreads();
+    double dot = 0.0;
+    for (int k0 = 0; k0 < F; k0 += EMB_TK) {
+        for (int e = threadIdx.x; e < EMB_TR * EMB_TK; e += blockDim.x) {
+            const int r = e / EMB_TK, k = e % EMB_TK;
+            const int slot = slot_of[r];
+            sa[r][k] = (slot >= 0 && k0 + k < F) ? s.emb[(size_t)slot * F + k0 + k] : 0.0;
+        }
+        for (int e = threadIdx.x; e < EMB_TD * EMB_TK; e += blockDim.x) {
+            const int d = e / EMB_TK, k = e % EMB_TK;
+            sb[d][k] = (d0 + d < D && k0 + k < F) ? s.embs[(size_t)(d0 + d) * F + k0 + k] : 0.f;
+        }
+        __syncthreads();
+#pragma unroll 8
+        for (int k = 0; k < EMB_TK; ++k) dot += (double)sb[td][k] * sa[tr][k];
+        __syncthreads();
+    }
+    const int slot = slot_of[tr];
+    if (slot >= 0 && d0 + td < D) s.embq[(size_t)(d0 + td) * cfg.cap_tracks + slot] = dot;
+}
+
+__global__ void __launch_bounds__(256) k_bt_frame(const BtCfg cfg, BtStream* streams, int jv_in_smem) {
+    extern __shared__ __align__(16) unsigned char dyn_smem[];
+    BtStream s = streams[blockIdx.x];
+    s.jv_wide = jv_in_smem >> 1;
+    if (jv_in_smem & 1) {
+        const int MX = cfg.cap_tracks > cfg.cap_dets ? cfg.cap_tracks : cfg.cap_dets;
+        double* pd = reinterpret_cast<double*>(dyn_smem);
+        s.lap_v = pd; pd += MX;
+        s.lap_spc = pd; pd += MX;
+        int* pi = reinterpret_cast<int*>(pd);
+        s.lap_x = pi; pi += MX;
+        s.lap_y = pi; pi += MX;
+        s.lap_path = pi; pi += MX;
+        s.lap_tl = pi; pi += MX;
+        s.lap_sc = pi; pi += MX;
+        s.lap_insc = pi;
+    }
+    bt_frame(cfg, s);
+}
+
 // DeepOCSORT embeds every detection above det_thresh (deepocsort.py:333-343)
 // ordered (stream, detection) crop list built by one warp with ballot compaction
 template <typename Keep>
@@ -244,6 +301,18 @@ __global__ void k_build_crops_docs(const DocsCfg cfg, DocsStream* streams, int n
                          [thr](const float* r) { return r[4] > thr; });
     }
     if (threadIdx.x == 0) { *n_crops = n; if (hint) *hint = n; }   // hint: host-mapped, read without synchronisation
+}
+
+// BoostTrack embeds EVERY detection row: which rows survive the confidence boosts depends on the track state, so a
+// survivor list would put the ReID behind the association; the frame kernel picks the survivors' rows
+__global__ void k_build_crops_bt(const BtCfg cfg, BtStream* streams, int n_streams, CropDesc* crops, int* n_crops, int* hint) {
+    if (threadIdx.x >= 32 || blockIdx.x != 0) return;
+    int n = 0;
+    for (int sidx = 0; sidx < n_streams; ++sidx) {
+        const BtStream& s = streams[sidx];
+        n = append_crops(s.dets, min(*s.n_dets, cfg.cap_dets), sidx, cfg.cap_dets, crops, n, [](const float*) { return true; });
+    }
+    if (threadIdx.x == 0) { *n_crops = n; if (hint) *hint = n; }
 }
 
 // crop list for on-device ReID: one entry per first-round detection, ordered by (stream, detection).
@@ -309,10 +378,12 @@ void Engine::construct(const BoxMOTB200TrackerConfig& p) {
     if (p.n_streams < 1) throw std::runtime_error("n_streams must be >= 1");
     if (p.cap_tracks < 8 || p.cap_dets < 1) throw std::runtime_error("cap_tracks >= 8 and cap_dets >= 1 required");
     if (p.tracker != BOXMOT_B200_TRACKER_BOTSORT && p.tracker != BOXMOT_B200_TRACKER_BYTETRACK &&
-        p.tracker != BOXMOT_B200_TRACKER_DEEPOCSORT && p.tracker != BOXMOT_B200_TRACKER_STRONGSORT)
+        p.tracker != BOXMOT_B200_TRACKER_DEEPOCSORT && p.tracker != BOXMOT_B200_TRACKER_STRONGSORT &&
+        p.tracker != BOXMOT_B200_TRACKER_BOOSTTRACK)
         throw std::runtime_error("unknown tracker kind");
     is_docs = p.tracker == BOXMOT_B200_TRACKER_DEEPOCSORT;
     is_ss = p.tracker == BOXMOT_B200_TRACKER_STRONGSORT;
+    is_bt = p.tracker == BOXMOT_B200_TRACKER_BOOSTTRACK;
     if (p.tracker == BOXMOT_B200_TRACKER_BOTSORT && p.removed_stracks_buffer < 1)
         throw std::runtime_error("removed_stracks_buffer must be >= 1");
     int ndev = 0;
@@ -345,6 +416,21 @@ void Engine::construct(const BoxMOTB200TrackerConfig& p) {
         cfg.feat_dim = p.feat_dim;
         cfg.cap_tracks = p.cap_tracks; cfg.cap_dets = p.cap_dets;
     }
+    if (is_bt) {
+        if (p.max_age < 0 || p.max_age > 100000) throw std::runtime_error("max_age must be in [0, 100000]");
+        if (p.min_hits < 0) throw std::runtime_error("min_hits must be >= 0");
+        btcfg.cap_tracks = p.cap_tracks; btcfg.cap_dets = p.cap_dets;
+        btcfg.max_age = p.max_age; btcfg.min_hits = p.min_hits; btcfg.with_reid = p.with_reid ? 1 : 0;
+        btcfg.use_dlo = p.use_dlo_boost ? 1 : 0; btcfg.use_duo = p.use_duo_boost ? 1 : 0;
+        btcfg.rich_s = p.use_rich_s ? 1 : 0; btcfg.use_sb = p.use_sb ? 1 : 0; btcfg.use_vt = p.use_vt ? 1 : 0;
+        btcfg.s_sim_corr = p.s_sim_corr ? 1 : 0;
+        btcfg.det_thresh = p.det_thresh; btcfg.iou_threshold = p.iou_threshold;
+        btcfg.lambda_iou = p.lambda_iou; btcfg.lambda_mhd = p.lambda_mhd; btcfg.lambda_shape = p.lambda_shape;
+        btcfg.dlo_coef = p.dlo_boost_coef; btcfg.min_box_area = p.min_box_area; btcfg.ar_thresh = p.aspect_ratio_thresh;
+        cfg.with_reid = btcfg.with_reid;
+        cfg.feat_dim = cfg.with_reid ? p.feat_dim : 0;
+        cfg.cap_tracks = p.cap_tracks; cfg.cap_dets = p.cap_dets;
+    }
     if (cfg.with_reid && cfg.feat_dim < 1) throw std::runtime_error("feat_dim must be set when with_reid");
     S = p.n_streams;
     CUDA_OK(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
@@ -356,12 +442,14 @@ void Engine::construct(const BoxMOTB200TrackerConfig& p) {
         }
     }
     if (is_docs) dcfg.feat_dim = cfg.feat_dim;
+    if (is_bt) btcfg.feat_dim = cfg.feat_dim;
     if (is_ss) {
         scfg.feat_dim = cfg.feat_dim;
         if (scfg.feat_dim % 4) throw std::runtime_error("StrongSORT feat_dim must be a multiple of 4");
     }
     stream_bytes = is_docs ? carve_docs(dcfg, nullptr, nullptr, &persistent_bytes)
                  : is_ss   ? carve_ss(scfg, nullptr, nullptr, &persistent_bytes)
+                 : is_bt   ? carve_bt(btcfg, nullptr, nullptr, &persistent_bytes)
                            : carve_stream(cfg, nullptr, nullptr, &persistent_bytes);
     persistent_bytes = (persistent_bytes + 15) & ~(size_t)15;
     CUDA_OK(cudaMalloc(&d_mem, stream_bytes * S));
@@ -396,6 +484,25 @@ void Engine::construct(const BoxMOTB200TrackerConfig& p) {
         }
         CUDA_OK(cudaMalloc(&d_ss, sizeof(SsStream) * S));
         CUDA_OK(cudaMemcpy(d_ss, h_ss.data(), sizeof(SsStream) * S, cudaMemcpyHostToDevice));
+    } else if (is_bt) {
+        // KalmanBoxTracker.get_confidence: 0.9 ** k with the host's pow, which is what python's float power calls
+        std::vector<double> pw((size_t)(p.max_age + 2 > 8 ? p.max_age + 2 : 8));
+        for (size_t k = 0; k < pw.size(); ++k) pw[k] = pow(0.9, (double)k);
+        CUDA_OK(cudaMalloc(&d_conf_pow, sizeof(double) * pw.size()));
+        CUDA_OK(cudaMemcpy(d_conf_pow, pw.data(), sizeof(double) * pw.size(), cudaMemcpyHostToDevice));
+        btcfg.conf_pow = d_conf_pow;
+        btcfg.n_conf_pow = (int)pw.size();
+        h_bt.resize(S);
+        for (int i = 0; i < S; ++i) {
+            carve_bt(btcfg, d_mem + stream_bytes * i, &h_bt[i], nullptr);
+            h_bt[i].dets = d_dets + (size_t)i * CD * 6;
+            h_bt[i].n_dets = d_ndets + i;
+            h_bt[i].embs = cfg.with_reid ? d_embs + (size_t)i * CD * F : nullptr;
+            h_bt[i].warp = d_warp + (size_t)i * 8;
+            out_ptr[i] = h_bt[i].out; scalars_ptr[i] = h_bt[i].scalars; timers_ptr[i] = h_bt[i].timers;
+        }
+        CUDA_OK(cudaMalloc(&d_bt, sizeof(BtStream) * S));
+        CUDA_OK(cudaMemcpy(d_bt, h_bt.data(), sizeof(BtStream) * S, cudaMemcpyHostToDevice));
     } else if (is_docs) {
         h_docs.resize(S);
         for (int i = 0; i < S; ++i) {
@@ -437,6 +544,15 @@ void Engine::construct(const BoxMOTB200TrackerConfig& p) {
             }
             CUDA_OK(cudaMalloc(&d_ss_alt, sizeof(SsStream) * S));
             CUDA_OK(cudaMemcpy(d_ss_alt, alt.data(), sizeof(SsStream) * S, cudaMemcpyHostToDevice));
+        } else if (is_bt) {
+            std::vector<BtStream> alt = h_bt;
+            for (int i = 0; i < S; ++i) {
+                alt[i].dets = d_dets_alt + (size_t)i * CD * 6;
+                alt[i].n_dets = d_ndets_alt + i;
+                alt[i].embs = d_embs_alt + (size_t)i * CD * F;
+            }
+            CUDA_OK(cudaMalloc(&d_bt_alt, sizeof(BtStream) * S));
+            CUDA_OK(cudaMemcpy(d_bt_alt, alt.data(), sizeof(BtStream) * S, cudaMemcpyHostToDevice));
         } else if (is_docs) {
             std::vector<DocsStream> alt = h_docs;
             for (int i = 0; i < S; ++i) {
@@ -510,13 +626,13 @@ void Engine::release() {
             if (ev_assoc_done[k]) cudaEventDestroy(ev_assoc_done[k]);
         }
         cudaFree(d_dets_alt); cudaFree(d_ndets_alt); cudaFree(d_embs_alt); cudaFree(d_streams_alt);
-        cudaFree(d_docs_alt); cudaFree(d_ss_alt);
+        cudaFree(d_docs_alt); cudaFree(d_ss_alt); cudaFree(d_bt_alt);
     }
     if (reid) reid_free(reid);
     cudaFree(d_cmc_prev); cudaFree(d_cmc_cur); cudaFree(d_cmc_has_prev); cudaFree(d_cmc_gate);
     if (sof) sof_state_free(sof);
     cudaFree(d_warp); cudaFree(d_mem); cudaFree(d_dets); cudaFree(d_ndets); cudaFree(d_embs); cudaFree(d_out);
-    cudaFree(d_scalars_out); cudaFree(d_streams); cudaFree(d_docs); cudaFree(d_ss); cudaFree(d_crops); cudaFree(d_ncrops); cudaFree(d_images);
+    cudaFree(d_scalars_out); cudaFree(d_streams); cudaFree(d_docs); cudaFree(d_ss); cudaFree(d_bt); cudaFree(d_conf_pow); cudaFree(d_crops); cudaFree(d_ncrops); cudaFree(d_images);
     cudaFreeHost(h_dets); cudaFreeHost(h_ndets); cudaFreeHost(h_out); cudaFreeHost(h_scalars);
     cudaFreeHost(h_embs); cudaFreeHost(h_images); cudaFreeHost(h_ndets_ring);
     if (mark[0]) cudaEventDestroy(mark[0]);
@@ -530,7 +646,7 @@ void Engine::reset() {
     if (reid_stream) CUDA_OK(cudaStreamSynchronize(reid_stream));
     if (d_cmc_has_prev) CUDA_OK(cudaMemsetAsync(d_cmc_has_prev, 0, sizeof(int) * S, stream));   // ECC.prev_img = None
     if (sof) sof_state_reset(sof, stream);   // a fresh SOF: the next frame initialises
-    if (is_docs || is_ss) {
+    if (is_docs || is_ss || is_bt) {
         CUDA_OK(cudaStreamSynchronize(stream));
         for (int i = 0; i < S; ++i) CUDA_OK(cudaMemsetAsync(d_mem + stream_bytes * i, 0, persistent_bytes, stream));
         CUDA_OK(cudaStreamSynchronize(stream));
@@ -575,6 +691,30 @@ void Engine::enqueue_frame(const float* embs_dev, const uint8_t* images_dev, int
             CUDA_OK(cudaMemsetAsync(d_warp, 0, sizeof(double) * 8 * S, stream));
             warp_dirty = false;
         }
+        CUDA_OK(cudaEventRecord(ev[2], stream));
+        if (profile) {
+            CUDA_OK(cudaStreamSynchronize(stream));
+            float b = 0.f;
+            cudaEventElapsedTime(&b, ev[1], ev[2]);
+            assoc_ms_accum += b;
+            assoc_frames += 1;
+        }
+        return;
+    }
+    if (is_bt) {
+        if (cfg.with_reid && !embs_dev) {
+            if (!reid) throw std::runtime_error("BoostTrack with_reid needs embeddings or a ReID model");
+            if (!images_dev) throw std::runtime_error("ReID inside update() needs an image");
+            k_build_crops_bt<<<1, 32, 0, stream>>>(btcfg, d_bt, S, d_crops, d_ncrops, d_crops_hint);
+            ++launches;
+            launches += run_reid(stream, images_dev, rows, cols, max_dets_total, d_embs);
+        } else if (cfg.with_reid && embs_dev && embs_dev != d_embs) {
+            CUDA_OK(cudaMemcpyAsync(d_embs, embs_dev, sizeof(float) * (size_t)cfg.feat_dim * cfg.cap_dets * S,
+                                    cudaMemcpyDeviceToDevice, stream));
+        }
+        CUDA_OK(cudaEventRecord(ev[1], stream));
+        enqueue_bt(d_bt);
+        CUDA_OK(cudaGetLastError());
         CUDA_OK(cudaEventRecord(ev[2], stream));
         if (profile) {
             CUDA_OK(cudaStreamSynchronize(stream));
@@ -657,6 +797,7 @@ void Engine::enqueue_frame(const float* embs_dev, const uint8_t* images_dev, int
 // crop list of the tracker family from input set `parity` (0: d_dets / d_ndets, 1: the alternate set)
 void Engine::enqueue_crops(int parity, cudaStream_t st) {
     if (is_ss) ss_build_crops(scfg, parity ? d_ss_alt : d_ss, S, d_crops, d_ncrops, d_crops_hint, st);
+    else if (is_bt) k_build_crops_bt<<<1, 32, 0, st>>>(btcfg, parity ? d_bt_alt : d_bt, S, d_crops, d_ncrops, d_crops_hint);
     else if (is_docs) k_build_crops_docs<<<1, 32, 0, st>>>(dcfg, parity ? d_docs_alt : d_docs, S, d_crops, d_ncrops, d_crops_hint);
     else k_build_crops<<<1, 32, 0, st>>>(cfg, parity ? d_streams_alt : d_streams, S, d_crops, d_ncrops, d_crops_hint);
     ++launches;
@@ -670,6 +811,8 @@ void Engine::enqueue_family_association(int parity) {
             CUDA_OK(cudaMemsetAsync(d_warp, 0, sizeof(double) * 8 * S, stream));
             warp_dirty = false;
         }
+    } else if (is_bt) {
+        enqueue_bt(parity ? d_bt_alt : d_bt);
     } else if (is_docs) {
         DocsStream* ds = parity ? d_docs_alt : d_docs;
         if (cfg.with_reid) {
@@ -692,6 +835,29 @@ void Engine::enqueue_family_association(int parity) {
         enqueue_association(parity ? d_streams_alt : d_streams, cfg.with_reid ? (parity ? d_embs_alt : d_embs) : nullptr);
     }
     CUDA_OK(cudaGetLastError());
+}
+
+// BoostTrack: embedding dot products (wide grid) and the per-stream frame kernel on `stream`; a supplied or estimated
+// warp applies to this frame only
+void Engine::enqueue_bt(BtStream* streams_dev) {
+    BtCfg c = btcfg;
+    c.cmc_every_frame = cmc_mode != 0;   // boosttrack.py:318-321: camera_update runs whenever an estimator exists
+    if (cfg.with_reid) {
+        dim3 g((c.cap_dets + EMB_TD - 1) / EMB_TD, (c.cap_tracks + EMB_TR - 1) / EMB_TR, S);
+        k_bt_embcost<<<g, 256, 0, stream>>>(c, streams_dev);
+        ++launches;
+    }
+    const int MX = c.cap_tracks > c.cap_dets ? c.cap_tracks : c.cap_dets;
+    const size_t jb = jv_smem_bytes(MX);
+    const bool in_smem = jb <= 200 * 1024;
+    if (in_smem && jb > 48 * 1024)
+        CUDA_OK(cudaFuncSetAttribute(k_bt_frame, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)jb));
+    k_bt_frame<<<S, 256, in_smem ? jb : 0, stream>>>(c, streams_dev, (in_smem ? 1 : 0) | (jv_wide_default() << 1));
+    ++launches;
+    if (warp_dirty) {
+        CUDA_OK(cudaMemsetAsync(d_warp, 0, sizeof(double) * 8 * S, stream));
+        warp_dirty = false;
+    }
 }
 
 // crop list (already built on main_stream) -> embeddings; slices of the list run concurrently on the helper streams
@@ -754,7 +920,7 @@ void Engine::set_cmc(const char* method) {
     if (strcmp(method, "sof") == 0) {
         // botsort.py:142,301 (every frame, every detection row) and deepocsort.py:330-349 (every frame, the rows with
         // conf > det_thresh); StrongSORT's estimator is ECC
-        if (is_ss || (!is_docs && cfg.kind != KIND_XYWH))
+        if (is_ss || (!is_docs && !is_bt && cfg.kind != KIND_XYWH))
             throw std::runtime_error("on-device SOF applies to BoT-SORT and DeepOCSORT (StrongSORT's estimator is ecc)");
         if (!sof) sof = sof_state_create(S, 0.15, 8, 0.2, 3.0);
         else if (cmc_mode != 2) sof_state_reset(sof, stream);
@@ -764,7 +930,7 @@ void Engine::set_cmc(const char* method) {
     if (strcmp(method, "ecc") != 0)
         throw std::runtime_error(std::string("camera-motion method '") + method + "' is not built on the device (ecc, sof, "
                                  "none); orb / sift warps can be supplied through set_warp");
-    if ((!is_ss && !is_docs && cfg.kind != KIND_XYWH) || is_docs)
+    if ((!is_ss && !is_docs && !is_bt && cfg.kind != KIND_XYWH) || is_docs)
         throw std::runtime_error("on-device ECC applies to BoT-SORT and StrongSORT (ByteTrack has no CMC, DeepOCSORT's is sof)");
     if (is_ss && !d_cmc_gate) {   // StrongSORT estimates only while tracks exist
         std::vector<const int*> g(S);
@@ -803,7 +969,7 @@ void Engine::enqueue_cmc(const uint8_t* images_dev, int rows, int cols) {
 
 void Engine::set_warp(int sidx, const double* warp6) {
     if (sidx < 0 || sidx >= S) throw std::runtime_error("stream index out of range");
-    if (!is_ss && !is_docs && cfg.kind != KIND_XYWH)
+    if (!is_ss && !is_docs && !is_bt && cfg.kind != KIND_XYWH)
         throw std::runtime_error("camera-motion warps apply to BoT-SORT, DeepOCSORT and StrongSORT (ByteTrack has none)");
     double w[8] = {warp6[0], warp6[1], warp6[2], warp6[3], warp6[4], warp6[5], 1.0, 0.0};
     CUDA_OK(cudaStreamSynchronize(stream));
@@ -832,7 +998,7 @@ void Engine::profile_read(double* ms, int* launch_counts) {
     for (int c = 0; c < REID_N_CLASSES + 1; ++c) { ms[c] = 0.0; launch_counts[c] = 0; }
     if (reid) reid_profile_collect(reid, ms, launch_counts);
     ms[REID_N_CLASSES] = assoc_ms_accum;
-    launch_counts[REID_N_CLASSES] = assoc_frames * (is_docs ? (cfg.with_reid ? 2 : 1) : (cfg.with_reid ? 4 : 1));
+    launch_counts[REID_N_CLASSES] = assoc_frames * ((is_docs || is_bt) ? (cfg.with_reid ? 2 : 1) : (cfg.with_reid ? 4 : 1));
     assoc_ms_accum = 0.0;
     assoc_frames = 0;
 }
@@ -1020,6 +1186,25 @@ int Engine::snapshot(int sidx, int* ids, double* means, double* covs, int cap) {
         }
         return n;
     }
+    if (is_bt) {
+        const BtStream& s = h_bt[sidx];
+        const int CT = cfg.cap_tracks;
+        std::vector<int> sc(SC_COUNT), lst(CT), idv(CT);
+        std::vector<double> xs((size_t)CT * 8), ps((size_t)CT * 64);
+        CUDA_OK(cudaMemcpy(sc.data(), s.scalars, sizeof(int) * SC_COUNT, cudaMemcpyDeviceToHost));
+        CUDA_OK(cudaMemcpy(lst.data(), s.tracks, sizeof(int) * CT, cudaMemcpyDeviceToHost));
+        CUDA_OK(cudaMemcpy(idv.data(), s.id, sizeof(int) * CT, cudaMemcpyDeviceToHost));
+        CUDA_OK(cudaMemcpy(xs.data(), s.x, sizeof(double) * 8 * CT, cudaMemcpyDeviceToHost));
+        CUDA_OK(cudaMemcpy(ps.data(), s.P, sizeof(double) * 64 * CT, cudaMemcpyDeviceToHost));
+        int n = 0;
+        for (int k = 0; k < sc[SC_N_ACTIVE] && n < cap; ++k, ++n) {
+            const int t = lst[k];
+            ids[n] = idv[t];
+            memcpy(means + (size_t)n * 8, xs.data() + (size_t)t * 8, sizeof(double) * 8);
+            memcpy(covs + (size_t)n * 64, ps.data() + (size_t)t * 64, sizeof(double) * 64);
+        }
+        return n;
+    }
     if (is_docs) {
         const DocsStream& s = h_docs[sidx];
         const int CT = cfg.cap_tracks;
@@ -1076,11 +1261,11 @@ int Engine::track_ids(int sidx, int which, int* ids, int cap) {
     const int CT = cfg.cap_tracks;
     std::vector<int> sc(SC_COUNT), lst(CT), idv(CT);
     int n = 0;
-    if (is_ss || is_docs) {
+    if (is_ss || is_docs || is_bt) {
         if (which != 0) return 0;
-        const int* scal = is_ss ? h_ss[sidx].scalars : h_docs[sidx].scalars;
-        const int* trk = is_ss ? h_ss[sidx].tracks : h_docs[sidx].tracks;
-        const int* idp = is_ss ? h_ss[sidx].id : h_docs[sidx].id;
+        const int* scal = is_ss ? h_ss[sidx].scalars : is_bt ? h_bt[sidx].scalars : h_docs[sidx].scalars;
+        const int* trk = is_ss ? h_ss[sidx].tracks : is_bt ? h_bt[sidx].tracks : h_docs[sidx].tracks;
+        const int* idp = is_ss ? h_ss[sidx].id : is_bt ? h_bt[sidx].id : h_docs[sidx].id;
         CUDA_OK(cudaMemcpy(sc.data(), scal, sizeof(int) * SC_COUNT, cudaMemcpyDeviceToHost));
         CUDA_OK(cudaMemcpy(lst.data(), trk, sizeof(int) * CT, cudaMemcpyDeviceToHost));
         CUDA_OK(cudaMemcpy(idv.data(), idp, sizeof(int) * CT, cudaMemcpyDeviceToHost));

@@ -183,3 +183,39 @@ inline size_t carve_ss(const SsCfg& c, uint8_t* base, SsStream* s, size_t* persi
 }
 
 }  // namespace bmb
+
+#include "bt_core.cuh"
+
+namespace bmb {
+
+// BoostTrack: the (row, track) matrices dominate the scratch
+inline size_t carve_bt(const BtCfg& c, uint8_t* base, BtStream* s, size_t* persistent_bytes) {
+    const size_t CT = (size_t)c.cap_tracks, CD = (size_t)c.cap_dets, F = (size_t)(c.feat_dim > 0 ? c.feat_dim : 1);
+    const size_t MX = CT > CD ? CT : CD;
+    Carver k{base, 0};
+    BtStream t{};
+    t.scalars = k.take<int>(SC_COUNT);
+    t.timers = k.take<long long>(16);
+    t.age = k.take<int>(CT); t.hit_streak = k.take<int>(CT); t.tsu = k.take<int>(CT); t.id = k.take<int>(CT);
+    t.tracks = k.take<int>(CT);
+    t.x = k.take<double>(CT * 8); t.P = k.take<double>(CT * 64);
+    t.conf = k.take<double>(CT); t.cls = k.take<double>(CT); t.det_ind = k.take<double>(CT);
+    t.emb = k.take<double>(CT * F);
+    if (persistent_bytes) *persistent_bytes = k.off;
+    t.rconf = k.take<double>(CD); t.dz = k.take<double>(CD * 4); t.tbox = k.take<double>(CT * 5);
+    t.iou = k.take<double>(CD * CT); t.md = k.take<double>(CD * CT); t.ex = k.take<double>(CD * CT);
+    t.embq = k.take<double>(CD * CT);
+    t.colsum = k.take<double>(CT); t.ovmax = k.take<double>(CD);
+    t.kdet = k.take<int>(CD); t.cand = k.take<int>(CD); t.flag = k.take<int>(MX); t.mrow = k.take<int>(CD);
+    t.und = k.take<int>(CD); t.tmp_a = k.take<int>(CT); t.tmp_b = k.take<int>(CT); t.mark = k.take<int>(CT);
+    t.free_l = k.take<int>(CT + MB_COUNT);
+    t.cost = k.take<double>(MX * MX);
+    t.lap_x = k.take<int>(MX); t.lap_y = k.take<int>(MX);
+    t.lap_u = k.take<double>(MX); t.lap_v = k.take<double>(MX); t.lap_spc = k.take<double>(MX);
+    t.lap_path = k.take<int>(MX); t.lap_insc = k.take<int>(MX); t.lap_tl = k.take<int>(MX); t.lap_sc = k.take<int>(MX);
+    t.out = k.take<float>(CD * 8);
+    if (s) *s = t;
+    return (k.off + 255) & ~(size_t)255;
+}
+
+}  // namespace bmb

@@ -9,6 +9,7 @@ This module is tensor plumbing only; there is no CPU implementation behind it.
 from __future__ import annotations
 
 import ctypes
+import sys
 from typing import Any, Optional, Sequence
 
 import numpy as np
@@ -255,9 +256,35 @@ class MultiStreamTracker:
             cfg.with_reid = 1
             p.setdefault("track_buffer", 0)
             p.setdefault("frame_rate", 30)
+        elif kind == "boosttrack":
+            p = dict(BOOSTTRACK_ENGINE_DEFAULTS)
+            unknown = set(params) - set(p)
+            if unknown:
+                raise TypeError(f"unknown BoostTrack parameters: {sorted(unknown)}")
+            p.update(params)
+            for name in ("det_thresh", "iou_threshold", "lambda_iou", "lambda_mhd", "lambda_shape", "dlo_boost_coef",
+                         "min_box_area", "aspect_ratio_thresh"):
+                if not np.isfinite(float(p[name])):
+                    raise ValueError(f"BoostTrack {name} must be finite, got {p[name]}")
+            if not 0.0 <= float(p["det_thresh"]) < 1.0:
+                raise ValueError(f"BoostTrack det_thresh must be in [0, 1), got {p['det_thresh']}")
+            if int(p["max_age"]) < 0 or int(p["min_hits"]) < 0:
+                raise ValueError("BoostTrack max_age and min_hits must be >= 0")
+            cfg.tracker = _lib.TRACKER_BOOSTTRACK
+            cfg.max_age, cfg.min_hits = int(p["max_age"]), int(p["min_hits"])
+            cfg.det_thresh, cfg.iou_threshold = float(p["det_thresh"]), float(p["iou_threshold"])
+            cfg.use_dlo_boost, cfg.use_duo_boost = int(bool(p["use_dlo_boost"])), int(bool(p["use_duo_boost"]))
+            cfg.use_rich_s, cfg.use_sb, cfg.use_vt = int(bool(p["use_rich_s"])), int(bool(p["use_sb"])), int(bool(p["use_vt"]))
+            cfg.s_sim_corr = int(bool(p["s_sim_corr"]))
+            cfg.dlo_boost_coef, cfg.min_box_area, cfg.aspect_ratio_thresh = (float(p["dlo_boost_coef"]), float(p["min_box_area"]),
+                                                                              float(p["aspect_ratio_thresh"]))
+            cfg.lambda_iou, cfg.lambda_mhd, cfg.lambda_shape = float(p["lambda_iou"]), float(p["lambda_mhd"]), float(p["lambda_shape"])
+            cfg.with_reid = int(bool(p["with_reid"]))
+            p.setdefault("track_buffer", 0)
+            p.setdefault("frame_rate", 30)
         else:
             raise ValueError(f"tracker '{tracker}' is not part of the B200 hot path "
-                             "(bytetrack, botsort, deepocsort, strongsort)")
+                             "(bytetrack, botsort, deepocsort, strongsort, boosttrack)")
         cfg.n_streams = int(n_streams)
         cfg.cap_tracks = int(cap_tracks)
         cfg.cap_dets = int(cap_dets)
@@ -495,7 +522,7 @@ class _SingleStreamTracker:
             # the reference's un-freeze replay looks its pre-gap anchor up in a history deque of max_obs entries
             # (xysr.py:384-399) and silently skips the replay once a gap has pushed it out; the device keeps the anchor
             raise NotImplementedError("DeepOCSORT needs max_obs >= max_age + 4 (history window of the un-freeze replay)")
-        if self._kind == "deepocsort":  # BaseTracker settings that DeepOCSORT's update actually reads
+        if self._kind in ("deepocsort", "boosttrack"):  # BaseTracker settings their updates actually read
             params = dict(params, det_thresh=det_thresh, max_age=max_age, min_hits=min_hits, iou_threshold=iou_threshold)
         if self._kind == "strongsort":  # Tracker(max_age=self.max_age) (strongsort.py:56-64)
             params = dict(params, max_age=max_age)
@@ -536,7 +563,12 @@ class _SingleStreamTracker:
                 raise B200Error("with_reid=True needs reid_model=, embs=, or with_reid=False")
             # the device re-derives the split from the float32 rows it receives: decide on the same rounded values
             conf = np.asarray(dets, dtype=np.float32)[:, 4].astype(np.float64)
-            first = conf >= eng.params["min_conf"] if eng.kind == "strongsort" else conf > eng.params["track_high_thresh"]
+            if eng.kind == "boosttrack":   # every row: which rows survive the confidence boosts is decided on the device
+                first = np.ones(len(conf), dtype=bool)
+            elif eng.kind == "strongsort":
+                first = conf >= eng.params["min_conf"]
+            else:
+                first = conf > eng.params["track_high_thresh"]
             embs = np.zeros((len(dets), eng.feat_dim), np.float32)
             if first.any():
                 embs[first] = np.asarray(self.model.get_features(dets[first][:, :4], img), dtype=np.float32)
@@ -691,6 +723,64 @@ class StrongSort(_SingleStreamTracker):
             self._engine.set_cmc("ecc")
 
 
+# BoostTrack (boxmot/trackers/bbox/boosttrack/boosttrack.py:241-296 + the BaseTracker settings it reads): the engine's
+# parameters with the constructor's defaults, and configs/trackers/boosttrack.yaml (BoostTrack++), the defaults
+# create_tracker("boosttrack") starts from
+BOOSTTRACK_ENGINE_DEFAULTS = dict(min_box_area=10, aspect_ratio_thresh=1.6, lambda_iou=0.5, lambda_mhd=0.25,
+                                  lambda_shape=0.25, use_dlo_boost=True, use_duo_boost=True, dlo_boost_coef=0.65,
+                                  s_sim_corr=False, use_rich_s=False, use_sb=False, use_vt=False, with_reid=False,
+                                  det_thresh=0.3, max_age=30, min_hits=3, iou_threshold=0.3)
+BOOSTTRACK_YAML_DEFAULTS = dict(max_age=60, min_hits=3, det_thresh=0.6, iou_threshold=0.3, use_cmc=True, cmc_method="ecc",
+                                min_box_area=10, aspect_ratio_thresh=1.6, lambda_iou=0.5, lambda_mhd=0.25,
+                                lambda_shape=0.25, use_dlo_boost=True, use_duo_boost=True, dlo_boost_coef=0.65,
+                                s_sim_corr=False, use_rich_s=True, use_sb=True, use_vt=True, with_reid=True,
+                                adaptive_kf=False)
+
+
+class BoostTrack(_SingleStreamTracker):
+    """BoostTrack / BoostTrack++ on the GPU; arguments and defaults as boxmot/trackers/bbox/boosttrack/boosttrack.py:241-296
+    (BoostTrack++ is `use_rich_s=use_sb=use_vt=True`, configs/trackers/boosttrack.yaml).  Everything per frame runs on the
+    device: the XYHR Kalman filter, both confidence boosts, the cost (IoU, confidence-weighted IoU, Mahalanobis softmax,
+    shape, appearance), lapjv and the track lifecycle.  `use_cmc=True` estimates the camera warp with `cmc_method` "ecc"
+    or "sof" on the device from `img` on every frame; `update(..., warp=)` applies a warp obtained elsewhere.
+
+    As in the reference, ReID is on only with a model (`with_reid and reid_model is not None`); without one, supplied
+    `embs` are ignored.  A model with a `.b200reid` blob (`B200ReID`) embeds on the device; any other object with
+    `get_features` is called on every detection row.  Ids start at 1 per tracker (the reference's class-level counter
+    continues across instances).  Not implemented (NotImplementedError): `adaptive_kf=True`, OBB, `per_class=True`, and
+    class-specific Kalman noise (a non-empty `per_class_noise` registry, the counterpart of the reference's
+    `ConstantNoiseXYHR._per_class_noise`, empty by default)."""
+
+    _kind = "boosttrack"
+    per_class_noise: dict = {}
+
+    def __init__(self, reid_model: Any = None, use_cmc: bool = True, min_box_area: int = 10,
+                 aspect_ratio_thresh: float = 1.6, cmc_method: str = "ecc", lambda_iou: float = 0.5,
+                 lambda_mhd: float = 0.25, lambda_shape: float = 0.25, use_dlo_boost: bool = True,
+                 use_duo_boost: bool = True, dlo_boost_coef: float = 0.65, s_sim_corr: bool = False,
+                 use_rich_s: bool = False, use_sb: bool = False, use_vt: bool = False, with_reid: bool = False,
+                 adaptive_kf: bool = False, **kwargs: Any):
+        if adaptive_kf:
+            raise NotImplementedError("BoostTrack adaptive_kf=True (innovation-window process noise) is not implemented "
+                                      "on the B200 path")
+        ref = sys.modules.get("boxmot.motion.kalman_filters.xyhr")
+        if self.per_class_noise or (ref is not None and getattr(ref.ConstantNoiseXYHR, "_per_class_noise", None)):
+            raise NotImplementedError("class-specific Kalman noise (a non-empty per-class noise registry) is not "
+                                      "implemented for BoostTrack on the B200 path")
+        if use_cmc and cmc_method not in ("ecc", "sof"):
+            raise NotImplementedError(f"use_cmc=True with cmc_method='{cmc_method}': 'ecc' and 'sof' are estimated on the "
+                                      "device (pass use_cmc=False and supply the warp through update(..., warp=))")
+        with_reid = bool(with_reid) and reid_model is not None
+        super().__init__(reid_model=reid_model if with_reid else None, min_box_area=min_box_area,
+                         aspect_ratio_thresh=aspect_ratio_thresh, lambda_iou=lambda_iou, lambda_mhd=lambda_mhd,
+                         lambda_shape=lambda_shape, use_dlo_boost=use_dlo_boost, use_duo_boost=use_duo_boost,
+                         dlo_boost_coef=dlo_boost_coef, s_sim_corr=s_sim_corr, use_rich_s=use_rich_s, use_sb=use_sb,
+                         use_vt=use_vt, with_reid=with_reid, **kwargs)
+        self.use_cmc, self.cmc_method = bool(use_cmc), cmc_method
+        if use_cmc:
+            self._engine.set_cmc(cmc_method)
+
+
 def _flatten_yaml_defaults(node, acc=None):
     """`<param>: {default: ...}` entries of a reference tracker YAML, nested conditional parameters included
     (what `flatten_yaml_config` + `details["default"]` produce in tracker_zoo.py:112-119)."""
@@ -718,7 +808,8 @@ def resolve_tracker_args(tracker_type, tracker_config=None, evolve_param_dict=No
     import inspect
 
     kind = str(tracker_type).lower()
-    classes = {"bytetrack": ByteTrack, "botsort": BotSort, "deepocsort": DeepOcSort, "strongsort": StrongSort, "ocsort": OcSort}
+    classes = {"bytetrack": ByteTrack, "botsort": BotSort, "deepocsort": DeepOcSort, "strongsort": StrongSort, "ocsort": OcSort,
+               "boosttrack": BoostTrack}
     if kind not in classes:
         raise ValueError(f"Unknown tracker type: '{tracker_type}'. Available trackers are: {', '.join(classes)} "
                          "(the trackers that are part of the B200 hot path)")
@@ -730,7 +821,7 @@ def resolve_tracker_args(tracker_type, tracker_config=None, evolve_param_dict=No
         with open(tracker_config, "r", encoding="utf-8") as f:
             args = _flatten_yaml_defaults(yaml.safe_load(f) or {})
     else:
-        args = dict(TRACKER_DEFAULTS[kind])
+        args = dict(TRACKER_DEFAULTS[kind] if kind in TRACKER_DEFAULTS else BOOSTTRACK_YAML_DEFAULTS)
     args.update(overrides or {})
     cls = classes[kind]
     accepted = set(inspect.signature(cls.__init__).parameters) | set(
@@ -753,6 +844,9 @@ def resolve_tracker_args(tracker_type, tracker_config=None, evolve_param_dict=No
                       f"({method if kind == 'botsort' else 'sof'}); this tracker is built with it off and applies a warp supplied "
                       "through update(..., warp=), without one it behaves as with CMC off -- call tracker.set_cmc('sof') "
                       "(BoT-SORT, DeepOCSORT) to estimate SOF on the device like the reference", stacklevel=3)
+    if kind == "boosttrack":   # both of its estimators run on the device: the configuration stays as it is
+        args.pop("per_class", None)
+        return kind, cls, args
     args.pop("cmc_method", None)
     if kind == "botsort":
         args["use_cmc"] = bot_ecc
@@ -773,7 +867,8 @@ def create_tracker(tracker_type, tracker_config=None, reid_weights=None, device=
     the four trackers of the path; `tracker_backend` "python" and "cpp" both resolve to this library.
 
     `reid_weights` may be a `.pt` state dict or a `.b200reid` blob; it is converted once and loaded on the GPU.
-    `**overrides` (an extension) are applied on top of the configuration.  CMC is always off (see BotSort)."""
+    `**overrides` (an extension) are applied on top of the configuration.  CMC: see `resolve_tracker_args` (BoostTrack keeps
+    its configuration's on-device estimator)."""
     kind, cls, args = resolve_tracker_args(tracker_type, tracker_config, evolve_param_dict, overrides)
     per_class = bool(per_class)
     if kind in ("bytetrack", "ocsort"):   # motion-only trackers: no ReID backend (tracker_zoo.py:124-130)

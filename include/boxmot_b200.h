@@ -114,6 +114,7 @@ BOXMOT_B200_API const char* boxmot_botsort_last_error(void);
 #define BOXMOT_B200_TRACKER_BOTSORT 1
 #define BOXMOT_B200_TRACKER_DEEPOCSORT 2
 #define BOXMOT_B200_TRACKER_STRONGSORT 3
+#define BOXMOT_B200_TRACKER_BOOSTTRACK 4
 
 /* Every parameter of the reference Python constructors (bytetrack.py:226-257, botsort.py:66-118), in
  * double precision so thresholds compare exactly as python floats do. */
@@ -164,6 +165,20 @@ typedef struct BoxMOTB200TrackerConfig {
     /* crop staging of the on-device ReID (reid/core/preprocessing.py): 0 = "resize" (the Python default), 1 = "resize_pad"
      * (aspect-preserving resize + ImageNet-mean border, the native default when the name is NULL) */
     int reid_preprocess;
+    /* BoostTrack / BoostTrack++ (trackers/bbox/boosttrack/boosttrack.py:241-296; det_thresh, max_age, min_hits,
+     * iou_threshold and with_reid above are shared); ignored by the other trackers */
+    int use_dlo_boost;
+    int use_duo_boost;
+    int use_rich_s;
+    int use_sb;
+    int use_vt;
+    int s_sim_corr;
+    double dlo_boost_coef;
+    double lambda_iou;
+    double lambda_mhd;
+    double lambda_shape;
+    double min_box_area;
+    double aspect_ratio_thresh;
 } BoxMOTB200TrackerConfig;
 
 typedef struct BoxMOTB200Tracker BoxMOTB200Tracker;
@@ -211,7 +226,8 @@ BOXMOT_B200_API int boxmot_b200_tracker_last_device_ms(BoxMOTB200Tracker* handle
  * (trackers/bbox/botsort/botsort_track.py:117-132); StrongSORT through Track.camera_update
  * (trackers/bbox/strongsort/sort/track.py:139-148; without a supplied warp it runs with the identity, as the
  * reference does whenever tracks exist); DeepOCSORT through KalmanBoxTracker.apply_affine_correction before the
- * predict step (trackers/bbox/deepocsort/deepocsort.py:189-206, 345-348; motion/kalman_filters/xysr.py:311-366).
+ * predict step (trackers/bbox/deepocsort/deepocsort.py:189-206, 345-348; motion/kalman_filters/xysr.py:311-366);
+ * BoostTrack through KalmanBoxTracker.camera_update before the predict step (boosttrack.py:132-172, 318-321).
  * A supplied warp is how the estimators that are not built on the device (sof, orb, sift) reach the trackers. */
 BOXMOT_B200_API int boxmot_b200_tracker_set_warp(BoxMOTB200Tracker* handle, int stream, const double* warp2x3);
 /* Camera-motion ESTIMATION on the device, every frame, from the frame passed to update (SURVEY 8f-3): method "ecc" is
@@ -221,8 +237,9 @@ BOXMOT_B200_API int boxmot_b200_tracker_set_warp(BoxMOTB200Tracker* handle, int 
  * cmc_method="ecc" (trackers/bbox/botsort/botsort.py:78,116-117,142) -- BoT-SORT and StrongSORT handles.  Method "sof"
  * is the reference's SOF estimator with its defaults (boxmot/motion/cmc/sof.py; as boxmot_b200_cmc_sof_*) on every
  * frame, with the detection boxes the reference masks: every row for BoT-SORT (botsort.py:301), the rows with
- * conf > det_thresh for DeepOCSORT (deepocsort.py:330-349) -- BoT-SORT and DeepOCSORT handles.  "none" / "" / NULL
- * turns it off again.  The estimate replaces a warp supplied for the same frame; reset restarts the estimator. */
+ * conf > det_thresh for DeepOCSORT (deepocsort.py:330-349) -- BoT-SORT and DeepOCSORT handles.  BoostTrack handles
+ * take both, run the estimator on every frame with every detection row (boosttrack.py:318-321) and apply its result --
+ * the identity when it returns none -- to every track.  "none" / "" / NULL turns it off again.  The estimate replaces a warp supplied for the same frame; reset restarts the estimator. */
 BOXMOT_B200_API int boxmot_b200_tracker_set_cmc(BoxMOTB200Tracker* handle, const char* method);
 /* Device timing on the handle's own CUDA stream: record mark 0 / mark 1 around a region, then read the elapsed
  * milliseconds (synchronises on mark 1). */
