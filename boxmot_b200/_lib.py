@@ -17,6 +17,7 @@ TRACKER_BOTSORT = 1
 TRACKER_DEEPOCSORT = 2
 TRACKER_STRONGSORT = 3
 TRACKER_BOOSTTRACK = 4
+TRACKER_OCCLUBOOST = 5
 
 
 class BoxMOTByteTrackConfig(ctypes.Structure):
@@ -51,7 +52,15 @@ class BoxMOTB200TrackerConfig(ctypes.Structure):
                 ("use_dlo_boost", c_int), ("use_duo_boost", c_int), ("use_rich_s", c_int), ("use_sb", c_int),
                 ("use_vt", c_int), ("s_sim_corr", c_int), ("dlo_boost_coef", c_double), ("lambda_iou", c_double),
                 ("lambda_mhd", c_double), ("lambda_shape", c_double), ("min_box_area", c_double),
-                ("aspect_ratio_thresh", c_double)]
+                ("aspect_ratio_thresh", c_double),
+                ("use_second_pass", c_int), ("recovery_max_age", c_int), ("second_pass_max_age", c_int),
+                ("second_pass_min_hits", c_int), ("confirm_hits", c_int), ("tentative_max_age", c_int),
+                ("ams_enabled", c_int), ("ams_buffer_size", c_int), ("gta_enabled", c_int),
+                ("gta_min_track_length", c_int), ("gta_max_gap", c_int), ("lambda_emb_multiplier", c_double),
+                ("recovery_appearance_thresh", c_double), ("recovery_iou_thresh", c_double), ("feat_alpha", c_double),
+                ("second_iou_thresh", c_double), ("second_appearance_thresh", c_double),
+                ("instant_confirm_thresh", c_double), ("duplicate_iou_thresh", c_double), ("ams_alpha0", c_double),
+                ("ams_threshold", c_double), ("ams_shrink_ratio", c_double), ("gta_appearance_thresh", c_double)]
 
 
 # every symbol include/boxmot_b200.h declares: name -> (restype, argtypes)
@@ -93,6 +102,7 @@ SYMBOLS = {
     "boxmot_b200_tracker_snapshot": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int,
                                              POINTER(c_int)]),
     "boxmot_b200_tracker_track_ids": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, POINTER(c_int)]),
+    "boxmot_b200_tracker_gta_events": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, POINTER(c_int)]),
     "boxmot_b200_tracker_last_launches": (c_int, [c_void_p, POINTER(c_int)]),
     "boxmot_b200_tracker_last_device_ms": (c_int, [c_void_p, POINTER(c_double), POINTER(c_double)]),
     "boxmot_b200_tracker_set_warp": (c_int, [c_void_p, c_int, c_void_p]),

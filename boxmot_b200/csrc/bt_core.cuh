@@ -128,9 +128,10 @@ BMB_FN void bt_predict(double* x, double* P) {
     bt_enforce(x, P);
 }
 
-// KalmanFilterXYHR.update (xyhr.py:339-377): plain Cholesky of S = H P H^T + R, K = P H^T S^-1, x += K (z - Hx),
-// P -= K S K^T, geometry clamp + symmetrise
-BMB_FN void bt_kf_update(double* x, double* P, const double* z) {
+// KalmanFilterXYHR.update (xyhr.py:339-377): plain Cholesky of S = H P H^T + R, K = P H^T S^-1,
+// x += alpha * (K (z - Hx)), P -= K S K^T, geometry clamp + symmetrise.  alpha is OccluBoost's abnormal-motion gain
+// factor; BoostTrack passes 1.0, and x + 1.0 * v is x + v bit for bit.
+BMB_FN void bt_kf_update(double* x, double* P, const double* z, double alpha) {
     const double Rd[4] = {1.0, 1.0, 10.0, 0.01};
     double m[4] = {z[0], z[1], py_max(z[2], 1e-4), py_max(z[3], 1e-4)};
     double S[16], Lc[16];
@@ -168,7 +169,7 @@ BMB_FN void bt_kf_update(double* x, double* P, const double* z) {
     for (int r = 0; r < 8; ++r) {
         double acc = 0.0;
         for (int i = 0; i < 4; ++i) acc += yv[i] * K[r * 4 + i];
-        x[r] = x[r] + acc;
+        x[r] = x[r] + alpha * acc;
     }
     double KS[32];
     for (int r = 0; r < 8; ++r)
@@ -264,21 +265,29 @@ BMB_FN double bt_mh_sim(const BtStream& s, int i, int row, int k, int LD) {
     return s.md[(size_t)row * LD + k] > BT_MH_LIMIT ? 0.0 : s.ex[(size_t)i * LD + k] / s.colsum[k];
 }
 
-BMB_FN void bt_frame(const BtCfg& c, BtStream& s) {
-    const int CT = c.cap_tracks, CD = c.cap_dets, F = c.feat_dim;
-    const int LD = CT;
-    const int LD2 = CT > CD ? CT : CD;
-    int* mb = s.free_l;
-    int* free_slots = s.free_l + MB_COUNT;
+// What the phases of one frame hand to each other.  t_prev carries the phase clock (BMB_PHASE) across them.
+struct BtFrame {
+    int D, T, frame, nk, n_und, n_ufail;
+    bool use_emb;
+    long long _t_prev;
+};
+
+// ---- camera_update on every track, then predict (boosttrack.py:318-331); IoU and Mahalanobis distance of every row
+// against every track (get_mh_dist_matrix) ----
+BMB_FN BtFrame bt_predict_phase(const BtCfg& c, BtStream& s) {
+    const int CD = c.cap_dets;
+    const int LD = c.cap_tracks;
+    BtFrame f{};
     int D = *s.n_dets;
     if (D > CD) { if (BMB_TID == 0) s.scalars[SC_ERROR] = ERR_DET_CAPACITY; D = CD; }
-    const int frame = s.scalars[SC_FRAME] + 1;
-    const int T = s.scalars[SC_N_ACTIVE];
-    const bool use_emb = c.with_reid && s.embs != nullptr;
-    long long _t_prev = BMB_CLOCK();   // phase clocks: 0 camera update + predict, 1 matrices, 2 boosts, 3 cost + match,
-    BMB_SYNC();                        // 4 updates, 5 births, 6 emit + cull
+    f.D = D;
+    f.frame = s.scalars[SC_FRAME] + 1;
+    const int T = f.T = s.scalars[SC_N_ACTIVE];
+    f.use_emb = c.with_reid && s.embs != nullptr;
+    long long& _t_prev = f._t_prev;   // phase clocks: 0 camera update + predict, 1 matrices, 2 boosts, 3 cost + match,
+    _t_prev = BMB_CLOCK();            // 4 updates, 5 births, 6 emit + cull
+    BMB_SYNC();
 
-    // ---- camera_update on every track, then predict (boosttrack.py:318-331) ----
     const bool warp_pending = s.warp != nullptr && s.warp[6] != 0.0;
     const double ident[6] = {1.0, 0.0, 0.0, 0.0, 1.0, 0.0};
     const double* W = warp_pending ? s.warp : ident;
@@ -300,7 +309,6 @@ BMB_FN void bt_frame(const BtCfg& c, BtStream& s) {
     BMB_SYNC();
     BMB_PHASE(0);
 
-    // ---- IoU and Mahalanobis distance of every row against every track (get_mh_dist_matrix) ----
     for (int e = BMB_TID; e < D * T; e += BMB_NT) {
         const int d = e / T, k = e - d * T;
         const float* r = s.dets + d * 6;
@@ -320,8 +328,17 @@ BMB_FN void bt_frame(const BtCfg& c, BtStream& s) {
     }
     BMB_SYNC();
     BMB_PHASE(1);
+    return f;
+}
 
-    // ---- DLO boost (boosttrack.py:489-529) over every row ----
+// ---- DLO boost (boosttrack.py:489-529) over every row, then the DUO boost (boosttrack.py:447-487): far from every
+// track and below the threshold, boosted unless a more confident candidate overlaps it; then the survivors
+// conf >= det_thresh ----
+BMB_FN void bt_boost_phase(const BtCfg& c, BtStream& s, BtFrame& f) {
+    const int LD = c.cap_tracks;
+    const int D = f.D, T = f.T;
+    int* mb = s.free_l;
+    long long& _t_prev = f._t_prev;
     if (c.use_dlo && D > 0 && T > 0) {
         if (c.rich_s) bt_mh_softmax(s, D, T, LD, [](int i) { return i; });
         for (int d = BMB_TID; d < D; d += BMB_NT) {
@@ -348,8 +365,6 @@ BMB_FN void bt_frame(const BtCfg& c, BtStream& s) {
         }
         BMB_SYNC();
     }
-    // ---- DUO boost (boosttrack.py:447-487): far from every track and below the threshold, boosted unless a more
-    // confident candidate overlaps it ----
     if (c.use_duo && D > 0 && T > 0) {
         if (BMB_WARP == 0) {
             const int n = warp_append(D, s.cand, 0, [&](int d) {
@@ -387,24 +402,35 @@ BMB_FN void bt_frame(const BtCfg& c, BtStream& s) {
             if (s.flag[i]) s.rconf[s.cand[i]] = c.det_thresh + 1e-4;
         BMB_SYNC();
     }
-    // ---- survivors: conf >= det_thresh ----
     if (BMB_WARP == 0) {
         const int n = warp_append(D, s.kdet, 0, [&](int d) { return s.rconf[d] >= c.det_thresh; }, [&](int d) { return d; });
         if (BMB_LANE == 0) mb[1] = n;
     }
     BMB_SYNC();
-    const int nk = mb[1];
+    f.nk = mb[1];
     BMB_PHASE(2);
+}
 
-    // ---- association (assoc.py:156-201, 106-153) ----
-    int n_und = 0;
+// ---- association (assoc.py:156-201, 106-153) with lambda_emb = (1 + l_iou + l_shape + l_mhd) * lambda_emb_mult.
+// mrow[i]: matched track position of survivor i or -1; und[0..n_und): unmatched survivors (unmatched ascending, then
+// the matches that fail the validity test, in row order); tmp_b[0..n_ufail): the track positions of those failed
+// matches, in the same order (the tail of the reference's unmatched_trks) ----
+BMB_FN void bt_match_phase(const BtCfg& c, BtStream& s, BtFrame& f, double lambda_emb_mult) {
+    const int CT = c.cap_tracks;
+    const int LD = CT;
+    const int LD2 = CT > c.cap_dets ? CT : c.cap_dets;
+    const int T = f.T, nk = f.nk;
+    const bool use_emb = f.use_emb;
+    int* mb = s.free_l;
+    long long& _t_prev = f._t_prev;
+    int n_und = 0, n_ufail = 0;
     if (T == 0 || nk == 0) {
         for (int i = BMB_TID; i < nk; i += BMB_NT) { s.mrow[i] = -1; s.und[i] = i; }
         n_und = nk;
         BMB_SYNC();
     } else {
         bt_mh_softmax(s, nk, T, LD, [&](int i) { return s.kdet[i]; });
-        const double lambda_emb = (((1 + c.lambda_iou) + c.lambda_shape) + c.lambda_mhd) * 1.5;
+        const double lambda_emb = (((1 + c.lambda_iou) + c.lambda_shape) + c.lambda_mhd) * lambda_emb_mult;
         auto cost_at = [&](int i, int k) {
             const int d = s.kdet[i];
             const float* r = s.dets + d * 6;
@@ -467,22 +493,36 @@ BMB_FN void bt_frame(const BtCfg& c, BtStream& s) {
                 const double io = s.iou[(size_t)d * LD + k];
                 const bool ok = io >= c.iou_threshold ||
                                 (use_emb && io >= c.iou_threshold / 2 && s.embq[(size_t)d * CT + s.tracks[k]] >= 0.75);
-                if (!ok) { s.und[n_und++] = i; s.mrow[i] = -1; }
+                if (!ok) { s.und[n_und++] = i; s.tmp_b[n_ufail++] = k; s.mrow[i] = -1; }
             }
             mb[4] = n_und;
+            mb[8] = n_ufail;
         }
         BMB_SYNC();
         n_und = mb[4];
+        n_ufail = mb[8];
+        BMB_SYNC();
     }
+    f.n_und = n_und;
+    f.n_ufail = n_ufail;
     BMB_PHASE(3);
+}
 
-    // ---- updates of the matched tracks (boosttrack.py:378-387) ----
+// ---- BoostTrack's tail: updates of the matched tracks (boosttrack.py:378-387), births in unmatched order
+// (389-393), emit in list order with the aspect / area filter (395-421), cull ----
+BMB_FN void bt_tail_phase(const BtCfg& c, BtStream& s, BtFrame& f) {
+    const int CT = c.cap_tracks, CD = c.cap_dets, F = c.feat_dim;
+    const int T = f.T, nk = f.nk, n_und = f.n_und, frame = f.frame;
+    const bool use_emb = f.use_emb;
+    int* mb = s.free_l;
+    int* free_slots = s.free_l + MB_COUNT;
+    long long& _t_prev = f._t_prev;
     for (int i = BMB_TID; i < nk; i += BMB_NT) {
         if (s.mrow[i] < 0) continue;
         const int t = s.tracks[s.mrow[i]], d = s.kdet[i];
         s.tsu[t] = 0;
         s.hit_streak[t] += 1;
-        bt_kf_update(s.x + t * 8, s.P + t * 64, s.dz + d * 4);
+        bt_kf_update(s.x + t * 8, s.P + t * 64, s.dz + d * 4, 1.0);
         s.conf[t] = s.rconf[d];
         s.cls[t] = (double)s.dets[d * 6 + 5];
         s.det_ind[t] = (double)d;
@@ -591,6 +631,14 @@ BMB_FN void bt_frame(const BtCfg& c, BtStream& s) {
     }
     BMB_SYNC();
     BMB_PHASE(6);
+}
+
+
+BMB_FN void bt_frame(const BtCfg& c, BtStream& s) {
+    BtFrame f = bt_predict_phase(c, s);
+    bt_boost_phase(c, s, f);
+    bt_match_phase(c, s, f, 1.5);
+    bt_tail_phase(c, s, f);
 }
 
 }  // namespace bmb

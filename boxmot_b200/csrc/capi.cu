@@ -135,6 +135,13 @@ int boxmot_b200_tracker_track_ids(BoxMOTB200Tracker* h, int stream, int which, i
         if (out_count) *out_count = n;
     });
 }
+int boxmot_b200_tracker_gta_events(BoxMOTB200Tracker* h, int stream, int clear_graveyard, double* events, int capacity,
+                                   int* out_count) {
+    return guard([&] {
+        int n = as_engine(h)->gta_events(stream, clear_graveyard, events, capacity);
+        if (out_count) *out_count = n;
+    });
+}
 int boxmot_b200_tracker_last_launches(BoxMOTB200Tracker* h, int* out_launches) {
     return guard([&] { *out_launches = as_engine(h)->launches; });
 }

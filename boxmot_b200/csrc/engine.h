@@ -13,6 +13,7 @@
 #include "docs_core.cuh"
 #include "ss_core.cuh"
 #include "bt_core.cuh"
+#include "ob_core.cuh"
 
 namespace bmb {
 
@@ -71,6 +72,10 @@ struct Engine {
     BtCfg btcfg{};
     BtStream* d_bt = nullptr;
     std::vector<BtStream> h_bt;
+    bool is_ob = false;                // OccluBoost engine (ob_core.cuh): is_bt too, d_bt / h_bt hold its BoostTrack part
+    ObCfg obcfg{};
+    ObStream* d_ob = nullptr;
+    std::vector<ObStream> h_ob;
     double* d_conf_pow = nullptr;      // 0.9 ** k, k = 0 .. max_age + 1 (KalmanBoxTracker.get_confidence)
     std::vector<float*> out_ptr;       // per-stream output rows / scalars / timers (either family)
     std::vector<int*> scalars_ptr;
@@ -131,6 +136,7 @@ struct Engine {
     DocsStream* d_docs_alt = nullptr;
     SsStream* d_ss_alt = nullptr;
     BtStream* d_bt_alt = nullptr;
+    ObStream* d_ob_alt = nullptr;
     cudaEvent_t ev_reid_done[2]{};
     cudaEvent_t ev_assoc_done[2]{};
     int pipe_parity = 0;
@@ -153,6 +159,7 @@ struct Engine {
     void fetch(float* const* out, const int* out_cap, int* out_rows);
     int snapshot(int stream_index, int* ids, double* means, double* covs, int cap);
     int track_ids(int stream_index, int which, int* ids, int cap);
+    int gta_events(int stream_index, int clear_graveyard, double* events, int cap);
     void set_warp(int stream_index, const double* warp6);
     void set_cmc(const char* method);   // "ecc" | "sof" | "none" / "" / NULL
     void read_timers(int stream_index, long long* out16, bool reset);
@@ -171,7 +178,7 @@ struct Engine {
     void enqueue_association(TrkStream* streams_dev, const float* embs_src);
     void enqueue_crops(int parity, cudaStream_t st);            // crop list of the family, from input set `parity`
     void enqueue_family_association(int parity);                // association launches of the family on `stream`
-    void enqueue_bt(BtStream* streams_dev);                      // BoostTrack: embedding cost + frame kernel
+    void enqueue_bt(BtStream* streams_dev, ObStream* ob_dev);    // BoostTrack / OccluBoost: embedding cost + frame kernel
     int run_reid(cudaStream_t main_stream, const uint8_t* images_dev, int rows, int cols, int total, float* embs_out);
     void enqueue_fetch();
     void finish_fetch(float* const* out, const int* out_cap, int* out_rows);

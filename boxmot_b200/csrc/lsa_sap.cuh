@@ -17,6 +17,33 @@
 
 namespace bmb {
 
+template <typename S>
+BMB_FN void lsa_solve(S& s, const double* cost, int nr, int nc, int ld);
+
+// scipy.optimize.linear_sum_assignment(cost) of an R x C matrix given by cost_at(r, c): scipy solves the transpose when
+// C < R.  buf receives the laid-out problem (min(R, C) x max(R, C), leading dimension max(R, C)); rowcol[r] is the
+// column assigned to row r, or -1.  Called by the whole CTA.
+template <typename S, typename CostAt>
+BMB_FN void lsa_rect(S& s, double* buf, int R, int C, CostAt cost_at, int* rowcol) {
+    const bool transposed = C < R;
+    const int nr = transposed ? C : R, nc = transposed ? R : C;
+    for (int e = BMB_TID; e < R * C; e += BMB_NT) {
+        const int r = e / C, cc = e - r * C;
+        buf[transposed ? (size_t)cc * nc + r : (size_t)r * nc + cc] = cost_at(r, cc);
+    }
+    BMB_SYNC();
+    lsa_solve(s, buf, nr, nc, nc);
+    for (int r = BMB_TID; r < R; r += BMB_NT) rowcol[r] = -1;
+    BMB_SYNC();
+    for (int i = BMB_TID; i < nr; i += BMB_NT) {
+        const int j = s.lsa_col4row[i];
+        if (j < 0) continue;
+        if (transposed) rowcol[j] = i;
+        else rowcol[i] = j;
+    }
+    BMB_SYNC();
+}
+
 // S provides lsa_u [>=nr], lsa_v, lsa_spc [>=nc] (double) and lsa_path, lsa_row4col, lsa_rem, lsa_sc [>=nc],
 // lsa_col4row, lsa_sr [>=nr] (int).  cost is row-major (nr x nc, leading dimension ld), nr <= nc, finite.
 // Result: lsa_col4row[i] for every row.  Called by the whole CTA.

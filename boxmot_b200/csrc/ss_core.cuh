@@ -298,26 +298,17 @@ template <typename CostAt, typename ColVal>
 BMB_FN void ss_match_stage(SsStream& s, int R, int C, double max_distance, CostAt cost_at, ColVal col_val,
                            int* und_out, int* mb, int mb_slot) {
     const bool transposed = C < R;
-    const int nr = transposed ? C : R, nc = transposed ? R : C;
+    const int nc = transposed ? R : C;
     const double clipv = max_distance + 1e-5;
-    for (int e = BMB_TID; e < R * C; e += BMB_NT) {
-        const int r = e / C, cc = e - r * C;
-        double v = cost_at(r, cc);
-        if (v > max_distance) v = clipv;
-        s.cost[transposed ? (size_t)cc * nc + r : (size_t)r * nc + cc] = v;
-    }
-    BMB_SYNC();
-    lsa_solve(s, s.cost, nr, nc, nc);
-    for (int r = BMB_TID; r < R; r += BMB_NT) s.rowcol[r] = -1;
+    // raw assignment (clipped pairs included) in original orientation
+    lsa_rect(s, s.cost, R, C, [&](int r, int cc) {
+        const double v = cost_at(r, cc);
+        return v > max_distance ? clipv : v;
+    }, s.rowcol);
     for (int cc = BMB_TID; cc < C; cc += BMB_NT) s.colrow[cc] = -1;
     BMB_SYNC();
-    // raw assignment (clipped pairs included) in original orientation
-    for (int i = BMB_TID; i < nr; i += BMB_NT) {
-        const int j = s.lsa_col4row[i];
-        if (j < 0) continue;
-        if (transposed) { s.rowcol[j] = i; s.colrow[i] = j; }
-        else { s.rowcol[i] = j; s.colrow[j] = i; }
-    }
+    for (int r = BMB_TID; r < R; r += BMB_NT)
+        if (s.rowcol[r] >= 0) s.colrow[s.rowcol[r]] = r;
     BMB_SYNC();
     if (BMB_WARP == 0) {
         int n = warp_append(C, und_out, 0, [&](int cc) { return s.colrow[cc] < 0; }, col_val);

@@ -268,6 +268,27 @@ __global__ void __launch_bounds__(256) k_bt_frame(const BtCfg cfg, BtStream* str
     bt_frame(cfg, s);
 }
 
+// OccluBoost: the BoostTrack phases with lapjv's scratch in shared memory as k_bt_frame, then its own passes
+__global__ void __launch_bounds__(256) k_ob_frame(const ObCfg cfg, ObStream* streams, int jv_in_smem) {
+    extern __shared__ __align__(16) unsigned char dyn_smem[];
+    ObStream s = streams[blockIdx.x];
+    s.b.jv_wide = jv_in_smem >> 1;
+    if (jv_in_smem & 1) {
+        const int MX = cfg.bt.cap_tracks > cfg.bt.cap_dets ? cfg.bt.cap_tracks : cfg.bt.cap_dets;
+        double* pd = reinterpret_cast<double*>(dyn_smem);
+        s.b.lap_v = pd; pd += MX;
+        s.b.lap_spc = pd; pd += MX;
+        int* pi = reinterpret_cast<int*>(pd);
+        s.b.lap_x = pi; pi += MX;
+        s.b.lap_y = pi; pi += MX;
+        s.b.lap_path = pi; pi += MX;
+        s.b.lap_tl = pi; pi += MX;
+        s.b.lap_sc = pi; pi += MX;
+        s.b.lap_insc = pi;
+    }
+    ob_frame(cfg, s);
+}
+
 // DeepOCSORT embeds every detection above det_thresh (deepocsort.py:333-343)
 // ordered (stream, detection) crop list built by one warp with ballot compaction
 template <typename Keep>
@@ -379,11 +400,12 @@ void Engine::construct(const BoxMOTB200TrackerConfig& p) {
     if (p.cap_tracks < 8 || p.cap_dets < 1) throw std::runtime_error("cap_tracks >= 8 and cap_dets >= 1 required");
     if (p.tracker != BOXMOT_B200_TRACKER_BOTSORT && p.tracker != BOXMOT_B200_TRACKER_BYTETRACK &&
         p.tracker != BOXMOT_B200_TRACKER_DEEPOCSORT && p.tracker != BOXMOT_B200_TRACKER_STRONGSORT &&
-        p.tracker != BOXMOT_B200_TRACKER_BOOSTTRACK)
+        p.tracker != BOXMOT_B200_TRACKER_BOOSTTRACK && p.tracker != BOXMOT_B200_TRACKER_OCCLUBOOST)
         throw std::runtime_error("unknown tracker kind");
     is_docs = p.tracker == BOXMOT_B200_TRACKER_DEEPOCSORT;
     is_ss = p.tracker == BOXMOT_B200_TRACKER_STRONGSORT;
-    is_bt = p.tracker == BOXMOT_B200_TRACKER_BOOSTTRACK;
+    is_ob = p.tracker == BOXMOT_B200_TRACKER_OCCLUBOOST;
+    is_bt = p.tracker == BOXMOT_B200_TRACKER_BOOSTTRACK || is_ob;   // OccluBoost runs on the BoostTrack stream
     if (p.tracker == BOXMOT_B200_TRACKER_BOTSORT && p.removed_stracks_buffer < 1)
         throw std::runtime_error("removed_stracks_buffer must be >= 1");
     int ndev = 0;
@@ -443,12 +465,36 @@ void Engine::construct(const BoxMOTB200TrackerConfig& p) {
     }
     if (is_docs) dcfg.feat_dim = cfg.feat_dim;
     if (is_bt) btcfg.feat_dim = cfg.feat_dim;
+    if (is_ob) {
+        if (p.confirm_hits < 1 || p.tentative_max_age < 0 || p.ams_buffer_size < 2 || p.ams_buffer_size > 4096 ||
+            p.gta_min_track_length < 1 || p.gta_max_gap < 1)
+            throw std::runtime_error("OccluBoost needs confirm_hits >= 1, tentative_max_age >= 0, ams_buffer_size in "
+                                     "[2, 4096], gta_min_track_length >= 1 and gta_max_gap >= 1");
+        obcfg.bt = btcfg;
+        obcfg.use_second_pass = p.use_second_pass ? 1 : 0;
+        obcfg.recovery_max_age = p.recovery_max_age; obcfg.second_pass_max_age = p.second_pass_max_age;
+        obcfg.second_pass_min_hits = p.second_pass_min_hits; obcfg.confirm_hits = p.confirm_hits;
+        obcfg.tentative_max_age = p.tentative_max_age;
+        obcfg.ams_on = p.ams_enabled && p.ams_alpha0 < 1.0;   // occluboost.py:791: alpha0 >= 1 never damps nor records
+        obcfg.ams_buffer_size = p.ams_buffer_size;
+        obcfg.gta = p.gta_enabled && btcfg.with_reid;
+        obcfg.gta_min_track_length = p.gta_min_track_length; obcfg.gta_max_gap = p.gta_max_gap;
+        obcfg.lambda_emb_mult = p.lambda_emb_multiplier;
+        obcfg.recovery_appearance_thresh = p.recovery_appearance_thresh; obcfg.recovery_iou_thresh = p.recovery_iou_thresh;
+        obcfg.feat_alpha = p.feat_alpha; obcfg.track_low_thresh = p.track_low_thresh;
+        obcfg.second_iou_thresh = p.second_iou_thresh; obcfg.second_appearance_thresh = p.second_appearance_thresh;
+        obcfg.new_track_thresh = p.new_track_thresh; obcfg.instant_confirm_thresh = p.instant_confirm_thresh;
+        obcfg.duplicate_iou_thresh = p.duplicate_iou_thresh; obcfg.ams_alpha0 = p.ams_alpha0;
+        obcfg.ams_threshold = p.ams_threshold; obcfg.ams_shrink_ratio = p.ams_shrink_ratio;
+        obcfg.gta_appearance_thresh = p.gta_appearance_thresh;
+    }
     if (is_ss) {
         scfg.feat_dim = cfg.feat_dim;
         if (scfg.feat_dim % 4) throw std::runtime_error("StrongSORT feat_dim must be a multiple of 4");
     }
     stream_bytes = is_docs ? carve_docs(dcfg, nullptr, nullptr, &persistent_bytes)
                  : is_ss   ? carve_ss(scfg, nullptr, nullptr, &persistent_bytes)
+                 : is_ob   ? carve_ob(obcfg, nullptr, nullptr, &persistent_bytes)
                  : is_bt   ? carve_bt(btcfg, nullptr, nullptr, &persistent_bytes)
                            : carve_stream(cfg, nullptr, nullptr, &persistent_bytes);
     persistent_bytes = (persistent_bytes + 15) & ~(size_t)15;
@@ -492,9 +538,16 @@ void Engine::construct(const BoxMOTB200TrackerConfig& p) {
         CUDA_OK(cudaMemcpy(d_conf_pow, pw.data(), sizeof(double) * pw.size(), cudaMemcpyHostToDevice));
         btcfg.conf_pow = d_conf_pow;
         btcfg.n_conf_pow = (int)pw.size();
+        obcfg.bt = btcfg;
         h_bt.resize(S);
+        if (is_ob) h_ob.resize(S);
         for (int i = 0; i < S; ++i) {
-            carve_bt(btcfg, d_mem + stream_bytes * i, &h_bt[i], nullptr);
+            if (is_ob) {
+                carve_ob(obcfg, d_mem + stream_bytes * i, &h_ob[i], nullptr);
+                h_bt[i] = h_ob[i].b;
+            } else {
+                carve_bt(btcfg, d_mem + stream_bytes * i, &h_bt[i], nullptr);
+            }
             h_bt[i].dets = d_dets + (size_t)i * CD * 6;
             h_bt[i].n_dets = d_ndets + i;
             h_bt[i].embs = cfg.with_reid ? d_embs + (size_t)i * CD * F : nullptr;
@@ -503,6 +556,11 @@ void Engine::construct(const BoxMOTB200TrackerConfig& p) {
         }
         CUDA_OK(cudaMalloc(&d_bt, sizeof(BtStream) * S));
         CUDA_OK(cudaMemcpy(d_bt, h_bt.data(), sizeof(BtStream) * S, cudaMemcpyHostToDevice));
+        if (is_ob) {
+            for (int i = 0; i < S; ++i) h_ob[i].b = h_bt[i];
+            CUDA_OK(cudaMalloc(&d_ob, sizeof(ObStream) * S));
+            CUDA_OK(cudaMemcpy(d_ob, h_ob.data(), sizeof(ObStream) * S, cudaMemcpyHostToDevice));
+        }
     } else if (is_docs) {
         h_docs.resize(S);
         for (int i = 0; i < S; ++i) {
@@ -553,6 +611,12 @@ void Engine::construct(const BoxMOTB200TrackerConfig& p) {
             }
             CUDA_OK(cudaMalloc(&d_bt_alt, sizeof(BtStream) * S));
             CUDA_OK(cudaMemcpy(d_bt_alt, alt.data(), sizeof(BtStream) * S, cudaMemcpyHostToDevice));
+            if (is_ob) {
+                std::vector<ObStream> alt_ob = h_ob;
+                for (int i = 0; i < S; ++i) alt_ob[i].b = alt[i];
+                CUDA_OK(cudaMalloc(&d_ob_alt, sizeof(ObStream) * S));
+                CUDA_OK(cudaMemcpy(d_ob_alt, alt_ob.data(), sizeof(ObStream) * S, cudaMemcpyHostToDevice));
+            }
         } else if (is_docs) {
             std::vector<DocsStream> alt = h_docs;
             for (int i = 0; i < S; ++i) {
@@ -626,13 +690,13 @@ void Engine::release() {
             if (ev_assoc_done[k]) cudaEventDestroy(ev_assoc_done[k]);
         }
         cudaFree(d_dets_alt); cudaFree(d_ndets_alt); cudaFree(d_embs_alt); cudaFree(d_streams_alt);
-        cudaFree(d_docs_alt); cudaFree(d_ss_alt); cudaFree(d_bt_alt);
+        cudaFree(d_docs_alt); cudaFree(d_ss_alt); cudaFree(d_bt_alt); cudaFree(d_ob_alt);
     }
     if (reid) reid_free(reid);
     cudaFree(d_cmc_prev); cudaFree(d_cmc_cur); cudaFree(d_cmc_has_prev); cudaFree(d_cmc_gate);
     if (sof) sof_state_free(sof);
     cudaFree(d_warp); cudaFree(d_mem); cudaFree(d_dets); cudaFree(d_ndets); cudaFree(d_embs); cudaFree(d_out);
-    cudaFree(d_scalars_out); cudaFree(d_streams); cudaFree(d_docs); cudaFree(d_ss); cudaFree(d_bt); cudaFree(d_conf_pow); cudaFree(d_crops); cudaFree(d_ncrops); cudaFree(d_images);
+    cudaFree(d_scalars_out); cudaFree(d_streams); cudaFree(d_docs); cudaFree(d_ss); cudaFree(d_bt); cudaFree(d_ob); cudaFree(d_conf_pow); cudaFree(d_crops); cudaFree(d_ncrops); cudaFree(d_images);
     cudaFreeHost(h_dets); cudaFreeHost(h_ndets); cudaFreeHost(h_out); cudaFreeHost(h_scalars);
     cudaFreeHost(h_embs); cudaFreeHost(h_images); cudaFreeHost(h_ndets_ring);
     if (mark[0]) cudaEventDestroy(mark[0]);
@@ -713,7 +777,7 @@ void Engine::enqueue_frame(const float* embs_dev, const uint8_t* images_dev, int
                                     cudaMemcpyDeviceToDevice, stream));
         }
         CUDA_OK(cudaEventRecord(ev[1], stream));
-        enqueue_bt(d_bt);
+        enqueue_bt(d_bt, d_ob);
         CUDA_OK(cudaGetLastError());
         CUDA_OK(cudaEventRecord(ev[2], stream));
         if (profile) {
@@ -812,7 +876,7 @@ void Engine::enqueue_family_association(int parity) {
             warp_dirty = false;
         }
     } else if (is_bt) {
-        enqueue_bt(parity ? d_bt_alt : d_bt);
+        enqueue_bt(parity ? d_bt_alt : d_bt, parity ? d_ob_alt : d_ob);
     } else if (is_docs) {
         DocsStream* ds = parity ? d_docs_alt : d_docs;
         if (cfg.with_reid) {
@@ -839,7 +903,7 @@ void Engine::enqueue_family_association(int parity) {
 
 // BoostTrack: embedding dot products (wide grid) and the per-stream frame kernel on `stream`; a supplied or estimated
 // warp applies to this frame only
-void Engine::enqueue_bt(BtStream* streams_dev) {
+void Engine::enqueue_bt(BtStream* streams_dev, ObStream* ob_dev) {
     BtCfg c = btcfg;
     c.cmc_every_frame = cmc_mode != 0;   // boosttrack.py:318-321: camera_update runs whenever an estimator exists
     if (cfg.with_reid) {
@@ -850,9 +914,18 @@ void Engine::enqueue_bt(BtStream* streams_dev) {
     const int MX = c.cap_tracks > c.cap_dets ? c.cap_tracks : c.cap_dets;
     const size_t jb = jv_smem_bytes(MX);
     const bool in_smem = jb <= 200 * 1024;
-    if (in_smem && jb > 48 * 1024)
-        CUDA_OK(cudaFuncSetAttribute(k_bt_frame, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)jb));
-    k_bt_frame<<<S, 256, in_smem ? jb : 0, stream>>>(c, streams_dev, (in_smem ? 1 : 0) | (jv_wide_default() << 1));
+    const int jv_arg = (in_smem ? 1 : 0) | (jv_wide_default() << 1);
+    if (is_ob) {
+        ObCfg oc = obcfg;
+        oc.bt = c;
+        if (in_smem && jb > 48 * 1024)
+            CUDA_OK(cudaFuncSetAttribute(k_ob_frame, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)jb));
+        k_ob_frame<<<S, 256, in_smem ? jb : 0, stream>>>(oc, ob_dev, jv_arg);
+    } else {
+        if (in_smem && jb > 48 * 1024)
+            CUDA_OK(cudaFuncSetAttribute(k_bt_frame, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)jb));
+        k_bt_frame<<<S, 256, in_smem ? jb : 0, stream>>>(c, streams_dev, jv_arg);
+    }
     ++launches;
     if (warp_dirty) {
         CUDA_OK(cudaMemsetAsync(d_warp, 0, sizeof(double) * 8 * S, stream));
@@ -1254,6 +1327,24 @@ int Engine::snapshot(int sidx, int* ids, double* means, double* covs, int cap) {
 // (BaseTracker attributes active_tracks / lost_stracks / removed_stracks, basetracker.py:386-390).  BoT-SORT's removed list
 // is its deque(maxlen=removed_stracks_buffer) oldest first; ByteTrack's unbounded list is kept as a per-slot flag, so it
 // comes back in slot order.  DeepOCSORT and StrongSORT keep a single list (the reference never fills the other two).
+// OccluBoost resurrection events of one stream (ob_core.cuh), taken and cleared; optionally the graveyard too
+int Engine::gta_events(int sidx, int clear_graveyard, double* events, int cap) {
+    if (!is_ob) throw std::runtime_error("GTA events exist on OccluBoost handles only");
+    if (sidx < 0 || sidx >= S) throw std::runtime_error("stream index out of range");
+    if (reid_stream) CUDA_OK(cudaStreamSynchronize(reid_stream));
+    CUDA_OK(cudaStreamSynchronize(stream));
+    const ObStream& s = h_ob[sidx];
+    int meta[2];
+    CUDA_OK(cudaMemcpy(meta, s.gv_meta, sizeof(meta), cudaMemcpyDeviceToHost));
+    if (meta[1] > cap) throw std::runtime_error("GTA event buffer too small");
+    if (meta[1] > 0) CUDA_OK(cudaMemcpy(events, s.ev, sizeof(double) * OB_EV * meta[1], cudaMemcpyDeviceToHost));
+    const int n = meta[1];
+    meta[1] = 0;
+    if (clear_graveyard) meta[0] = 0;
+    CUDA_OK(cudaMemcpy(s.gv_meta, meta, sizeof(meta), cudaMemcpyHostToDevice));
+    return n;
+}
+
 int Engine::track_ids(int sidx, int which, int* ids, int cap) {
     if (sidx < 0 || sidx >= S) throw std::runtime_error("stream index out of range");
     if (which < 0 || which > 2) throw std::runtime_error("list index must be 0 (active), 1 (lost) or 2 (removed)");

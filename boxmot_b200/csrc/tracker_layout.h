@@ -219,3 +219,36 @@ inline size_t carve_bt(const BtCfg& c, uint8_t* base, BtStream* s, size_t* persi
 }
 
 }  // namespace bmb
+
+#include "ob_core.cuh"
+
+namespace bmb {
+
+// OccluBoost: BoostTrack's stream, then its own state.  The persistent part is the whole stream (reset clears it all):
+// the graveyard and the event log sit after BoostTrack's scratch.
+inline size_t carve_ob(const ObCfg& c, uint8_t* base, ObStream* s, size_t* persistent_bytes) {
+    const size_t CT = (size_t)c.bt.cap_tracks, CD = (size_t)c.bt.cap_dets;
+    const size_t F = (size_t)(c.bt.feat_dim > 0 ? c.bt.feat_dim : 1), B = (size_t)(c.ams_buffer_size > 0 ? c.ams_buffer_size : 1);
+    const size_t MX = CT > CD ? CT : CD;
+    ObStream t{};
+    const size_t nb = carve_bt(c.bt, base, s ? &t.b : nullptr, nullptr);
+    Carver k{base, nb};
+    t.activated = k.take<int>(CT); t.ams = k.take<double>(CT * B * 4); t.ams_n = k.take<int>(CT); t.ams_head = k.take<int>(CT);
+    t.gv_meta = k.take<int>(2); t.gv_order = k.take<int>(CT); t.gv_id = k.take<int>(CT); t.gv_frame = k.take<int>(CT);
+    t.gv_box = k.take<double>(CT * 4); t.gv_conf = k.take<double>(CT); t.gv_cls = k.take<double>(CT);
+    t.gv_emb = k.take<double>(CT * F); t.ev = k.take<double>(CT * OB_EV);
+    t.unt = k.take<int>(CT); t.elig = k.take<int>(CT); t.low = k.take<int>(CD); t.rowcol = k.take<int>(CD);
+    t.nsrc = k.take<int>(CD); t.nid = k.take<int>(CD); t.emit = k.take<int>(CT);
+    t.gate = t.b.ex;
+    t.scalars = t.b.scalars; t.timers = t.b.timers;   // BoostTrack's softmax scratch is free once the association is done
+    t.lsa_u = k.take<double>(MX); t.lsa_v = k.take<double>(MX); t.lsa_spc = k.take<double>(MX);
+    t.lsa_path = k.take<int>(MX); t.lsa_row4col = k.take<int>(MX); t.lsa_col4row = k.take<int>(MX);
+    t.lsa_rem = k.take<int>(MX); t.lsa_sc = k.take<int>(MX); t.lsa_sr = k.take<int>(MX);
+    const size_t total = (k.off + 255) & ~(size_t)255;
+    if (persistent_bytes) *persistent_bytes = total;
+    if (s) *s = t;
+    return total;
+}
+
+}  // namespace bmb
+

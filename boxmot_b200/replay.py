@@ -328,6 +328,11 @@ def replay_sequences(tracker, caches: Sequence[SequenceCache], conf_threshold: f
         step += 1
         if on_step is not None:
             on_step(step)
+    if getattr(tracker, "kind", None) == "occluboost":   # online GTA gap rows at the end, as process_sequence
+        for i in range(S):
+            gta = tracker.flush_gta(i)
+            if gta.size:
+                rows[i].append(np.asarray(gta, dtype=np.float32))
     return [np.concatenate(r, axis=0) if r else np.empty((0, 9), dtype=np.float32) for r in rows]
 
 

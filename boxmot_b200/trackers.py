@@ -256,11 +256,11 @@ class MultiStreamTracker:
             cfg.with_reid = 1
             p.setdefault("track_buffer", 0)
             p.setdefault("frame_rate", 30)
-        elif kind == "boosttrack":
-            p = dict(BOOSTTRACK_ENGINE_DEFAULTS)
+        elif kind in ("boosttrack", "occluboost"):
+            p = dict(BOOSTTRACK_ENGINE_DEFAULTS, **(OCCLUBOOST_ENGINE_DEFAULTS if kind == "occluboost" else {}))
             unknown = set(params) - set(p)
             if unknown:
-                raise TypeError(f"unknown BoostTrack parameters: {sorted(unknown)}")
+                raise TypeError(f"unknown {'BoostTrack' if kind == 'boosttrack' else 'OccluBoost'} parameters: {sorted(unknown)}")
             p.update(params)
             for name in ("det_thresh", "iou_threshold", "lambda_iou", "lambda_mhd", "lambda_shape", "dlo_boost_coef",
                          "min_box_area", "aspect_ratio_thresh"):
@@ -270,7 +270,7 @@ class MultiStreamTracker:
                 raise ValueError(f"BoostTrack det_thresh must be in [0, 1), got {p['det_thresh']}")
             if int(p["max_age"]) < 0 or int(p["min_hits"]) < 0:
                 raise ValueError("BoostTrack max_age and min_hits must be >= 0")
-            cfg.tracker = _lib.TRACKER_BOOSTTRACK
+            cfg.tracker = _lib.TRACKER_BOOSTTRACK if kind == "boosttrack" else _lib.TRACKER_OCCLUBOOST
             cfg.max_age, cfg.min_hits = int(p["max_age"]), int(p["min_hits"])
             cfg.det_thresh, cfg.iou_threshold = float(p["det_thresh"]), float(p["iou_threshold"])
             cfg.use_dlo_boost, cfg.use_duo_boost = int(bool(p["use_dlo_boost"])), int(bool(p["use_duo_boost"]))
@@ -280,11 +280,13 @@ class MultiStreamTracker:
                                                                               float(p["aspect_ratio_thresh"]))
             cfg.lambda_iou, cfg.lambda_mhd, cfg.lambda_shape = float(p["lambda_iou"]), float(p["lambda_mhd"]), float(p["lambda_shape"])
             cfg.with_reid = int(bool(p["with_reid"]))
+            if kind == "occluboost":
+                _occluboost_cfg(cfg, p)
             p.setdefault("track_buffer", 0)
             p.setdefault("frame_rate", 30)
         else:
             raise ValueError(f"tracker '{tracker}' is not part of the B200 hot path "
-                             "(bytetrack, botsort, deepocsort, strongsort, boosttrack)")
+                             "(bytetrack, botsort, deepocsort, strongsort, boosttrack, occluboost)")
         cfg.n_streams = int(n_streams)
         cfg.cap_tracks = int(cap_tracks)
         cfg.cap_dets = int(cap_dets)
@@ -314,6 +316,8 @@ class MultiStreamTracker:
             raise B200Error(f"tracker create failed: {_lib.last_error(self.lib)}")
         self.frame_count = 0
         self.cmc = None
+        self._gta_on = kind == "occluboost" and bool(p["gta_enabled"]) and self.with_reid
+        self._gta_events = [[] for _ in range(self.n_streams)]
 
     def set_cmc(self, method: Optional[str]) -> None:
         """Camera-motion ESTIMATION on the device from the frames passed to `update`: "ecc" (BoT-SORT, StrongSORT) = the
@@ -342,6 +346,7 @@ class MultiStreamTracker:
         if not self.lib.boxmot_b200_tracker_reset(self.handle):
             raise B200Error(_lib.last_error(self.lib))
         self.frame_count = 0
+        self._gta_events = [[] for _ in range(self.n_streams)]
 
     def set_warp(self, stream: int, warp) -> None:
         """Camera-motion warp (2x3) to apply on the next update of `stream` (BoT-SORT multi_gmc, StrongSORT
@@ -400,7 +405,37 @@ class MultiStreamTracker:
         if not ok:
             raise B200Error(_lib.last_error(self.lib))
         self.frame_count += 1
+        if self._gta_on:   # the device log holds cap_tracks events: take them every frame
+            for i in range(S):
+                self._take_gta(i, False)
         return [TrackResults(outs[i][: o_rows[i], :8].copy()) for i in range(S)]
+
+    # ---- OccluBoost online GTA --------------------------------------------------------------------------------------
+    def _take_gta(self, stream: int, clear_graveyard: bool) -> None:
+        ev = np.empty((self.cap_tracks, 13), np.float64)
+        n = ctypes.c_int(0)
+        if not self.lib.boxmot_b200_tracker_gta_events(self.handle, int(stream), int(clear_graveyard), ev.ctypes.data,
+                                                       self.cap_tracks, ctypes.byref(n)):
+            raise B200Error(_lib.last_error(self.lib))
+        if n.value:
+            self._gta_events[stream].append(ev[: n.value].copy())
+
+    def flush_gta(self, stream: int = 0) -> np.ndarray:
+        """OccluBoost: the interpolated (and, with gta_smooth_tau > 0, Gaussian-process smoothed) gap rows of the tracks
+        `stream` resurrected since the last flush, MOT layout `[frame, id, x1, y1, x2, y2, conf, cls, -1]` float64, as
+        the reference's flush_gta (occluboost.py:710-768).  Like the reference it also empties the graveyard when there
+        are rows.  Other trackers: no rows."""
+        if self.kind != "occluboost":
+            return np.empty((0, 9))
+        if self._gta_on:
+            self._take_gta(stream, False)
+        ev = np.concatenate(self._gta_events[stream], 0) if self._gta_events[stream] else np.empty((0, 13))
+        p = self.params
+        rows = gta_rows(ev, bool(p["gta_interpolate"]), max(int(p["gta_max_gap"]), 1), float(p["gta_smooth_tau"]))
+        if len(rows):
+            self._gta_events[stream] = []
+            self._take_gta(stream, True)
+        return rows
 
     # ---- device-resident frame loop (SURVEY 8f-1) ---------------------------------------------------------------
     @staticmethod
@@ -522,7 +557,7 @@ class _SingleStreamTracker:
             # the reference's un-freeze replay looks its pre-gap anchor up in a history deque of max_obs entries
             # (xysr.py:384-399) and silently skips the replay once a gap has pushed it out; the device keeps the anchor
             raise NotImplementedError("DeepOCSORT needs max_obs >= max_age + 4 (history window of the un-freeze replay)")
-        if self._kind in ("deepocsort", "boosttrack"):  # BaseTracker settings their updates actually read
+        if self._kind in ("deepocsort", "boosttrack", "occluboost"):  # BaseTracker settings their updates actually read
             params = dict(params, det_thresh=det_thresh, max_age=max_age, min_hits=min_hits, iou_threshold=iou_threshold)
         if self._kind == "strongsort":  # Tracker(max_age=self.max_age) (strongsort.py:56-64)
             params = dict(params, max_age=max_age)
@@ -563,7 +598,7 @@ class _SingleStreamTracker:
                 raise B200Error("with_reid=True needs reid_model=, embs=, or with_reid=False")
             # the device re-derives the split from the float32 rows it receives: decide on the same rounded values
             conf = np.asarray(dets, dtype=np.float32)[:, 4].astype(np.float64)
-            if eng.kind == "boosttrack":   # every row: which rows survive the confidence boosts is decided on the device
+            if eng.kind in ("boosttrack", "occluboost"):   # every row: which rows survive the confidence boosts is decided on the device
                 first = np.ones(len(conf), dtype=bool)
             elif eng.kind == "strongsort":
                 first = conf >= eng.params["min_conf"]
@@ -781,6 +816,145 @@ class BoostTrack(_SingleStreamTracker):
             self._engine.set_cmc(cmc_method)
 
 
+# OccluBoost (boxmot/trackers/bbox/occluboost/occluboost.py:84-183): its own parameters with the constructor's defaults,
+# and configs/trackers/occluboost.yaml, the defaults create_tracker("occluboost") starts from
+OCCLUBOOST_ENGINE_DEFAULTS = dict(
+    recovery_appearance_thresh=0.99, recovery_iou_thresh=0.1, recovery_max_age=1, feat_alpha=0.95, track_low_thresh=0.1,
+    second_iou_thresh=0.6, second_appearance_thresh=0.5, second_pass_max_age=1, second_pass_min_hits=3,
+    use_second_pass=False, new_track_thresh=0.6, confirm_hits=2, instant_confirm_thresh=0.7, tentative_max_age=1,
+    duplicate_iou_thresh=0.85, ams_enabled=True, ams_alpha0=0.4, ams_threshold=0.5, ams_buffer_size=30,
+    ams_shrink_ratio=0.75, lambda_emb_multiplier=1.5, gta_enabled=True, gta_appearance_thresh=0.5,
+    gta_min_track_length=5, gta_smooth_tau=5.0, gta_interpolate=True, gta_max_gap=60)
+OCCLUBOOST_YAML_DEFAULTS = dict(
+    max_age=146, min_hits=1, det_thresh=0.5678626013369781, iou_threshold=0.2957128153631725, use_cmc=True,
+    cmc_method="sof", min_box_area=73, aspect_ratio_thresh=1.4888137942764672, lambda_iou=1.0784558316374715,
+    lambda_mhd=0.304435887183232, lambda_shape=1.6709449476805447, use_dlo_boost=True, dlo_boost_coef=1.2061962091907352,
+    use_duo_boost=False, s_sim_corr=False, use_rich_s=False, use_sb=True, use_vt=True, with_reid=True,
+    recovery_appearance_thresh=0.6732855110134396, recovery_iou_thresh=0.24380051350243462, recovery_max_age=113,
+    feat_alpha=0.8324072665785186, track_low_thresh=0.04473431588067598, use_second_pass=True,
+    second_iou_thresh=0.8131671757478834, second_appearance_thresh=0.364089272226479, second_pass_max_age=8,
+    second_pass_min_hits=7, new_track_thresh=0.7128242784621849, confirm_hits=2,
+    instant_confirm_thresh=0.6783889178413256, tentative_max_age=3, duplicate_iou_thresh=0.9571823233925608,
+    ams_enabled=True, ams_alpha0=0.8732388616784778, ams_threshold=0.9206232808452425, ams_buffer_size=57,
+    ams_shrink_ratio=0.6934881647679682, lambda_emb_multiplier=2.9476295884842885, gta_enabled=False,
+    gta_appearance_thresh=0.7125445489563044, gta_min_track_length=7, gta_smooth_tau=14.757519908748044,
+    gta_interpolate=False, gta_max_gap=40, adaptive_kf=False)
+
+
+def _occluboost_cfg(cfg, p) -> None:
+    """OccluBoost's fields of the engine configuration, with the clamps the reference constructor applies."""
+    for name in ("recovery_appearance_thresh", "recovery_iou_thresh", "feat_alpha", "track_low_thresh",
+                 "second_iou_thresh", "second_appearance_thresh", "new_track_thresh", "instant_confirm_thresh",
+                 "duplicate_iou_thresh", "ams_alpha0", "ams_threshold", "ams_shrink_ratio", "lambda_emb_multiplier",
+                 "gta_appearance_thresh", "gta_smooth_tau"):
+        if not np.isfinite(float(p[name])):
+            raise ValueError(f"OccluBoost {name} must be finite, got {p[name]}")
+    cfg.use_second_pass = int(bool(p["use_second_pass"]))
+    cfg.recovery_max_age, cfg.second_pass_max_age = int(p["recovery_max_age"]), int(p["second_pass_max_age"])
+    cfg.second_pass_min_hits = int(p["second_pass_min_hits"])
+    cfg.confirm_hits, cfg.tentative_max_age = max(int(p["confirm_hits"]), 1), max(int(p["tentative_max_age"]), 0)
+    cfg.ams_enabled, cfg.ams_buffer_size = int(bool(p["ams_enabled"])), int(max(p["ams_buffer_size"], 2))
+    cfg.gta_enabled = int(bool(p["gta_enabled"]))
+    cfg.gta_min_track_length, cfg.gta_max_gap = max(int(p["gta_min_track_length"]), 1), max(int(p["gta_max_gap"]), 1)
+    cfg.lambda_emb_multiplier = float(p["lambda_emb_multiplier"])
+    cfg.recovery_appearance_thresh, cfg.recovery_iou_thresh = float(p["recovery_appearance_thresh"]), float(p["recovery_iou_thresh"])
+    cfg.feat_alpha, cfg.track_low_thresh = float(p["feat_alpha"]), float(p["track_low_thresh"])
+    cfg.second_iou_thresh, cfg.second_appearance_thresh = float(p["second_iou_thresh"]), float(p["second_appearance_thresh"])
+    cfg.new_track_thresh = max(float(p["new_track_thresh"]), 0.0)
+    cfg.instant_confirm_thresh, cfg.duplicate_iou_thresh = float(p["instant_confirm_thresh"]), float(p["duplicate_iou_thresh"])
+    cfg.ams_alpha0 = float(np.clip(p["ams_alpha0"], 0.0, 1.0))
+    cfg.ams_threshold = float(max(p["ams_threshold"], 0.0))
+    cfg.ams_shrink_ratio = float(np.clip(p["ams_shrink_ratio"], 0.0, 1.0))
+    cfg.gta_appearance_thresh = float(p["gta_appearance_thresh"])
+
+
+def gta_rows(events, interpolate: bool, max_gap: int, smooth_tau: float) -> np.ndarray:
+    """Gap rows of OccluBoost's resurrection events (`[grave id, death frame, frame, box at death (4), new box (4), conf,
+    cls]`, in order): for a gap of 2 .. max_gap frames, one linearly interpolated `[frame, id, x1, y1, x2, y2, conf, cls,
+    -1]` row per missing frame (occluboost.py:680-698); then, with smooth_tau > 0 and at least 3 rows, every id's rows
+    (at least 3) are replaced by a Gaussian-process regression with a fixed RBF length scale (occluboost.py:731-768;
+    left unsmoothed when scikit-learn is absent, as there)."""
+    rows = []
+    for e in np.asarray(events, np.float64).reshape(-1, 13):
+        gid, death, frame = int(e[0]), int(e[1]), int(e[2])
+        gap = frame - death
+        if not interpolate or not (1 < gap <= max_gap):
+            continue
+        last, cur = e[3:7].copy(), e[7:11].copy()
+        for t in range(1, gap):
+            a = t / gap
+            b = (1.0 - a) * last + a * cur
+            rows.append(np.array([death + t, gid, b[0], b[1], b[2], b[3], e[11], e[12], -1.0], dtype=float))
+    if not rows:
+        return np.empty((0, 9))
+    if smooth_tau > 0 and len(rows) >= 3:
+        try:
+            from sklearn.gaussian_process import GaussianProcessRegressor
+            from sklearn.gaussian_process.kernels import RBF
+        except ImportError:
+            return np.vstack(rows)
+        groups: dict = {}
+        for k, r in enumerate(rows):
+            groups.setdefault(int(r[1]), []).append(k)
+        tau = smooth_tau
+        for idx in groups.values():
+            if len(idx) < 3:
+                continue
+            frames = np.array([rows[k][0] for k in idx]).reshape(-1, 1)
+            boxes = np.array([rows[k][2:6] for k in idx])
+            ls = np.clip(tau * np.log(max(tau ** 3 / len(idx), 1e-6)), tau ** -1, tau ** 2)
+            sm = GaussianProcessRegressor(RBF(ls, length_scale_bounds="fixed")).fit(frames, boxes).predict(frames)
+            for j, k in enumerate(idx):
+                rows[k][2:6] = sm[j]
+    return np.vstack(rows)
+
+
+class OccluBoost(BoostTrack):
+    """OccluBoost on the GPU; arguments and defaults as boxmot/trackers/bbox/occluboost/occluboost.py:84-183 plus
+    BoostTrack's (including `use_cmc=True, cmc_method="ecc"`).  The whole update runs on the device on top of the
+    BoostTrack core: original-confidence low set, associate with `lambda_emb_multiplier`, OccluTrack abnormal-motion
+    suppression of the Kalman gain, the ReID recovery pass, the low-confidence second pass, online GTA (appearance
+    recovery and resurrection from a graveyard of dead tracks, which reuses the dead id), tentative tracks, duplicate
+    suppression and the cull.  `flush_gta()` returns the gap rows of the resurrections, as the reference's.
+
+    Differences from the reference: ids start at 1 per tracker; `reset()` also clears the graveyard and the pending gap
+    rows.  Not implemented (NotImplementedError): OBB, `per_class=True`, `adaptive_kf=True`, class-specific Kalman
+    noise, and `cmc_method` other than "ecc" / "sof"."""
+
+    _kind = "occluboost"
+
+    def __init__(self, reid_model: Any = None, recovery_appearance_thresh: float = 0.99,
+                 recovery_iou_thresh: float = 0.1, recovery_max_age: int = 1, feat_alpha: float = 0.95,
+                 track_low_thresh: float = 0.1, second_iou_thresh: float = 0.6, second_appearance_thresh: float = 0.5,
+                 second_pass_max_age: int = 1, second_pass_min_hits: int = 3, use_second_pass: bool = False,
+                 new_track_thresh: float = 0.6, confirm_hits: int = 2, instant_confirm_thresh: float = 0.7,
+                 tentative_max_age: int = 1, duplicate_iou_thresh: float = 0.85, ams_enabled: bool = True,
+                 ams_alpha0: float = 0.4, ams_threshold: float = 0.5, ams_buffer_size: int = 30,
+                 ams_shrink_ratio: float = 0.75, lambda_emb_multiplier: float = 1.5, gta_enabled: bool = True,
+                 gta_appearance_thresh: float = 0.5, gta_min_track_length: int = 5, gta_smooth_tau: float = 5.0,
+                 gta_interpolate: bool = True, gta_max_gap: int = 60, adaptive_kf: bool = False, **kwargs: Any):
+        if adaptive_kf:
+            raise NotImplementedError("OccluBoost adaptive_kf=True (innovation-window process noise) is not implemented "
+                                      "on the B200 path")
+        super().__init__(reid_model=reid_model, recovery_appearance_thresh=recovery_appearance_thresh,
+                         recovery_iou_thresh=recovery_iou_thresh, recovery_max_age=recovery_max_age,
+                         feat_alpha=feat_alpha, track_low_thresh=track_low_thresh, second_iou_thresh=second_iou_thresh,
+                         second_appearance_thresh=second_appearance_thresh, second_pass_max_age=second_pass_max_age,
+                         second_pass_min_hits=second_pass_min_hits, use_second_pass=use_second_pass,
+                         new_track_thresh=new_track_thresh, confirm_hits=confirm_hits,
+                         instant_confirm_thresh=instant_confirm_thresh, tentative_max_age=tentative_max_age,
+                         duplicate_iou_thresh=duplicate_iou_thresh, ams_enabled=ams_enabled, ams_alpha0=ams_alpha0,
+                         ams_threshold=ams_threshold, ams_buffer_size=ams_buffer_size, ams_shrink_ratio=ams_shrink_ratio,
+                         lambda_emb_multiplier=lambda_emb_multiplier, gta_enabled=gta_enabled,
+                         gta_appearance_thresh=gta_appearance_thresh, gta_min_track_length=gta_min_track_length,
+                         gta_smooth_tau=gta_smooth_tau, gta_interpolate=gta_interpolate, gta_max_gap=gta_max_gap,
+                         **kwargs)
+
+    def flush_gta(self) -> np.ndarray:
+        """Interpolated gap rows of the resurrected tracks, MOT layout (9 columns); see `MultiStreamTracker.flush_gta`."""
+        return self._engine.flush_gta(0)
+
+
 def _flatten_yaml_defaults(node, acc=None):
     """`<param>: {default: ...}` entries of a reference tracker YAML, nested conditional parameters included
     (what `flatten_yaml_config` + `details["default"]` produce in tracker_zoo.py:112-119)."""
@@ -809,7 +983,7 @@ def resolve_tracker_args(tracker_type, tracker_config=None, evolve_param_dict=No
 
     kind = str(tracker_type).lower()
     classes = {"bytetrack": ByteTrack, "botsort": BotSort, "deepocsort": DeepOcSort, "strongsort": StrongSort, "ocsort": OcSort,
-               "boosttrack": BoostTrack}
+               "boosttrack": BoostTrack, "occluboost": OccluBoost}
     if kind not in classes:
         raise ValueError(f"Unknown tracker type: '{tracker_type}'. Available trackers are: {', '.join(classes)} "
                          "(the trackers that are part of the B200 hot path)")
@@ -821,11 +995,14 @@ def resolve_tracker_args(tracker_type, tracker_config=None, evolve_param_dict=No
         with open(tracker_config, "r", encoding="utf-8") as f:
             args = _flatten_yaml_defaults(yaml.safe_load(f) or {})
     else:
-        args = dict(TRACKER_DEFAULTS[kind] if kind in TRACKER_DEFAULTS else BOOSTTRACK_YAML_DEFAULTS)
+        args = dict(TRACKER_DEFAULTS[kind] if kind in TRACKER_DEFAULTS
+                    else OCCLUBOOST_YAML_DEFAULTS if kind == "occluboost" else BOOSTTRACK_YAML_DEFAULTS)
     args.update(overrides or {})
     cls = classes[kind]
-    accepted = set(inspect.signature(cls.__init__).parameters) | set(
-        inspect.signature(_SingleStreamTracker.__init__).parameters) | {"cap_tracks", "cap_dets", "feat_dim"}
+    accepted = {"cap_tracks", "cap_dets", "feat_dim"}
+    for base in cls.__mro__:   # OccluBoost forwards BoostTrack's parameters, as the reference subclass does
+        if issubclass(base, _SingleStreamTracker):
+            accepted |= set(inspect.signature(base.__init__).parameters)
     accepted -= {"self", "params", "kwargs"}
     args = {k: v for k, v in args.items() if k in accepted}   # the reference's **kwargs swallows the rest
     # Camera-motion estimation: ECC runs on the device (StrongSORT always uses it in the reference; BoT-SORT when
@@ -844,7 +1021,7 @@ def resolve_tracker_args(tracker_type, tracker_config=None, evolve_param_dict=No
                       f"({method if kind == 'botsort' else 'sof'}); this tracker is built with it off and applies a warp supplied "
                       "through update(..., warp=), without one it behaves as with CMC off -- call tracker.set_cmc('sof') "
                       "(BoT-SORT, DeepOCSORT) to estimate SOF on the device like the reference", stacklevel=3)
-    if kind == "boosttrack":   # both of its estimators run on the device: the configuration stays as it is
+    if kind in ("boosttrack", "occluboost"):   # both estimators run on the device: the configuration stays as it is
         args.pop("per_class", None)
         return kind, cls, args
     args.pop("cmc_method", None)

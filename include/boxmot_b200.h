@@ -115,6 +115,7 @@ BOXMOT_B200_API const char* boxmot_botsort_last_error(void);
 #define BOXMOT_B200_TRACKER_DEEPOCSORT 2
 #define BOXMOT_B200_TRACKER_STRONGSORT 3
 #define BOXMOT_B200_TRACKER_BOOSTTRACK 4
+#define BOXMOT_B200_TRACKER_OCCLUBOOST 5
 
 /* Every parameter of the reference Python constructors (bytetrack.py:226-257, botsort.py:66-118), in
  * double precision so thresholds compare exactly as python floats do. */
@@ -179,6 +180,33 @@ typedef struct BoxMOTB200TrackerConfig {
     double lambda_shape;
     double min_box_area;
     double aspect_ratio_thresh;
+    /* OccluBoost (trackers/bbox/occluboost/occluboost.py:84-183; the BoostTrack fields above are shared, and so are
+     * track_low_thresh and new_track_thresh); ignored by the other trackers.  Values as the reference stores them
+     * after its clamps (confirm_hits >= 1, tentative_max_age >= 0, ams_buffer_size >= 2, gta_min_track_length >= 1,
+     * gta_max_gap >= 1, ams_alpha0 and ams_shrink_ratio in [0, 1], ams_threshold >= 0, new_track_thresh >= 0). */
+    int use_second_pass;
+    int recovery_max_age;
+    int second_pass_max_age;
+    int second_pass_min_hits;
+    int confirm_hits;
+    int tentative_max_age;
+    int ams_enabled;
+    int ams_buffer_size;
+    int gta_enabled;
+    int gta_min_track_length;
+    int gta_max_gap;
+    double lambda_emb_multiplier;
+    double recovery_appearance_thresh;
+    double recovery_iou_thresh;
+    double feat_alpha;
+    double second_iou_thresh;
+    double second_appearance_thresh;
+    double instant_confirm_thresh;
+    double duplicate_iou_thresh;
+    double ams_alpha0;
+    double ams_threshold;
+    double ams_shrink_ratio;
+    double gta_appearance_thresh;
 } BoxMOTB200TrackerConfig;
 
 typedef struct BoxMOTB200Tracker BoxMOTB200Tracker;
@@ -218,6 +246,12 @@ BOXMOT_B200_API int boxmot_b200_tracker_snapshot(BoxMOTB200Tracker* handle, int 
  * BaseTracker.active_tracks / lost_stracks / removed_stracks (boxmot/trackers/basetracker.py:386-390, 465-466). */
 BOXMOT_B200_API int boxmot_b200_tracker_track_ids(BoxMOTB200Tracker* handle, int stream, int which, int* ids,
                                                   int capacity, int* out_count);
+/* OccluBoost: the graveyard resurrections of `stream` logged since the last call, oldest first, OB_EV = 13 doubles
+ * each: grave id, death frame, resurrection frame, box at death [x1,y1,x2,y2], box of the new track, conf and cls at
+ * death -- what trackers/bbox/occluboost/occluboost.py:680-698 interpolates into gap rows.  The log is cleared;
+ * clear_graveyard != 0 also empties the graveyard (flush_gta, occluboost.py:727-728).  Synchronises the handle. */
+BOXMOT_B200_API int boxmot_b200_tracker_gta_events(BoxMOTB200Tracker* handle, int stream, int clear_graveyard,
+                                                   double* events, int capacity, int* out_count);
 /* Kernel launches issued by the last update call, and CUDA stream / device-time accessors for benchmarks. */
 BOXMOT_B200_API int boxmot_b200_tracker_last_launches(BoxMOTB200Tracker* handle, int* out_launches);
 BOXMOT_B200_API int boxmot_b200_tracker_last_device_ms(BoxMOTB200Tracker* handle, double* reid_ms, double* assoc_ms);
