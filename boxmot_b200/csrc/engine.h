@@ -58,31 +58,39 @@ struct Engine {
     ReidModel* reid = nullptr;
     uint8_t* d_mem = nullptr;
     size_t stream_bytes = 0, persistent_bytes = 0;
-    TrkStream* d_streams = nullptr;
-    std::vector<TrkStream> h_streams;
-    bool is_docs = false;              // DeepOCSORT engine (docs_core.cuh) instead of the STrack family
+    // Which tracker runs: the STrack family (ByteTrack / BoT-SORT, tracker_core.cuh), DeepOCSORT / OC-SORT (docs_core.cuh),
+    // StrongSORT (ss_core.cuh), BoostTrack (bt_core.cuh) or OccluBoost (ob_core.cuh, whose streams wrap a BtStream).
+    enum class Family { STrack, Docs, StrongSort, Boost, Occlu };
+    Family family = Family::STrack;
+    bool on_bt_stream() const { return family == Family::Boost || family == Family::Occlu; }
+    bool is_bytetrack() const { return family == Family::STrack && cfg.kind != KIND_XYWH; }
+    // family configs and host copies of the stream structs of input set 0 (h_bt holds OccluBoost's BoostTrack part too)
     DocsCfg dcfg{};
-    DocsStream* d_docs = nullptr;
-    std::vector<DocsStream> h_docs;
-    bool is_ss = false;                // StrongSORT engine (ss_core.cuh)
     SsCfg scfg{};
-    SsStream* d_ss = nullptr;
-    std::vector<SsStream> h_ss;
-    bool is_bt = false;                // BoostTrack engine (bt_core.cuh)
     BtCfg btcfg{};
-    BtStream* d_bt = nullptr;
-    std::vector<BtStream> h_bt;
-    bool is_ob = false;                // OccluBoost engine (ob_core.cuh): is_bt too, d_bt / h_bt hold its BoostTrack part
     ObCfg obcfg{};
-    ObStream* d_ob = nullptr;
+    std::vector<TrkStream> h_streams;
+    std::vector<DocsStream> h_docs;
+    std::vector<SsStream> h_ss;
+    std::vector<BtStream> h_bt;
     std::vector<ObStream> h_ob;
+    // One set of frame inputs and the family's device stream array that reads it.  Set 0 serves update() and the
+    // synchronous device path; set 1 exists with on-device ReID, for the frame pipeline of update_device.
+    struct InputSet {
+        float* dets = nullptr;
+        int* ndets = nullptr;
+        float* embs = nullptr;
+        TrkStream* trk = nullptr;
+        DocsStream* docs = nullptr;
+        SsStream* ss = nullptr;
+        BtStream* bt = nullptr;
+        ObStream* ob = nullptr;
+    };
+    InputSet in[2];
     double* d_conf_pow = nullptr;      // 0.9 ** k, k = 0 .. max_age + 1 (KalmanBoxTracker.get_confidence)
     std::vector<float*> out_ptr;       // per-stream output rows / scalars / timers (either family)
     std::vector<int*> scalars_ptr;
     std::vector<long long*> timers_ptr;
-    float* d_dets = nullptr;
-    int* d_ndets = nullptr;
-    float* d_embs = nullptr;
     double* d_warp = nullptr;      // [S][8] pending camera-motion warps (slot 6 = pending flag)
     bool warp_dirty = false;
     // on-device camera-motion estimation: 0 = off (warps are supplied), 1 = the reference's ECC defaults (cmc_ecc.cuh),
@@ -116,7 +124,7 @@ struct Engine {
     double assoc_ms_accum = 0.0;
     int assoc_frames = 0;
     // frame pipeline of the device-resident path (update_device): ReID of frame f+1 runs on its own stream while
-    // the single-CTA-per-stream association of frame f runs on `stream`; inputs are double-buffered (BoT-SORT family)
+    // the single-CTA-per-stream association of frame f runs on `stream`; inputs are double-buffered (in[0] / in[1])
     cudaStream_t reid_stream = nullptr;
     // extra ReID workspaces: slices of a frame's crop list run concurrently on helper streams (the tile kernels
     // are latency-bound with short waves; concurrent slices fill each other's tails)
@@ -128,15 +136,6 @@ struct Engine {
     int* h_crops_hint = nullptr;           // mapped host word: crop count of a recent frame (slice balancing hint)
     int* d_crops_hint = nullptr;
     cudaEvent_t ev_slice_done[MAX_SPLIT - 1]{};
-    float* d_dets_alt = nullptr;
-    int* d_ndets_alt = nullptr;
-    float* d_embs_alt = nullptr;
-    TrkStream* d_streams_alt = nullptr;
-    std::vector<TrkStream> h_streams_alt;
-    DocsStream* d_docs_alt = nullptr;
-    SsStream* d_ss_alt = nullptr;
-    BtStream* d_bt_alt = nullptr;
-    ObStream* d_ob_alt = nullptr;
     cudaEvent_t ev_reid_done[2]{};
     cudaEvent_t ev_assoc_done[2]{};
     int pipe_parity = 0;
@@ -175,10 +174,14 @@ struct Engine {
     void enqueue_cmc(const uint8_t* images_dev, int rows, int cols);
     void enqueue_frame(const float* embs_dev, const uint8_t* images_dev, int rows, int cols, int max_dets_total);
     bool can_pipeline() const { return reid_stream != nullptr && !profile; }
+    template <typename St> void wire_streams(std::vector<St>& h, int set, St** dev);
     void enqueue_association(TrkStream* streams_dev, const float* embs_src);
     void enqueue_crops(int parity, cudaStream_t st);            // crop list of the family, from input set `parity`
-    void enqueue_family_association(int parity);                // association launches of the family on `stream`
+    // association launches of the family on `stream`; the STrack family reads `embs_src` in place (null: the set's own)
+    void enqueue_family_association(int parity, const float* embs_src = nullptr);
     void enqueue_bt(BtStream* streams_dev, ObStream* ob_dev);    // BoostTrack / OccluBoost: embedding cost + frame kernel
+    struct TrackView;
+    TrackView track_view(int stream_index) const;
     int run_reid(cudaStream_t main_stream, const uint8_t* images_dev, int rows, int cols, int total, float* embs_out);
     void enqueue_fetch();
     void finish_fetch(float* const* out, const int* out_cap, int* out_rows);

@@ -191,11 +191,38 @@ __host__ __device__ inline size_t jv_smem_bytes(int MX) {
     return (size_t)MX * (2 * sizeof(double) + 6 * sizeof(int)) + 16;
 }
 
+// lapjv's scratch of a stream copy re-pointed into the frame kernel's dynamic shared memory (jv_smem_bytes(MX) bytes)
+template <typename St>
+__device__ __forceinline__ void jv_scratch_to_smem(St& s, unsigned char* smem, int MX) {
+    double* pd = reinterpret_cast<double*>(smem);
+    s.lap_v = pd; pd += MX;
+    s.lap_spc = pd; pd += MX;
+    int* pi = reinterpret_cast<int*>(pd);
+    s.lap_x = pi; pi += MX;
+    s.lap_y = pi; pi += MX;
+    s.lap_path = pi; pi += MX;
+    s.lap_tl = pi; pi += MX;
+    s.lap_sc = pi; pi += MX;
+    s.lap_insc = pi;
+}
+
+// Dynamic shared memory for a launch of `frame_kernel` (lapjv's scratch, when it fits) and the kernel's jv_in_smem
+// argument: bit 0 = the scratch lives there, the bits above = the dense-JV augmentation mode
+template <typename Kernel>
+static int jv_launch_setup(Kernel frame_kernel, int cap_tracks, int cap_dets, size_t* smem_bytes) {
+    const size_t jb = jv_smem_bytes(cap_tracks > cap_dets ? cap_tracks : cap_dets);
+    const bool in_smem = jb <= 200 * 1024;
+    if (in_smem && jb > 48 * 1024)
+        CUDA_OK(cudaFuncSetAttribute(frame_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)jb));
+    *smem_bytes = in_smem ? jb : 0;
+    return (in_smem ? 1 : 0) | (jv_wide_default() << 1);
+}
+
 __global__ void __launch_bounds__(256) k_docs_frame(const DocsCfg cfg, DocsStream* streams, int jv_in_smem) {
     extern __shared__ __align__(16) unsigned char dyn_smem[];
     DocsStream s = streams[blockIdx.x];
     s.jv_wide = jv_in_smem >> 1;
-    if (jv_in_smem & 1) {
+    if (jv_in_smem & 1) {   // jv_scratch_to_smem, written out: at 255 registers with spills, this kernel's allocation moves with the helper
         const int MX = cfg.cap_tracks > cfg.cap_dets ? cfg.cap_tracks : cfg.cap_dets;
         double* pd = reinterpret_cast<double*>(dyn_smem);
         s.lap_v = pd; pd += MX;
@@ -252,19 +279,7 @@ __global__ void __launch_bounds__(256) k_bt_frame(const BtCfg cfg, BtStream* str
     extern __shared__ __align__(16) unsigned char dyn_smem[];
     BtStream s = streams[blockIdx.x];
     s.jv_wide = jv_in_smem >> 1;
-    if (jv_in_smem & 1) {
-        const int MX = cfg.cap_tracks > cfg.cap_dets ? cfg.cap_tracks : cfg.cap_dets;
-        double* pd = reinterpret_cast<double*>(dyn_smem);
-        s.lap_v = pd; pd += MX;
-        s.lap_spc = pd; pd += MX;
-        int* pi = reinterpret_cast<int*>(pd);
-        s.lap_x = pi; pi += MX;
-        s.lap_y = pi; pi += MX;
-        s.lap_path = pi; pi += MX;
-        s.lap_tl = pi; pi += MX;
-        s.lap_sc = pi; pi += MX;
-        s.lap_insc = pi;
-    }
+    if (jv_in_smem & 1) jv_scratch_to_smem(s, dyn_smem, max(cfg.cap_tracks, cfg.cap_dets));
     bt_frame(cfg, s);
 }
 
@@ -273,23 +288,10 @@ __global__ void __launch_bounds__(256) k_ob_frame(const ObCfg cfg, ObStream* str
     extern __shared__ __align__(16) unsigned char dyn_smem[];
     ObStream s = streams[blockIdx.x];
     s.b.jv_wide = jv_in_smem >> 1;
-    if (jv_in_smem & 1) {
-        const int MX = cfg.bt.cap_tracks > cfg.bt.cap_dets ? cfg.bt.cap_tracks : cfg.bt.cap_dets;
-        double* pd = reinterpret_cast<double*>(dyn_smem);
-        s.b.lap_v = pd; pd += MX;
-        s.b.lap_spc = pd; pd += MX;
-        int* pi = reinterpret_cast<int*>(pd);
-        s.b.lap_x = pi; pi += MX;
-        s.b.lap_y = pi; pi += MX;
-        s.b.lap_path = pi; pi += MX;
-        s.b.lap_tl = pi; pi += MX;
-        s.b.lap_sc = pi; pi += MX;
-        s.b.lap_insc = pi;
-    }
+    if (jv_in_smem & 1) jv_scratch_to_smem(s.b, dyn_smem, max(cfg.bt.cap_tracks, cfg.bt.cap_dets));
     ob_frame(cfg, s);
 }
 
-// DeepOCSORT embeds every detection above det_thresh (deepocsort.py:333-343)
 // ordered (stream, detection) crop list built by one warp with ballot compaction
 template <typename Keep>
 __device__ __forceinline__ int append_crops(const float* dets, int D, int sidx, int cap_dets, CropDesc* crops, int n, Keep keep) {
@@ -311,41 +313,23 @@ __device__ __forceinline__ int append_crops(const float* dets, int D, int sidx, 
     return n;
 }
 
-__global__ void k_build_crops_docs(const DocsCfg cfg, DocsStream* streams, int n_streams, CropDesc* crops, int* n_crops,
-                                   int* hint) {
-    if (threadIdx.x >= 32 || blockIdx.x != 0) return;
-    int n = 0;
-    for (int sidx = 0; sidx < n_streams; ++sidx) {
-        const DocsStream& s = streams[sidx];
-        const float thr = cfg.det_thresh_f32;
-        n = append_crops(s.dets, min(*s.n_dets, cfg.cap_dets), sidx, cfg.cap_dets, crops, n,
-                         [thr](const float* r) { return r[4] > thr; });
-    }
-    if (threadIdx.x == 0) { *n_crops = n; if (hint) *hint = n; }   // hint: host-mapped, read without synchronisation
-}
-
-// BoostTrack embeds EVERY detection row: which rows survive the confidence boosts depends on the track state, so a
+// Which detection rows a family embeds.  The STrack family: the first-round detections
+__device__ __forceinline__ bool keep_crop(const TrkCfg& cfg, const float* r) { return (double)r[4] > cfg.high_thresh; }
+// DeepOCSORT: every detection above det_thresh (deepocsort.py:333-343)
+__device__ __forceinline__ bool keep_crop(const DocsCfg& cfg, const float* r) { return r[4] > cfg.det_thresh_f32; }
+// BoostTrack: EVERY detection row.  Which rows survive the confidence boosts depends on the track state, so a
 // survivor list would put the ReID behind the association; the frame kernel picks the survivors' rows
-__global__ void k_build_crops_bt(const BtCfg cfg, BtStream* streams, int n_streams, CropDesc* crops, int* n_crops, int* hint) {
-    if (threadIdx.x >= 32 || blockIdx.x != 0) return;
-    int n = 0;
-    for (int sidx = 0; sidx < n_streams; ++sidx) {
-        const BtStream& s = streams[sidx];
-        n = append_crops(s.dets, min(*s.n_dets, cfg.cap_dets), sidx, cfg.cap_dets, crops, n, [](const float*) { return true; });
-    }
-    if (threadIdx.x == 0) { *n_crops = n; if (hint) *hint = n; }
-}
+__device__ __forceinline__ bool keep_crop(const BtCfg&, const float*) { return true; }
 
-// crop list for on-device ReID: one entry per first-round detection, ordered by (stream, detection).
-__global__ void k_build_crops(const TrkCfg cfg, TrkStream* streams, int n_streams, CropDesc* crops, int* n_crops,
-                              int* hint) {
+// crop list for on-device ReID: one entry per embedded detection, ordered by (stream, detection)
+template <typename Cfg, typename St>
+__global__ void k_build_crops(const Cfg cfg, St* streams, int n_streams, CropDesc* crops, int* n_crops, int* hint) {
     if (threadIdx.x >= 32 || blockIdx.x != 0) return;
     int n = 0;
     for (int sidx = 0; sidx < n_streams; ++sidx) {
-        const TrkStream& s = streams[sidx];
-        const double thr = cfg.high_thresh;
+        const St& s = streams[sidx];
         n = append_crops(s.dets, min(*s.n_dets, cfg.cap_dets), sidx, cfg.cap_dets, crops, n,
-                         [thr](const float* r) { return (double)r[4] > thr; });
+                         [&cfg](const float* r) { return keep_crop(cfg, r); });
     }
     if (threadIdx.x == 0) { *n_crops = n; if (hint) *hint = n; }   // hint: host-mapped, read without synchronisation
 }
@@ -386,6 +370,31 @@ static TrkCfg make_core_cfg(const BoxMOTB200TrackerConfig& p) {
     return c;
 }
 
+template <typename St>
+static void upload_streams(const std::vector<St>& h, St** dev) {
+    CUDA_OK(cudaMalloc(dev, sizeof(St) * h.size()));
+    CUDA_OK(cudaMemcpy(*dev, h.data(), sizeof(St) * h.size(), cudaMemcpyHostToDevice));
+}
+
+// TrkStream has no embeddings pointer: the STrack family's appearance prep is handed the source with each launch
+static void set_embs(TrkStream&, float*) {}
+template <typename St> static void set_embs(St& s, float* embs) { s.embs = embs; }
+
+// Point the carved streams `h` at their slices of input set `set` and of the pending warps, and upload them to *dev.
+// Set 0 also records where each stream keeps its output rows, scalars and timers.
+template <typename St>
+void Engine::wire_streams(std::vector<St>& h, int set, St** dev) {
+    const size_t CD = cfg.cap_dets, F = cfg.feat_dim > 0 ? cfg.feat_dim : 1;
+    for (int i = 0; i < S; ++i) {
+        h[i].dets = in[set].dets + (size_t)i * CD * 6;
+        h[i].n_dets = in[set].ndets + i;
+        set_embs(h[i], cfg.with_reid ? in[set].embs + (size_t)i * CD * F : nullptr);
+        h[i].warp = d_warp + (size_t)i * 8;
+        if (set == 0) { out_ptr[i] = h[i].out; scalars_ptr[i] = h[i].scalars; timers_ptr[i] = h[i].timers; }
+    }
+    upload_streams(h, dev);
+}
+
 Engine::Engine(const BoxMOTB200TrackerConfig& p) {
     try {
         construct(p);
@@ -398,21 +407,22 @@ Engine::Engine(const BoxMOTB200TrackerConfig& p) {
 void Engine::construct(const BoxMOTB200TrackerConfig& p) {
     if (p.n_streams < 1) throw std::runtime_error("n_streams must be >= 1");
     if (p.cap_tracks < 8 || p.cap_dets < 1) throw std::runtime_error("cap_tracks >= 8 and cap_dets >= 1 required");
-    if (p.tracker != BOXMOT_B200_TRACKER_BOTSORT && p.tracker != BOXMOT_B200_TRACKER_BYTETRACK &&
-        p.tracker != BOXMOT_B200_TRACKER_DEEPOCSORT && p.tracker != BOXMOT_B200_TRACKER_STRONGSORT &&
-        p.tracker != BOXMOT_B200_TRACKER_BOOSTTRACK && p.tracker != BOXMOT_B200_TRACKER_OCCLUBOOST)
-        throw std::runtime_error("unknown tracker kind");
-    is_docs = p.tracker == BOXMOT_B200_TRACKER_DEEPOCSORT;
-    is_ss = p.tracker == BOXMOT_B200_TRACKER_STRONGSORT;
-    is_ob = p.tracker == BOXMOT_B200_TRACKER_OCCLUBOOST;
-    is_bt = p.tracker == BOXMOT_B200_TRACKER_BOOSTTRACK || is_ob;   // OccluBoost runs on the BoostTrack stream
+    switch (p.tracker) {
+        case BOXMOT_B200_TRACKER_BOTSORT:
+        case BOXMOT_B200_TRACKER_BYTETRACK: family = Family::STrack; break;
+        case BOXMOT_B200_TRACKER_DEEPOCSORT: family = Family::Docs; break;
+        case BOXMOT_B200_TRACKER_STRONGSORT: family = Family::StrongSort; break;
+        case BOXMOT_B200_TRACKER_BOOSTTRACK: family = Family::Boost; break;
+        case BOXMOT_B200_TRACKER_OCCLUBOOST: family = Family::Occlu; break;
+        default: throw std::runtime_error("unknown tracker kind");
+    }
     if (p.tracker == BOXMOT_B200_TRACKER_BOTSORT && p.removed_stracks_buffer < 1)
         throw std::runtime_error("removed_stracks_buffer must be >= 1");
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
         throw std::runtime_error("no CUDA device: boxmot_b200 has no CPU fallback");
     cfg = make_core_cfg(p);
-    if (is_docs) {
+    if (family == Family::Docs) {
         if (p.delta_t < 1 || p.delta_t >= DOCS_RING) throw std::runtime_error("delta_t must be in [1, 7]");
         if (p.max_age < 1 || p.max_age > 46) throw std::runtime_error("max_age must be in [1, 46] (reference history window)");
         dcfg.cap_tracks = p.cap_tracks; dcfg.cap_dets = p.cap_dets; dcfg.feat_dim = p.feat_dim;
@@ -426,7 +436,7 @@ void Engine::construct(const BoxMOTB200TrackerConfig& p) {
         cfg.feat_dim = cfg.with_reid ? p.feat_dim : 0;
         cfg.cap_tracks = p.cap_tracks; cfg.cap_dets = p.cap_dets;
     }
-    if (is_ss) {
+    if (family == Family::StrongSort) {
         if (p.n_init < 1) throw std::runtime_error("n_init must be >= 1");
         if (p.nn_budget < 1) throw std::runtime_error("nn_budget must be >= 1 (the reference's None = unbounded is not supported)");
         if (p.max_age < 1) throw std::runtime_error("max_age must be >= 1");
@@ -438,7 +448,7 @@ void Engine::construct(const BoxMOTB200TrackerConfig& p) {
         cfg.feat_dim = p.feat_dim;
         cfg.cap_tracks = p.cap_tracks; cfg.cap_dets = p.cap_dets;
     }
-    if (is_bt) {
+    if (on_bt_stream()) {
         if (p.max_age < 0 || p.max_age > 100000) throw std::runtime_error("max_age must be in [0, 100000]");
         if (p.min_hits < 0) throw std::runtime_error("min_hits must be >= 0");
         btcfg.cap_tracks = p.cap_tracks; btcfg.cap_dets = p.cap_dets;
@@ -463,9 +473,9 @@ void Engine::construct(const BoxMOTB200TrackerConfig& p) {
             cfg.feat_dim = reid_feature_dim(reid);
         }
     }
-    if (is_docs) dcfg.feat_dim = cfg.feat_dim;
-    if (is_bt) btcfg.feat_dim = cfg.feat_dim;
-    if (is_ob) {
+    if (family == Family::Docs) dcfg.feat_dim = cfg.feat_dim;
+    if (on_bt_stream()) btcfg.feat_dim = cfg.feat_dim;
+    if (family == Family::Occlu) {
         if (p.confirm_hits < 1 || p.tentative_max_age < 0 || p.ams_buffer_size < 2 || p.ams_buffer_size > 4096 ||
             p.gta_min_track_length < 1 || p.gta_max_gap < 1)
             throw std::runtime_error("OccluBoost needs confirm_hits >= 1, tentative_max_age >= 0, ams_buffer_size in "
@@ -488,27 +498,38 @@ void Engine::construct(const BoxMOTB200TrackerConfig& p) {
         obcfg.ams_threshold = p.ams_threshold; obcfg.ams_shrink_ratio = p.ams_shrink_ratio;
         obcfg.gta_appearance_thresh = p.gta_appearance_thresh;
     }
-    if (is_ss) {
+    if (family == Family::StrongSort) {
         scfg.feat_dim = cfg.feat_dim;
         if (scfg.feat_dim % 4) throw std::runtime_error("StrongSORT feat_dim must be a multiple of 4");
     }
-    stream_bytes = is_docs ? carve_docs(dcfg, nullptr, nullptr, &persistent_bytes)
-                 : is_ss   ? carve_ss(scfg, nullptr, nullptr, &persistent_bytes)
-                 : is_ob   ? carve_ob(obcfg, nullptr, nullptr, &persistent_bytes)
-                 : is_bt   ? carve_bt(btcfg, nullptr, nullptr, &persistent_bytes)
-                           : carve_stream(cfg, nullptr, nullptr, &persistent_bytes);
+    // every stream's slab of d_mem and the host copy of the struct carved out of it
+    auto carve_all = [&](auto carve, const auto& c, auto& h) {
+        stream_bytes = carve(c, nullptr, nullptr, &persistent_bytes);
+        CUDA_OK(cudaMalloc(&d_mem, stream_bytes * S));
+        CUDA_OK(cudaMemset(d_mem, 0, stream_bytes * S));
+        h.resize(S);
+        for (int i = 0; i < S; ++i) carve(c, d_mem + stream_bytes * i, &h[i], nullptr);
+    };
+    switch (family) {
+        case Family::STrack: carve_all(carve_stream, cfg, h_streams); break;
+        case Family::Docs: carve_all(carve_docs, dcfg, h_docs); break;
+        case Family::StrongSort: carve_all(carve_ss, scfg, h_ss); break;
+        case Family::Boost: carve_all(carve_bt, btcfg, h_bt); break;
+        case Family::Occlu:   // its BoostTrack part is what gets wired below; it is put back before the upload
+            carve_all(carve_ob, obcfg, h_ob);
+            for (const ObStream& o : h_ob) h_bt.push_back(o.b);
+            break;
+    }
     persistent_bytes = (persistent_bytes + 15) & ~(size_t)15;
-    CUDA_OK(cudaMalloc(&d_mem, stream_bytes * S));
-    CUDA_OK(cudaMemset(d_mem, 0, stream_bytes * S));
     const size_t CD = cfg.cap_dets, F = cfg.feat_dim > 0 ? cfg.feat_dim : 1;
-    CUDA_OK(cudaMalloc(&d_dets, sizeof(float) * 6 * CD * S));
+    CUDA_OK(cudaMalloc(&in[0].dets, sizeof(float) * 6 * CD * S));
     CUDA_OK(cudaMalloc(&d_warp, sizeof(double) * 8 * S));
     CUDA_OK(cudaMemset(d_warp, 0, sizeof(double) * 8 * S));
-    CUDA_OK(cudaMalloc(&d_ndets, sizeof(int) * S));
-    CUDA_OK(cudaMemset(d_ndets, 0, sizeof(int) * S));
+    CUDA_OK(cudaMalloc(&in[0].ndets, sizeof(int) * S));
+    CUDA_OK(cudaMemset(in[0].ndets, 0, sizeof(int) * S));
     if (cfg.with_reid) {
-        CUDA_OK(cudaMalloc(&d_embs, sizeof(float) * F * CD * S));
-        CUDA_OK(cudaMemset(d_embs, 0, sizeof(float) * F * CD * S));
+        CUDA_OK(cudaMalloc(&in[0].embs, sizeof(float) * F * CD * S));
+        CUDA_OK(cudaMemset(in[0].embs, 0, sizeof(float) * F * CD * S));
     }
     CUDA_OK(cudaMallocHost(&h_dets, sizeof(float) * 6 * CD * S));
     CUDA_OK(cudaMallocHost(&h_ndets, sizeof(int) * S));
@@ -518,19 +539,7 @@ void Engine::construct(const BoxMOTB200TrackerConfig& p) {
     CUDA_OK(cudaMalloc(&d_out, sizeof(float) * 8 * CD * S));
     CUDA_OK(cudaMalloc(&d_scalars_out, sizeof(int) * SC_COUNT * S));
     out_ptr.resize(S); scalars_ptr.resize(S); timers_ptr.resize(S);
-    if (is_ss) {
-        h_ss.resize(S);
-        for (int i = 0; i < S; ++i) {
-            carve_ss(scfg, d_mem + stream_bytes * i, &h_ss[i], nullptr);
-            h_ss[i].dets = d_dets + (size_t)i * CD * 6;
-            h_ss[i].n_dets = d_ndets + i;
-            h_ss[i].embs = d_embs + (size_t)i * CD * F;
-            h_ss[i].warp = d_warp + (size_t)i * 8;
-            out_ptr[i] = h_ss[i].out; scalars_ptr[i] = h_ss[i].scalars; timers_ptr[i] = h_ss[i].timers;
-        }
-        CUDA_OK(cudaMalloc(&d_ss, sizeof(SsStream) * S));
-        CUDA_OK(cudaMemcpy(d_ss, h_ss.data(), sizeof(SsStream) * S, cudaMemcpyHostToDevice));
-    } else if (is_bt) {
+    if (on_bt_stream()) {
         // KalmanBoxTracker.get_confidence: 0.9 ** k with the host's pow, which is what python's float power calls
         std::vector<double> pw((size_t)(p.max_age + 2 > 8 ? p.max_age + 2 : 8));
         for (size_t k = 0; k < pw.size(); ++k) pw[k] = pow(0.9, (double)k);
@@ -538,106 +547,32 @@ void Engine::construct(const BoxMOTB200TrackerConfig& p) {
         CUDA_OK(cudaMemcpy(d_conf_pow, pw.data(), sizeof(double) * pw.size(), cudaMemcpyHostToDevice));
         btcfg.conf_pow = d_conf_pow;
         btcfg.n_conf_pow = (int)pw.size();
-        obcfg.bt = btcfg;
-        h_bt.resize(S);
-        if (is_ob) h_ob.resize(S);
-        for (int i = 0; i < S; ++i) {
-            if (is_ob) {
-                carve_ob(obcfg, d_mem + stream_bytes * i, &h_ob[i], nullptr);
-                h_bt[i] = h_ob[i].b;
-            } else {
-                carve_bt(btcfg, d_mem + stream_bytes * i, &h_bt[i], nullptr);
-            }
-            h_bt[i].dets = d_dets + (size_t)i * CD * 6;
-            h_bt[i].n_dets = d_ndets + i;
-            h_bt[i].embs = cfg.with_reid ? d_embs + (size_t)i * CD * F : nullptr;
-            h_bt[i].warp = d_warp + (size_t)i * 8;
-            out_ptr[i] = h_bt[i].out; scalars_ptr[i] = h_bt[i].scalars; timers_ptr[i] = h_bt[i].timers;
-        }
-        CUDA_OK(cudaMalloc(&d_bt, sizeof(BtStream) * S));
-        CUDA_OK(cudaMemcpy(d_bt, h_bt.data(), sizeof(BtStream) * S, cudaMemcpyHostToDevice));
-        if (is_ob) {
-            for (int i = 0; i < S; ++i) h_ob[i].b = h_bt[i];
-            CUDA_OK(cudaMalloc(&d_ob, sizeof(ObStream) * S));
-            CUDA_OK(cudaMemcpy(d_ob, h_ob.data(), sizeof(ObStream) * S, cudaMemcpyHostToDevice));
-        }
-    } else if (is_docs) {
-        h_docs.resize(S);
-        for (int i = 0; i < S; ++i) {
-            carve_docs(dcfg, d_mem + stream_bytes * i, &h_docs[i], nullptr);
-            h_docs[i].dets = d_dets + (size_t)i * CD * 6;
-            h_docs[i].n_dets = d_ndets + i;
-            h_docs[i].embs = cfg.with_reid ? d_embs + (size_t)i * CD * F : nullptr;
-            h_docs[i].warp = d_warp + (size_t)i * 8;
-            out_ptr[i] = h_docs[i].out; scalars_ptr[i] = h_docs[i].scalars; timers_ptr[i] = h_docs[i].timers;
-        }
-        CUDA_OK(cudaMalloc(&d_docs, sizeof(DocsStream) * S));
-        CUDA_OK(cudaMemcpy(d_docs, h_docs.data(), sizeof(DocsStream) * S, cudaMemcpyHostToDevice));
-        // ids start at 1 (KalmanBoxTracker.count = 1 in DeepOcSort.__init__); SC_NEXT_ID holds the last id used
-    } else {
-        h_streams.resize(S);
-        for (int i = 0; i < S; ++i) {
-            carve_stream(cfg, d_mem + stream_bytes * i, &h_streams[i], nullptr);
-            h_streams[i].dets = d_dets + (size_t)i * CD * 6;
-            h_streams[i].n_dets = d_ndets + i;
-            h_streams[i].warp = d_warp + (size_t)i * 8;
-            out_ptr[i] = h_streams[i].out; scalars_ptr[i] = h_streams[i].scalars; timers_ptr[i] = h_streams[i].timers;
-        }
-        CUDA_OK(cudaMalloc(&d_streams, sizeof(TrkStream) * S));
-        CUDA_OK(cudaMemcpy(d_streams, h_streams.data(), sizeof(TrkStream) * S, cudaMemcpyHostToDevice));
+        obcfg.bt = btcfg;   // again: the copy taken with the OccluBoost parameters above predates conf_pow
     }
-    if (reid && cfg.with_reid) {   // second input set for the frame pipeline of update_device (all families)
+    const bool two_sets = reid && cfg.with_reid;   // second input set for the frame pipeline of update_device
+    if (two_sets) {
         CUDA_OK(cudaStreamCreateWithFlags(&reid_stream, cudaStreamNonBlocking));
-        CUDA_OK(cudaMalloc(&d_dets_alt, sizeof(float) * 6 * CD * S));
-        CUDA_OK(cudaMalloc(&d_ndets_alt, sizeof(int) * S));
-        CUDA_OK(cudaMemset(d_ndets_alt, 0, sizeof(int) * S));
-        CUDA_OK(cudaMalloc(&d_embs_alt, sizeof(float) * F * CD * S));
-        CUDA_OK(cudaMemset(d_embs_alt, 0, sizeof(float) * F * CD * S));
-        if (is_ss) {
-            std::vector<SsStream> alt = h_ss;
-            for (int i = 0; i < S; ++i) {
-                alt[i].dets = d_dets_alt + (size_t)i * CD * 6;
-                alt[i].n_dets = d_ndets_alt + i;
-                alt[i].embs = d_embs_alt + (size_t)i * CD * F;
-            }
-            CUDA_OK(cudaMalloc(&d_ss_alt, sizeof(SsStream) * S));
-            CUDA_OK(cudaMemcpy(d_ss_alt, alt.data(), sizeof(SsStream) * S, cudaMemcpyHostToDevice));
-        } else if (is_bt) {
-            std::vector<BtStream> alt = h_bt;
-            for (int i = 0; i < S; ++i) {
-                alt[i].dets = d_dets_alt + (size_t)i * CD * 6;
-                alt[i].n_dets = d_ndets_alt + i;
-                alt[i].embs = d_embs_alt + (size_t)i * CD * F;
-            }
-            CUDA_OK(cudaMalloc(&d_bt_alt, sizeof(BtStream) * S));
-            CUDA_OK(cudaMemcpy(d_bt_alt, alt.data(), sizeof(BtStream) * S, cudaMemcpyHostToDevice));
-            if (is_ob) {
-                std::vector<ObStream> alt_ob = h_ob;
-                for (int i = 0; i < S; ++i) alt_ob[i].b = alt[i];
-                CUDA_OK(cudaMalloc(&d_ob_alt, sizeof(ObStream) * S));
-                CUDA_OK(cudaMemcpy(d_ob_alt, alt_ob.data(), sizeof(ObStream) * S, cudaMemcpyHostToDevice));
-            }
-        } else if (is_docs) {
-            std::vector<DocsStream> alt = h_docs;
-            for (int i = 0; i < S; ++i) {
-                alt[i].dets = d_dets_alt + (size_t)i * CD * 6;
-                alt[i].n_dets = d_ndets_alt + i;
-                alt[i].embs = d_embs_alt + (size_t)i * CD * F;
-            }
-            CUDA_OK(cudaMalloc(&d_docs_alt, sizeof(DocsStream) * S));
-            CUDA_OK(cudaMemcpy(d_docs_alt, alt.data(), sizeof(DocsStream) * S, cudaMemcpyHostToDevice));
-        } else {
-            h_streams_alt = h_streams;
-            for (int i = 0; i < S; ++i) {
-                h_streams_alt[i].dets = d_dets_alt + (size_t)i * CD * 6;
-                h_streams_alt[i].n_dets = d_ndets_alt + i;
-            }
-            CUDA_OK(cudaMalloc(&d_streams_alt, sizeof(TrkStream) * S));
-            CUDA_OK(cudaMemcpy(d_streams_alt, h_streams_alt.data(), sizeof(TrkStream) * S, cudaMemcpyHostToDevice));
-        }
+        CUDA_OK(cudaMalloc(&in[1].dets, sizeof(float) * 6 * CD * S));
+        CUDA_OK(cudaMalloc(&in[1].ndets, sizeof(int) * S));
+        CUDA_OK(cudaMemset(in[1].ndets, 0, sizeof(int) * S));
+        CUDA_OK(cudaMalloc(&in[1].embs, sizeof(float) * F * CD * S));
+        CUDA_OK(cudaMemset(in[1].embs, 0, sizeof(float) * F * CD * S));
         for (int k = 0; k < 2; ++k) {
             CUDA_OK(cudaEventCreateWithFlags(&ev_reid_done[k], cudaEventDisableTiming));
             CUDA_OK(cudaEventCreateWithFlags(&ev_assoc_done[k], cudaEventDisableTiming));
+        }
+    }
+    for (int set = two_sets ? 1 : 0; set >= 0; --set) {   // set 0 last: the host copies stay pointed at it
+        switch (family) {
+            case Family::STrack: wire_streams(h_streams, set, &in[set].trk); break;
+            case Family::Docs: wire_streams(h_docs, set, &in[set].docs); break;
+            case Family::StrongSort: wire_streams(h_ss, set, &in[set].ss); break;
+            case Family::Boost: wire_streams(h_bt, set, &in[set].bt); break;
+            case Family::Occlu:
+                wire_streams(h_bt, set, &in[set].bt);
+                for (int i = 0; i < S; ++i) h_ob[i].b = h_bt[i];
+                upload_streams(h_ob, &in[set].ob);
+                break;
         }
     }
     if (reid) {
@@ -689,14 +624,16 @@ void Engine::release() {
             if (ev_reid_done[k]) cudaEventDestroy(ev_reid_done[k]);
             if (ev_assoc_done[k]) cudaEventDestroy(ev_assoc_done[k]);
         }
-        cudaFree(d_dets_alt); cudaFree(d_ndets_alt); cudaFree(d_embs_alt); cudaFree(d_streams_alt);
-        cudaFree(d_docs_alt); cudaFree(d_ss_alt); cudaFree(d_bt_alt); cudaFree(d_ob_alt);
     }
     if (reid) reid_free(reid);
     cudaFree(d_cmc_prev); cudaFree(d_cmc_cur); cudaFree(d_cmc_has_prev); cudaFree(d_cmc_gate);
     if (sof) sof_state_free(sof);
-    cudaFree(d_warp); cudaFree(d_mem); cudaFree(d_dets); cudaFree(d_ndets); cudaFree(d_embs); cudaFree(d_out);
-    cudaFree(d_scalars_out); cudaFree(d_streams); cudaFree(d_docs); cudaFree(d_ss); cudaFree(d_bt); cudaFree(d_ob); cudaFree(d_conf_pow); cudaFree(d_crops); cudaFree(d_ncrops); cudaFree(d_images);
+    for (InputSet& s : in) {
+        cudaFree(s.dets); cudaFree(s.ndets); cudaFree(s.embs);
+        cudaFree(s.trk); cudaFree(s.docs); cudaFree(s.ss); cudaFree(s.bt); cudaFree(s.ob);
+    }
+    cudaFree(d_warp); cudaFree(d_mem); cudaFree(d_out); cudaFree(d_scalars_out); cudaFree(d_conf_pow);
+    cudaFree(d_crops); cudaFree(d_ncrops); cudaFree(d_images);
     cudaFreeHost(h_dets); cudaFreeHost(h_ndets); cudaFreeHost(h_out); cudaFreeHost(h_scalars);
     cudaFreeHost(h_embs); cudaFreeHost(h_images); cudaFreeHost(h_ndets_ring);
     if (mark[0]) cudaEventDestroy(mark[0]);
@@ -710,13 +647,13 @@ void Engine::reset() {
     if (reid_stream) CUDA_OK(cudaStreamSynchronize(reid_stream));
     if (d_cmc_has_prev) CUDA_OK(cudaMemsetAsync(d_cmc_has_prev, 0, sizeof(int) * S, stream));   // ECC.prev_img = None
     if (sof) sof_state_reset(sof, stream);   // a fresh SOF: the next frame initialises
-    if (is_docs || is_ss || is_bt) {
+    if (family != Family::STrack) {
         CUDA_OK(cudaStreamSynchronize(stream));
         for (int i = 0; i < S; ++i) CUDA_OK(cudaMemsetAsync(d_mem + stream_bytes * i, 0, persistent_bytes, stream));
         CUDA_OK(cudaStreamSynchronize(stream));
         return;
     }
-    k_reset_streams<<<S, 256, 0, stream>>>(d_streams, persistent_bytes);
+    k_reset_streams<<<S, 256, 0, stream>>>(in[0].trk, persistent_bytes);
     CUDA_OK(cudaGetLastError());
     CUDA_OK(cudaStreamSynchronize(stream));
 }
@@ -732,122 +669,29 @@ void Engine::ensure_images(int rows, int cols, bool host_too) {
     if (host_too && !h_images) CUDA_OK(cudaMallocHost(&h_images, image_bytes * S));
 }
 
-// Enqueue the device work of one frame.  Inputs already in d_dets / d_ndets (+ embs or images).
+// Enqueue the device work of one frame.  Inputs already in input set 0 (+ embs or images).
 void Engine::enqueue_frame(const float* embs_dev, const uint8_t* images_dev, int rows, int cols, int max_dets_total) {
     launches = 0;
     CUDA_OK(cudaEventRecord(ev[0], stream));
     ev_recorded = true;
     if (cmc_mode) enqueue_cmc(images_dev, rows, cols);
-    if (is_ss) {
-        const size_t CD = cfg.cap_dets, F = cfg.feat_dim;
-        if (!embs_dev) {
-            if (!reid) throw std::runtime_error("StrongSORT needs embeddings or a ReID model");
-            if (!images_dev) throw std::runtime_error("ReID inside update() needs an image");
-            ss_build_crops(scfg, d_ss, S, d_crops, d_ncrops, d_crops_hint, stream);
-            ++launches;
-            launches += run_reid(stream, images_dev, rows, cols, max_dets_total, d_embs);
-        } else if (embs_dev != d_embs) {
-            CUDA_OK(cudaMemcpyAsync(d_embs, embs_dev, sizeof(float) * F * CD * S, cudaMemcpyDeviceToDevice, stream));
-        }
-        CUDA_OK(cudaEventRecord(ev[1], stream));
-        launches += ss_enqueue_frame(scfg, d_ss, S, stream);
-        if (warp_dirty) {
-            CUDA_OK(cudaMemsetAsync(d_warp, 0, sizeof(double) * 8 * S, stream));
-            warp_dirty = false;
-        }
-        CUDA_OK(cudaEventRecord(ev[2], stream));
-        if (profile) {
-            CUDA_OK(cudaStreamSynchronize(stream));
-            float b = 0.f;
-            cudaEventElapsedTime(&b, ev[1], ev[2]);
-            assoc_ms_accum += b;
-            assoc_frames += 1;
-        }
-        return;
+    if (cfg.with_reid && !embs_dev) {
+        if (!reid)
+            throw std::runtime_error(family == Family::StrongSort ? "StrongSORT needs embeddings or a ReID model"
+                                     : family == Family::Docs     ? "DeepOCSORT needs embeddings, a ReID model, or embedding_off"
+                                     : on_bt_stream()             ? "BoostTrack with_reid needs embeddings or a ReID model"
+                                                                  : "with_reid tracker needs embeddings or a ReID model");
+        if (!images_dev) throw std::runtime_error("ReID inside update() needs an image");
+        enqueue_crops(0, stream);
+        launches += run_reid(stream, images_dev, rows, cols, max_dets_total, in[0].embs);
+    } else if (cfg.with_reid && family != Family::STrack && embs_dev != in[0].embs) {
+        // caller-supplied device embeddings (update_device / DeviceFrameLoop): these families' kernels read the engine's
+        // buffer through their stream structs; the STrack family's appearance prep reads the caller's pointer in place
+        CUDA_OK(cudaMemcpyAsync(in[0].embs, embs_dev, sizeof(float) * (size_t)cfg.feat_dim * cfg.cap_dets * S,
+                                cudaMemcpyDeviceToDevice, stream));
     }
-    if (is_bt) {
-        if (cfg.with_reid && !embs_dev) {
-            if (!reid) throw std::runtime_error("BoostTrack with_reid needs embeddings or a ReID model");
-            if (!images_dev) throw std::runtime_error("ReID inside update() needs an image");
-            k_build_crops_bt<<<1, 32, 0, stream>>>(btcfg, d_bt, S, d_crops, d_ncrops, d_crops_hint);
-            ++launches;
-            launches += run_reid(stream, images_dev, rows, cols, max_dets_total, d_embs);
-        } else if (cfg.with_reid && embs_dev && embs_dev != d_embs) {
-            CUDA_OK(cudaMemcpyAsync(d_embs, embs_dev, sizeof(float) * (size_t)cfg.feat_dim * cfg.cap_dets * S,
-                                    cudaMemcpyDeviceToDevice, stream));
-        }
-        CUDA_OK(cudaEventRecord(ev[1], stream));
-        enqueue_bt(d_bt, d_ob);
-        CUDA_OK(cudaGetLastError());
-        CUDA_OK(cudaEventRecord(ev[2], stream));
-        if (profile) {
-            CUDA_OK(cudaStreamSynchronize(stream));
-            float b = 0.f;
-            cudaEventElapsedTime(&b, ev[1], ev[2]);
-            assoc_ms_accum += b;
-            assoc_frames += 1;
-        }
-        return;
-    }
-    if (is_docs) {
-        if (cfg.with_reid && !embs_dev) {
-            if (!reid) throw std::runtime_error("DeepOCSORT needs embeddings, a ReID model, or embedding_off");
-            if (!images_dev) throw std::runtime_error("ReID inside update() needs an image");
-            k_build_crops_docs<<<1, 32, 0, stream>>>(dcfg, d_docs, S, d_crops, d_ncrops, d_crops_hint);
-            ++launches;
-            launches += run_reid(stream, images_dev, rows, cols, max_dets_total, d_embs);
-        } else if (cfg.with_reid && embs_dev && embs_dev != d_embs) {
-            // caller-supplied device embeddings (update_device / DeviceFrameLoop): the kernels read the engine's buffer
-            CUDA_OK(cudaMemcpyAsync(d_embs, embs_dev, sizeof(float) * (size_t)cfg.feat_dim * cfg.cap_dets * S,
-                                    cudaMemcpyDeviceToDevice, stream));
-        }
-        CUDA_OK(cudaEventRecord(ev[1], stream));
-        if (cfg.with_reid) {
-            dim3 g((dcfg.cap_dets + EMB_TD - 1) / EMB_TD, (dcfg.cap_tracks + EMB_TR - 1) / EMB_TR, S);
-            k_docs_embcost<<<g, 256, 0, stream>>>(dcfg, d_docs);
-            ++launches;
-        }
-        {
-            const int MX = dcfg.cap_tracks > dcfg.cap_dets ? dcfg.cap_tracks : dcfg.cap_dets;
-            const size_t jb = jv_smem_bytes(MX);
-            const bool in_smem = jb <= 200 * 1024;
-            if (in_smem && jb > 48 * 1024)
-                CUDA_OK(cudaFuncSetAttribute(k_docs_frame, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)jb));
-            k_docs_frame<<<S, 256, in_smem ? jb : 0, stream>>>(dcfg, d_docs, (in_smem ? 1 : 0) | (jv_wide_default() << 1));
-        }
-        ++launches;
-        if (warp_dirty) {  // a supplied camera-motion warp applies to exactly one frame
-            CUDA_OK(cudaMemsetAsync(d_warp, 0, sizeof(double) * 8 * S, stream));
-            warp_dirty = false;
-        }
-        CUDA_OK(cudaGetLastError());
-        CUDA_OK(cudaEventRecord(ev[2], stream));
-        if (profile) {
-            CUDA_OK(cudaStreamSynchronize(stream));
-            float b = 0.f;
-            cudaEventElapsedTime(&b, ev[1], ev[2]);
-            assoc_ms_accum += b;
-            assoc_frames += 1;
-        }
-        return;
-    }
-    if (cfg.with_reid) {
-        const float* src = embs_dev;
-        if (!src) {
-            if (!reid) throw std::runtime_error("with_reid tracker needs embeddings or a ReID model");
-            if (!images_dev) throw std::runtime_error("ReID inside update() needs an image");
-            k_build_crops<<<1, 32, 0, stream>>>(cfg, d_streams, S, d_crops, d_ncrops, d_crops_hint);
-            ++launches;
-            launches += run_reid(stream, images_dev, rows, cols, max_dets_total, d_embs);
-            src = d_embs;
-        }
-        CUDA_OK(cudaEventRecord(ev[1], stream));
-        enqueue_association(d_streams, src);
-    } else {
-        CUDA_OK(cudaEventRecord(ev[1], stream));
-        enqueue_association(d_streams, nullptr);
-    }
-    CUDA_OK(cudaGetLastError());
+    CUDA_OK(cudaEventRecord(ev[1], stream));
+    enqueue_family_association(0, embs_dev);
     CUDA_OK(cudaEventRecord(ev[2], stream));
     if (profile) {  // profiling pass: serialise and attribute device time per kernel class
         CUDA_OK(cudaStreamSynchronize(stream));
@@ -858,51 +702,49 @@ void Engine::enqueue_frame(const float* embs_dev, const uint8_t* images_dev, int
     }
 }
 
-// crop list of the tracker family from input set `parity` (0: d_dets / d_ndets, 1: the alternate set)
+// crop list of the tracker family from input set `parity`
 void Engine::enqueue_crops(int parity, cudaStream_t st) {
-    if (is_ss) ss_build_crops(scfg, parity ? d_ss_alt : d_ss, S, d_crops, d_ncrops, d_crops_hint, st);
-    else if (is_bt) k_build_crops_bt<<<1, 32, 0, st>>>(btcfg, parity ? d_bt_alt : d_bt, S, d_crops, d_ncrops, d_crops_hint);
-    else if (is_docs) k_build_crops_docs<<<1, 32, 0, st>>>(dcfg, parity ? d_docs_alt : d_docs, S, d_crops, d_ncrops, d_crops_hint);
-    else k_build_crops<<<1, 32, 0, st>>>(cfg, parity ? d_streams_alt : d_streams, S, d_crops, d_ncrops, d_crops_hint);
+    const InputSet& set = in[parity];
+    switch (family) {
+        case Family::STrack: k_build_crops<<<1, 32, 0, st>>>(cfg, set.trk, S, d_crops, d_ncrops, d_crops_hint); break;
+        case Family::Docs: k_build_crops<<<1, 32, 0, st>>>(dcfg, set.docs, S, d_crops, d_ncrops, d_crops_hint); break;
+        case Family::StrongSort: ss_build_crops(scfg, set.ss, S, d_crops, d_ncrops, d_crops_hint, st); break;
+        case Family::Boost:
+        case Family::Occlu: k_build_crops<<<1, 32, 0, st>>>(btcfg, set.bt, S, d_crops, d_ncrops, d_crops_hint); break;
+    }
     ++launches;
 }
 
-// association launches of the family on `stream`, reading input set `parity` (embeddings included)
-void Engine::enqueue_family_association(int parity) {
-    if (is_ss) {
-        launches += ss_enqueue_frame(scfg, parity ? d_ss_alt : d_ss, S, stream);
-        if (warp_dirty) {
-            CUDA_OK(cudaMemsetAsync(d_warp, 0, sizeof(double) * 8 * S, stream));
-            warp_dirty = false;
-        }
-    } else if (is_bt) {
-        enqueue_bt(parity ? d_bt_alt : d_bt, parity ? d_ob_alt : d_ob);
-    } else if (is_docs) {
-        DocsStream* ds = parity ? d_docs_alt : d_docs;
-        if (cfg.with_reid) {
-            dim3 g((dcfg.cap_dets + EMB_TD - 1) / EMB_TD, (dcfg.cap_tracks + EMB_TR - 1) / EMB_TR, S);
-            k_docs_embcost<<<g, 256, 0, stream>>>(dcfg, ds);
+// association launches of the family on `stream`, reading input set `parity` (embeddings included, except that the
+// STrack family reads `embs_src` when one is given); a supplied or estimated camera-motion warp applies to this frame only
+void Engine::enqueue_family_association(int parity, const float* embs_src) {
+    const InputSet& set = in[parity];
+    switch (family) {
+        case Family::STrack: enqueue_association(set.trk, embs_src ? embs_src : set.embs); break;
+        case Family::StrongSort: launches += ss_enqueue_frame(scfg, set.ss, S, stream); break;
+        case Family::Boost:
+        case Family::Occlu: enqueue_bt(set.bt, set.ob); break;
+        case Family::Docs: {
+            if (cfg.with_reid) {
+                dim3 g((dcfg.cap_dets + EMB_TD - 1) / EMB_TD, (dcfg.cap_tracks + EMB_TR - 1) / EMB_TR, S);
+                k_docs_embcost<<<g, 256, 0, stream>>>(dcfg, set.docs);
+                ++launches;
+            }
+            size_t smem;
+            const int jv_arg = jv_launch_setup(k_docs_frame, dcfg.cap_tracks, dcfg.cap_dets, &smem);
+            k_docs_frame<<<S, 256, smem, stream>>>(dcfg, set.docs, jv_arg);
             ++launches;
+            break;
         }
-        const int MX = dcfg.cap_tracks > dcfg.cap_dets ? dcfg.cap_tracks : dcfg.cap_dets;
-        const size_t jb = jv_smem_bytes(MX);
-        const bool in_smem = jb <= 200 * 1024;
-        if (in_smem && jb > 48 * 1024)
-            CUDA_OK(cudaFuncSetAttribute(k_docs_frame, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)jb));
-        k_docs_frame<<<S, 256, in_smem ? jb : 0, stream>>>(dcfg, ds, (in_smem ? 1 : 0) | (jv_wide_default() << 1));
-        ++launches;
-        if (warp_dirty) {
-            CUDA_OK(cudaMemsetAsync(d_warp, 0, sizeof(double) * 8 * S, stream));
-            warp_dirty = false;
-        }
-    } else {
-        enqueue_association(parity ? d_streams_alt : d_streams, cfg.with_reid ? (parity ? d_embs_alt : d_embs) : nullptr);
+    }
+    if (warp_dirty) {
+        CUDA_OK(cudaMemsetAsync(d_warp, 0, sizeof(double) * 8 * S, stream));
+        warp_dirty = false;
     }
     CUDA_OK(cudaGetLastError());
 }
 
-// BoostTrack: embedding dot products (wide grid) and the per-stream frame kernel on `stream`; a supplied or estimated
-// warp applies to this frame only
+// BoostTrack / OccluBoost: embedding dot products (wide grid) and the per-stream frame kernel on `stream`
 void Engine::enqueue_bt(BtStream* streams_dev, ObStream* ob_dev) {
     BtCfg c = btcfg;
     c.cmc_every_frame = cmc_mode != 0;   // boosttrack.py:318-321: camera_update runs whenever an estimator exists
@@ -911,26 +753,17 @@ void Engine::enqueue_bt(BtStream* streams_dev, ObStream* ob_dev) {
         k_bt_embcost<<<g, 256, 0, stream>>>(c, streams_dev);
         ++launches;
     }
-    const int MX = c.cap_tracks > c.cap_dets ? c.cap_tracks : c.cap_dets;
-    const size_t jb = jv_smem_bytes(MX);
-    const bool in_smem = jb <= 200 * 1024;
-    const int jv_arg = (in_smem ? 1 : 0) | (jv_wide_default() << 1);
-    if (is_ob) {
+    size_t smem;
+    if (family == Family::Occlu) {
         ObCfg oc = obcfg;
         oc.bt = c;
-        if (in_smem && jb > 48 * 1024)
-            CUDA_OK(cudaFuncSetAttribute(k_ob_frame, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)jb));
-        k_ob_frame<<<S, 256, in_smem ? jb : 0, stream>>>(oc, ob_dev, jv_arg);
+        const int jv_arg = jv_launch_setup(k_ob_frame, c.cap_tracks, c.cap_dets, &smem);
+        k_ob_frame<<<S, 256, smem, stream>>>(oc, ob_dev, jv_arg);
     } else {
-        if (in_smem && jb > 48 * 1024)
-            CUDA_OK(cudaFuncSetAttribute(k_bt_frame, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)jb));
-        k_bt_frame<<<S, 256, in_smem ? jb : 0, stream>>>(c, streams_dev, jv_arg);
+        const int jv_arg = jv_launch_setup(k_bt_frame, c.cap_tracks, c.cap_dets, &smem);
+        k_bt_frame<<<S, 256, smem, stream>>>(c, streams_dev, jv_arg);
     }
     ++launches;
-    if (warp_dirty) {
-        CUDA_OK(cudaMemsetAsync(d_warp, 0, sizeof(double) * 8 * S, stream));
-        warp_dirty = false;
-    }
 }
 
 // crop list (already built on main_stream) -> embeddings; slices of the list run concurrently on the helper streams
@@ -978,10 +811,6 @@ void Engine::enqueue_association(TrkStream* streams_dev, const float* embs_src) 
         k_feat_ema<<<dim3((cfg.cap_dets + 7) / 8, S), 256, 0, stream>>>(cfg, streams_dev);
         ++launches;
     }
-    if (warp_dirty) {  // a supplied camera-motion warp applies to exactly one frame
-        CUDA_OK(cudaMemsetAsync(d_warp, 0, sizeof(double) * 8 * S, stream));
-        warp_dirty = false;
-    }
 }
 
 // On-device camera-motion estimation: the reference's ECC estimator with its defaults (motion/cmc/ecc.py:23-31), used
@@ -993,7 +822,7 @@ void Engine::set_cmc(const char* method) {
     if (strcmp(method, "sof") == 0) {
         // botsort.py:142,301 (every frame, every detection row) and deepocsort.py:330-349 (every frame, the rows with
         // conf > det_thresh); StrongSORT's estimator is ECC
-        if (is_ss || (!is_docs && !is_bt && cfg.kind != KIND_XYWH))
+        if (family == Family::StrongSort || is_bytetrack())
             throw std::runtime_error("on-device SOF applies to BoT-SORT and DeepOCSORT (StrongSORT's estimator is ecc)");
         if (!sof) sof = sof_state_create(S, 0.15, 8, 0.2, 3.0);
         else if (cmc_mode != 2) sof_state_reset(sof, stream);
@@ -1003,9 +832,9 @@ void Engine::set_cmc(const char* method) {
     if (strcmp(method, "ecc") != 0)
         throw std::runtime_error(std::string("camera-motion method '") + method + "' is not built on the device (ecc, sof, "
                                  "none); orb / sift warps can be supplied through set_warp");
-    if ((!is_ss && !is_docs && !is_bt && cfg.kind != KIND_XYWH) || is_docs)
+    if (is_bytetrack() || family == Family::Docs)
         throw std::runtime_error("on-device ECC applies to BoT-SORT and StrongSORT (ByteTrack has no CMC, DeepOCSORT's is sof)");
-    if (is_ss && !d_cmc_gate) {   // StrongSORT estimates only while tracks exist
+    if (family == Family::StrongSort && !d_cmc_gate) {   // StrongSORT estimates only while tracks exist
         std::vector<const int*> g(S);
         for (int i = 0; i < S; ++i) g[i] = h_ss[i].scalars + SC_N_ACTIVE;
         CUDA_OK(cudaMalloc(&d_cmc_gate, sizeof(const int*) * S));
@@ -1020,8 +849,9 @@ void Engine::enqueue_cmc(const uint8_t* images_dev, int rows, int cols) {
     cmc_scaled_size(rows, cols, cmc_scale, &h, &w);
     if (h < 3 || w < 3) throw std::runtime_error("camera-motion estimation: frame too small for the registration scale");
     if (cmc_mode == 2) {
-        launches += sof_state_enqueue(sof, images_dev, (size_t)rows * cols * 3, rows, cols, d_dets, d_ndets, (int)cfg.cap_dets,
-                                      6, is_docs ? 4 : -1, is_docs ? dcfg.det_thresh_f32 : 0.f, d_warp, stream);
+        const bool docs = family == Family::Docs;
+        launches += sof_state_enqueue(sof, images_dev, (size_t)rows * cols * 3, rows, cols, in[0].dets, in[0].ndets,
+                                      (int)cfg.cap_dets, 6, docs ? 4 : -1, docs ? dcfg.det_thresh_f32 : 0.f, d_warp, stream);
         warp_dirty = true;   // the estimate applies to this frame only
         return;
     }
@@ -1042,7 +872,7 @@ void Engine::enqueue_cmc(const uint8_t* images_dev, int rows, int cols) {
 
 void Engine::set_warp(int sidx, const double* warp6) {
     if (sidx < 0 || sidx >= S) throw std::runtime_error("stream index out of range");
-    if (!is_ss && !is_docs && !is_bt && cfg.kind != KIND_XYWH)
+    if (is_bytetrack())
         throw std::runtime_error("camera-motion warps apply to BoT-SORT, DeepOCSORT and StrongSORT (ByteTrack has none)");
     double w[8] = {warp6[0], warp6[1], warp6[2], warp6[3], warp6[4], warp6[5], 1.0, 0.0};
     CUDA_OK(cudaStreamSynchronize(stream));
@@ -1071,7 +901,7 @@ void Engine::profile_read(double* ms, int* launch_counts) {
     for (int c = 0; c < REID_N_CLASSES + 1; ++c) { ms[c] = 0.0; launch_counts[c] = 0; }
     if (reid) reid_profile_collect(reid, ms, launch_counts);
     ms[REID_N_CLASSES] = assoc_ms_accum;
-    launch_counts[REID_N_CLASSES] = assoc_frames * ((is_docs || is_bt) ? (cfg.with_reid ? 2 : 1) : (cfg.with_reid ? 4 : 1));
+    launch_counts[REID_N_CLASSES] = assoc_frames * ((family == Family::Docs || on_bt_stream()) ? (cfg.with_reid ? 2 : 1) : (cfg.with_reid ? 4 : 1));
     assoc_ms_accum = 0.0;
     assoc_frames = 0;
 }
@@ -1149,14 +979,14 @@ void Engine::update_batch(const float* const* dets, const int* det_rows, const f
             memcpy(h_embs + (size_t)i * CD * F, embs[i], sizeof(float) * F * n);
         }
     }
-    CUDA_OK(cudaMemcpyAsync(d_ndets, h_ndets, sizeof(int) * S, cudaMemcpyHostToDevice, stream));
+    CUDA_OK(cudaMemcpyAsync(in[0].ndets, h_ndets, sizeof(int) * S, cudaMemcpyHostToDevice, stream));
     // one strided copy moves every stream's occupied prefix; simpler: copy whole staging when small
     for (int i = 0; i < S; ++i) {
         if (!h_ndets[i]) continue;
-        CUDA_OK(cudaMemcpyAsync(d_dets + (size_t)i * CD * 6, h_dets + (size_t)i * CD * 6,
+        CUDA_OK(cudaMemcpyAsync(in[0].dets + (size_t)i * CD * 6, h_dets + (size_t)i * CD * 6,
                                 sizeof(float) * 6 * h_ndets[i], cudaMemcpyHostToDevice, stream));
         if (have_embs)
-            CUDA_OK(cudaMemcpyAsync(d_embs + (size_t)i * CD * F, h_embs + (size_t)i * CD * F,
+            CUDA_OK(cudaMemcpyAsync(in[0].embs + (size_t)i * CD * F, h_embs + (size_t)i * CD * F,
                                     sizeof(float) * F * h_ndets[i], cudaMemcpyHostToDevice, stream));
     }
     const uint8_t* img_dev = nullptr;
@@ -1187,7 +1017,7 @@ void Engine::update_batch(const float* const* dets, const int* det_rows, const f
         }
         img_dev = d_images;
     }
-    enqueue_frame(have_embs ? d_embs : nullptr, img_dev, rows, cols, total);
+    enqueue_frame(have_embs ? in[0].embs : nullptr, img_dev, rows, cols, total);
     enqueue_fetch();
     finish_fetch(out, out_cap, out_rows);
 }
@@ -1207,17 +1037,15 @@ void Engine::update_device(const float* dets_dev, const int* det_rows, const flo
         // embeddings are there; the ReID of the next frame overlaps this frame's association
         const int pp = pipe_parity;
         pipe_parity ^= 1;
-        float* dd = pp ? d_dets_alt : d_dets;
-        int* dn = pp ? d_ndets_alt : d_ndets;
-        float* de = pp ? d_embs_alt : d_embs;
+        const InputSet& set = in[pp];
         CUDA_OK(cudaStreamWaitEvent(reid_stream, ev_assoc_done[pp], 0));   // set p is free again
-        CUDA_OK(cudaMemcpyAsync(dn, slot, sizeof(int) * S, cudaMemcpyHostToDevice, reid_stream));
-        if (dets_dev != dd)
-            CUDA_OK(cudaMemcpyAsync(dd, dets_dev, sizeof(float) * 6 * CD * S, cudaMemcpyDeviceToDevice, reid_stream));
+        CUDA_OK(cudaMemcpyAsync(set.ndets, slot, sizeof(int) * S, cudaMemcpyHostToDevice, reid_stream));
+        if (dets_dev != set.dets)
+            CUDA_OK(cudaMemcpyAsync(set.dets, dets_dev, sizeof(float) * 6 * CD * S, cudaMemcpyDeviceToDevice, reid_stream));
         launches = 0;
         ev_recorded = false;   // the per-frame ReID / association split is not timed in pipelined mode
         enqueue_crops(pp, reid_stream);
-        launches += run_reid(reid_stream, images_dev, rows, cols, total, de);
+        launches += run_reid(reid_stream, images_dev, rows, cols, total, set.embs);
         CUDA_OK(cudaEventRecord(ev_reid_done[pp], reid_stream));
         CUDA_OK(cudaStreamWaitEvent(stream, ev_reid_done[pp], 0));
         enqueue_family_association(pp);
@@ -1225,9 +1053,9 @@ void Engine::update_device(const float* dets_dev, const int* det_rows, const flo
         return;
     }
     if (reid_stream) CUDA_OK(cudaStreamSynchronize(reid_stream));   // leave the pipelined mode in order
-    CUDA_OK(cudaMemcpyAsync(d_ndets, slot, sizeof(int) * S, cudaMemcpyHostToDevice, stream));
-    if (dets_dev != d_dets)
-        CUDA_OK(cudaMemcpyAsync(d_dets, dets_dev, sizeof(float) * 6 * CD * S, cudaMemcpyDeviceToDevice, stream));
+    CUDA_OK(cudaMemcpyAsync(in[0].ndets, slot, sizeof(int) * S, cudaMemcpyHostToDevice, stream));
+    if (dets_dev != in[0].dets)
+        CUDA_OK(cudaMemcpyAsync(in[0].dets, dets_dev, sizeof(float) * 6 * CD * S, cudaMemcpyDeviceToDevice, stream));
     enqueue_frame(cfg.with_reid ? embs_dev : nullptr, images_dev, rows, cols, total);
     if (sync) CUDA_OK(cudaStreamSynchronize(stream));
 }
@@ -1237,99 +1065,72 @@ void Engine::fetch(float* const* out, const int* out_cap, int* out_rows) {
     finish_fetch(out, out_cap, out_rows);
 }
 
+// Where one stream keeps its ordered slot lists and the per-slot identity and Kalman state they index
+struct Engine::TrackView {
+    const int* scalars;
+    int n_lists;                  // list k holds scalars[count[k]] slots
+    const int* list[2];
+    int count[2];
+    const int* id;
+    const double* state;          // [cap_tracks][8], the first `dim` used
+    const double* cov;            // [cap_tracks][cov_stride], dim x dim row-major
+    int dim, cov_stride;
+};
+
+Engine::TrackView Engine::track_view(int sidx) const {
+    switch (family) {
+        case Family::STrack: {
+            const TrkStream& s = h_streams[sidx];
+            return {s.scalars, 2, {s.active, s.lost}, {SC_N_ACTIVE, SC_N_LOST}, s.id, s.mean, s.cov, 8, 64};
+        }
+        case Family::StrongSort: {
+            const SsStream& s = h_ss[sidx];
+            return {s.scalars, 1, {s.tracks, nullptr}, {SC_N_ACTIVE, 0}, s.id, s.mean, s.cov, 8, 64};
+        }
+        case Family::Docs: {
+            const DocsStream& s = h_docs[sidx];
+            return {s.scalars, 1, {s.tracks, nullptr}, {SC_N_ACTIVE, 0}, s.id, s.x, s.P, 7, 56};
+        }
+        default: {
+            const BtStream& s = h_bt[sidx];
+            return {s.scalars, 1, {s.tracks, nullptr}, {SC_N_ACTIVE, 0}, s.id, s.x, s.P, 8, 64};
+        }
+    }
+}
+
+// Id, state and covariance of every track of the stream's lists in list order, widened to 8 / 8 x 8 with zeros
 int Engine::snapshot(int sidx, int* ids, double* means, double* covs, int cap) {
     if (sidx < 0 || sidx >= S) throw std::runtime_error("stream index out of range");
     CUDA_OK(cudaStreamSynchronize(stream));
-    if (is_ss) {
-        const SsStream& s = h_ss[sidx];
-        const int CT = cfg.cap_tracks;
-        std::vector<int> sc(SC_COUNT), lst(CT), idv(CT);
-        std::vector<double> mean((size_t)CT * 8), cov((size_t)CT * 64);
-        CUDA_OK(cudaMemcpy(sc.data(), s.scalars, sizeof(int) * SC_COUNT, cudaMemcpyDeviceToHost));
-        CUDA_OK(cudaMemcpy(lst.data(), s.tracks, sizeof(int) * CT, cudaMemcpyDeviceToHost));
-        CUDA_OK(cudaMemcpy(idv.data(), s.id, sizeof(int) * CT, cudaMemcpyDeviceToHost));
-        CUDA_OK(cudaMemcpy(mean.data(), s.mean, sizeof(double) * 8 * CT, cudaMemcpyDeviceToHost));
-        CUDA_OK(cudaMemcpy(cov.data(), s.cov, sizeof(double) * 64 * CT, cudaMemcpyDeviceToHost));
-        int n = 0;
-        for (int k = 0; k < sc[SC_N_ACTIVE] && n < cap; ++k, ++n) {
-            const int t = lst[k];
-            ids[n] = idv[t];
-            memcpy(means + (size_t)n * 8, mean.data() + (size_t)t * 8, sizeof(double) * 8);
-            memcpy(covs + (size_t)n * 64, cov.data() + (size_t)t * 64, sizeof(double) * 64);
-        }
-        return n;
-    }
-    if (is_bt) {
-        const BtStream& s = h_bt[sidx];
-        const int CT = cfg.cap_tracks;
-        std::vector<int> sc(SC_COUNT), lst(CT), idv(CT);
-        std::vector<double> xs((size_t)CT * 8), ps((size_t)CT * 64);
-        CUDA_OK(cudaMemcpy(sc.data(), s.scalars, sizeof(int) * SC_COUNT, cudaMemcpyDeviceToHost));
-        CUDA_OK(cudaMemcpy(lst.data(), s.tracks, sizeof(int) * CT, cudaMemcpyDeviceToHost));
-        CUDA_OK(cudaMemcpy(idv.data(), s.id, sizeof(int) * CT, cudaMemcpyDeviceToHost));
-        CUDA_OK(cudaMemcpy(xs.data(), s.x, sizeof(double) * 8 * CT, cudaMemcpyDeviceToHost));
-        CUDA_OK(cudaMemcpy(ps.data(), s.P, sizeof(double) * 64 * CT, cudaMemcpyDeviceToHost));
-        int n = 0;
-        for (int k = 0; k < sc[SC_N_ACTIVE] && n < cap; ++k, ++n) {
-            const int t = lst[k];
-            ids[n] = idv[t];
-            memcpy(means + (size_t)n * 8, xs.data() + (size_t)t * 8, sizeof(double) * 8);
-            memcpy(covs + (size_t)n * 64, ps.data() + (size_t)t * 64, sizeof(double) * 64);
-        }
-        return n;
-    }
-    if (is_docs) {
-        const DocsStream& s = h_docs[sidx];
-        const int CT = cfg.cap_tracks;
-        std::vector<int> sc(SC_COUNT), lst(CT), idv(CT);
-        std::vector<double> xs((size_t)CT * 8), ps((size_t)CT * 56);
-        CUDA_OK(cudaMemcpy(sc.data(), s.scalars, sizeof(int) * SC_COUNT, cudaMemcpyDeviceToHost));
-        CUDA_OK(cudaMemcpy(lst.data(), s.tracks, sizeof(int) * CT, cudaMemcpyDeviceToHost));
-        CUDA_OK(cudaMemcpy(idv.data(), s.id, sizeof(int) * CT, cudaMemcpyDeviceToHost));
-        CUDA_OK(cudaMemcpy(xs.data(), s.x, sizeof(double) * 8 * CT, cudaMemcpyDeviceToHost));
-        CUDA_OK(cudaMemcpy(ps.data(), s.P, sizeof(double) * 56 * CT, cudaMemcpyDeviceToHost));
-        int n = 0;
-        for (int k = 0; k < sc[SC_N_ACTIVE] && n < cap; ++k, ++n) {
-            const int t = lst[k];
-            ids[n] = idv[t];
-            for (int i = 0; i < 8; ++i) means[(size_t)n * 8 + i] = i < 7 ? xs[(size_t)t * 8 + i] : 0.0;
-            for (int i = 0; i < 64; ++i) covs[(size_t)n * 64 + i] = 0.0;
-            for (int i = 0; i < 7; ++i)
-                for (int j = 0; j < 7; ++j) covs[(size_t)n * 64 + i * 8 + j] = ps[(size_t)t * 56 + i * 7 + j];
-        }
-        return n;
-    }
-    const TrkStream& s = h_streams[sidx];
+    const TrackView v = track_view(sidx);
     const int CT = cfg.cap_tracks;
-    std::vector<int> sc(SC_COUNT), act(CT), lost(CT), idv(CT);
-    std::vector<double> mean((size_t)CT * 8), cov((size_t)CT * 64);
-    CUDA_OK(cudaMemcpy(sc.data(), s.scalars, sizeof(int) * SC_COUNT, cudaMemcpyDeviceToHost));
-    CUDA_OK(cudaMemcpy(act.data(), s.active, sizeof(int) * CT, cudaMemcpyDeviceToHost));
-    CUDA_OK(cudaMemcpy(lost.data(), s.lost, sizeof(int) * CT, cudaMemcpyDeviceToHost));
-    CUDA_OK(cudaMemcpy(idv.data(), s.id, sizeof(int) * CT, cudaMemcpyDeviceToHost));
-    CUDA_OK(cudaMemcpy(mean.data(), s.mean, sizeof(double) * 8 * CT, cudaMemcpyDeviceToHost));
-    CUDA_OK(cudaMemcpy(cov.data(), s.cov, sizeof(double) * 64 * CT, cudaMemcpyDeviceToHost));
+    std::vector<int> sc(SC_COUNT), lst[2], idv(CT);
+    std::vector<double> state((size_t)CT * 8), cov((size_t)CT * v.cov_stride);
+    CUDA_OK(cudaMemcpy(sc.data(), v.scalars, sizeof(int) * SC_COUNT, cudaMemcpyDeviceToHost));
+    for (int l = 0; l < v.n_lists; ++l) {
+        lst[l].resize(CT);
+        CUDA_OK(cudaMemcpy(lst[l].data(), v.list[l], sizeof(int) * CT, cudaMemcpyDeviceToHost));
+    }
+    CUDA_OK(cudaMemcpy(idv.data(), v.id, sizeof(int) * CT, cudaMemcpyDeviceToHost));
+    CUDA_OK(cudaMemcpy(state.data(), v.state, sizeof(double) * state.size(), cudaMemcpyDeviceToHost));
+    CUDA_OK(cudaMemcpy(cov.data(), v.cov, sizeof(double) * cov.size(), cudaMemcpyDeviceToHost));
     int n = 0;
-    for (int pass = 0; pass < 2; ++pass) {
-        const int cnt = sc[pass == 0 ? SC_N_ACTIVE : SC_N_LOST];
-        const std::vector<int>& lst = pass == 0 ? act : lost;
-        for (int k = 0; k < cnt && n < cap; ++k, ++n) {
-            const int t = lst[k];
+    for (int l = 0; l < v.n_lists; ++l) {
+        for (int k = 0; k < sc[v.count[l]] && n < cap; ++k, ++n) {
+            const int t = lst[l][k];
             ids[n] = idv[t];
-            memcpy(means + (size_t)n * 8, mean.data() + (size_t)t * 8, sizeof(double) * 8);
-            memcpy(covs + (size_t)n * 64, cov.data() + (size_t)t * 64, sizeof(double) * 64);
+            for (int i = 0; i < 8; ++i) means[(size_t)n * 8 + i] = i < v.dim ? state[(size_t)t * 8 + i] : 0.0;
+            for (int i = 0; i < 64; ++i) covs[(size_t)n * 64 + i] = 0.0;
+            for (int i = 0; i < v.dim; ++i)
+                for (int j = 0; j < v.dim; ++j) covs[(size_t)n * 64 + i * 8 + j] = cov[(size_t)t * v.cov_stride + i * v.dim + j];
         }
     }
     return n;
 }
 
-// Ids of one of the tracker's lists, in list order: 0 = active (the rows `update` may emit), 1 = lost, 2 = removed
-// (BaseTracker attributes active_tracks / lost_stracks / removed_stracks, basetracker.py:386-390).  BoT-SORT's removed list
-// is its deque(maxlen=removed_stracks_buffer) oldest first; ByteTrack's unbounded list is kept as a per-slot flag, so it
-// comes back in slot order.  DeepOCSORT and StrongSORT keep a single list (the reference never fills the other two).
 // OccluBoost resurrection events of one stream (ob_core.cuh), taken and cleared; optionally the graveyard too
 int Engine::gta_events(int sidx, int clear_graveyard, double* events, int cap) {
-    if (!is_ob) throw std::runtime_error("GTA events exist on OccluBoost handles only");
+    if (family != Family::Occlu) throw std::runtime_error("GTA events exist on OccluBoost handles only");
     if (sidx < 0 || sidx >= S) throw std::runtime_error("stream index out of range");
     if (reid_stream) CUDA_OK(cudaStreamSynchronize(reid_stream));
     CUDA_OK(cudaStreamSynchronize(stream));
@@ -1345,33 +1146,27 @@ int Engine::gta_events(int sidx, int clear_graveyard, double* events, int cap) {
     return n;
 }
 
+// Ids of one of the tracker's lists, in list order: 0 = active (the rows `update` may emit), 1 = lost, 2 = removed
+// (BaseTracker attributes active_tracks / lost_stracks / removed_stracks, basetracker.py:386-390).  BoT-SORT's removed list
+// is its deque(maxlen=removed_stracks_buffer) oldest first; ByteTrack's unbounded list is kept as a per-slot flag, so it
+// comes back in slot order.  The other families keep a single list (the reference never fills the other two).
 int Engine::track_ids(int sidx, int which, int* ids, int cap) {
     if (sidx < 0 || sidx >= S) throw std::runtime_error("stream index out of range");
     if (which < 0 || which > 2) throw std::runtime_error("list index must be 0 (active), 1 (lost) or 2 (removed)");
     CUDA_OK(cudaStreamSynchronize(stream));
+    const TrackView v = track_view(sidx);
+    if (which >= v.n_lists && family != Family::STrack) return 0;
     const int CT = cfg.cap_tracks;
     std::vector<int> sc(SC_COUNT), lst(CT), idv(CT);
     int n = 0;
-    if (is_ss || is_docs || is_bt) {
-        if (which != 0) return 0;
-        const int* scal = is_ss ? h_ss[sidx].scalars : is_bt ? h_bt[sidx].scalars : h_docs[sidx].scalars;
-        const int* trk = is_ss ? h_ss[sidx].tracks : is_bt ? h_bt[sidx].tracks : h_docs[sidx].tracks;
-        const int* idp = is_ss ? h_ss[sidx].id : is_bt ? h_bt[sidx].id : h_docs[sidx].id;
-        CUDA_OK(cudaMemcpy(sc.data(), scal, sizeof(int) * SC_COUNT, cudaMemcpyDeviceToHost));
-        CUDA_OK(cudaMemcpy(lst.data(), trk, sizeof(int) * CT, cudaMemcpyDeviceToHost));
-        CUDA_OK(cudaMemcpy(idv.data(), idp, sizeof(int) * CT, cudaMemcpyDeviceToHost));
-        for (int k = 0; k < sc[SC_N_ACTIVE] && n < cap; ++k) ids[n++] = idv[lst[k]];
+    CUDA_OK(cudaMemcpy(sc.data(), v.scalars, sizeof(int) * SC_COUNT, cudaMemcpyDeviceToHost));
+    CUDA_OK(cudaMemcpy(idv.data(), v.id, sizeof(int) * CT, cudaMemcpyDeviceToHost));
+    if (which < v.n_lists) {
+        CUDA_OK(cudaMemcpy(lst.data(), v.list[which], sizeof(int) * CT, cudaMemcpyDeviceToHost));
+        for (int k = 0; k < sc[v.count[which]] && n < cap; ++k) ids[n++] = idv[lst[k]];
         return n;
     }
     const TrkStream& s = h_streams[sidx];
-    CUDA_OK(cudaMemcpy(sc.data(), s.scalars, sizeof(int) * SC_COUNT, cudaMemcpyDeviceToHost));
-    CUDA_OK(cudaMemcpy(idv.data(), s.id, sizeof(int) * CT, cudaMemcpyDeviceToHost));
-    if (which < 2) {
-        CUDA_OK(cudaMemcpy(lst.data(), which == 0 ? s.active : s.lost, sizeof(int) * CT, cudaMemcpyDeviceToHost));
-        const int cnt = sc[which == 0 ? SC_N_ACTIVE : SC_N_LOST];
-        for (int k = 0; k < cnt && n < cap; ++k) ids[n++] = idv[lst[k]];
-        return n;
-    }
     if (cfg.removed_cap > 0) {
         std::vector<int> ring(cfg.removed_cap);
         CUDA_OK(cudaMemcpy(ring.data(), s.removed_ring, sizeof(int) * cfg.removed_cap, cudaMemcpyDeviceToHost));
