@@ -18,6 +18,7 @@ TRACKER_DEEPOCSORT = 2
 TRACKER_STRONGSORT = 3
 TRACKER_BOOSTTRACK = 4
 TRACKER_OCCLUBOOST = 5
+TRACKER_SFSORT = 6
 
 
 class BoxMOTByteTrackConfig(ctypes.Structure):
@@ -60,7 +61,21 @@ class BoxMOTB200TrackerConfig(ctypes.Structure):
                 ("recovery_appearance_thresh", c_double), ("recovery_iou_thresh", c_double), ("feat_alpha", c_double),
                 ("second_iou_thresh", c_double), ("second_appearance_thresh", c_double),
                 ("instant_confirm_thresh", c_double), ("duplicate_iou_thresh", c_double), ("ams_alpha0", c_double),
-                ("ams_threshold", c_double), ("ams_shrink_ratio", c_double), ("gta_appearance_thresh", c_double)]
+                ("ams_threshold", c_double), ("ams_shrink_ratio", c_double), ("gta_appearance_thresh", c_double),
+                ("sf_high_th", c_double), ("sf_match_th_first", c_double), ("sf_new_track_th", c_double),
+                ("sf_low_th", c_double), ("sf_match_th_second", c_double), ("sf_dynamic_tuning", c_int),
+                ("sf_cth", c_double), ("sf_high_th_m", c_double), ("sf_new_track_th_m", c_double),
+                ("sf_match_th_first_m", c_double), ("sf_marginal_timeout", c_int), ("sf_central_timeout", c_int),
+                ("sf_frame_width", c_int), ("sf_frame_height", c_int), ("sf_horizontal_margin", c_double),
+                ("sf_vertical_margin", c_double), ("sf_log10_table", c_void_p), ("sf_log10_count", c_int)]
+
+
+class BoxMOTSFSORTConfig(ctypes.Structure):
+    _fields_ = [("high_th", c_float), ("match_th_first", c_float), ("new_track_th", c_float), ("low_th", c_float),
+                ("match_th_second", c_float), ("dynamic_tuning", c_int), ("cth", c_float), ("high_th_m", c_float),
+                ("new_track_th_m", c_float), ("match_th_first_m", c_float), ("obb_theta_damping", c_float),
+                ("marginal_timeout", c_int), ("central_timeout", c_int), ("frame_width", c_int), ("frame_height", c_int),
+                ("horizontal_margin", c_int), ("vertical_margin", c_int), ("frame_rate", c_int), ("max_obs", c_int)]
 
 
 # every symbol include/boxmot_b200.h declares: name -> (restype, argtypes)
@@ -91,6 +106,12 @@ SYMBOLS = {
     "boxmot_botsort_last_reid_process_time_ms": (c_int, [c_void_p, POINTER(c_double)]),
     "boxmot_botsort_last_reid_postprocess_time_ms": (c_int, [c_void_p, POINTER(c_double)]),
     "boxmot_botsort_last_error": (c_char_p, []),
+    "boxmot_sfsort_create": (c_void_p, [POINTER(BoxMOTSFSORTConfig)]),
+    "boxmot_sfsort_destroy": (None, [c_void_p]),
+    "boxmot_sfsort_reset": (c_int, [c_void_p]),
+    "boxmot_sfsort_update": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_int, c_int, c_int,
+                                     c_void_p, c_int, c_int, POINTER(c_int), POINTER(c_int)]),
+    "boxmot_sfsort_last_error": (c_char_p, []),
     "boxmot_b200_tracker_create": (c_void_p, [POINTER(BoxMOTB200TrackerConfig)]),
     "boxmot_b200_tracker_destroy": (None, [c_void_p]),
     "boxmot_b200_tracker_reset": (c_int, [c_void_p]),
@@ -107,6 +128,7 @@ SYMBOLS = {
     "boxmot_b200_tracker_last_device_ms": (c_int, [c_void_p, POINTER(c_double), POINTER(c_double)]),
     "boxmot_b200_tracker_set_warp": (c_int, [c_void_p, c_int, c_void_p]),
     "boxmot_b200_tracker_set_cmc": (c_int, [c_void_p, c_char_p]),
+    "boxmot_b200_tracker_set_frame_size": (c_int, [c_void_p, c_int, c_int, c_int]),
     "boxmot_b200_cmc_ecc": (c_int, [c_void_p, c_void_p, c_int, c_int, c_double, c_double, c_int, c_void_p, POINTER(c_int),
                                     c_void_p]),
     "boxmot_b200_cmc_sof_create": (c_void_p, [c_double, c_int, c_double, c_double]),

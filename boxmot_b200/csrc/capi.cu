@@ -1,6 +1,8 @@
 // capi.cu -- the extern "C" surface of libboxmot_b200.so (see include/boxmot_b200.h for the contract and the
 // reference interfaces each symbol replaces).  Errors never cross the ABI: every entry point is wrapped, the
 // message is kept in a thread-local string (native_runtime.hpp:17-29 GuardCall convention).
+#include <cstdio>
+#include <cstdlib>
 #include <cstring>
 #include <exception>
 #include <stdexcept>
@@ -79,6 +81,7 @@ extern "C" {
 const char* boxmot_b200_last_error(void) { return g_error.c_str(); }
 const char* boxmot_bytetrack_last_error(void) { return g_error.c_str(); }
 const char* boxmot_botsort_last_error(void) { return g_error.c_str(); }
+const char* boxmot_sfsort_last_error(void) { return g_error.c_str(); }
 
 int boxmot_b200_device_count(void) {
     int n = 0;
@@ -159,6 +162,9 @@ int boxmot_b200_tracker_set_warp(BoxMOTB200Tracker* h, int stream, const double*
         as_engine(h)->set_warp(stream, warp2x3);
     });
 }
+int boxmot_b200_tracker_set_frame_size(BoxMOTB200Tracker* h, int stream, int rows, int cols) {
+    return guard([&] { as_engine(h)->set_frame_size(stream, rows, cols); });
+}
 int boxmot_b200_tracker_set_cmc(BoxMOTB200Tracker* h, const char* method) {
     return guard([&] { as_engine(h)->set_cmc(method); });
 }
@@ -205,6 +211,55 @@ int boxmot_bytetrack_reset(BoxMOTByteTrackHandle* h) { return guard([&] { as_eng
 int boxmot_bytetrack_update(BoxMOTByteTrackHandle* h, const float* dets, int det_rows, int det_cols,
                             const uint8_t* image, int rows, int cols, int ch, float* out, int out_cap, int out_cols,
                             int* out_rows, int* out_is_obb) {
+    return single_update(h, dets, det_rows, det_cols, nullptr, 0, 0, image, rows, cols, ch, out, out_cap, out_cols,
+                         out_rows, out_is_obb);
+}
+
+// ---- SFSORT (reference ABI) -------------------------------------------------------------------------------
+// The python float a float32 configuration member stands for: the shortest decimal that rounds to it (0.6f -> 0.6),
+// so thresholds compare as the Python class's do
+static double py_float(float f) {
+    char buf[32];
+    for (int p = 6; p < 10; ++p) {
+        snprintf(buf, sizeof(buf), "%.*g", p, (double)f);
+        if (strtof(buf, nullptr) == f) return strtod(buf, nullptr);
+    }
+    return (double)f;
+}
+BoxMOTSFSORTHandle* boxmot_sfsort_create(const BoxMOTSFSORTConfig* c) {
+    Engine* e = nullptr;
+    guard([&] {
+        if (!c) throw std::runtime_error("NULL config");
+        BoxMOTB200TrackerConfig p{};
+        p.tracker = BOXMOT_B200_TRACKER_SFSORT;
+        p.n_streams = 1;
+        p.cap_tracks = 1024;   // the SFSORT class's defaults (boxmot_b200/trackers.py)
+        p.cap_dets = 1024;
+        p.frame_rate = c->frame_rate;
+        p.sf_high_th = py_float(c->high_th);
+        p.sf_match_th_first = py_float(c->match_th_first);
+        p.sf_new_track_th = py_float(c->new_track_th);
+        p.sf_low_th = py_float(c->low_th);
+        p.sf_match_th_second = py_float(c->match_th_second);
+        p.sf_dynamic_tuning = c->dynamic_tuning;
+        p.sf_cth = py_float(c->cth);
+        p.sf_high_th_m = py_float(c->high_th_m);
+        p.sf_new_track_th_m = py_float(c->new_track_th_m);
+        p.sf_match_th_first_m = py_float(c->match_th_first_m);
+        p.sf_marginal_timeout = c->marginal_timeout;
+        p.sf_central_timeout = c->central_timeout;
+        p.sf_frame_width = c->frame_width;
+        p.sf_frame_height = c->frame_height;
+        p.sf_horizontal_margin = c->horizontal_margin;
+        p.sf_vertical_margin = c->vertical_margin;
+        e = new Engine(p);
+    });
+    return reinterpret_cast<BoxMOTSFSORTHandle*>(e);
+}
+void boxmot_sfsort_destroy(BoxMOTSFSORTHandle* h) { guard([&] { delete reinterpret_cast<Engine*>(h); }); }
+int boxmot_sfsort_reset(BoxMOTSFSORTHandle* h) { return guard([&] { as_engine(h)->reset(); }); }
+int boxmot_sfsort_update(BoxMOTSFSORTHandle* h, const float* dets, int det_rows, int det_cols, const uint8_t* image,
+                         int rows, int cols, int ch, float* out, int out_cap, int out_cols, int* out_rows, int* out_is_obb) {
     return single_update(h, dets, det_rows, det_cols, nullptr, 0, 0, image, rows, cols, ch, out, out_cap, out_cols,
                          out_rows, out_is_obb);
 }

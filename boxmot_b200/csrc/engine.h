@@ -14,6 +14,7 @@
 #include "ss_core.cuh"
 #include "bt_core.cuh"
 #include "ob_core.cuh"
+#include "sf_core.cuh"
 
 namespace bmb {
 
@@ -59,8 +60,9 @@ struct Engine {
     uint8_t* d_mem = nullptr;
     size_t stream_bytes = 0, persistent_bytes = 0;
     // Which tracker runs: the STrack family (ByteTrack / BoT-SORT, tracker_core.cuh), DeepOCSORT / OC-SORT (docs_core.cuh),
-    // StrongSORT (ss_core.cuh), BoostTrack (bt_core.cuh) or OccluBoost (ob_core.cuh, whose streams wrap a BtStream).
-    enum class Family { STrack, Docs, StrongSort, Boost, Occlu };
+    // StrongSORT (ss_core.cuh), BoostTrack (bt_core.cuh), OccluBoost (ob_core.cuh, whose streams wrap a BtStream) or
+    // SFSORT (sf_core.cuh).
+    enum class Family { STrack, Docs, StrongSort, Boost, Occlu, SfSort };
     Family family = Family::STrack;
     bool on_bt_stream() const { return family == Family::Boost || family == Family::Occlu; }
     bool is_bytetrack() const { return family == Family::STrack && cfg.kind != KIND_XYWH; }
@@ -69,11 +71,13 @@ struct Engine {
     SsCfg scfg{};
     BtCfg btcfg{};
     ObCfg obcfg{};
+    SfCfg sfcfg{};
     std::vector<TrkStream> h_streams;
     std::vector<DocsStream> h_docs;
     std::vector<SsStream> h_ss;
     std::vector<BtStream> h_bt;
     std::vector<ObStream> h_ob;
+    std::vector<SfStream> h_sf;
     // One set of frame inputs and the family's device stream array that reads it.  Set 0 serves update() and the
     // synchronous device path; set 1 exists with on-device ReID, for the frame pipeline of update_device.
     struct InputSet {
@@ -85,9 +89,13 @@ struct Engine {
         SsStream* ss = nullptr;
         BtStream* bt = nullptr;
         ObStream* ob = nullptr;
+        SfStream* sf = nullptr;
     };
     InputSet in[2];
     double* d_conf_pow = nullptr;      // 0.9 ** k, k = 0 .. max_age + 1 (KalmanBoxTracker.get_confidence)
+    double* d_log10 = nullptr;         // SFSORT: log10(k), k = 0 .. cap_dets (_dynamic_thresholds)
+    int* d_frame_hw = nullptr;         // SFSORT: [S][2] frame size of each stream (its margins come from the first)
+    std::vector<int> h_frame_hw;
     std::vector<float*> out_ptr;       // per-stream output rows / scalars / timers (either family)
     std::vector<int*> scalars_ptr;
     std::vector<long long*> timers_ptr;
@@ -161,6 +169,7 @@ struct Engine {
     int gta_events(int stream_index, int clear_graveyard, double* events, int cap);
     void set_warp(int stream_index, const double* warp6);
     void set_cmc(const char* method);   // "ecc" | "sof" | "none" / "" / NULL
+    void set_frame_size(int stream_index, int rows, int cols);   // SFSORT: the size of the stream's frames
     void read_timers(int stream_index, long long* out16, bool reset);
     void set_profile(bool on);
     void profile_read(double* ms, int* launch_counts);  // REID_N_CLASSES + 1 entries (last = association)

@@ -292,6 +292,16 @@ __global__ void __launch_bounds__(256) k_ob_frame(const ObCfg cfg, ObStream* str
     ob_frame(cfg, s);
 }
 
+// SFSORT: lapjv's scratch in shared memory as k_bt_frame (the square problem is cap_tracks + cap_dets wide); the frames
+// themselves never reach the device, only each stream's frame size (margins)
+__global__ void __launch_bounds__(256) k_sf_frame(const SfCfg cfg, SfStream* streams, int jv_in_smem) {
+    extern __shared__ __align__(16) unsigned char dyn_smem[];
+    SfStream s = streams[blockIdx.x];
+    s.jv_wide = jv_in_smem >> 1;
+    if (jv_in_smem & 1) jv_scratch_to_smem(s, dyn_smem, cfg.cap_tracks + cfg.cap_dets);
+    sf_frame(cfg, s);
+}
+
 // ordered (stream, detection) crop list built by one warp with ballot compaction
 template <typename Keep>
 __device__ __forceinline__ int append_crops(const float* dets, int D, int sidx, int cap_dets, CropDesc* crops, int n, Keep keep) {
@@ -414,6 +424,7 @@ void Engine::construct(const BoxMOTB200TrackerConfig& p) {
         case BOXMOT_B200_TRACKER_STRONGSORT: family = Family::StrongSort; break;
         case BOXMOT_B200_TRACKER_BOOSTTRACK: family = Family::Boost; break;
         case BOXMOT_B200_TRACKER_OCCLUBOOST: family = Family::Occlu; break;
+        case BOXMOT_B200_TRACKER_SFSORT: family = Family::SfSort; break;
         default: throw std::runtime_error("unknown tracker kind");
     }
     if (p.tracker == BOXMOT_B200_TRACKER_BOTSORT && p.removed_stracks_buffer < 1)
@@ -461,6 +472,35 @@ void Engine::construct(const BoxMOTB200TrackerConfig& p) {
         btcfg.dlo_coef = p.dlo_boost_coef; btcfg.min_box_area = p.min_box_area; btcfg.ar_thresh = p.aspect_ratio_thresh;
         cfg.with_reid = btcfg.with_reid;
         cfg.feat_dim = cfg.with_reid ? p.feat_dim : 0;
+        cfg.cap_tracks = p.cap_tracks; cfg.cap_dets = p.cap_dets;
+    }
+    if (family == Family::SfSort) {
+        if (p.reid_model_path && p.reid_model_path[0]) throw std::runtime_error("SFSORT has no ReID: pass no ReID blob");
+        // the constructor's _resolve_or_default clamps (sfsort.py:205-237)
+        auto clamp = [](double v, double lo, double hi) { const double m = hi < v ? hi : v; return m > lo ? m : lo; };
+        SfCfg& c = sfcfg;
+        c.cap_tracks = p.cap_tracks; c.cap_dets = p.cap_dets;
+        c.high_th = clamp(p.sf_high_th, 0.0, 1.0);
+        c.match_th_first = clamp(p.sf_match_th_first, 0.0, 0.67);
+        c.new_track_th = clamp(p.sf_new_track_th, c.high_th, 1.0);
+        c.low_th = clamp(p.sf_low_th, 0.0, c.high_th);
+        c.match_th_second = clamp(p.sf_match_th_second, 0.0, 1.0);
+        c.cth = clamp(p.sf_cth, c.low_th, 1.0);
+        c.dynamic = c.hth_f64 = c.nth_f64 = p.sf_dynamic_tuning ? 1 : 0;   // the tuned thresholds are np.float64
+        c.high_th_m = c.dynamic ? clamp(p.sf_high_th_m, 0.02, 0.1) : p.sf_high_th_m;
+        c.new_track_th_m = c.dynamic ? clamp(p.sf_new_track_th_m, 0.02, 0.08) : p.sf_new_track_th_m;
+        c.match_th_first_m = c.dynamic ? clamp(p.sf_match_th_first_m, 0.02, 0.08) : p.sf_match_th_first_m;
+        c.marginal_timeout = (int)clamp(p.sf_marginal_timeout, 0, 500);
+        c.central_timeout = (int)clamp(p.sf_central_timeout, 0, 1000);
+        c.h_margin = p.sf_horizontal_margin; c.v_margin = p.sf_vertical_margin;
+        c.margins_given = p.sf_frame_width > 0 && p.sf_frame_height > 0;
+        if (c.margins_given) {
+            const double W = p.sf_frame_width, H = p.sf_frame_height;
+            c.margin[0] = (float)clamp(c.h_margin, 0.0, W); c.margin[1] = (float)clamp(W - c.h_margin, 0.0, W);
+            c.margin[2] = (float)clamp(c.v_margin, 0.0, H); c.margin[3] = (float)clamp(H - c.v_margin, 0.0, H);
+        }
+        cfg.with_reid = 0;
+        cfg.feat_dim = 0;
         cfg.cap_tracks = p.cap_tracks; cfg.cap_dets = p.cap_dets;
     }
     if (cfg.with_reid && cfg.feat_dim < 1) throw std::runtime_error("feat_dim must be set when with_reid");
@@ -519,6 +559,7 @@ void Engine::construct(const BoxMOTB200TrackerConfig& p) {
             carve_all(carve_ob, obcfg, h_ob);
             for (const ObStream& o : h_ob) h_bt.push_back(o.b);
             break;
+        case Family::SfSort: carve_all(carve_sf, sfcfg, h_sf); break;
     }
     persistent_bytes = (persistent_bytes + 15) & ~(size_t)15;
     const size_t CD = cfg.cap_dets, F = cfg.feat_dim > 0 ? cfg.feat_dim : 1;
@@ -549,6 +590,23 @@ void Engine::construct(const BoxMOTB200TrackerConfig& p) {
         btcfg.n_conf_pow = (int)pw.size();
         obcfg.bt = btcfg;   // again: the copy taken with the OccluBoost parameters above predates conf_pow
     }
+    if (family == Family::SfSort) {
+        std::vector<double> lg((size_t)p.cap_dets + 1);
+        if (p.sf_log10_table) {
+            if (p.sf_log10_count < p.cap_dets + 1) throw std::runtime_error("sf_log10_table needs cap_dets + 1 entries");
+            lg.assign(p.sf_log10_table, p.sf_log10_table + lg.size());
+        } else {
+            sf_log10_table((int)lg.size(), lg.data());
+        }
+        CUDA_OK(cudaMalloc(&d_log10, sizeof(double) * lg.size()));
+        CUDA_OK(cudaMemcpy(d_log10, lg.data(), sizeof(double) * lg.size(), cudaMemcpyHostToDevice));
+        sfcfg.log10_tab = d_log10;
+        sfcfg.n_log10 = (int)lg.size();
+        h_frame_hw.assign((size_t)S * 2, 0);
+        CUDA_OK(cudaMalloc(&d_frame_hw, sizeof(int) * 2 * S));
+        CUDA_OK(cudaMemset(d_frame_hw, 0, sizeof(int) * 2 * S));
+        for (int i = 0; i < S; ++i) h_sf[i].frame_hw = d_frame_hw + 2 * i;
+    }
     const bool two_sets = reid && cfg.with_reid;   // second input set for the frame pipeline of update_device
     if (two_sets) {
         CUDA_OK(cudaStreamCreateWithFlags(&reid_stream, cudaStreamNonBlocking));
@@ -573,6 +631,7 @@ void Engine::construct(const BoxMOTB200TrackerConfig& p) {
                 for (int i = 0; i < S; ++i) h_ob[i].b = h_bt[i];
                 upload_streams(h_ob, &in[set].ob);
                 break;
+            case Family::SfSort: wire_streams(h_sf, set, &in[set].sf); break;
         }
     }
     if (reid) {
@@ -630,9 +689,10 @@ void Engine::release() {
     if (sof) sof_state_free(sof);
     for (InputSet& s : in) {
         cudaFree(s.dets); cudaFree(s.ndets); cudaFree(s.embs);
-        cudaFree(s.trk); cudaFree(s.docs); cudaFree(s.ss); cudaFree(s.bt); cudaFree(s.ob);
+        cudaFree(s.trk); cudaFree(s.docs); cudaFree(s.ss); cudaFree(s.bt); cudaFree(s.ob); cudaFree(s.sf);
     }
-    cudaFree(d_warp); cudaFree(d_mem); cudaFree(d_out); cudaFree(d_scalars_out); cudaFree(d_conf_pow);
+    cudaFree(d_warp); cudaFree(d_mem); cudaFree(d_out); cudaFree(d_scalars_out); cudaFree(d_conf_pow); cudaFree(d_log10);
+    cudaFree(d_frame_hw);
     cudaFree(d_crops); cudaFree(d_ncrops); cudaFree(d_images);
     cudaFreeHost(h_dets); cudaFreeHost(h_ndets); cudaFreeHost(h_out); cudaFreeHost(h_scalars);
     cudaFreeHost(h_embs); cudaFreeHost(h_images); cudaFreeHost(h_ndets_ring);
@@ -691,6 +751,8 @@ void Engine::enqueue_frame(const float* embs_dev, const uint8_t* images_dev, int
                                 cudaMemcpyDeviceToDevice, stream));
     }
     CUDA_OK(cudaEventRecord(ev[1], stream));
+    if (family == Family::SfSort && rows > 0 && cols > 0)   // a frame size given with the batch holds for every stream
+        for (int i = 0; i < S; ++i) set_frame_size(i, rows, cols);
     enqueue_family_association(0, embs_dev);
     CUDA_OK(cudaEventRecord(ev[2], stream));
     if (profile) {  // profiling pass: serialise and attribute device time per kernel class
@@ -711,6 +773,7 @@ void Engine::enqueue_crops(int parity, cudaStream_t st) {
         case Family::StrongSort: ss_build_crops(scfg, set.ss, S, d_crops, d_ncrops, d_crops_hint, st); break;
         case Family::Boost:
         case Family::Occlu: k_build_crops<<<1, 32, 0, st>>>(btcfg, set.bt, S, d_crops, d_ncrops, d_crops_hint); break;
+        case Family::SfSort: throw std::runtime_error("SFSORT embeds no detections");
     }
     ++launches;
 }
@@ -733,6 +796,13 @@ void Engine::enqueue_family_association(int parity, const float* embs_src) {
             size_t smem;
             const int jv_arg = jv_launch_setup(k_docs_frame, dcfg.cap_tracks, dcfg.cap_dets, &smem);
             k_docs_frame<<<S, 256, smem, stream>>>(dcfg, set.docs, jv_arg);
+            ++launches;
+            break;
+        }
+        case Family::SfSort: {
+            size_t smem;
+            const int jv_arg = jv_launch_setup(k_sf_frame, sfcfg.cap_tracks + sfcfg.cap_dets, 0, &smem);
+            k_sf_frame<<<S, 256, smem, stream>>>(sfcfg, set.sf, jv_arg);
             ++launches;
             break;
         }
@@ -819,6 +889,7 @@ void Engine::enqueue_association(TrkStream* streams_dev, const float* embs_src) 
 void Engine::set_cmc(const char* method) {
     const bool off = !method || !method[0] || strcmp(method, "none") == 0 || strcmp(method, "None") == 0;
     if (off) { cmc_mode = 0; return; }
+    if (family == Family::SfSort) throw std::runtime_error("SFSORT has no camera-motion compensation");
     if (strcmp(method, "sof") == 0) {
         // botsort.py:142,301 (every frame, every detection row) and deepocsort.py:330-349 (every frame, the rows with
         // conf > det_thresh); StrongSORT's estimator is ECC
@@ -841,6 +912,19 @@ void Engine::set_cmc(const char* method) {
         CUDA_OK(cudaMemcpy(d_cmc_gate, g.data(), sizeof(const int*) * S, cudaMemcpyHostToDevice));
     }
     cmc_mode = 1;
+}
+
+// SFSORT takes a stream's margins from the size of its first frame (BaseTracker._preprocess sets self.w / self.h); the
+// frames themselves never reach the device.  Stream-ordered: frames enqueued before the change keep the old size.
+void Engine::set_frame_size(int sidx, int rows, int cols) {
+    if (family != Family::SfSort) throw std::runtime_error("frame sizes are read by SFSORT handles only");
+    if (sidx < 0 || sidx >= S) throw std::runtime_error("stream index out of range");
+    if (rows <= 0 || cols <= 0) throw std::runtime_error("frame size must be positive");
+    int* hw = h_frame_hw.data() + 2 * sidx;
+    if (hw[0] == rows && hw[1] == cols) return;
+    hw[0] = rows; hw[1] = cols;
+    // pageable source: the copy is staged before the call returns, so h_frame_hw may change afterwards
+    CUDA_OK(cudaMemcpyAsync(d_frame_hw + 2 * sidx, hw, sizeof(int) * 2, cudaMemcpyHostToDevice, stream));
 }
 
 void Engine::enqueue_cmc(const uint8_t* images_dev, int rows, int cols) {
@@ -872,8 +956,8 @@ void Engine::enqueue_cmc(const uint8_t* images_dev, int rows, int cols) {
 
 void Engine::set_warp(int sidx, const double* warp6) {
     if (sidx < 0 || sidx >= S) throw std::runtime_error("stream index out of range");
-    if (is_bytetrack())
-        throw std::runtime_error("camera-motion warps apply to BoT-SORT, DeepOCSORT and StrongSORT (ByteTrack has none)");
+    if (is_bytetrack() || family == Family::SfSort)
+        throw std::runtime_error("camera-motion warps apply to BoT-SORT, DeepOCSORT and StrongSORT (ByteTrack and SFSORT have none)");
     double w[8] = {warp6[0], warp6[1], warp6[2], warp6[3], warp6[4], warp6[5], 1.0, 0.0};
     CUDA_OK(cudaStreamSynchronize(stream));
     CUDA_OK(cudaMemcpy(d_warp + (size_t)sidx * 8, w, sizeof(w), cudaMemcpyHostToDevice));
@@ -1091,6 +1175,10 @@ Engine::TrackView Engine::track_view(int sidx) const {
             const DocsStream& s = h_docs[sidx];
             return {s.scalars, 1, {s.tracks, nullptr}, {SC_N_ACTIVE, 0}, s.id, s.x, s.P, 7, 56};
         }
+        case Family::SfSort: {   // no motion state: ids only
+            const SfStream& s = h_sf[sidx];
+            return {s.scalars, 2, {s.active, s.lost}, {SC_N_ACTIVE, SC_N_LOST}, s.id, nullptr, nullptr, 0, 0};
+        }
         default: {
             const BtStream& s = h_bt[sidx];
             return {s.scalars, 1, {s.tracks, nullptr}, {SC_N_ACTIVE, 0}, s.id, s.x, s.P, 8, 64};
@@ -1112,8 +1200,10 @@ int Engine::snapshot(int sidx, int* ids, double* means, double* covs, int cap) {
         CUDA_OK(cudaMemcpy(lst[l].data(), v.list[l], sizeof(int) * CT, cudaMemcpyDeviceToHost));
     }
     CUDA_OK(cudaMemcpy(idv.data(), v.id, sizeof(int) * CT, cudaMemcpyDeviceToHost));
-    CUDA_OK(cudaMemcpy(state.data(), v.state, sizeof(double) * state.size(), cudaMemcpyDeviceToHost));
-    CUDA_OK(cudaMemcpy(cov.data(), v.cov, sizeof(double) * cov.size(), cudaMemcpyDeviceToHost));
+    if (v.dim) {
+        CUDA_OK(cudaMemcpy(state.data(), v.state, sizeof(double) * state.size(), cudaMemcpyDeviceToHost));
+        CUDA_OK(cudaMemcpy(cov.data(), v.cov, sizeof(double) * cov.size(), cudaMemcpyDeviceToHost));
+    }
     int n = 0;
     for (int l = 0; l < v.n_lists; ++l) {
         for (int k = 0; k < sc[v.count[l]] && n < cap; ++k, ++n) {

@@ -252,3 +252,32 @@ inline size_t carve_ob(const ObCfg& c, uint8_t* base, ObStream* s, size_t* persi
 
 }  // namespace bmb
 
+
+#include "sf_core.cuh"
+
+namespace bmb {
+
+// SFSORT: boxes and the two ordered lists persist; lapjv's (CT + CD) square problem dominates the scratch
+inline size_t carve_sf(const SfCfg& c, uint8_t* base, SfStream* s, size_t* persistent_bytes) {
+    const size_t CT = (size_t)c.cap_tracks, CD = (size_t)c.cap_dets, MX = CT + CD;
+    Carver k{base, 0};
+    SfStream t{};
+    t.scalars = k.take<int>(SC_COUNT);
+    t.timers = k.take<long long>(16);
+    t.box = k.take<float>(CT * 4); t.conf = k.take<float>(CT); t.cls = k.take<float>(CT);
+    t.det_ind = k.take<int>(CT); t.last_frame = k.take<int>(CT); t.id = k.take<int>(CT); t.state = k.take<int>(CT);
+    t.active = k.take<int>(CT); t.lost = k.take<int>(CT); t.margins = k.take<float>(4);
+    if (persistent_bytes) *persistent_bytes = k.off;
+    t.high = k.take<int>(CD); t.mid = k.take<int>(CD);
+    t.pool = k.take<int>(CT); t.unm = k.take<int>(CT); t.nxt = k.take<int>(CT); t.nlost = k.take<int>(CT);
+    t.mark = k.take<int>(CT); t.next_lost = k.take<int>(CT); t.mb = k.take<int>(SF_MB_COUNT); t.th = k.take<double>(4);
+    t.free_l = k.take<int>(MB_COUNT);
+    t.cost = k.take<double>(MX * MX);
+    t.lap_x = k.take<int>(MX); t.lap_y = k.take<int>(MX); t.lap_v = k.take<double>(MX); t.lap_spc = k.take<double>(MX);
+    t.lap_path = k.take<int>(MX); t.lap_insc = k.take<int>(MX); t.lap_tl = k.take<int>(MX); t.lap_sc = k.take<int>(MX);
+    t.out = k.take<float>(CD * 8);
+    if (s) *s = t;
+    return (k.off + 255) & ~(size_t)255;
+}
+
+}  // namespace bmb

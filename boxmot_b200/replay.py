@@ -185,11 +185,14 @@ def fps_mask(frames: np.ndarray, orig_fps: int, target_fps: int) -> np.ndarray:
 
 
 class SequenceCache:
-    """One cached sequence: `(frame_id, x1, y1, x2, y2, conf, cls)` rows + row-aligned embeddings."""
+    """One cached sequence: `(frame_id, x1, y1, x2, y2, conf, cls)` rows + row-aligned embeddings.  `frame_hw`: the
+    `(H, W)` of the sequence's images (the reference hands every update a frame of that size; SFSORT's margins read it)."""
 
     def __init__(self, dets, embs=None, *, frame_ids: Optional[Sequence[int]] = None, name: str = "",
-                 orig_fps: Optional[int] = None, target_fps: Optional[int] = None):
+                 orig_fps: Optional[int] = None, target_fps: Optional[int] = None,
+                 frame_hw: Optional[Tuple[int, int]] = None):
         self.name = name
+        self.frame_hw = None if frame_hw is None else (int(frame_hw[0]), int(frame_hw[1]))
         self.dets = np.load(dets, mmap_mode="r") if isinstance(dets, (str, os.PathLike)) else np.asarray(dets)
         if self.dets.ndim != 2 or (self.dets.shape[0] and self.dets.shape[1] != 7):
             raise ValueError(f"dets cache of {name!r} must be (rows, 7): frame_id, x1, y1, x2, y2, conf, cls")
@@ -293,6 +296,10 @@ def replay_sequences(tracker, caches: Sequence[SequenceCache], conf_threshold: f
     if getattr(tracker, "n_streams", S) != S:
         raise ValueError(f"tracker has {tracker.n_streams} streams for {S} sequences")
     feeds = [_frame_inputs(c, conf_threshold) for c in caches]
+    if getattr(tracker, "kind", None) == "sfsort":   # each stream's margins come from its sequence's frame size
+        for i, c in enumerate(caches):
+            if c.frame_hw is not None:
+                tracker.set_frame_size(i, c.frame_hw)
     rows: List[List[np.ndarray]] = [[] for _ in range(S)]
     feat_dim = int(getattr(tracker, "feat_dim", 0))
     wants_embs = bool(getattr(tracker, "with_reid", False))

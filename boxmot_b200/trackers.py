@@ -177,6 +177,7 @@ class MultiStreamTracker:
         self.lib = _lib.require_device()
         cfg = BoxMOTB200TrackerConfig()
         kind = tracker.lower()
+        needs_frame_size = False
         if kind == "bytetrack":
             p = dict(min_conf=0.1, track_thresh=0.45, match_thresh=0.8, track_buffer=25, frame_rate=30)
             unknown = set(params) - set(p)
@@ -284,9 +285,34 @@ class MultiStreamTracker:
                 _occluboost_cfg(cfg, p)
             p.setdefault("track_buffer", 0)
             p.setdefault("frame_rate", 30)
+        elif kind == "sfsort":
+            p = dict(SFSORT_ENGINE_DEFAULTS)
+            unknown = set(params) - set(p)
+            if unknown:
+                raise TypeError(f"unknown SFSORT parameters: {sorted(unknown)}")
+            p.update(params)
+            r = sfsort_resolve(**p)
+            cfg.tracker = _lib.TRACKER_SFSORT
+            for name in ("high_th", "match_th_first", "new_track_th", "low_th", "match_th_second", "cth", "high_th_m",
+                         "new_track_th_m", "match_th_first_m", "horizontal_margin", "vertical_margin"):
+                setattr(cfg, "sf_" + name, float(r[name]))
+            cfg.sf_dynamic_tuning = int(r["dynamic_tuning"])
+            cfg.sf_marginal_timeout, cfg.sf_central_timeout = r["marginal_timeout"], r["central_timeout"]
+            given = r["frame_width"] is not None and r["frame_height"] is not None
+            # the margins decide a lost track's state, which only matters when the two timeouts differ
+            needs_frame_size = not given and r["central_timeout"] != r["marginal_timeout"]
+            cfg.sf_frame_width = int(r["frame_width"]) if given else 0
+            cfg.sf_frame_height = int(r["frame_height"]) if given else 0
+            cfg.with_reid = 0
+            # np.log10(count) of _dynamic_thresholds, from this process's numpy (its vectorised log10 and libm's differ
+            # in the last bit for some counts)
+            self._log10 = sfsort_log10_table(int(cap_dets) + 1)
+            cfg.sf_log10_table, cfg.sf_log10_count = self._log10.ctypes.data, len(self._log10)
+            p.setdefault("track_buffer", 0)
+            p.setdefault("frame_rate", 30)
         else:
             raise ValueError(f"tracker '{tracker}' is not part of the B200 hot path "
-                             "(bytetrack, botsort, deepocsort, strongsort, boosttrack, occluboost)")
+                             "(bytetrack, botsort, deepocsort, strongsort, boosttrack, occluboost, sfsort)")
         cfg.n_streams = int(n_streams)
         cfg.cap_tracks = int(cap_tracks)
         cfg.cap_dets = int(cap_dets)
@@ -316,6 +342,8 @@ class MultiStreamTracker:
             raise B200Error(f"tracker create failed: {_lib.last_error(self.lib)}")
         self.frame_count = 0
         self.cmc = None
+        self._frame_hw = [None] * self.n_streams   # SFSORT: the frame size each stream was given
+        self._needs_frame_size = needs_frame_size
         self._gta_on = kind == "occluboost" and bool(p["gta_enabled"]) and self.with_reid
         self._gta_events = [[] for _ in range(self.n_streams)]
 
@@ -330,6 +358,23 @@ class MultiStreamTracker:
         if not self.lib.boxmot_b200_tracker_set_cmc(self.handle, m.encode() if m else None):
             raise B200Error(_lib.last_error(self.lib))
         self.cmc = m
+
+    def set_frame_size(self, stream: int, hw: Sequence[int]) -> None:
+        """SFSORT: the size `(H, W)` of `stream`'s frames.  A stream takes its margins from the first size it is given,
+        as the reference takes them from its first image; `update(dets, imgs)` and `update_device(..., image_hw=)` call
+        this for every stream."""
+        h, w = int(hw[0]), int(hw[1])
+        if self._frame_hw[stream] == (h, w):
+            return
+        if not self.lib.boxmot_b200_tracker_set_frame_size(self.handle, int(stream), h, w):
+            raise B200Error(_lib.last_error(self.lib))
+        self._frame_hw[stream] = (h, w)
+
+    def _check_frame_sizes(self) -> None:
+        if self._needs_frame_size and None in self._frame_hw:
+            raise B200Error(f"SFSORT stream {self._frame_hw.index(None)} has no frame size: with central_timeout != "
+                            "marginal_timeout its margins decide which timeout a lost track gets -- pass the frames, "
+                            "image_hw, frame_width / frame_height, or call set_frame_size")
 
     def close(self):
         if getattr(self, "handle", None):
@@ -383,6 +428,11 @@ class MultiStreamTracker:
                 e_ptr[i] = e.ctypes.data
         i_ptr, ih, iw = None, 0, 0
         i_arr = []
+        if self.kind == "sfsort":   # each stream's frame size sets its margins; the frames stay on the host
+            for i, im in enumerate(imgs if imgs is not None else []):
+                if im is not None:
+                    self.set_frame_size(i, np.shape(im)[:2])
+            self._check_frame_sizes()
         if (self.with_reid and e_ptr is None) or self.cmc:
             if imgs is None:
                 raise B200Error("camera-motion estimation needs the frames" if self.cmc and not (self.with_reid and e_ptr is None)
@@ -468,9 +518,16 @@ class MultiStreamTracker:
         decoded frames): `d_dets` `[n_streams][cap_dets][6]` float32, `d_embs` `[n_streams][cap_dets][feat_dim]`
         float32 or None, `d_images` `[n_streams][H][W][3]` uint8 or None, `det_rows` host ints.  With `sync=False`
         the call returns after enqueueing: ReID of the next frame overlaps this frame's association.  Rows stay on
-        the device until `fetch()`."""
+        the device until `fetch()`.  SFSORT: `image_hw` is one `(H, W)` for every stream or one per stream."""
         S = self.n_streams
         assert len(det_rows) == S, f"expected {S} detection counts"
+        if self.kind == "sfsort":
+            if image_hw is not None:
+                per_stream = np.ndim(image_hw) == 2
+                for i in range(S):
+                    self.set_frame_size(i, image_hw[i] if per_stream else image_hw)
+                image_hw = None
+            self._check_frame_sizes()
         if max(det_rows, default=0) > self.cap_dets:
             raise B200Error(f"{max(det_rows)} detections exceed cap_dets={self.cap_dets}")
         rows = (ctypes.c_int * S)(*[int(r) for r in det_rows])
@@ -955,6 +1012,99 @@ class OccluBoost(BoostTrack):
         return self._engine.flush_gta(0)
 
 
+# SFSORT (boxmot/trackers/bbox/sfsort/sfsort.py:180-237): the constructor's defaults, and configs/trackers/sfsort.yaml, the
+# defaults create_tracker("sfsort") starts from
+SFSORT_ENGINE_DEFAULTS = dict(high_th=0.6, match_th_first=0.67, new_track_th=0.7, low_th=0.1, match_th_second=0.3,
+                              dynamic_tuning=False, cth=0.5, high_th_m=0.0, new_track_th_m=0.0, match_th_first_m=0.0,
+                              marginal_timeout=0, central_timeout=0, frame_width=None, frame_height=None,
+                              horizontal_margin=None, vertical_margin=None)
+SFSORT_YAML_DEFAULTS = dict(high_th=0.6, match_th_first=0.67, new_track_th=0.7, low_th=0.1, match_th_second=0.3,
+                            dynamic_tuning=False, cth=0.5, high_th_m=0.0, new_track_th_m=0.0, match_th_first_m=0.0,
+                            marginal_timeout=0, central_timeout=0, horizontal_margin=0, vertical_margin=0)
+
+
+def sfsort_log10_table(n: int) -> np.ndarray:
+    """np.log10(k) for k = 0 .. n - 1, as `_dynamic_thresholds` evaluates it for k scores above cth."""
+    with np.errstate(divide="ignore"):
+        return np.ascontiguousarray(np.log10(np.arange(n, dtype=np.float64)))
+
+
+def sfsort_resolve(high_th=0.6, match_th_first=0.67, new_track_th=0.7, low_th=0.1, match_th_second=0.3,
+                   dynamic_tuning=False, cth=0.5, high_th_m=0.0, new_track_th_m=0.0, match_th_first_m=0.0,
+                   marginal_timeout=0, central_timeout=0, frame_width=None, frame_height=None, horizontal_margin=None,
+                   vertical_margin=None) -> dict:
+    """The constructor's `_resolve_or_default` clamps (sfsort.py:205-237); margins of None count as 0."""
+    def rd(v, d, lo, hi):
+        return max(lo, min(d if v is None else v, hi))
+
+    r = dict(high_th=rd(high_th, 0.6, 0.0, 1.0), match_th_first=rd(match_th_first, 0.67, 0.0, 0.67))
+    r["new_track_th"] = rd(new_track_th, 0.7, r["high_th"], 1.0)
+    r["low_th"] = rd(low_th, 0.1, 0.0, r["high_th"])
+    r["match_th_second"] = rd(match_th_second, 0.3, 0.0, 1.0)
+    r["dynamic_tuning"] = bool(dynamic_tuning)
+    r["cth"] = rd(cth, 0.5, r["low_th"], 1.0)
+    for name, v, hi in (("high_th_m", high_th_m, 0.1), ("new_track_th_m", new_track_th_m, 0.08),
+                        ("match_th_first_m", match_th_first_m, 0.08)):
+        r[name] = rd(v, 0.0, 0.02, hi) if dynamic_tuning else (0.0 if v is None else float(v))
+    r["marginal_timeout"] = int(rd(marginal_timeout, 0, 0, 500))
+    r["central_timeout"] = int(rd(central_timeout, 0, 0, 1000))
+    r["frame_width"], r["frame_height"] = frame_width, frame_height
+    r["horizontal_margin"], r["vertical_margin"] = horizontal_margin or 0, vertical_margin or 0
+    return r
+
+
+class SFSORT(_SingleStreamTracker):
+    """SFSORT on the GPU; arguments and defaults as boxmot/trackers/bbox/sfsort/sfsort.py:180-237 plus `cap_tracks` /
+    `cap_dets`.  Ids are 0-based per tracker, as in the reference.  `obb_theta_damping`, `max_age`, `min_hits`,
+    `iou_threshold` and `asso_func` are accepted and never read, as there.
+
+    Deviation: `reset()` clears every track and restarts ids at 0 (the reference's native backend rebuilds its tracker;
+    the Python class inherits BaseTracker's no-op reset).
+
+    Device memory: lapjv's square problem takes `8 * (cap_tracks + cap_dets) ** 2` bytes per stream, 34 MB at the
+    defaults (1024 tracks, 1024 detections per frame)."""
+
+    _kind = "sfsort"
+
+    def __init__(self, high_th: Optional[float] = 0.6, match_th_first: Optional[float] = 0.67,
+                 new_track_th: Optional[float] = 0.7, low_th: Optional[float] = 0.1,
+                 match_th_second: Optional[float] = 0.3, dynamic_tuning: bool = False, cth: Optional[float] = 0.5,
+                 high_th_m: Optional[float] = 0.0, new_track_th_m: Optional[float] = 0.0,
+                 match_th_first_m: Optional[float] = 0.0, obb_theta_damping: float = 0.8,
+                 marginal_timeout: Optional[int] = 0, central_timeout: Optional[int] = 0,
+                 frame_width: Optional[int] = None, frame_height: Optional[int] = None,
+                 horizontal_margin: Optional[int] = None, vertical_margin: Optional[int] = None, **kwargs: Any):
+        args = dict(high_th=high_th, match_th_first=match_th_first, new_track_th=new_track_th, low_th=low_th,
+                    match_th_second=match_th_second, dynamic_tuning=dynamic_tuning, cth=cth, high_th_m=high_th_m,
+                    new_track_th_m=new_track_th_m, match_th_first_m=match_th_first_m, marginal_timeout=marginal_timeout,
+                    central_timeout=central_timeout, frame_width=frame_width, frame_height=frame_height,
+                    horizontal_margin=horizontal_margin, vertical_margin=vertical_margin)
+        if kwargs.get("reid_model") is not None:
+            raise NotImplementedError("SFSORT has no ReID")
+        kwargs.setdefault("det_thresh", 0.6 if high_th is None else float(high_th))
+        kwargs.setdefault("cap_tracks", 1024)
+        kwargs.setdefault("cap_dets", 1024)
+        self.asso_func_name = kwargs.pop("asso_func", "iou")   # accepted and never read, as in the reference
+        super().__init__(**kwargs, **args)
+        r = sfsort_resolve(**args)
+        for name in ("high_th", "match_th_first", "new_track_th", "low_th", "match_th_second", "dynamic_tuning", "cth",
+                     "high_th_m", "new_track_th_m", "match_th_first_m", "marginal_timeout", "central_timeout"):
+            setattr(self, name, r[name])
+        self.obb_theta_damping = max(0.0, min(0.8 if obb_theta_damping is None else obb_theta_damping, 1.0))
+        self.frame_width, self.frame_height = frame_width, frame_height
+        self.horizontal_margin, self.vertical_margin = horizontal_margin, vertical_margin
+
+    def update(self, dets, img=None, embs=None, masks=None, warp=None) -> TrackResults:
+        if isinstance(dets, np.ndarray) and dets.ndim == 2 and dets.shape[1] == 7:
+            raise NotImplementedError("OBB detections (7 columns) are out of scope for the B200 hot path")
+        return super().update(dets, img, None, masks, warp)
+
+    @property
+    def lost_tracks(self):
+        """Lost tracks (`lost_tracks`) in list order: ids only (SFSORT keeps no motion state)."""
+        return self._views(1)
+
+
 def _flatten_yaml_defaults(node, acc=None):
     """`<param>: {default: ...}` entries of a reference tracker YAML, nested conditional parameters included
     (what `flatten_yaml_config` + `details["default"]` produce in tracker_zoo.py:112-119)."""
@@ -983,7 +1133,7 @@ def resolve_tracker_args(tracker_type, tracker_config=None, evolve_param_dict=No
 
     kind = str(tracker_type).lower()
     classes = {"bytetrack": ByteTrack, "botsort": BotSort, "deepocsort": DeepOcSort, "strongsort": StrongSort, "ocsort": OcSort,
-               "boosttrack": BoostTrack, "occluboost": OccluBoost}
+               "boosttrack": BoostTrack, "occluboost": OccluBoost, "sfsort": SFSORT}
     if kind not in classes:
         raise ValueError(f"Unknown tracker type: '{tracker_type}'. Available trackers are: {', '.join(classes)} "
                          "(the trackers that are part of the B200 hot path)")
@@ -996,7 +1146,8 @@ def resolve_tracker_args(tracker_type, tracker_config=None, evolve_param_dict=No
             args = _flatten_yaml_defaults(yaml.safe_load(f) or {})
     else:
         args = dict(TRACKER_DEFAULTS[kind] if kind in TRACKER_DEFAULTS
-                    else OCCLUBOOST_YAML_DEFAULTS if kind == "occluboost" else BOOSTTRACK_YAML_DEFAULTS)
+                    else OCCLUBOOST_YAML_DEFAULTS if kind == "occluboost" else SFSORT_YAML_DEFAULTS if kind == "sfsort"
+                    else BOOSTTRACK_YAML_DEFAULTS)
     args.update(overrides or {})
     cls = classes[kind]
     accepted = {"cap_tracks", "cap_dets", "feat_dim"}
@@ -1048,7 +1199,7 @@ def create_tracker(tracker_type, tracker_config=None, reid_weights=None, device=
     its configuration's on-device estimator)."""
     kind, cls, args = resolve_tracker_args(tracker_type, tracker_config, evolve_param_dict, overrides)
     per_class = bool(per_class)
-    if kind in ("bytetrack", "ocsort"):   # motion-only trackers: no ReID backend (tracker_zoo.py:124-130)
+    if kind in ("bytetrack", "ocsort", "sfsort"):   # motion-only trackers: no ReID backend (tracker_zoo.py:124-130)
         return cls(per_class=per_class, **args)
     wants_reid = args.get("with_reid", True) and not args.get("embedding_off", False)
     if reid_model is None and reid_weights is not None and wants_reid:

@@ -107,6 +107,44 @@ BOXMOT_B200_API int boxmot_botsort_last_reid_process_time_ms(BoxMOTBotSortHandle
 BOXMOT_B200_API int boxmot_botsort_last_reid_postprocess_time_ms(BoxMOTBotSortHandle* handle, double* out_time_ms);
 BOXMOT_B200_API const char* boxmot_botsort_last_error(void);
 
+/* SFSORT (sfsort/include/sfsort/c_api.hpp): the configuration member for member.  frame_rate and max_obs are accepted and
+ * unused, as there; frame_width / frame_height of 0 take the margins from the first frame's size.  Results follow the
+ * Python class (0-based ids); float members stand for the python float they print as (0.6f is 0.6).  det_cols must be
+ * 6 (OBB is out of scope); out_is_obb is always 0.  The handle holds 1024 tracks and 1024 detections per frame; lapjv's
+ * square problem takes 8 * (1024 + 1024)^2 bytes (34 MB) of device memory. */
+typedef struct BoxMOTSFSORTConfig {
+    float high_th;
+    float match_th_first;
+    float new_track_th;
+    float low_th;
+    float match_th_second;
+    int dynamic_tuning;
+    float cth;
+    float high_th_m;
+    float new_track_th_m;
+    float match_th_first_m;
+    float obb_theta_damping;
+    int marginal_timeout;
+    int central_timeout;
+    int frame_width;
+    int frame_height;
+    int horizontal_margin;
+    int vertical_margin;
+    int frame_rate;
+    int max_obs;
+} BoxMOTSFSORTConfig;
+
+typedef struct BoxMOTSFSORTHandle BoxMOTSFSORTHandle;
+
+BOXMOT_B200_API BoxMOTSFSORTHandle* boxmot_sfsort_create(const BoxMOTSFSORTConfig* config);
+BOXMOT_B200_API void boxmot_sfsort_destroy(BoxMOTSFSORTHandle* handle);
+BOXMOT_B200_API int boxmot_sfsort_reset(BoxMOTSFSORTHandle* handle);
+BOXMOT_B200_API int boxmot_sfsort_update(BoxMOTSFSORTHandle* handle, const float* dets, int det_rows, int det_cols,
+                                         const uint8_t* image_data, int image_rows, int image_cols, int image_channels,
+                                         float* out_tracks, int out_capacity_rows, int out_cols, int* out_rows,
+                                         int* out_is_obb);
+BOXMOT_B200_API const char* boxmot_sfsort_last_error(void);
+
 /* ------------------------------------------------------------------------------------------------ */
 /* Part 2: B200 extension                                                                            */
 /* ------------------------------------------------------------------------------------------------ */
@@ -116,6 +154,7 @@ BOXMOT_B200_API const char* boxmot_botsort_last_error(void);
 #define BOXMOT_B200_TRACKER_STRONGSORT 3
 #define BOXMOT_B200_TRACKER_BOOSTTRACK 4
 #define BOXMOT_B200_TRACKER_OCCLUBOOST 5
+#define BOXMOT_B200_TRACKER_SFSORT 6
 
 /* Every parameter of the reference Python constructors (bytetrack.py:226-257, botsort.py:66-118), in
  * double precision so thresholds compare exactly as python floats do. */
@@ -207,6 +246,28 @@ typedef struct BoxMOTB200TrackerConfig {
     double ams_threshold;
     double ams_shrink_ratio;
     double gta_appearance_thresh;
+    /* SFSORT (sfsort.py:180-237); the engine applies the constructor's clamps.  frame_width / frame_height of 0: the
+     * margins come from the first frame's size. */
+    double sf_high_th;
+    double sf_match_th_first;
+    double sf_new_track_th;
+    double sf_low_th;
+    double sf_match_th_second;
+    int sf_dynamic_tuning;
+    double sf_cth;
+    double sf_high_th_m;
+    double sf_new_track_th_m;
+    double sf_match_th_first_m;
+    int sf_marginal_timeout;
+    int sf_central_timeout;
+    int sf_frame_width;
+    int sf_frame_height;
+    double sf_horizontal_margin;
+    double sf_vertical_margin;
+    /* log10(k) for k = 0 .. sf_log10_count - 1 (at least cap_dets + 1 entries), the value the density-tuned thresholds
+     * use for k scores above cth; the Python layer passes numpy's.  NULL: the host libm's log10. */
+    const double* sf_log10_table;
+    int sf_log10_count;
 } BoxMOTB200TrackerConfig;
 
 typedef struct BoxMOTB200Tracker BoxMOTB200Tracker;
@@ -275,6 +336,10 @@ BOXMOT_B200_API int boxmot_b200_tracker_set_warp(BoxMOTB200Tracker* handle, int 
  * take both, run the estimator on every frame with every detection row (boosttrack.py:318-321) and apply its result --
  * the identity when it returns none -- to every track.  "none" / "" / NULL turns it off again.  The estimate replaces a warp supplied for the same frame; reset restarts the estimator. */
 BOXMOT_B200_API int boxmot_b200_tracker_set_cmc(BoxMOTB200Tracker* handle, const char* method);
+/* SFSORT handles: the size (rows x cols) of one stream's frames.  A stream takes its margins from the first size it is
+ * given (the reference's first image); update calls that pass image_rows / image_cols > 0 set every stream's size.
+ * Streams of different resolutions in one handle need this call.  Other handles: an error. */
+BOXMOT_B200_API int boxmot_b200_tracker_set_frame_size(BoxMOTB200Tracker* handle, int stream, int rows, int cols);
 /* Device timing on the handle's own CUDA stream: record mark 0 / mark 1 around a region, then read the elapsed
  * milliseconds (synchronises on mark 1). */
 BOXMOT_B200_API int boxmot_b200_tracker_mark(BoxMOTB200Tracker* handle, int which);
