@@ -386,6 +386,10 @@ int boxmot_b200_pointwise_gemm(const float* a, int m, int k, const float* w, int
                                const float* residual, int relu, int use_tensor_cores, float* out, float* elapsed_ms) {
     return guard([&] { standalone_pointwise(a, m, k, w, n, bias, residual, relu, use_tensor_cores, out, elapsed_ms); });
 }
+int boxmot_b200_instance_norm(const float* x, int n, int h, int w, int c, const float* gamma, const float* beta,
+                              const float* residual, int relu, int pool, float* out) {
+    return guard([&] { standalone_instance_norm(x, n, h, w, c, gamma, beta, residual, relu, pool, out); });
+}
 int boxmot_b200_cosine_cost(const float* a, int rows, const float* b, int cols, int dim, double* out) {
     return guard([&] { standalone_cosine(a, rows, b, cols, dim, out); });
 }

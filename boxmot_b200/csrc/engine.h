@@ -243,5 +243,7 @@ void standalone_iou(const double* t, int T, const float* d, int D, double* out);
 void standalone_cosine(const float* a, int T, const float* b, int D, int F, double* out);
 void standalone_pointwise(const float* A, int M, int K, const float* W, int N, const float* bias, const float* residual,
                           int relu, int use_tc, float* out, float* elapsed_ms);
+void standalone_instance_norm(const float* x, int n, int H, int W, int C, const float* gamma, const float* beta,
+                              const float* residual, int relu, int pool, float* out);
 
 }  // namespace bmb

@@ -136,7 +136,10 @@ __global__ void __launch_bounds__(256) k_crop_resize_norm(const uint8_t* __restr
 // CTA = 8 output rows x 64 columns of one crop; the 21 x 134 x 3 input window and the weight chunk live in
 // shared memory; a thread owns two output pixels (x, x+32) x 16 output channels.
 // ---------------------------------------------------------------------------------------------------
+// RAW (the instance-norm stem of OSNet-AIN / OSNet-IBN): no bias, no ReLU; the instance norm and the ReLU are applied by
+// k_maxpool3s2_in.
 constexpr int ST_R = 8, ST_IR = 2 * ST_R + 5, ST_IC = IN_W + 6;
+template <bool RAW = false>
 __global__ void __launch_bounds__(256) k_stem(const float* __restrict__ blob, const float* __restrict__ w,
                                               const float* __restrict__ bias, int C0, const int* __restrict__ d_n,
                                               int off, int cap, float* __restrict__ out, int in_h) {
@@ -191,6 +194,11 @@ __global__ void __launch_bounds__(256) k_stem(const float* __restrict__ blob, co
         float* o1 = o0 + (size_t)32 * C0;
 #pragma unroll
         for (int q = 0; q < 4; ++q) {
+            if (RAW) {
+                reinterpret_cast<float4*>(o0)[q] = make_float4(acc0[q * 2].x, acc0[q * 2].y, acc0[q * 2 + 1].x, acc0[q * 2 + 1].y);
+                reinterpret_cast<float4*>(o1)[q] = make_float4(acc1[q * 2].x, acc1[q * 2].y, acc1[q * 2 + 1].x, acc1[q * 2 + 1].y);
+                continue;
+            }
             const float4 b = *reinterpret_cast<const float4*>(bias + co0 + q * 4);
             float4 r0 = make_float4(fmaxf(acc0[q * 2].x + b.x, 0.f), fmaxf(acc0[q * 2].y + b.y, 0.f),
                                     fmaxf(acc0[q * 2 + 1].x + b.z, 0.f), fmaxf(acc0[q * 2 + 1].y + b.w, 0.f));
@@ -250,6 +258,118 @@ __global__ void k_avgpool2(const float* __restrict__ in, int H, int W, int C, co
         o.x = (a.x + b.x + c.x + d.x) * 0.25f; o.y = (a.y + b.y + c.y + d.y) * 0.25f;
         o.z = (a.z + b.z + c.z + d.z) * 0.25f; o.w = (a.w + b.w + c.w + d.w) * 0.25f;
         *reinterpret_cast<float4*>(out + (((size_t)n * OH + oy) * OW + ox) * C + c4 * 4) = o;
+    }
+}
+
+// ---------------------------------------------------------------------------------------------------
+// K4b: InstanceNorm2d(affine=True, track_running_stats=False) of OSNet-AIN / OSNet-IBN on NHWC maps [crops][HW][C]:
+//   y = (x - mean_nc) / sqrt(var_nc + 1e-5) * gamma_c + beta_c,  mean / biased var over the crop's H x W.
+// Statistics: one CTA per (32-channel group, crop); lane = channel, eight pixel stripes of four float64 partial sums
+// each, combined in a fixed order, so a crop's statistics do not depend on the chunk it lands in or its position in it.
+// No floating-point atomics.  Output per (crop, channel): {mean, 1 / sqrt(var + eps)} in float64.
+// Apply: (x - mean) is taken in float64 and rounded once, then scaled by gamma * rstd and shifted by beta in float32
+// (no cancellation between x * scale and mean * scale when a channel is nearly constant).
+// ---------------------------------------------------------------------------------------------------
+constexpr int INS_LANES = 32, INS_STRIPES = 8;
+__global__ void __launch_bounds__(INS_LANES * INS_STRIPES) k_in_stats(const float* __restrict__ x, int HW, int C,
+                                                                      const int* __restrict__ d_n, int off, int cap,
+                                                                      double2* __restrict__ stats) {
+    const int n = blockIdx.y;
+    if (n >= chunk_count(d_n, off, cap)) return;
+    const int lane = threadIdx.x % INS_LANES, g = threadIdx.x / INS_LANES;
+    const int c = blockIdx.x * INS_LANES + lane;
+    __shared__ double s_sum[INS_STRIPES][INS_LANES], s_sq[INS_STRIPES][INS_LANES];
+    double s[4] = {0.0, 0.0, 0.0, 0.0}, q[4] = {0.0, 0.0, 0.0, 0.0};
+    if (c < C) {
+        const float* xp = x + (size_t)n * HW * C + c;
+        int p = g;
+        for (; p + 3 * INS_STRIPES < HW; p += 4 * INS_STRIPES) {
+#pragma unroll
+            for (int u = 0; u < 4; ++u) {
+                const double v = (double)__ldg(xp + (size_t)(p + u * INS_STRIPES) * C);
+                s[u] += v;
+                q[u] = fma(v, v, q[u]);
+            }
+        }
+        for (; p < HW; p += INS_STRIPES) {
+            const double v = (double)__ldg(xp + (size_t)p * C);
+            s[0] += v;
+            q[0] = fma(v, v, q[0]);
+        }
+    }
+    s_sum[g][lane] = (s[0] + s[1]) + (s[2] + s[3]);
+    s_sq[g][lane] = (q[0] + q[1]) + (q[2] + q[3]);
+    __syncthreads();
+    if (g == 0 && c < C) {
+        double ts = 0.0, tq = 0.0;
+        for (int k = 0; k < INS_STRIPES; ++k) { ts += s_sum[k][lane]; tq += s_sq[k][lane]; }
+        const double mean = ts / (double)HW;
+        const double var = fmax(tq / (double)HW - mean * mean, 0.0);
+        stats[(size_t)n * C + c] = make_double2(mean, 1.0 / sqrt(var + 1e-5));
+    }
+}
+
+__device__ __forceinline__ float in_apply1(float x, double2 st, float gamma, float beta) {
+    return fmaf((float)((double)x - st.x), (float)(st.y * (double)gamma), beta);
+}
+
+// out = act(IN(x) * gamma + beta (+ residual)); out may alias x or residual (element-wise, each element read once
+// before it is written).  act: 0 none, 1 ReLU.
+__global__ void k_in_apply(const float* x, const float* residual, float* out, int HW, int C,
+                           const float* __restrict__ gamma, const float* __restrict__ beta,
+                           const double2* __restrict__ stats, int relu, const int* __restrict__ d_n, int off, int cap) {
+    const int n_crops = chunk_count(d_n, off, cap);
+    const int C4 = C / 4;
+    const size_t per_crop = (size_t)HW * C4, total = (size_t)n_crops * per_crop;
+    for (size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (size_t)gridDim.x * blockDim.x) {
+        const int c = (int)(e % C4) * 4;
+        const size_t n = e / per_crop;
+        const double2* st = stats + n * C + c;
+        const float4 v = reinterpret_cast<const float4*>(x)[e];
+        const float4 gm = *reinterpret_cast<const float4*>(gamma + c);
+        const float4 bt = *reinterpret_cast<const float4*>(beta + c);
+        float4 y = make_float4(in_apply1(v.x, st[0], gm.x, bt.x), in_apply1(v.y, st[1], gm.y, bt.y),
+                               in_apply1(v.z, st[2], gm.z, bt.z), in_apply1(v.w, st[3], gm.w, bt.w));
+        if (residual) {
+            const float4 r = reinterpret_cast<const float4*>(residual)[e];
+            y.x += r.x; y.y += r.y; y.z += r.z; y.w += r.w;
+        }
+        if (relu) { y.x = fmaxf(y.x, 0.f); y.y = fmaxf(y.y, 0.f); y.z = fmaxf(y.z, 0.f); y.w = fmaxf(y.w, 0.f); }
+        reinterpret_cast<float4*>(out)[e] = y;
+    }
+}
+
+// K3 with the instance-norm stem fused in: max over the 3x3 window of relu(IN(x) * gamma + beta), applied per element
+// before the max (gamma may be negative, so the norm does not commute with the max).
+__global__ void k_maxpool3s2_in(const float* __restrict__ in, int H, int W, int C, const float* __restrict__ gamma,
+                                const float* __restrict__ beta, const double2* __restrict__ stats,
+                                const int* __restrict__ d_n, int off, int cap, float* __restrict__ out) {
+    const int n_crops = chunk_count(d_n, off, cap);
+    const int OH = H / 2, OW = W / 2, C4 = C / 4;
+    const size_t total = (size_t)n_crops * OH * OW * C4;
+    for (size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (size_t)gridDim.x * blockDim.x) {
+        const int c4 = (int)(e % C4);
+        size_t r = e / C4;
+        const int ox = (int)(r % OW); r /= OW;
+        const int oy = (int)(r % OH);
+        const int n = (int)(r / OH);
+        const double2* st = stats + (size_t)n * C + c4 * 4;
+        const double2 s0 = st[0], s1 = st[1], s2 = st[2], s3 = st[3];
+        const float4 gm = *reinterpret_cast<const float4*>(gamma + c4 * 4);
+        const float4 bt = *reinterpret_cast<const float4*>(beta + c4 * 4);
+        float4 m = make_float4(0.f, 0.f, 0.f, 0.f);   // every window holds a valid pixel and ReLU output is >= 0
+        for (int ky = 0; ky < 3; ++ky) {
+            const int iy = oy * 2 - 1 + ky;
+            if (iy < 0 || iy >= H) continue;
+            for (int kx = 0; kx < 3; ++kx) {
+                const int ix = ox * 2 - 1 + kx;
+                if (ix < 0 || ix >= W) continue;
+                const float4 v = *reinterpret_cast<const float4*>(in + (((size_t)n * H + iy) * W + ix) * C + c4 * 4);
+                m.x = fmaxf(m.x, in_apply1(v.x, s0, gm.x, bt.x)); m.y = fmaxf(m.y, in_apply1(v.y, s1, gm.y, bt.y));
+                m.z = fmaxf(m.z, in_apply1(v.z, s2, gm.z, bt.z)); m.w = fmaxf(m.w, in_apply1(v.w, s3, gm.w, bt.w));
+            }
+        }
+        *reinterpret_cast<float4*>(out + (((size_t)n * OH + oy) * OW + ox) * C + c4 * 4) = m;
     }
 }
 
@@ -1199,7 +1319,12 @@ struct BlockW {
     size_t cw, cb;
     TcW tc_c1, tc_c;
     TcW light_tc[10];   // LightConv 1x1 weights packed for the tensor-core stage (mid % 16 == 0)
+    // arch 4: instance norm of the block (IN_NONE / IN_BEFORE_RESIDUAL / IN_AFTER_RESIDUAL), its gamma / beta, and for
+    // IN_BEFORE_RESIDUAL with a downsample the downsample's own weights (cw / cb are then conv3 alone)
+    int in_mode = 0;
+    size_t ing = 0, inb = 0, dsw = 0, dsb = 0;
 };
+enum { IN_NONE = 0, IN_BEFORE_RESIDUAL = 1, IN_AFTER_RESIDUAL = 2 };
 
 namespace tcx { struct Plan; }
 
@@ -1220,8 +1345,11 @@ struct LmbnW {
 };
 
 struct ReidModel {
-    int arch = 1;                 // 1 OSNet, 2 MobileNetV2, 3 LMBN_n
+    int arch = 1;                 // 1 OSNet, 2 MobileNetV2, 3 LMBN_n, 4 OSNet with instance norms (AIN / IBN)
     int in_h = IN_H;              // crop height (the width is IN_W for every model)
+    bool stem_in = false;         // arch 4: conv 7x7 -> IN -> ReLU stem (stem_b is then gamma, stem_beta beta)
+    size_t stem_beta = 0;
+    float* in_tmp = nullptr;      // arch 4: conv3 output of an IN_BEFORE_RESIDUAL block with a downsample
     LmbnW lm;
     std::vector<MbBlock> mb;      // MobileNetV2 bottlenecks
     int mb_stem = 0, mb_stemp = 0, mb_last = 0;
@@ -1287,7 +1415,7 @@ ReidModel* reid_load(const char* path) {
     if (!f) throw std::runtime_error(std::string("cannot open ReID blob: ") + path);
     int32_t hdr[16];
     f.read(reinterpret_cast<char*>(hdr), sizeof(hdr));
-    if (!f || (uint32_t)hdr[0] != BLOB_MAGIC || hdr[1] != 1 || hdr[2] < 1 || hdr[2] > 3)
+    if (!f || (uint32_t)hdr[0] != BLOB_MAGIC || hdr[1] != 1 || hdr[2] < 1 || hdr[2] > 4)
         throw std::runtime_error("not a version-1 .b200reid blob (export it with boxmot_b200.weights.export_blob)");
     ReidModel* m = new ReidModel();
     if (hdr[2] == 2) {
@@ -1363,12 +1491,22 @@ ReidModel* reid_load(const char* path) {
                 throw std::runtime_error("unsupported LMBN_n blob header (expected 384x128 input, widths 64/256/384/512, 3584-d)");
             m->in_h = hdr[9];
         }
+        int in_modes[6] = {0, 0, 0, 0, 0, 0};
+        if (m->arch == 4) {   // header word 9: stem IN flag; words 10-15: per-block IN placement
+            m->stem_in = hdr[9] != 0;
+            for (int i = 0; i < 6; ++i) {
+                in_modes[i] = hdr[10 + i];
+                if (in_modes[i] < IN_NONE || in_modes[i] > IN_AFTER_RESIDUAL)
+                    throw std::runtime_error("bad instance-norm placement in an arch-4 ReID blob header");
+            }
+        }
         std::vector<float> host(n_floats);
         f.read(reinterpret_cast<char*>(host.data()), sizeof(float) * n_floats);
         if (!f) throw std::runtime_error("truncated ReID blob");
         size_t o = 0;
         auto take = [&](size_t n) { size_t r = o; o += (n + 3) / 4 * 4; return r; };  // 16-byte aligned tensors
-        auto take_block = [&](BlockW& b, int cin, int cout) {
+        auto take_block = [&](BlockW& b, int cin, int cout, int in_mode = IN_NONE) {
+            b.in_mode = in_mode;
             b.cin = cin;
             b.cout = cout;
             b.mid = b.cout / 4;
@@ -1386,11 +1524,26 @@ ReidModel* reid_load(const char* path) {
             b.g1b = take(b.hid);
             b.g2w = take((size_t)b.hid * b.mid);
             b.g2b = take(b.mid);
-            b.cw = take((size_t)(b.mid + (b.has_ds ? b.cin : 0)) * b.cout);
-            b.cb = take(b.cout);
+            if (in_mode == IN_BEFORE_RESIDUAL) {   // conv3 alone (zero bias), then the downsample on its own
+                b.cw = take((size_t)b.mid * b.cout);
+                b.cb = take(b.cout);
+                if (b.has_ds) {
+                    b.dsw = take((size_t)b.cin * b.cout);
+                    b.dsb = take(b.cout);
+                }
+            } else {
+                b.cw = take((size_t)(b.mid + (b.has_ds ? b.cin : 0)) * b.cout);
+                b.cb = take(b.cout);
+            }
+            if (in_mode != IN_NONE) {
+                if (b.cout % 4) throw std::runtime_error("unsupported OSNet width (instance-norm channels)");
+                b.ing = take(b.cout);
+                b.inb = take(b.cout);
+            }
         };
         m->stem_w = take((size_t)147 * m->c[0]);
         m->stem_b = take(m->c[0]);
+        if (m->stem_in) m->stem_beta = take(m->c[0]);
         if (m->arch == 3) {   // weights.fold_lmbn_n walk order
             LmbnW& lm = m->lm;
             take_block(lm.trunk[0], 64, 256);
@@ -1417,7 +1570,8 @@ ReidModel* reid_load(const char* path) {
             lm.ch_st = take((size_t)4 * LMBN_C);
         } else {
             for (int s = 0; s < 3; ++s) {
-                for (int j = 0; j < 2; ++j) take_block(m->blocks[s * 2 + j], j == 0 ? m->c[s] : m->c[s + 1], m->c[s + 1]);
+                for (int j = 0; j < 2; ++j)
+                    take_block(m->blocks[s * 2 + j], j == 0 ? m->c[s] : m->c[s + 1], m->c[s + 1], in_modes[s * 2 + j]);
                 if (s < 2) {
                     m->trans_w[s] = take((size_t)m->c[s + 1] * m->c[s + 1]);
                     m->trans_b[s] = take(m->c[s + 1]);
@@ -1502,6 +1656,14 @@ ReidModel* reid_load(const char* path) {
             RCUDA_OK(cudaMalloc(&m->sums[b], sizeof(float) * CH * 64 * (m->c[3] / 4)));
         }
         RCUDA_OK(cudaMalloc(&m->gates, sizeof(float) * CH * 4 * (m->c[3] / 4)));
+        // arch 4: the instance-norm statistics ({mean, rstd} per crop and channel, 4 floats) live in sums[0], which
+        // holds 16 * c3 >= 4 * C floats per crop and is free whenever they are needed (the stem runs before any block;
+        // a block's norm follows its gates kernel, the last reader of the branch sums).  The one extra buffer is the
+        // conv3 output of an IN_BEFORE_RESIDUAL block whose downsample GEMM writes the block output.
+        if (m->arch == 4)
+            for (const BlockW& b : m->blocks)
+                if (b.in_mode == IN_BEFORE_RESIDUAL && b.has_ds && !m->in_tmp)
+                    RCUDA_OK(cudaMalloc(&m->in_tmp, sizeof(float) * CH * big));
         if (m->arch == 3) {
             RCUDA_OK(cudaMalloc(&m->trunk, sizeof(float) * CH * (m->in_h / 8) * 16 * m->c[2]));
             RCUDA_OK(cudaMalloc(&m->pooled, sizeof(float) * CH * LMBN_POOLS * LMBN_C));
@@ -1522,7 +1684,7 @@ void reid_free(ReidModel* m) {
     if (!m) return;
     cudaFree(m->d_w); cudaFree(m->d_wtc); cudaFree(m->blob); cudaFree(m->bufA); cudaFree(m->bufB); cudaFree(m->x1);
     for (int b = 0; b < 4; ++b) { cudaFree(m->Y[b][0]); cudaFree(m->Y[b][1]); cudaFree(m->sums[b]); }
-    cudaFree(m->gates); cudaFree(m->trunk); cudaFree(m->pooled);
+    cudaFree(m->gates); cudaFree(m->trunk); cudaFree(m->pooled); cudaFree(m->in_tmp);
     tcx::plan_free(m->tc);
     delete m;
 }
@@ -1695,6 +1857,21 @@ struct Launcher {
 #undef BMB_LIGHT2
         return false;
     }
+    // instance norm (arch 4): statistics of x [crops][HW][C] into stats, timed under `cls`
+    void in_stats(const float* x, int HW, int C, double2* stats, int cls) {
+        begin(cls);
+        k_in_stats<<<dim3((C + INS_LANES - 1) / INS_LANES, upper), INS_LANES * INS_STRIPES, 0, st>>>(x, HW, C, d_n, off,
+                                                                                                       cap, stats);
+        end();
+        ++launches;
+    }
+    void in_apply(const float* x, const float* residual, float* out, int HW, int C, const float* gamma,
+                  const float* beta, const double2* stats, int relu, int cls) {
+        begin(cls);
+        k_in_apply<<<m->sms * 8, 256, 0, st>>>(x, residual, out, HW, C, gamma, beta, stats, relu, d_n, off, cap);
+        end();
+        ++launches;
+    }
     void light(const LightArgs& a, int n_branches, int threads) {
         if (m->light_v2 && light2(a, n_branches)) return;
         const int tiles = (a.H + a.R - 1) / a.R;
@@ -1758,11 +1935,34 @@ bool run_front(Launcher& L, const FrameIn& fi, StageTaps& stop_here) {
     L.end();
     ++L.launches;
     if (stop_here(m->blob, (size_t)m->in_h * IN_W * 3)) return true;
+    if (m->stem_in) {   // conv 7x7 -> IN -> ReLU -> max pool: the norm and the ReLU are applied inside the pool
+        const size_t smem = sizeof(float) * ((size_t)((ST_IR * ST_IC * 3 + 3) & ~3) + 147 * 16);
+        RCUDA_OK(cudaFuncSetAttribute(k_stem<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        L.begin(CLS_STEM);
+        k_stem<true><<<dim3(m->in_h / 2 / ST_R, L.upper), 256, smem, L.st>>>(m->blob, W + m->stem_w, nullptr, m->c[0],
+                                                                             L.d_n, L.off, L.cap, m->bufA, m->in_h);
+        L.end();
+        ++L.launches;
+        const int HW = (m->in_h / 2) * 64;
+        double2* stats = reinterpret_cast<double2*>(m->sums[0]);
+        L.in_stats(m->bufA, HW, m->c[0], stats, CLS_MAXPOOL);
+        if (m->debug_stop == 1) {   // the stem tap is the map after IN + ReLU, which the fused pool never writes
+            L.in_apply(m->bufA, nullptr, m->bufA, HW, m->c[0], W + m->stem_b, W + m->stem_beta, stats, 1, CLS_MAXPOOL);
+            return stop_here(m->bufA, (size_t)HW * m->c[0]);   // tap 1
+        }
+        ++stop_here.idx;   // tap 1 is only materialised when it is the one asked for
+        L.begin(CLS_MAXPOOL);
+        k_maxpool3s2_in<<<m->sms * 8, 256, 0, L.st>>>(m->bufA, m->in_h / 2, 64, m->c[0], W + m->stem_b, W + m->stem_beta,
+                                                      stats, L.d_n, L.off, L.cap, m->bufB);
+        L.end();
+        ++L.launches;
+        return stop_here(m->bufB, (size_t)(m->in_h / 4) * 32 * m->c[0]);
+    }
     {
         const size_t smem = sizeof(float) * ((size_t)((ST_IR * ST_IC * 3 + 3) & ~3) + 147 * 16);
-        RCUDA_OK(cudaFuncSetAttribute(k_stem, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        RCUDA_OK(cudaFuncSetAttribute(k_stem<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         L.begin(CLS_STEM);
-        k_stem<<<dim3(m->in_h / 2 / ST_R, L.upper), 256, smem, L.st>>>(m->blob, W + m->stem_w, W + m->stem_b, m->c[0],
+        k_stem<false><<<dim3(m->in_h / 2 / ST_R, L.upper), 256, smem, L.st>>>(m->blob, W + m->stem_w, W + m->stem_b, m->c[0],
                                                                        L.d_n, L.off, L.cap, m->bufA, m->in_h);
         L.end();
         ++L.launches;
@@ -1777,7 +1977,8 @@ bool run_front(Launcher& L, const FrameIn& fi, StageTaps& stop_here) {
 
 // One OSBlock (osnet.py:213-260): conv1 -> the four LightConv3x3 branches -> shared ChannelGate -> conv3 (+ downsample,
 // or the identity) + ReLU.  X [crops][H][Wd][cin] -> Xo [crops][H][Wd][cout] (Xo != X); scratch m->x1, m->Y, m->sums,
-// m->gates.
+// m->gates (and m->in_tmp).  b.in_mode places an instance norm before (OSNet-AIN) or after (OSNet-IBN) the residual
+// add; IN_NONE launches exactly the OSNet sequence.
 void run_osblock(Launcher& L, const BlockW& b, const float* X, float* Xo, int H, int Wd) {
     ReidModel* m = L.m;
     const float* W = m->d_w;
@@ -1831,12 +2032,36 @@ void run_osblock(Launcher& L, const BlockW& b, const float* X, float* Xo, int H,
     PwArgs c{};
     for (int br = 0; br < 4; ++br) c.branch[br] = m->Y[br][kDepth[br] & 1];
     c.gates = m->gates; c.mid = b.mid;
+    if (b.in_mode == IN_BEFORE_RESIDUAL) {
+        // OSBlockINin (osnet_ain.py): out = relu(IN(conv3(x2)) + identity').  conv3 (no bias, no ReLU) goes to a
+        // cout-wide scratch (Xo itself when the identity is X); the downsample GEMM writes Xo; the norm pass reads both.
+        float* x3 = b.has_ds ? m->in_tmp : Xo;
+        c.w = W + b.cw; c.bias = W + b.cb; c.out = x3;
+        c.K = b.mid; c.N = b.cout; c.HW = HW; c.relu = 0;
+        L.pointwise(c);
+        if (b.has_ds) {
+            PwArgs d{};
+            d.in = X; d.w = W + b.dsw; d.bias = W + b.dsb; d.out = Xo;
+            d.K = b.cin; d.N = b.cout; d.HW = HW; d.relu = 0;
+            L.pointwise(d);
+        }
+        double2* stats = reinterpret_cast<double2*>(m->sums[0]);
+        L.in_stats(x3, HW, b.cout, stats, CLS_POINTWISE);
+        L.in_apply(x3, b.has_ds ? Xo : X, Xo, HW, b.cout, W + b.ing, W + b.inb, stats, 1, CLS_POINTWISE);
+        return;
+    }
     c.in = b.has_ds ? X : nullptr;
     c.residual = b.has_ds ? nullptr : X;
     c.w = W + b.cw; c.bias = W + b.cb; c.out = Xo;
     c.K = b.mid + (b.has_ds ? b.cin : 0); c.N = b.cout; c.HW = HW; c.relu = 1;
     c.w_tc = b.tc_c.w; c.Kpad = b.tc_c.Kpad; c.Npad = b.tc_c.Npad;
+    if (b.in_mode == IN_AFTER_RESIDUAL) c.relu = 0;   // OSBlock(IN=True): out = relu(IN(conv3(x2) + identity'))
     L.pointwise(c);
+    if (b.in_mode == IN_AFTER_RESIDUAL) {
+        double2* stats = reinterpret_cast<double2*>(m->sums[0]);
+        L.in_stats(Xo, HW, b.cout, stats, CLS_POINTWISE);
+        L.in_apply(Xo, nullptr, Xo, HW, b.cout, W + b.ing, W + b.inb, stats, 1, CLS_POINTWISE);
+    }
 }
 
 // Transition (osnet.py conv2[2], conv3[2]): 1x1 + folded BN + ReLU of X [crops][H][Wd][C] into tmp, then 2x2 average
@@ -2104,6 +2329,50 @@ void standalone_pointwise(const float* A, int M, int K, const float* W, int N, c
         if (elapsed_ms) *elapsed_ms = ms / 10.f;
         cudaEventDestroy(e0); cudaEventDestroy(e1);
         RCUDA_OK(cudaMemcpy(out, dO, sizeof(float) * (size_t)M * N, cudaMemcpyDeviceToHost));
+    } catch (...) {
+        cleanup();
+        throw;
+    }
+    cleanup();
+}
+
+// Standalone instance norm on host arrays (parity tests): x [n][H][W][C] float32.
+//   pool == 0: out [n][H][W][C] = act(IN(x) * gamma + beta (+ residual))     (k_in_stats + k_in_apply)
+//   pool == 1: out [n][H/2][W/2][C] = maxpool3x3s2(relu(IN(x) * gamma + beta)) (k_in_stats + k_maxpool3s2_in)
+void standalone_instance_norm(const float* x, int n, int H, int W, int C, const float* gamma, const float* beta,
+                              const float* residual, int relu, int pool, float* out) {
+    if (n <= 0 || H <= 0 || W <= 0 || C <= 0 || C % 4 || (pool && (H % 2 || W % 2)))
+        throw std::runtime_error("n, H, W, C > 0, C a multiple of 4 (and H, W even to pool) required");
+    const size_t elems = (size_t)n * H * W * C, out_elems = pool ? elems / 4 : elems;
+    float *dx = nullptr, *dg = nullptr, *db = nullptr, *dr = nullptr, *dout = nullptr;
+    double2* dst = nullptr;
+    int* dn = nullptr;
+    auto cleanup = [&] { cudaFree(dx); cudaFree(dg); cudaFree(db); cudaFree(dr); cudaFree(dout); cudaFree(dst); cudaFree(dn); };
+    try {
+        RCUDA_OK(cudaMalloc(&dx, sizeof(float) * elems));
+        RCUDA_OK(cudaMalloc(&dg, sizeof(float) * C));
+        RCUDA_OK(cudaMalloc(&db, sizeof(float) * C));
+        RCUDA_OK(cudaMalloc(&dout, sizeof(float) * out_elems));
+        RCUDA_OK(cudaMalloc(&dst, sizeof(double2) * (size_t)n * C));
+        RCUDA_OK(cudaMalloc(&dn, sizeof(int)));
+        RCUDA_OK(cudaMemcpy(dx, x, sizeof(float) * elems, cudaMemcpyHostToDevice));
+        RCUDA_OK(cudaMemcpy(dg, gamma, sizeof(float) * C, cudaMemcpyHostToDevice));
+        RCUDA_OK(cudaMemcpy(db, beta, sizeof(float) * C, cudaMemcpyHostToDevice));
+        if (residual && !pool) {
+            RCUDA_OK(cudaMalloc(&dr, sizeof(float) * elems));
+            RCUDA_OK(cudaMemcpy(dr, residual, sizeof(float) * elems, cudaMemcpyHostToDevice));
+        }
+        RCUDA_OK(cudaMemcpy(dn, &n, sizeof(int), cudaMemcpyHostToDevice));
+        ReidModel fake;
+        Launcher L{&fake, dn, 0, n, n, nullptr};
+        L.in_stats(dx, H * W, C, dst, CLS_POINTWISE);
+        if (pool)
+            k_maxpool3s2_in<<<fake.sms * 8, 256>>>(dx, H, W, C, dg, db, dst, dn, 0, n, dout);
+        else
+            L.in_apply(dx, dr, dout, H * W, C, dg, db, dst, relu, CLS_POINTWISE);
+        RCUDA_OK(cudaGetLastError());
+        RCUDA_OK(cudaDeviceSynchronize());
+        RCUDA_OK(cudaMemcpy(out, dout, sizeof(float) * out_elems, cudaMemcpyDeviceToHost));
     } catch (...) {
         cleanup();
         throw;

@@ -123,6 +123,94 @@ def make_osnet_state(arch: str = "osnet_x0_25", seed: int = 0, feature_dim: int 
     return sd
 
 
+def _in_affine(g, sd, name, c):
+    """InstanceNorm2d(affine=True) parameters: randomised gamma / beta (some gammas negative) so the affine path and
+    the sign handling of the fused ReLU + max pool are exercised."""
+    import torch
+
+    sd[name + ".weight"] = (0.5 + torch.rand(c, generator=g)) * torch.where(torch.rand(c, generator=g) < 0.15, -1.0, 1.0)
+    sd[name + ".bias"] = 0.2 * torch.randn(c, generator=g)
+
+
+# reid/backbones/osnet_ain.py: which blocks of conv2 / conv3 / conv4 are OSBlockINin (IN before the residual add)
+OSNET_AIN_ININ = ((True, True), (False, True), (True, False))
+
+
+def _osnet_arch(width: str) -> str:
+    """Width name: x0_75, osnet_x0_75 or osnet_ain_x0_75 -> osnet_x0_75."""
+    return "osnet_" + width[width.index("x"):]
+
+
+def make_osnet_ain_state(width: str = "x1_0", seed: int = 0, feature_dim: int = 512, num_classes: int = 4101):
+    """Seeded state dict with the parameter names of the reference's osnet_ain_x{1_0,0_75,0_5,0_25}
+    (reid/backbones/osnet_ain.py): stem conv + InstanceNorm, blocks `[[INin, INin], [OSBlock, INin], [INin, OSBlock]]`
+    whose branches are `conv2.{t}.layers.{i}`, transitions `pool2.0` / `pool3.0`.  `width` is e.g. "x0_75" or
+    "osnet_ain_x0_75"."""
+    import torch
+
+    ch = OSNET_ARCHS[_osnet_arch(width)]
+    g = torch.Generator().manual_seed(seed)
+    sd = {}
+    conv, bn, _ = _osnet_makers(g, sd)
+
+    def block(name, cin, cout, inin):
+        mid = cout // 4
+        conv(name + ".conv1.conv", mid, cin, 1)
+        bn(name + ".conv1.bn", mid)
+        for t in range(4):
+            for i in range(t + 1):
+                lname = f"{name}.conv2.{t}.layers.{i}"
+                conv(lname + ".conv1", mid, mid, 1)
+                conv(lname + ".conv2", mid, mid, 3, groups=mid)
+                bn(lname + ".bn", mid)
+        hid = mid // 16
+        conv(name + ".gate.fc1", hid, mid, 1)
+        sd[name + ".gate.fc1.bias"] = 0.1 * torch.randn(hid, generator=g)
+        conv(name + ".gate.fc2", mid, hid, 1)
+        sd[name + ".gate.fc2.bias"] = 0.1 * torch.randn(mid, generator=g)
+        conv(name + ".conv3.conv", cout, mid, 1, gain=0.1 if not inin else 1.0)
+        if not inin:
+            bn(name + ".conv3.bn", cout)
+        if cin != cout:
+            conv(name + ".downsample.conv", cout, cin, 1)
+            bn(name + ".downsample.bn", cout)
+        if inin:
+            _in_affine(g, sd, name + ".IN", cout)
+
+    conv("conv1.conv", ch[0], 3, 7)
+    _in_affine(g, sd, "conv1.bn", ch[0])
+    for s, (cin, cout) in enumerate(((ch[0], ch[1]), (ch[1], ch[2]), (ch[2], ch[3]))):
+        block(f"conv{s + 2}.0", cin, cout, OSNET_AIN_ININ[s][0])
+        block(f"conv{s + 2}.1", cout, cout, OSNET_AIN_ININ[s][1])
+        if s < 2:
+            conv(f"pool{s + 2}.0.conv", cout, cout, 1)
+            bn(f"pool{s + 2}.0.bn", cout)
+    conv("conv5.conv", ch[3], ch[3], 1)
+    bn("conv5.bn", ch[3])
+    sd["fc.0.weight"] = 0.05 * torch.randn(feature_dim, ch[3], generator=g)
+    sd["fc.0.bias"] = 0.05 * torch.randn(feature_dim, generator=g)
+    bn("fc.1", feature_dim)
+    sd["classifier.weight"] = 0.01 * torch.randn(num_classes, feature_dim, generator=g)
+    sd["classifier.bias"] = torch.zeros(num_classes)
+    return sd
+
+
+def make_osnet_ibn_state(seed: int = 0, feature_dim: int = 512, num_classes: int = 4101):
+    """Seeded state dict with the parameter names of the reference's osnet_ibn_x1_0 (reid/backbones/osnet.py:548,
+    `IN=True`): the osnet_x1_0 names, with the stem's `conv1.bn` an InstanceNorm (weight and bias only) and an
+    InstanceNorm `IN` after the residual add of conv2.0 and conv2.1."""
+    import torch
+
+    sd = make_osnet_state("osnet_x1_0", seed=seed, feature_dim=feature_dim, num_classes=num_classes)
+    g = torch.Generator().manual_seed(seed + 7919)
+    for k in [k for k in sd if k.startswith("conv1.bn.")]:
+        del sd[k]
+    _in_affine(g, sd, "conv1.bn", 64)
+    for j in range(2):
+        _in_affine(g, sd, f"conv2.{j}.IN", 256)
+    return sd
+
+
 LMBN_BRANCHES = ("global_branch", "partial_branch", "channel_branch")
 
 

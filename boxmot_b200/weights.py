@@ -18,6 +18,9 @@ followed by float32 parameters in the exact order csrc/reid_model.cu walks them:
     fc        W[c3][feat] (BatchNorm1d folded), b[feat]
 Arch 3 (LMBN_n, `fold_lmbn_n`) keeps the OSNet header dims (64, 256, 384, 512, feat 3584) and records the input
 height (384) in header word 9; its tensors reuse the OSBlock / transition layouts above.
+Arch 4 (OSNet-AIN / OSNet-IBN, `fold_osnet_in`) keeps the arch-1 layout and header dims; header word 9 flags the
+stem's instance norm and words 10-15 hold each block's IN placement (0 none, 1 before the residual add, 2 after it),
+with the gamma / beta arrays stored right after the tensors of the stem or block they belong to.
 All 1x1 weights are stored K-major ([cin][cout]) so a thread owning consecutive output channels loads
 consecutive floats; every tensor is zero-padded to a multiple of 4 floats (16-byte aligned float4 loads).
 """
@@ -35,6 +38,7 @@ VERSION = 1
 ARCH_OSNET = 1
 ARCH_MOBILENETV2 = 2
 ARCH_LMBN_N = 3
+ARCH_OSNET_IN = 4
 BRANCHES = (("conv2a", 1), ("conv2b", 2), ("conv2c", 3), ("conv2d", 4))
 EPS = 1e-5
 
@@ -178,6 +182,119 @@ def fold_lmbn_n(sd) -> List[np.ndarray]:
     return out
 
 
+# OSNet with instance norms (arch 4): osnet_ain_x{1_0,0_75,0_5,0_25} (reid/backbones/osnet_ain.py) and osnet_ibn_x1_0
+# (reid/backbones/osnet.py:548).  Per-block IN placement, recorded in header words 10-15:
+IN_NONE, IN_BEFORE_RESIDUAL, IN_AFTER_RESIDUAL = 0, 1, 2
+
+
+def _ignored(k: str) -> bool:
+    return k.startswith("classifier.") or k.endswith("num_batches_tracked")
+
+
+def _osnet_in_variant(sd):
+    """("ain" | "ibn", width name) for a state dict shaped like one of the OSNet-with-IN networks, else None."""
+    from .synthetic import OSNET_ARCHS
+
+    if "conv1.conv.weight" not in sd:
+        return None
+    c0 = sd["conv1.conv.weight"].shape[0]
+    width = next((name for name, ch in OSNET_ARCHS.items() if ch[0] == c0), None)
+    if "pool2.0.conv.weight" in sd or any(".layers." in k for k in sd):
+        return "ain", width
+    if any(".IN." in k for k in sd) or ("conv1.bn.weight" in sd and "conv1.bn.running_var" not in sd):
+        return "ibn", width
+    return None
+
+
+def _osnet_in_keys(variant, width):
+    from .synthetic import make_osnet_ain_state, make_osnet_ibn_state
+
+    if width is None or (variant == "ibn" and width != "osnet_x1_0"):
+        return None
+    sd = make_osnet_ain_state(width, 0, num_classes=1) if variant == "ain" else make_osnet_ibn_state(0, num_classes=1)
+    return {k for k in sd if not _ignored(k)}
+
+
+def _in_affine(sd, name):
+    return [_np(sd[name + ".weight"]), _np(sd[name + ".bias"])]
+
+
+def fold_osnet_in(sd):
+    """OSNet-AIN / OSNet-IBN state dict -> (dims, IN modes [stem, block 0..5], arrays) of the arch-4 blob.  The arrays
+    keep the arch-1 order; where an instance norm sits:
+        stem      W[147][c0] (no bias, no fold), gamma[c0], beta[c0]           (IN then ReLU, before the max pool)
+        IN_BEFORE_RESIDUAL block (OSBlockINin): ... gate, conv3 W[mid][cout], zero bias[cout],
+                  then (downsample) W[cin][cout] with its BN folded, b[cout], then gamma[cout], beta[cout]
+        IN_AFTER_RESIDUAL block (IBN conv2.0 / conv2.1): the arch-1 combine (conv3 rows, downsample rows, summed bias),
+                  then gamma[cout], beta[cout]
+    Refuses (ValueError, naming the keys) any state dict whose key set, apart from `classifier.*` and
+    `num_batches_tracked`, is not exactly the one of the variant its structure suggests."""
+    from .synthetic import OSNET_AIN_ININ, OSNET_ARCHS
+
+    variant, width = _osnet_in_variant(sd) or (None, None)
+    want = _osnet_in_keys(variant, width) if variant else None
+    keys = {k for k in sd if not _ignored(k)}
+    if want is None or keys != want:
+        label = {"ain": "OSNet-AIN", "ibn": "OSNet-IBN x1_0"}.get(variant, "OSNet with instance norms")
+        extra, missing = sorted(keys - (want or set()))[:4], sorted((want or set()) - keys)[:4]
+        raise ValueError(f"not an {label} state dict of a known width (unexpected keys {extra}, missing keys "
+                         f"{missing}); osnet_ain_x1_0 / _x0_75 / _x0_5 / _x0_25 and osnet_ibn_x1_0 are supported")
+    chans = list(OSNET_ARCHS[width])
+    feat = sd["fc.0.weight"].shape[0]
+    w = _np(sd["conv1.conv.weight"])
+    out: List[np.ndarray] = [w.transpose(2, 3, 1, 0).reshape(147, chans[0])] + _in_affine(sd, "conv1.bn")
+    modes = [1]
+    for s in range(3):
+        for j in range(2):
+            name, cin, cout = f"conv{s + 2}.{j}", chans[s] if j == 0 else chans[s + 1], chans[s + 1]
+            if variant == "ain":
+                inin = OSNET_AIN_ININ[s][j]
+                out += _fold_ain_block(sd, name, cin, cout, inin)
+                modes.append(IN_BEFORE_RESIDUAL if inin else IN_NONE)
+            else:
+                out += _fold_osblock(sd, name, cin, cout)
+                if (name + ".IN.weight") in sd:
+                    out += _in_affine(sd, name + ".IN")
+                modes.append(IN_AFTER_RESIDUAL if (name + ".IN.weight") in sd else IN_NONE)
+        if s < 2:
+            t = f"pool{s + 2}.0" if variant == "ain" else f"conv{s + 2}.2.0"
+            out += list(_pw(sd, t + ".conv", t + ".bn"))
+    out += list(_pw(sd, "conv5.conv", "conv5.bn"))
+    wf, bf = _np(sd["fc.0.weight"]), _np(sd["fc.0.bias"])
+    scale, shift = _bn_fold(sd, "fc.1")
+    out += [(wf * scale[:, None]).T.copy(), bf * scale + shift]
+    return chans + [feat], modes, out
+
+
+def _fold_ain_block(sd, name, cin, cout, inin) -> List[np.ndarray]:
+    """osnet_ain.py OSBlock / OSBlockINin: the OSNet layout with the branches read from `conv2.{t}.layers.{i}`."""
+    mid = cout // 4
+    assert sd[name + ".conv1.conv.weight"].shape[:2] == (mid, cin)
+    out = list(_pw(sd, name + ".conv1.conv", name + ".conv1.bn"))
+    for t in range(4):
+        for i in range(t + 1):
+            lname = f"{name}.conv2.{t}.layers.{i}"
+            wpw, _ = _pw(sd, lname + ".conv1")
+            sc, sh = _bn_fold(sd, lname + ".bn")
+            wdw = _np(sd[lname + ".conv2.weight"])[:, 0] * sc[:, None, None]
+            out += [wpw, wdw.reshape(mid, 9).T.copy(), sh]
+    w1, b1 = _pw(sd, name + ".gate.fc1")
+    w2, b2 = _pw(sd, name + ".gate.fc2")
+    out += [w1, b1, w2, b2]
+    has_ds = (name + ".downsample.conv.weight") in sd
+    if not inin:
+        w3, b3 = _pw(sd, name + ".conv3.conv", name + ".conv3.bn")
+        if has_ds:
+            wd, bd = _pw(sd, name + ".downsample.conv", name + ".downsample.bn")
+            return out + [np.concatenate([w3, wd], 0), b3 + bd]
+        return out + [w3, b3]
+    w3, _ = _pw(sd, name + ".conv3.conv")   # Conv1x1Linear(bn=False): the instance norm follows directly
+    out += [w3, np.zeros(cout)]
+    if has_ds:
+        out += list(_pw(sd, name + ".downsample.conv", name + ".downsample.bn"))
+    return out + _in_affine(sd, name + ".IN")
+
+
 def _pad4(n: int) -> int:
     return (n + 3) // 4 * 4
 
@@ -247,10 +364,13 @@ def export_blob(weights, out_path=None) -> Path:
         sd = weights
         if out_path is None:
             raise ValueError("out_path is required when exporting an in-memory state dict")
-    table = []
+    table, in_modes = [], []
     if "conv9.conv.weight" in sd:
         stem_c, feat, table, arrays = fold_mobilenetv2(sd)
         arch, dims = ARCH_MOBILENETV2, [stem_c, len(table), 0, 0, feat]
+    elif _osnet_in_variant(sd) is not None:
+        dims, in_modes, arrays = fold_osnet_in(sd)
+        arch = ARCH_OSNET_IN
     elif "conv1.conv.weight" in sd and "conv5.conv.weight" in sd and "fc.0.weight" in sd:
         dims, arrays = fold_osnet(sd)
         arch = ARCH_OSNET
@@ -258,7 +378,8 @@ def export_blob(weights, out_path=None) -> Path:
         arrays = fold_lmbn_n(sd)
         arch, dims = ARCH_LMBN_N, [64, 256, 384, 512, LMBN_FEAT]
     else:
-        raise ValueError("only OSNet, MobileNetV2 and LMBN_n state dicts are implemented on the B200 ReID path")
+        raise ValueError("only OSNet, OSNet-AIN, OSNet-IBN, MobileNetV2 and LMBN_n state dicts are implemented on the "
+                         "B200 ReID path")
     # every tensor starts on a 16-byte boundary (the kernels read weights as float4)
     padded = []
     for a in arrays:
@@ -268,6 +389,8 @@ def export_blob(weights, out_path=None) -> Path:
     header = [MAGIC, VERSION, arch, *dims, int(payload.size)] + [0] * (16 - 9)
     if arch == ARCH_LMBN_N:
         header[9] = LMBN_INPUT_H
+    if arch == ARCH_OSNET_IN:
+        header[9:16] = in_modes
     out_path = Path(out_path)
     tmp = out_path.with_suffix(out_path.suffix + ".tmp")
     with open(tmp, "wb") as f:

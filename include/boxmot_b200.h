@@ -407,9 +407,16 @@ BOXMOT_B200_API int boxmot_b200_cosine_cost(const float* a, int rows, const floa
 BOXMOT_B200_API int boxmot_b200_pointwise_gemm(const float* a, int m, int k, const float* w, int n, const float* bias,
                                                const float* residual, int relu, int use_tensor_cores, float* out,
                                                float* elapsed_ms);
+/* Instance norm (InstanceNorm2d, affine, eps 1e-5, statistics per crop and channel) of OSNet-AIN / OSNet-IBN on host
+ * arrays, x (n,H,W,C) NHWC float32, C a multiple of 4.  pool = 0: out (n,H,W,C) = act(IN(x) * gamma + beta
+ * (+ residual, optional)), act = ReLU when relu = 1.  pool = 1: the stem form, out (n,H/2,W/2,C) = 3x3 stride-2
+ * max pool of relu(IN(x) * gamma + beta). */
+BOXMOT_B200_API int boxmot_b200_instance_norm(const float* x, int n, int h, int w, int c, const float* gamma,
+                                              const float* beta, const float* residual, int relu, int pool, float* out);
 BOXMOT_B200_API int boxmot_b200_device_count(void);
 /* Diagnostics for the ReID kernels: run the forward up to `stage` (0 input blob, 1 stem, 2 max-pool, 3..10 the
- * six OSBlocks and two transitions in order, 11 conv5) and copy that NHWC float32 tensor of the n crops out. */
+ * six OSBlocks and two transitions in order, 11 conv5) and copy that NHWC float32 tensor of the n crops out.  For
+ * OSNet-AIN / OSNet-IBN the stem tap is the map after the instance norm and the ReLU. */
 BOXMOT_B200_API int boxmot_b200_reid_debug_stage(void* reid_handle, const float* boxes_xyxy, int n_boxes,
                                                  const uint8_t* image_data, int image_rows, int image_cols,
                                                  int stage, float* out, int out_capacity_floats,
