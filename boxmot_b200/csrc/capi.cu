@@ -390,6 +390,14 @@ int boxmot_b200_instance_norm(const float* x, int n, int h, int w, int c, const 
                               const float* residual, int relu, int pool, float* out) {
     return guard([&] { standalone_instance_norm(x, n, h, w, c, gamma, beta, residual, relu, pool, out); });
 }
+int boxmot_b200_resnet_conv(const float* in0, int n, int h0, int w0, int c0, int k, int stride, const float* in1, int h1,
+                            int w1, int c1, int stride1, const float* w, int out_c, const float* bias,
+                            const float* residual, int relu, float* out, float* elapsed_ms) {
+    return guard([&] {
+        standalone_resnet_conv(in0, n, h0, w0, c0, k, stride, in1, h1, w1, c1, stride1, w, out_c, bias, residual, relu,
+                               out, elapsed_ms);
+    });
+}
 int boxmot_b200_cosine_cost(const float* a, int rows, const float* b, int cols, int dim, double* out) {
     return guard([&] { standalone_cosine(a, rows, b, cols, dim, out); });
 }

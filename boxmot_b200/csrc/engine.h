@@ -245,5 +245,8 @@ void standalone_pointwise(const float* A, int M, int K, const float* W, int N, c
                           int relu, int use_tc, float* out, float* elapsed_ms);
 void standalone_instance_norm(const float* x, int n, int H, int W, int C, const float* gamma, const float* beta,
                               const float* residual, int relu, int pool, float* out);
+void standalone_resnet_conv(const float* in0, int n, int h0, int w0, int c0, int k, int stride, const float* in1, int h1,
+                            int w1, int c1, int stride1, const float* w, int N, const float* bias, const float* residual,
+                            int relu, float* out, float* elapsed_ms);
 
 }  // namespace bmb

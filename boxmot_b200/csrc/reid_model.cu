@@ -24,6 +24,7 @@
 
 #include "engine.h"
 #include "pointwise_tc.cuh"
+#include "resnet_tc.cuh"
 
 namespace bmb {
 
@@ -1344,14 +1345,20 @@ struct LmbnW {
     size_t neck_w[5] = {0, 0, 0, 0, 0}, neck_b[5] = {0, 0, 0, 0, 0}, sh_w = 0, sh_b = 0, ch_st = 0;
 };
 
+// Bottleneck ResNet (arch 5): per convolution the folded bias (offset in d_w) and the tensor-core packing of its weights
+struct RnConv { size_t b = 0; const float* w = nullptr; };
+struct RnBlock { int cin, width, cout, stride; RnConv c1, c2, c3; };
+
 struct ReidModel {
-    int arch = 1;                 // 1 OSNet, 2 MobileNetV2, 3 LMBN_n, 4 OSNet with instance norms (AIN / IBN)
+    int arch = 1;                 // 1 OSNet, 2 MobileNetV2, 3 LMBN_n, 4 OSNet with instance norms (AIN / IBN), 5 ResNet
     int in_h = IN_H;              // crop height (the width is IN_W for every model)
     bool stem_in = false;         // arch 4: conv 7x7 -> IN -> ReLU stem (stem_b is then gamma, stem_beta beta)
     size_t stem_beta = 0;
     float* in_tmp = nullptr;      // arch 4: conv3 output of an IN_BEFORE_RESIDUAL block with a downsample
     LmbnW lm;
     std::vector<MbBlock> mb;      // MobileNetV2 bottlenecks
+    std::vector<RnBlock> rn;      // ResNet Bottlenecks, layer1.0 .. layer4.last
+    float* d_wrn = nullptr;       // ResNet: every convolution's weights packed by rn::pack_conv_weights
     int mb_stem = 0, mb_stemp = 0, mb_last = 0;
     size_t mb_stem_w = 0, mb_stem_b = 0, mb_c9w = 0, mb_c9b = 0;
     int c[4] = {0, 0, 0, 0};
@@ -1415,9 +1422,75 @@ ReidModel* reid_load(const char* path) {
     if (!f) throw std::runtime_error(std::string("cannot open ReID blob: ") + path);
     int32_t hdr[16];
     f.read(reinterpret_cast<char*>(hdr), sizeof(hdr));
-    if (!f || (uint32_t)hdr[0] != BLOB_MAGIC || hdr[1] != 1 || hdr[2] < 1 || hdr[2] > 4)
+    if (!f || (uint32_t)hdr[0] != BLOB_MAGIC || hdr[1] != 1 || hdr[2] < 1 || hdr[2] > 5)
         throw std::runtime_error("not a version-1 .b200reid blob (export it with boxmot_b200.weights.export_blob)");
     ReidModel* m = new ReidModel();
+    if (hdr[2] == 5) {
+        // ---- Bottleneck ResNet (reid/backbones/resnet.py resnet50 / resnet101): stem, layer1..4, GAP ----
+        try {
+            m->arch = 5;
+            m->c[0] = 64;
+            m->feat = hdr[7];
+            const size_t n_floats = (size_t)hdr[8];
+            for (int l = 0; l < 4; ++l)
+                if (hdr[3 + l] < 1 || hdr[3 + l] > 64) throw std::runtime_error("bad ResNet blob header (block counts)");
+            if (m->feat != 2048) throw std::runtime_error("bad ResNet blob header (feature dim)");
+            std::vector<float> host(n_floats);
+            f.read(reinterpret_cast<char*>(host.data()), sizeof(float) * n_floats);
+            if (!f) throw std::runtime_error("truncated ReID blob");
+            size_t o = 0;
+            auto take = [&](size_t n) { size_t r = o; o += (n + 3) / 4 * 4; return r; };
+            m->stem_w = take((size_t)147 * 64);
+            m->stem_b = take(64);
+            struct Todo { RnConv* dst; size_t w; int K, N; size_t at; };
+            std::vector<Todo> todo;
+            size_t packed_n = 0;
+            auto conv = [&](RnConv& c, int K, int N) {
+                const size_t w = take((size_t)K * N);
+                c.b = take(N);
+                todo.push_back({&c, w, K, N, packed_n});
+                packed_n += 2 * (size_t)K * N;
+            };
+            int cin = 64;
+            m->rn.reserve((size_t)hdr[3] + hdr[4] + hdr[5] + hdr[6]);   // `todo` keeps pointers into the blocks
+            for (int l = 0; l < 4; ++l)
+                for (int j = 0; j < hdr[3 + l]; ++j) {
+                    RnBlock b{};
+                    b.cin = cin; b.width = 64 << l; b.cout = 4 * b.width; b.stride = (j == 0 && l > 0) ? 2 : 1;
+                    m->rn.push_back(b);
+                    RnBlock& r = m->rn.back();
+                    conv(r.c1, r.cin, r.width);
+                    conv(r.c2, 9 * r.width, r.width);
+                    conv(r.c3, r.width + (j == 0 ? r.cin : 0), r.cout);
+                    cin = r.cout;
+                }
+            if (o != n_floats || cin != m->feat) throw std::runtime_error("ReID blob size does not match its header");
+            std::vector<float> packed(packed_n);
+            for (auto& t : todo) rn::pack_conv_weights(host.data() + t.w, t.K, t.N, packed.data() + t.at);
+            RCUDA_OK(cudaMalloc(&m->d_w, sizeof(float) * n_floats));
+            RCUDA_OK(cudaMemcpy(m->d_w, host.data(), sizeof(float) * n_floats, cudaMemcpyHostToDevice));
+            RCUDA_OK(cudaMalloc(&m->d_wrn, sizeof(float) * packed_n));
+            RCUDA_OK(cudaMemcpy(m->d_wrn, packed.data(), sizeof(float) * packed_n, cudaMemcpyHostToDevice));
+            for (auto& t : todo) t.dst->w = m->d_wrn + t.at;
+            if (const char* ce = getenv("BOXMOT_B200_REID_CHUNK")) {
+                const int v = atoi(ce);
+                if (v >= 8 && v <= 1024) m->chunk = v;
+            }
+            // per crop: the staged crop, two block maps as large as the stem output / layer1's 64x32x256, layer2.0's
+            // conv1 output (64x32x128) and layer1's conv2 output (64x32x64): 1.54 M floats, below the 2.36 M an
+            // OSNet_x1_0 chunk takes per crop, so the chunk keeps its size
+            const size_t CH = m->chunk, big = (size_t)128 * 64 * 64;
+            RCUDA_OK(cudaMalloc(&m->blob, sizeof(float) * CH * IN_H * IN_W * 3));
+            RCUDA_OK(cudaMalloc(&m->bufA, sizeof(float) * CH * big));
+            RCUDA_OK(cudaMalloc(&m->bufB, sizeof(float) * CH * big));
+            RCUDA_OK(cudaMalloc(&m->x1, sizeof(float) * CH * 64 * 32 * 128));
+            RCUDA_OK(cudaMalloc(&m->Y[0][0], sizeof(float) * CH * 64 * 32 * 64));
+        } catch (...) {
+            reid_free(m);
+            throw;
+        }
+        return m;
+    }
     if (hdr[2] == 2) {
         // ---- MobileNetV2 (reid/backbones/mobilenetv2.py): stem, 17 inverted-residual blocks, conv9, GAP ----
         try {
@@ -1684,7 +1757,7 @@ void reid_free(ReidModel* m) {
     if (!m) return;
     cudaFree(m->d_w); cudaFree(m->d_wtc); cudaFree(m->blob); cudaFree(m->bufA); cudaFree(m->bufB); cudaFree(m->x1);
     for (int b = 0; b < 4; ++b) { cudaFree(m->Y[b][0]); cudaFree(m->Y[b][1]); cudaFree(m->sums[b]); }
-    cudaFree(m->gates); cudaFree(m->trunk); cudaFree(m->pooled); cudaFree(m->in_tmp);
+    cudaFree(m->gates); cudaFree(m->trunk); cudaFree(m->pooled); cudaFree(m->in_tmp); cudaFree(m->d_wrn);
     tcx::plan_free(m->tc);
     delete m;
 }
@@ -1869,6 +1942,21 @@ struct Launcher {
                   const float* beta, const double2* stats, int relu, int cls) {
         begin(cls);
         k_in_apply<<<m->sms * 8, 256, 0, st>>>(x, residual, out, HW, C, gamma, beta, stats, relu, d_n, off, cap);
+        end();
+        ++launches;
+    }
+    // one ResNet convolution (rn::k_conv_tc) over the output pixels of at most `upper` crops
+    void conv_tc(const rn::ConvArgs& a) {
+        const int BN = rn::tile_n(a.N);
+        const dim3 grid((unsigned)(((size_t)upper * a.Ho * a.Wo + rn::BM - 1) / rn::BM), (unsigned)(a.N / BN));
+        begin(a.k0 == 3 ? CLS_LIGHTCONV : CLS_POINTWISE);
+        if (BN == 128) {
+            RCUDA_OK(cudaFuncSetAttribute(rn::k_conv_tc<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rn::smem_bytes<128>()));
+            rn::k_conv_tc<128><<<grid, rn::THREADS, rn::smem_bytes<128>(), st>>>(a, d_n, off, cap);
+        } else {
+            RCUDA_OK(cudaFuncSetAttribute(rn::k_conv_tc<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rn::smem_bytes<64>()));
+            rn::k_conv_tc<64><<<grid, rn::THREADS, rn::smem_bytes<64>(), st>>>(a, d_n, off, cap);
+        }
         end();
         ++launches;
     }
@@ -2140,6 +2228,48 @@ void run_lmbn_chunk(Launcher& L, const FrameIn& fi, float* d_out, int out_ld) {
     L.end();
     ++L.launches;
 }
+
+// Bottleneck ResNet, one chunk (resnet.py featuremaps + global average pool).  Taps: 0 crop, 1 stem, 2 pool, then
+// 3 + i after Bottleneck i (layer1.0 first).  Per Bottleneck: conv1 (1x1) and conv2 (3x3, the block's stride) with
+// bias + ReLU, then conv3 with the residual: block 0 of a stage runs conv3 and the strided downsample as one GEMM over
+// [conv2 out | x], the others add x in the epilogue.  The head pools layer4 and L2-normalises into the caller's rows.
+void run_resnet_chunk(Launcher& L, const FrameIn& fi, float* d_out, int out_ld) {
+    ReidModel* m = L.m;
+    const float* W = m->d_w;
+    StageTaps stop_here{m};
+    if (run_front(L, fi, stop_here)) return;
+    float* X = m->bufB;
+    float* Xo = m->bufA;
+    int H = IN_H / 4, Wd = IN_W / 4;
+    for (const RnBlock& b : m->rn) {
+        const int Ho = H / b.stride, Wo = Wd / b.stride;
+        rn::ConvArgs c{};
+        c.in0 = X; c.H0 = H; c.W0 = Wd; c.C0 = b.cin; c.k0 = 1; c.s0 = 1;
+        c.w = b.c1.w; c.bias = W + b.c1.b; c.out = m->x1; c.Ho = H; c.Wo = Wd; c.N = b.width; c.relu = 1;
+        L.conv_tc(c);
+        c = rn::ConvArgs{};
+        c.in0 = m->x1; c.H0 = H; c.W0 = Wd; c.C0 = b.width; c.k0 = 3; c.s0 = b.stride;
+        c.w = b.c2.w; c.bias = W + b.c2.b; c.out = m->Y[0][0]; c.Ho = Ho; c.Wo = Wo; c.N = b.width; c.relu = 1;
+        L.conv_tc(c);
+        c = rn::ConvArgs{};
+        c.in0 = m->Y[0][0]; c.H0 = Ho; c.W0 = Wo; c.C0 = b.width; c.k0 = 1; c.s0 = 1;
+        if (b.cin != b.cout || b.stride != 1) {
+            c.in1 = X; c.H1 = H; c.W1 = Wd; c.C1 = b.cin; c.s1 = b.stride;
+        } else {
+            c.residual = X;
+        }
+        c.w = b.c3.w; c.bias = W + b.c3.b; c.out = Xo; c.Ho = Ho; c.Wo = Wo; c.N = b.cout; c.relu = 1;
+        L.conv_tc(c);
+        std::swap(X, Xo);
+        H = Ho; Wd = Wo;
+        if (stop_here(X, (size_t)H * Wd * b.cout)) return;
+    }
+    L.begin(CLS_HEAD);
+    k_head<<<L.upper, 256, sizeof(float) * (2 * m->feat + 32), L.st>>>(X, H * Wd, m->feat, nullptr, nullptr, m->feat,
+                                                                       fi.crops, L.d_n, L.off, L.cap, d_out, out_ld);
+    L.end();
+    ++L.launches;
+}
 }  // namespace
 
 }  // namespace bmb
@@ -2205,11 +2335,12 @@ int reid_forward(ReidModel* m, const uint8_t* d_images, size_t image_stride, int
         return launches;
     }
     const FrameIn fi{d_images, image_stride, rows, cols, d_crops};
-    if (m->arch == 3) {
+    if (m->arch == 3 || m->arch == 5) {
         for (int off = first_crop; off < last_crop; off += m->chunk) {
             const int upper = (last_crop - off) < m->chunk ? (last_crop - off) : m->chunk;
             Launcher L{m, d_ncrops, off, upper, upper, st};
-            run_lmbn_chunk(L, fi, d_out, out_ld);
+            if (m->arch == 3) run_lmbn_chunk(L, fi, d_out, out_ld);
+            else run_resnet_chunk(L, fi, d_out, out_ld);
             launches += L.launches;
         }
         RCUDA_OK(cudaGetLastError());
@@ -2373,6 +2504,71 @@ void standalone_instance_norm(const float* x, int n, int H, int W, int C, const 
         RCUDA_OK(cudaGetLastError());
         RCUDA_OK(cudaDeviceSynchronize());
         RCUDA_OK(cudaMemcpy(out, dout, sizeof(float) * out_elems, cudaMemcpyDeviceToHost));
+    } catch (...) {
+        cleanup();
+        throw;
+    }
+    cleanup();
+}
+
+// Standalone ResNet convolution (rn::k_conv_tc) on host arrays (parity tests / micro-benchmarks):
+//   out [n][Ho][Wo][N] = act(conv_k(in0, stride) (+ conv_1x1(in1, stride1)) + bias (+ residual)),
+// in0 [n][h0][w0][c0] with k in {1, 3} (pad k / 2), in1 [n][h1][w1][c1] (c1 = 0: none), w [k*k*c0 + c1][N] K-major.
+void standalone_resnet_conv(const float* in0, int n, int h0, int w0, int c0, int k, int stride, const float* in1, int h1,
+                            int w1, int c1, int stride1, const float* w, int N, const float* bias, const float* residual,
+                            int relu, float* out, float* elapsed_ms) {
+    if (n <= 0 || h0 <= 0 || w0 <= 0 || c0 <= 0 || c0 % rn::KC || (k != 1 && k != 3) || stride < 1 || N <= 0 || N % 64 ||
+        c1 < 0 || c1 % rn::KC || (c1 && (!in1 || h1 <= 0 || w1 <= 0 || stride1 < 1)))
+        throw std::runtime_error("n, h0, w0 > 0, k in {1, 3}, c0 and c1 multiples of 32, N a multiple of 64 required");
+    const int pad = k / 2, Ho = (h0 + 2 * pad - k) / stride + 1, Wo = (w0 + 2 * pad - k) / stride + 1;
+    if (c1 && ((Ho - 1) * stride1 >= h1 || (Wo - 1) * stride1 >= w1))
+        throw std::runtime_error("the second operand does not cover the output grid");
+    const int K = k * k * c0 + c1;
+    const size_t n_in0 = (size_t)n * h0 * w0 * c0, n_in1 = (size_t)n * h1 * w1 * c1, n_out = (size_t)n * Ho * Wo * N;
+    float *d0 = nullptr, *d1 = nullptr, *dW = nullptr, *dB = nullptr, *dR = nullptr, *dO = nullptr;
+    int* dn = nullptr;
+    auto cleanup = [&] { cudaFree(d0); cudaFree(d1); cudaFree(dW); cudaFree(dB); cudaFree(dR); cudaFree(dO); cudaFree(dn); };
+    try {
+        std::vector<float> packed(2 * (size_t)K * N);
+        rn::pack_conv_weights(w, K, N, packed.data());
+        RCUDA_OK(cudaMalloc(&d0, sizeof(float) * n_in0));
+        RCUDA_OK(cudaMemcpy(d0, in0, sizeof(float) * n_in0, cudaMemcpyHostToDevice));
+        if (c1) {
+            RCUDA_OK(cudaMalloc(&d1, sizeof(float) * n_in1));
+            RCUDA_OK(cudaMemcpy(d1, in1, sizeof(float) * n_in1, cudaMemcpyHostToDevice));
+        }
+        RCUDA_OK(cudaMalloc(&dW, sizeof(float) * packed.size()));
+        RCUDA_OK(cudaMemcpy(dW, packed.data(), sizeof(float) * packed.size(), cudaMemcpyHostToDevice));
+        RCUDA_OK(cudaMalloc(&dB, sizeof(float) * N));
+        RCUDA_OK(cudaMemcpy(dB, bias, sizeof(float) * N, cudaMemcpyHostToDevice));
+        if (residual) {
+            RCUDA_OK(cudaMalloc(&dR, sizeof(float) * n_out));
+            RCUDA_OK(cudaMemcpy(dR, residual, sizeof(float) * n_out, cudaMemcpyHostToDevice));
+        }
+        RCUDA_OK(cudaMalloc(&dO, sizeof(float) * n_out));
+        RCUDA_OK(cudaMalloc(&dn, sizeof(int)));
+        RCUDA_OK(cudaMemcpy(dn, &n, sizeof(int), cudaMemcpyHostToDevice));
+        rn::ConvArgs c{};
+        c.in0 = d0; c.H0 = h0; c.W0 = w0; c.C0 = c0; c.k0 = k; c.s0 = stride;
+        c.in1 = d1; c.H1 = h1; c.W1 = w1; c.C1 = c1; c.s1 = stride1;
+        c.w = dW; c.bias = dB; c.residual = dR; c.out = dO; c.Ho = Ho; c.Wo = Wo; c.N = N; c.relu = relu;
+        ReidModel fake;
+        Launcher L{&fake, dn, 0, n, n, nullptr};
+        L.conv_tc(c);   // warm-up
+        RCUDA_OK(cudaGetLastError());
+        RCUDA_OK(cudaDeviceSynchronize());
+        cudaEvent_t e0, e1;
+        RCUDA_OK(cudaEventCreate(&e0));
+        RCUDA_OK(cudaEventCreate(&e1));
+        RCUDA_OK(cudaEventRecord(e0));
+        for (int r = 0; r < 10; ++r) L.conv_tc(c);
+        RCUDA_OK(cudaEventRecord(e1));
+        RCUDA_OK(cudaDeviceSynchronize());
+        float ms = 0.f;
+        cudaEventElapsedTime(&ms, e0, e1);
+        if (elapsed_ms) *elapsed_ms = ms / 10.f;
+        cudaEventDestroy(e0); cudaEventDestroy(e1);
+        RCUDA_OK(cudaMemcpy(out, dO, sizeof(float) * n_out, cudaMemcpyDeviceToHost));
     } catch (...) {
         cleanup();
         throw;

@@ -252,6 +252,56 @@ def make_lmbn_n_state(seed: int = 0, num_classes: int = 702):
     return sd
 
 
+RESNET_BLOCKS = {50: (3, 4, 6, 3), 101: (3, 4, 23, 3)}   # Bottleneck counts of layer1..4 (resnet.py resnet50 / resnet101)
+RESNET_FEAT = 2048
+
+
+def resnet_layout(depth: int):
+    """[(parameter prefix, kind, shape)] of the reference's Bottleneck ResNet (reid/backbones/resnet.py, torchvision
+    v1.5: the stride sits on the 3x3), kind "conv" (weight [co][ci][k][k]) or "bn" (BatchNorm2d of `shape[0]` channels),
+    in module order.  `classifier` and `fc` are not listed: the embedding is the pooled layer4 map."""
+    out = [("conv1", "conv", (64, 3, 7, 7)), ("bn1", "bn", (64,))]
+    cin = 64
+    for li, n_blocks in enumerate(RESNET_BLOCKS[depth]):
+        width = 64 << li
+        for j in range(n_blocks):
+            name = f"layer{li + 1}.{j}"
+            out += [(name + ".conv1", "conv", (width, cin, 1, 1)), (name + ".bn1", "bn", (width,)),
+                    (name + ".conv2", "conv", (width, width, 3, 3)), (name + ".bn2", "bn", (width,)),
+                    (name + ".conv3", "conv", (4 * width, width, 1, 1)), (name + ".bn3", "bn", (4 * width,))]
+            if j == 0:
+                out += [(name + ".downsample.0", "conv", (4 * width, cin, 1, 1)), (name + ".downsample.1", "bn", (4 * width,))]
+            cin = 4 * width
+    return out
+
+
+def make_resnet_state(depth: int = 50, seed: int = 0, with_fc512: bool = False, num_classes: int = 751):
+    """Seeded state dict with the parameter names of the reference's `resnet50` / `resnet101` (loads with strict=True).
+    with_fc512 adds the `fc.0` Linear(2048, 512) + `fc.1` BatchNorm1d head and a 512-wide classifier of a
+    resnet50_fc512 checkpoint, which the reference drops when it builds plain resnet50 for such a file.  BatchNorm
+    statistics are randomised so folding is exercised; conv3 starts small so activations stay O(1-10) through the
+    residual stream of resnet101."""
+    import torch
+
+    g = torch.Generator().manual_seed(seed)
+    sd = {}
+    conv, bn, _ = _osnet_makers(g, sd)
+    for name, kind, shape in resnet_layout(depth):
+        if kind == "bn":
+            bn(name, shape[0])
+        else:
+            conv(name, shape[0], shape[1], shape[2], gain=0.1 if name.endswith("conv3") else 1.0)
+    feat = RESNET_FEAT
+    if with_fc512:
+        feat = 512
+        sd["fc.0.weight"] = 0.05 * torch.randn(512, RESNET_FEAT, generator=g)
+        sd["fc.0.bias"] = 0.05 * torch.randn(512, generator=g)
+        bn("fc.1", 512)
+    sd["classifier.weight"] = 0.01 * torch.randn(num_classes, feat, generator=g)
+    sd["classifier.bias"] = torch.zeros(num_classes)
+    return sd
+
+
 MOBILENETV2_LAYERS = ((1, 16, 1, 1), (6, 24, 2, 2), (6, 32, 3, 2), (6, 64, 4, 2), (6, 96, 3, 1), (6, 160, 3, 2),
                       (6, 320, 1, 1))  # (expansion t, base channels c, repeats n, first stride s), mobilenetv2.py:91-99
 

@@ -21,6 +21,8 @@ height (384) in header word 9; its tensors reuse the OSBlock / transition layout
 Arch 4 (OSNet-AIN / OSNet-IBN, `fold_osnet_in`) keeps the arch-1 layout and header dims; header word 9 flags the
 stem's instance norm and words 10-15 hold each block's IN placement (0 none, 1 before the residual add, 2 after it),
 with the gamma / beta arrays stored right after the tensors of the stem or block they belong to.
+Arch 5 (Bottleneck ResNet50 / ResNet101, `fold_resnet`) records the Bottleneck counts of layer1..4 in words 3-6 and
+the 2048-d feature in word 7; its layout is listed above `fold_resnet`.
 All 1x1 weights are stored K-major ([cin][cout]) so a thread owning consecutive output channels loads
 consecutive floats; every tensor is zero-padded to a multiple of 4 floats (16-byte aligned float4 loads).
 """
@@ -39,6 +41,8 @@ ARCH_OSNET = 1
 ARCH_MOBILENETV2 = 2
 ARCH_LMBN_N = 3
 ARCH_OSNET_IN = 4
+ARCH_RESNET = 5
+RESNET_FEAT = 2048
 BRANCHES = (("conv2a", 1), ("conv2b", 2), ("conv2c", 3), ("conv2d", 4))
 EPS = 1e-5
 
@@ -295,6 +299,61 @@ def _fold_ain_block(sd, name, cin, cout, inin) -> List[np.ndarray]:
     return out + _in_affine(sd, name + ".IN")
 
 
+# Bottleneck ResNet (arch 5): resnet50 / resnet101 of reid/backbones/resnet.py.  Header words 3-6 hold the Bottleneck
+# counts of layer1..4 and word 7 the 2048-d feature; the arrays are
+#     stem      W[147][64] (k = (kh*7+kw)*3 + ci, bn1 folded), b[64]
+#     per Bottleneck (cin, width, cout = 4 width):
+#         conv1     W[cin][width], b[width]                      (bn1 folded)
+#         conv2     W[9 width][width] (k = (kh*3+kw)*width + ci), b[width]   (bn2 folded)
+#         conv3     W[width (+ cin, block 0)][cout], b[cout]     (bn3 folded; block 0 appends the downsample's rows and
+#                                                                 adds its folded bias: one GEMM over [conv2 out | x])
+def _resnet_ignored(k: str) -> bool:
+    return k.startswith(("fc.", "classifier.")) or k.endswith("num_batches_tracked")
+
+
+def is_resnet(sd) -> bool:
+    return "conv1.weight" in sd and any(k.startswith("layer1.0.") for k in sd)
+
+
+def fold_resnet(sd):
+    """ResNet state dict -> (block counts, arrays) of the arch-5 blob.  Only the Bottleneck resnet50 / resnet101 are
+    supported: anything else whose keys or shapes differ from those (resnet18/34's BasicBlocks, ResNeXt's grouped 3x3,
+    a missing BatchNorm key), apart from `fc.*`, `classifier.*` and `num_batches_tracked`, raises a ValueError naming
+    the keys."""
+    from .synthetic import RESNET_BLOCKS, resnet_layout
+
+    keys = {k for k in sd if not _resnet_ignored(k)}
+    n3 = len({k.split(".")[1] for k in keys if k.startswith("layer3.")})
+    depth = next((d for d, b in RESNET_BLOCKS.items() if b[2] == n3), None)
+    want = {}
+    for name, kind, shape in resnet_layout(depth) if depth else ():
+        if kind == "conv":
+            want[name + ".weight"] = shape
+        else:
+            for p in ("weight", "bias", "running_mean", "running_var"):
+                want[f"{name}.{p}"] = shape
+    bad_shape = sorted(k for k in keys & set(want) if tuple(sd[k].shape) != want[k])[:4]
+    if not want or keys != set(want) or bad_shape:
+        extra, missing = sorted(keys - set(want))[:4], sorted(set(want) - keys)[:4]
+        raise ValueError(f"not a Bottleneck resnet50 / resnet101 state dict (unexpected keys {extra}, missing keys "
+                         f"{missing}, unexpected shapes {bad_shape}); BasicBlock ResNets and ResNeXt are not supported")
+    out: List[np.ndarray] = _fold_stem(sd, "conv1", "bn1")
+    for li, n_blocks in enumerate(RESNET_BLOCKS[depth]):
+        for j in range(n_blocks):
+            name = f"layer{li + 1}.{j}"
+            out += list(_pw(sd, name + ".conv1", name + ".bn1"))
+            w2 = _np(sd[name + ".conv2.weight"])   # [co][ci][3][3]
+            sc, sh = _bn_fold(sd, name + ".bn2")
+            w2 = (w2 * sc[:, None, None, None]).transpose(2, 3, 1, 0).reshape(-1, w2.shape[0])
+            out += [w2, sh]
+            w3, b3 = _pw(sd, name + ".conv3", name + ".bn3")
+            if j == 0:
+                wd, bd = _pw(sd, name + ".downsample.0", name + ".downsample.1")
+                w3, b3 = np.concatenate([w3, wd], 0), b3 + bd
+            out += [w3, b3]
+    return list(RESNET_BLOCKS[depth]), out
+
+
 def _pad4(n: int) -> int:
     return (n + 3) // 4 * 4
 
@@ -377,9 +436,12 @@ def export_blob(weights, out_path=None) -> Path:
     elif is_lmbn(sd):
         arrays = fold_lmbn_n(sd)
         arch, dims = ARCH_LMBN_N, [64, 256, 384, 512, LMBN_FEAT]
+    elif is_resnet(sd):
+        blocks, arrays = fold_resnet(sd)
+        arch, dims = ARCH_RESNET, blocks + [RESNET_FEAT]
     else:
-        raise ValueError("only OSNet, OSNet-AIN, OSNet-IBN, MobileNetV2 and LMBN_n state dicts are implemented on the "
-                         "B200 ReID path")
+        raise ValueError("only OSNet, OSNet-AIN, OSNet-IBN, MobileNetV2, LMBN_n and ResNet50 / ResNet101 state dicts are "
+                         "implemented on the B200 ReID path")
     # every tensor starts on a 16-byte boundary (the kernels read weights as float4)
     padded = []
     for a in arrays:

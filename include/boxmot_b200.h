@@ -413,10 +413,21 @@ BOXMOT_B200_API int boxmot_b200_pointwise_gemm(const float* a, int m, int k, con
  * max pool of relu(IN(x) * gamma + beta). */
 BOXMOT_B200_API int boxmot_b200_instance_norm(const float* x, int n, int h, int w, int c, const float* gamma,
                                               const float* beta, const float* residual, int relu, int pool, float* out);
+/* One convolution of the ResNet50 / ResNet101 path (wgmma tf32x3 implicit GEMM) on host arrays, NHWC float32:
+ * out (n,Ho,Wo,out_c) = act(conv(in0) + conv1x1(in1) + bias (+ residual, optional)), act = ReLU when relu = 1.
+ * in0 (n,h0,w0,c0) is read by a k x k kernel (k 1 or 3, pad k/2) at `stride`; in1 (n,h1,w1,c1), optional (c1 = 0
+ * for none), by a 1x1 kernel at `stride1` over the same output grid (the fused conv3 + downsample of a stage's first
+ * Bottleneck).  w is (k*k*c0 + c1, out_c) K-major, k index (kh*k + kw)*c0 + ci then the c1 channels; c0 and c1
+ * multiples of 32, out_c a multiple of 64.  elapsed_ms (optional) receives the average device time of 10 launches. */
+BOXMOT_B200_API int boxmot_b200_resnet_conv(const float* in0, int n, int h0, int w0, int c0, int k, int stride,
+                                            const float* in1, int h1, int w1, int c1, int stride1, const float* w,
+                                            int out_c, const float* bias, const float* residual, int relu, float* out,
+                                            float* elapsed_ms);
 BOXMOT_B200_API int boxmot_b200_device_count(void);
 /* Diagnostics for the ReID kernels: run the forward up to `stage` (0 input blob, 1 stem, 2 max-pool, 3..10 the
  * six OSBlocks and two transitions in order, 11 conv5) and copy that NHWC float32 tensor of the n crops out.  For
- * OSNet-AIN / OSNet-IBN the stem tap is the map after the instance norm and the ReLU. */
+ * OSNet-AIN / OSNet-IBN the stem tap is the map after the instance norm and the ReLU.  For ResNet50 / ResNet101: 0 input
+ * blob, 1 stem, 2 max-pool, 3 + i the output of Bottleneck i (layer1.0 first). */
 BOXMOT_B200_API int boxmot_b200_reid_debug_stage(void* reid_handle, const float* boxes_xyxy, int n_boxes,
                                                  const uint8_t* image_data, int image_rows, int image_cols,
                                                  int stage, float* out, int out_capacity_floats,

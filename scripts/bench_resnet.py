@@ -1,0 +1,141 @@
+"""ResNet50 on bench.py's default workload: the BoT-SORT tracker, detection stream and frame ring of BASELINE config 2
+with ResNet50 (seeded weights, 2048-d rows, tensor-core convolutions) as the ReID backbone, alternated in one process
+with OSNet_x1_0 (float32 CUDA-core kernels) on the same workload, timed with bench.py's own device and end-to-end legs,
+plus parity of the first frames against the oracle tracker fed by the oracle ResNet50.  Prints one JSON line.
+
+    python scripts/bench_resnet.py [--steps 200] [--warmup 20] [--rounds 2] [--parity-frames 2]
+
+Writes nothing into the tree (the blobs go to a temporary directory).  The convolutions run as three-term TF32 wgmma,
+so the share of peak is against the data sheet's dense TF32 rate with the three MMAs per product counted (the
+algorithmic rate is also given against the dense FP32 rate a float32 implementation would be bounded by)."""
+from __future__ import annotations
+
+import argparse
+import json
+import subprocess
+import sys
+import tempfile
+from pathlib import Path
+
+import numpy as np
+
+ROOT = Path(__file__).resolve().parents[1]
+if str(ROOT) not in sys.path:
+    sys.path.insert(0, str(ROOT))
+
+import bench  # noqa: E402
+
+TF32_PEAK_TFLOPS = 495.0   # H100 SXM data sheet, dense TF32 (700 W)
+FP32_PEAK_TFLOPS = 67.0    # H100 SXM data sheet, dense FP32 on the CUDA cores (700 W)
+TC_TERMS = 3               # hi*hi + hi*lo + lo*hi per product
+
+
+def resnet_gflop_per_crop(blocks=(3, 4, 6, 3), in_h=256, in_w=128):
+    """Algorithmic GFLOP of one crop: 2 x MAC over every convolution of reid/backbones/resnet.py (stem, and per
+    Bottleneck conv1, conv2, conv3 and block 0's downsample)."""
+    h, w = in_h // 2, in_w // 2
+    macs = h * w * 64 * 3 * 49
+    h, w = h // 2, w // 2
+    cin = 64
+    for li, n in enumerate(blocks):
+        width = 64 << li
+        for j in range(n):
+            s = 2 if (j == 0 and li > 0) else 1
+            ho, wo = h // s, w // s
+            macs += h * w * cin * width + ho * wo * 9 * width * width + ho * wo * width * 4 * width
+            if j == 0:
+                macs += ho * wo * cin * 4 * width
+            h, w, cin = ho, wo, 4 * width
+    return 2 * macs / 1e9
+
+
+def power_limit():
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                             capture_output=True, text=True, timeout=30).stdout.strip()
+        return out.splitlines()[0] if out else "unknown"
+    except (OSError, subprocess.SubprocessError):
+        return "unknown"
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--steps", type=int, default=200)
+    ap.add_argument("--warmup", type=int, default=20)
+    ap.add_argument("--rounds", type=int, default=2, help="alternations of ResNet50 and OSNet_x1_0")
+    ap.add_argument("--parity-frames", type=int, default=2, help="first frames of stream 0 checked against the oracle (CPU)")
+    args = ap.parse_args()
+
+    import torch
+
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_resnet.py needs a CUDA device: boxmot_b200 has no CPU fallback")
+    torch.cuda.set_device(0)
+    from boxmot_b200.synthetic import make_osnet_state, make_resnet_state
+    from boxmot_b200.weights import export_blob
+
+    base = bench.CONFIGS[2]
+    tmp = Path(tempfile.mkdtemp(prefix="b200resnet_"))
+    sd = make_resnet_state(50, seed=0)
+    models = {
+        "resnet50": (dict(base, id=2, arch="resnet50", feat=2048), export_blob(sd, tmp / "resnet50_synthetic.b200reid")),
+        "osnet_x1_0": (dict(base, id=2, arch="osnet_x1_0", feat=512),
+                       export_blob(make_osnet_state("osnet_x1_0", seed=0), tmp / "osnet_x1_0_synthetic.b200reid")),
+    }
+    K, Wm = args.steps, max(3, args.warmup)
+    runs = {name: [] for name in models}
+    for _ in range(args.rounds):
+        for name, (cfg, blob) in models.items():
+            dev = bench.device_run(cfg, blob, K, Wm, None)
+            e2e_ms, _, api = bench.e2e_run(cfg, blob, dev["per_stream"], K, Wm, None, pinned=False)
+            reid_ms = sum(dev["prof"][c]["ms_per_step"] for c in bench.CLASSES if c != "association")
+            runs[name].append(dict(dev=dev, e2e_ms=e2e_ms, api=api, reid_ms=reid_ms))
+
+    cfg, blob = models["resnet50"]
+    first = runs["resnet50"][0]["dev"]
+    ps = first["per_stream"][0]
+    from oracle.resnet import OracleResNet
+    from oracle.trackers import BotSortOracle
+
+    orc = BotSortOracle(reid_model=OracleResNet(sd), **cfg["params"])
+    rows = [np.asarray(orc.update(ps[1][f], ps[0][f % cfg["ring"]]), np.float32).reshape(-1, 8)
+            for f in range(args.parity_frames)]
+    parity = bench.parity_check(cfg, blob, rows, first["per_stream"])
+
+    def summary(name):
+        rs = runs[name]
+        best = min(rs, key=lambda r: r["dev"]["value_ms"])
+        return {
+            "device_fps": [K / (r["dev"]["value_ms"] * 1e-3) for r in rs],
+            "e2e_fps": [K / (r["e2e_ms"] * 1e-3) for r in rs],
+            "reid_device_ms_per_frame": [r["reid_ms"] for r in rs],
+            "crops_per_frame": best["dev"]["crops"],
+            "kernel_classes": best["dev"]["prof"],
+        }
+
+    gflop_crop = resnet_gflop_per_crop()
+    res = summary("resnet50")
+    reid_ms = min(res["reid_device_ms_per_frame"])
+    gflop_frame = res["crops_per_frame"] * gflop_crop
+    achieved = gflop_frame / reid_ms   # GFLOP per ms = TFLOP/s
+    line = {
+        "metric": "tracker.update() frames/sec with ResNet50 ReID", "value": max(res["device_fps"]), "unit": "frames/s",
+        "steps": K, "warmup": Wm, "rounds": args.rounds, "data": "synthetic",
+        "workload": f"botsort workload of BASELINE config 2 ({base['dets']} dets/frame, {base['hw'][0]}x{base['hw'][1]}) "
+                    f"with ReID in update(); resnet50 and osnet_x1_0 alternated in one process",
+        "card": power_limit(),
+        "resnet50": res,
+        "osnet_x1_0": summary("osnet_x1_0"),
+        "roofline": {"kernel": "ResNet50 ReID (all kernels of a frame, serialised device time)",
+                     "gflop_per_crop": gflop_crop, "algorithmic_gflop_per_frame": gflop_frame,
+                     "achieved_tflops": achieved,
+                     "tf32x3_frac": achieved * TC_TERMS / TF32_PEAK_TFLOPS,
+                     "fp32_floor_ms_per_frame": gflop_frame / FP32_PEAK_TFLOPS,
+                     "peak_source": "H100 SXM data sheet (dense TF32 495 TFLOP/s, FP32 67 TFLOP/s, 700 W), not measured"},
+        "parity": parity,
+    }
+    print(json.dumps(line))
+
+
+if __name__ == "__main__":
+    main()
