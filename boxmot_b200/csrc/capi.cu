@@ -398,6 +398,12 @@ int boxmot_b200_resnet_conv(const float* in0, int n, int h0, int w0, int c0, int
                                out, elapsed_ms);
     });
 }
+int boxmot_b200_vit_layernorm(const float* x, int rows, const float* gamma, const float* beta, float* out) {
+    return guard([&] { standalone_vit_layernorm(x, rows, gamma, beta, out); });
+}
+int boxmot_b200_vit_attention(const float* qkv, int n, int tokens, float* out) {
+    return guard([&] { standalone_vit_attention(qkv, n, tokens, out); });
+}
 int boxmot_b200_cosine_cost(const float* a, int rows, const float* b, int cols, int dim, double* out) {
     return guard([&] { standalone_cosine(a, rows, b, cols, dim, out); });
 }

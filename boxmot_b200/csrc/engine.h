@@ -248,5 +248,7 @@ void standalone_instance_norm(const float* x, int n, int H, int W, int C, const 
 void standalone_resnet_conv(const float* in0, int n, int h0, int w0, int c0, int k, int stride, const float* in1, int h1,
                             int w1, int c1, int stride1, const float* w, int N, const float* bias, const float* residual,
                             int relu, float* out, float* elapsed_ms);
+void standalone_vit_layernorm(const float* x, int rows, const float* gamma, const float* beta, float* out);
+void standalone_vit_attention(const float* qkv, int n, int tokens, float* out);
 
 }  // namespace bmb

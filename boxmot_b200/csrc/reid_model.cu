@@ -25,6 +25,7 @@
 #include "engine.h"
 #include "pointwise_tc.cuh"
 #include "resnet_tc.cuh"
+#include "vit_tc.cuh"
 
 namespace bmb {
 
@@ -36,7 +37,8 @@ namespace bmb {
     } while (0)
 
 constexpr int IN_H = 256, IN_W = 128;
-constexpr int IN_H_MAX = 384;   // LMBN_n crops are 384x128 (the width of every model is 128)
+constexpr int IN_H_MAX = 384;   // LMBN_n crops are 384x128
+constexpr int IN_W_MAX = 256;   // CLIP vehicle crops are 256x256 (every other model's width is 128)
 constexpr uint32_t BLOB_MAGIC = 0x45523242u;
 
 // streaming multiprocessors of the current device: grid-stride kernels launch a few CTAs per SM
@@ -53,7 +55,7 @@ __device__ __forceinline__ int chunk_count(const int* d_n, int off, int cap) {
 }
 
 // ---------------------------------------------------------------------------------------------------
-// K1: crop + OpenCV-exact bilinear resize + BGR->RGB + /255 + mean/std  ->  (N,in_h,128,3) float32
+// K1: crop + OpenCV-exact bilinear resize + BGR->RGB + /255 + mean/std  ->  (N,in_h,in_w,3) float32
 // One CTA per crop.  cv2.resize(INTER_LINEAR) on uint8 is integer arithmetic: 11-bit coefficients derived from a
 // float32 phase, horizontal pass in int32, vertical (((b0*(S0>>4))>>16)+((b1*(S1>>4))>>16)+2)>>2.  x phases are
 // clamped at the borders, y rows are clipped at fetch (pinned against cv2 in tests/test_oracle_reid.py).
@@ -71,14 +73,19 @@ __device__ __forceinline__ void linear_coeff(int d, int src_n, double scale, boo
     a1 = (int)rintf(f * 2048.0f);
 }
 
+// per-channel (RGB) mean and std of the staged crop: ImageNet's for every model but CLIP (0.5, base_backend.py:52-54)
+struct CropNorm { float mean[3], std[3]; };
+constexpr CropNorm kImageNetNorm{{0.485f, 0.456f, 0.406f}, {0.229f, 0.224f, 0.225f}};
+
 __global__ void __launch_bounds__(256) k_crop_resize_norm(const uint8_t* __restrict__ images, size_t image_stride,
                                                           int rows, int cols, const CropDesc* __restrict__ crops,
                                                           const int* __restrict__ d_n, int off, int cap,
-                                                          float* __restrict__ blob, int pad_mode, int in_h) {
+                                                          float* __restrict__ blob, int pad_mode, int in_h, int in_w,
+                                                          CropNorm nm) {
     const int n = blockIdx.x;
     if (n >= chunk_count(d_n, off, cap)) return;
     const CropDesc cd = crops[off + n];
-    __shared__ int xi[IN_W], xa0[IN_W], xa1[IN_W];
+    __shared__ int xi[IN_W_MAX], xa0[IN_W_MAX], xa1[IN_W_MAX];
     __shared__ int yi[IN_H_MAX], ya0[IN_H_MAX], ya1[IN_H_MAX];
     // box.round().astype(int): round half to even
     const int x1 = (int)rintf(cd.x1), y1 = (int)rintf(cd.y1), x2 = (int)rintf(cd.x2), y2 = (int)rintf(cd.y2);
@@ -86,12 +93,12 @@ __global__ void __launch_bounds__(256) k_crop_resize_norm(const uint8_t* __restr
     const bool valid = cx2 > cx1 && cy2 > cy1;
     const int sw = cx2 - cx1, sh = cy2 - cy1;
     // resize_pad (preprocessing.py:21-45): scale = min(W / w, H / h); new = int(size * scale); centred, ImageNet-mean border
-    int nw = IN_W, nh = in_h, pl = 0, pt = 0;
+    int nw = in_w, nh = in_h, pl = 0, pt = 0;
     if (valid && pad_mode) {
-        const double sc = fmin((double)IN_W / (double)sw, (double)in_h / (double)sh);
+        const double sc = fmin((double)in_w / (double)sw, (double)in_h / (double)sh);
         nw = max(1, (int)((double)sw * sc));
         nh = max(1, (int)((double)sh * sc));
-        pl = (IN_W - nw) / 2;
+        pl = (in_w - nw) / 2;
         pt = (in_h - nh) / 2;
     }
     if (valid) {
@@ -101,11 +108,9 @@ __global__ void __launch_bounds__(256) k_crop_resize_norm(const uint8_t* __restr
     }
     __syncthreads();
     const uint8_t* img = images + (size_t)cd.image * image_stride;
-    float* out = blob + (size_t)n * in_h * IN_W * 3;
-    const float mean[3] = {0.485f, 0.456f, 0.406f};
-    const float stdv[3] = {0.229f, 0.224f, 0.225f};
-    for (int p = threadIdx.x; p < in_h * IN_W; p += blockDim.x) {
-        const int py = p / IN_W, px = p - py * IN_W;
+    float* out = blob + (size_t)n * in_h * in_w * 3;
+    for (int p = threadIdx.x; p < in_h * in_w; p += blockDim.x) {
+        const int py = p / in_w, px = p - py * in_w;
         const int dy = py - pt, dx = px - pl;
         int v[3] = {0, 0, 0};
         if (valid && (dx < 0 || dx >= nw || dy < 0 || dy >= nh)) {
@@ -127,7 +132,7 @@ __global__ void __launch_bounds__(256) k_crop_resize_norm(const uint8_t* __restr
 #pragma unroll
         for (int c = 0; c < 3; ++c) {  // output channel c is RGB: source channel 2-c
             const float f = __fdiv_rn((float)v[2 - c], 255.0f);
-            out[(size_t)p * 3 + c] = __fdiv_rn(f - mean[c], stdv[c]);
+            out[(size_t)p * 3 + c] = __fdiv_rn(f - nm.mean[c], nm.std[c]);
         }
     }
 }
@@ -1349,9 +1354,26 @@ struct LmbnW {
 struct RnConv { size_t b = 0; const float* w = nullptr; };
 struct RnBlock { int cin, width, cout, stride; RnConv c1, c2, c3; };
 
+// CLIP-ReID ViT-B/16 (arch 6): per residual block the offsets in d_w of its LayerNorm parameters and biases, and the
+// tensor-core packings of its four linear layers
+struct VitLayer {
+    size_t ln1g = 0, ln1b = 0, bin = 0, bout = 0, ln2g = 0, ln2b = 0, bfc = 0, bproj = 0;
+    const float *win = nullptr, *wout = nullptr, *wfc = nullptr, *wproj = nullptr;
+};
+struct VitW {
+    int tokens = 0, layers = 0;   // 1 + (in_h / 16) (in_w / 16)
+    size_t patch_b = 0, pos = 0, lnpre_g = 0, lnpre_b = 0, head_g = 0, head_b = 0, head_w = 0, head_pb = 0;
+    const float* patch_w = nullptr;
+    std::vector<VitLayer> layer;
+};
+
 struct ReidModel {
-    int arch = 1;                 // 1 OSNet, 2 MobileNetV2, 3 LMBN_n, 4 OSNet with instance norms (AIN / IBN), 5 ResNet
-    int in_h = IN_H;              // crop height (the width is IN_W for every model)
+    int arch = 1;                 // 1 OSNet, 2 MobileNetV2, 3 LMBN_n, 4 OSNet with instance norms (AIN / IBN), 5 ResNet,
+                                  // 6 CLIP-ReID ViT-B/16
+    int in_h = IN_H;              // crop height
+    int in_w = IN_W;              // crop width (256 only for CLIP's vehicle models)
+    CropNorm norm = kImageNetNorm;
+    VitW vit;
     bool stem_in = false;         // arch 4: conv 7x7 -> IN -> ReLU stem (stem_b is then gamma, stem_beta beta)
     size_t stem_beta = 0;
     float* in_tmp = nullptr;      // arch 4: conv3 output of an IN_BEFORE_RESIDUAL block with a downsample
@@ -1422,9 +1444,84 @@ ReidModel* reid_load(const char* path) {
     if (!f) throw std::runtime_error(std::string("cannot open ReID blob: ") + path);
     int32_t hdr[16];
     f.read(reinterpret_cast<char*>(hdr), sizeof(hdr));
-    if (!f || (uint32_t)hdr[0] != BLOB_MAGIC || hdr[1] != 1 || hdr[2] < 1 || hdr[2] > 5)
+    if (!f || (uint32_t)hdr[0] != BLOB_MAGIC || hdr[1] != 1 || hdr[2] < 1 || hdr[2] > 6)
         throw std::runtime_error("not a version-1 .b200reid blob (export it with boxmot_b200.weights.export_blob)");
     ReidModel* m = new ReidModel();
+    if (hdr[2] == 6) {
+        // ---- CLIP-ReID ViT-B/16 (reid/backbones/clip): patch embedding, ln_pre, 12 residual attention blocks, head ----
+        try {
+            m->arch = 6;
+            constexpr int D = vit::D;
+            if (hdr[3] != D || hdr[4] < 1 || hdr[4] > 64 || hdr[5] != vit::HEADS || hdr[6] != vit::PROJ ||
+                hdr[7] != vit::FEAT)
+                throw std::runtime_error("bad CLIP blob header (only ViT-B/16: width 768, 12 heads, 512-d projection)");
+            m->feat = hdr[7];
+            m->in_h = hdr[9];
+            m->in_w = hdr[10];
+            if (m->in_h != 256 || (m->in_w != 128 && m->in_w != 256) || hdr[11] != m->in_h / vit::PATCH ||
+                hdr[12] != m->in_w / vit::PATCH)
+                throw std::runtime_error("bad CLIP blob header (input 256x128 or 256x256, 16x16 patches)");
+            m->norm = CropNorm{{0.5f, 0.5f, 0.5f}, {0.5f, 0.5f, 0.5f}};
+            VitW& v = m->vit;
+            v.layers = hdr[4];
+            v.tokens = 1 + hdr[11] * hdr[12];
+            const size_t n_floats = (size_t)hdr[8];
+            std::vector<float> host(n_floats);
+            f.read(reinterpret_cast<char*>(host.data()), sizeof(float) * n_floats);
+            if (!f) throw std::runtime_error("truncated ReID blob");
+            size_t o = 0;
+            auto take = [&](size_t n) { size_t r = o; o += (n + 3) / 4 * 4; return r; };
+            struct Todo { const float** dst; size_t w; int K, N; size_t at; };
+            std::vector<Todo> todo;
+            size_t packed_n = 0;
+            auto linear = [&](const float*& dst, int K, int N) {
+                todo.push_back({&dst, take((size_t)K * N), K, N, packed_n});
+                packed_n += 2 * (size_t)K * N;
+            };
+            linear(v.patch_w, 3 * vit::PATCH * vit::PATCH, D);
+            v.patch_b = take(D);
+            v.pos = take((size_t)v.tokens * D);
+            v.lnpre_g = take(D); v.lnpre_b = take(D);
+            v.layer.resize(v.layers);   // `todo` keeps pointers into the layers
+            for (VitLayer& l : v.layer) {
+                l.ln1g = take(D); l.ln1b = take(D);
+                linear(l.win, D, 3 * D); l.bin = take(3 * D);
+                linear(l.wout, D, D); l.bout = take(D);
+                l.ln2g = take(D); l.ln2b = take(D);
+                linear(l.wfc, D, 4 * D); l.bfc = take(4 * D);
+                linear(l.wproj, 4 * D, D); l.bproj = take(D);
+            }
+            v.head_g = take(D); v.head_b = take(D);
+            v.head_w = take((size_t)D * vit::PROJ); v.head_pb = take(vit::PROJ);
+            if (o != n_floats) throw std::runtime_error("ReID blob size does not match its header");
+            std::vector<float> packed(packed_n);
+            for (auto& t : todo) rn::pack_conv_weights(host.data() + t.w, t.K, t.N, packed.data() + t.at);
+            RCUDA_OK(cudaMalloc(&m->d_w, sizeof(float) * n_floats));
+            RCUDA_OK(cudaMemcpy(m->d_w, host.data(), sizeof(float) * n_floats, cudaMemcpyHostToDevice));
+            RCUDA_OK(cudaMalloc(&m->d_wrn, sizeof(float) * packed_n));
+            RCUDA_OK(cudaMemcpy(m->d_wrn, packed.data(), sizeof(float) * packed_n, cudaMemcpyHostToDevice));
+            for (auto& t : todo) *t.dst = m->d_wrn + t.at;
+            if (const char* ce = getenv("BOXMOT_B200_REID_CHUNK")) {
+                const int c = atoi(ce);
+                if (c >= 8 && c <= 1024) m->chunk = c;
+            }
+            // per crop: the staged crop, the residual stream, the LayerNorm output and the attention output
+            // ([T][768] each), q | k | v ([T][2304]) and the MLP hidden layer ([T][3072], which also holds the patch
+            // rows): 1.09 M floats at 129 tokens, 2.17 M at 257, both below the 2.36 M an OSNet_x1_0 chunk takes per
+            // crop, so the chunk keeps its size
+            const size_t CH = m->chunk, T = v.tokens;
+            RCUDA_OK(cudaMalloc(&m->blob, sizeof(float) * CH * m->in_h * m->in_w * 3));
+            RCUDA_OK(cudaMalloc(&m->bufA, sizeof(float) * CH * T * D));
+            RCUDA_OK(cudaMalloc(&m->bufB, sizeof(float) * CH * T * D));
+            RCUDA_OK(cudaMalloc(&m->Y[0][0], sizeof(float) * CH * T * D));
+            RCUDA_OK(cudaMalloc(&m->x1, sizeof(float) * CH * T * 3 * D));
+            RCUDA_OK(cudaMalloc(&m->Y[0][1], sizeof(float) * CH * T * 4 * D));
+        } catch (...) {
+            reid_free(m);
+            throw;
+        }
+        return m;
+    }
     if (hdr[2] == 5) {
         // ---- Bottleneck ResNet (reid/backbones/resnet.py resnet50 / resnet101): stem, layer1..4, GAP ----
         try {
@@ -1960,6 +2057,25 @@ struct Launcher {
         end();
         ++launches;
     }
+    // CLIP: LayerNorm of T token rows per crop (EMBED: token assembly + ln_pre), timed under `gates`
+    void vit_layernorm(bool embed, const float* in, const float* pos, const float* g, const float* b, int T, float* out) {
+        const int grid = (int)std::min<size_t>(((size_t)upper * T + 7) / 8, (size_t)m->sms * 16);
+        begin(CLS_GATES);
+        if (embed) vit::k_vit_layernorm<true><<<grid, 256, 0, st>>>(in, pos, g, b, T, d_n, off, cap, out);
+        else vit::k_vit_layernorm<false><<<grid, 256, 0, st>>>(in, pos, g, b, T, d_n, off, cap, out);
+        end();
+        ++launches;
+    }
+    // CLIP: multi-head attention of every (crop, head, query block), timed under `lightconv`
+    void vit_attention(const float* qkv, int T, float* out) {
+        const size_t smem = vit::attention_smem_bytes(T);
+        RCUDA_OK(cudaFuncSetAttribute(vit::k_vit_attention, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        begin(CLS_LIGHTCONV);
+        vit::k_vit_attention<<<dim3((T + vit::ATT_QB - 1) / vit::ATT_QB, vit::HEADS, upper), vit::ATT_THREADS, smem, st>>>(
+            qkv, T, d_n, off, cap, out);
+        end();
+        ++launches;
+    }
     void light(const LightArgs& a, int n_branches, int threads) {
         if (m->light_v2 && light2(a, n_branches)) return;
         const int tiles = (a.H + a.R - 1) / a.R;
@@ -2019,7 +2135,7 @@ bool run_front(Launcher& L, const FrameIn& fi, StageTaps& stop_here) {
     const float* W = m->d_w;
     L.begin(CLS_CROP);
     k_crop_resize_norm<<<L.upper, 256, 0, L.st>>>(fi.images, fi.image_stride, fi.rows, fi.cols, fi.crops, L.d_n, L.off,
-                                                  L.cap, m->blob, m->preprocess, m->in_h);
+                                                  L.cap, m->blob, m->preprocess, m->in_h, IN_W, kImageNetNorm);
     L.end();
     ++L.launches;
     if (stop_here(m->blob, (size_t)m->in_h * IN_W * 3)) return true;
@@ -2270,6 +2386,64 @@ void run_resnet_chunk(Launcher& L, const FrameIn& fi, float* d_out, int out_ld) 
     L.end();
     ++L.launches;
 }
+
+// CLIP-ReID ViT-B/16, one chunk (clip/model.py VisionTransformer.forward + make_model.py build_transformer, eval,
+// NECK_FEAT "after").  Taps: 0 crop, 1 patch embedding ([P][768]), 2 ln_pre ([T][768]), 3 + l after residual block l,
+// 3 + layers the un-normalised 1280-d head row.  Every linear layer is rn::k_conv_tc over a [crops x T] x 1 map; the
+// two residual adds run in the epilogues of out_proj and c_proj, in place on the stream (each element is read and
+// written by the same thread).  Timing classes: crop, stem (patchify + patch GEMM), gates (LayerNorm), pointwise_gemm
+// (linear layers), lightconv (attention), head.
+void run_clip_chunk(Launcher& L, const FrameIn& fi, float* d_out, int out_ld) {
+    ReidModel* m = L.m;
+    const float* W = m->d_w;
+    const VitW& v = m->vit;
+    constexpr int D = vit::D;
+    const int T = v.tokens, P = T - 1;
+    StageTaps stop_here{m};
+    L.begin(CLS_CROP);
+    k_crop_resize_norm<<<L.upper, 256, 0, L.st>>>(fi.images, fi.image_stride, fi.rows, fi.cols, fi.crops, L.d_n, L.off,
+                                                  L.cap, m->blob, m->preprocess, m->in_h, m->in_w, m->norm);
+    L.end();
+    ++L.launches;
+    if (stop_here(m->blob, (size_t)m->in_h * m->in_w * 3)) return;
+    float* X = m->bufA;          // residual stream [T][768]
+    float* Xn = m->bufB;         // LayerNorm output
+    float* att = m->Y[0][0];     // attention output / patch embedding
+    float* hid = m->Y[0][1];     // MLP hidden layer / patch rows
+    float* qkv = m->x1;
+    L.begin(CLS_STEM);
+    vit::k_vit_patchify<<<m->sms * 8, 256, 0, L.st>>>(m->blob, m->in_h, m->in_w, L.d_n, L.off, L.cap, hid);
+    L.end();
+    ++L.launches;
+    auto linear = [&](const float* in, int K, const float* w, const float* bias, const float* residual, int N, int act,
+                      float* out, int rows) {
+        rn::ConvArgs c{};
+        c.in0 = in; c.H0 = rows; c.W0 = 1; c.C0 = K; c.k0 = 1; c.s0 = 1;
+        c.w = w; c.bias = bias; c.residual = residual; c.out = out; c.Ho = rows; c.Wo = 1; c.N = N; c.relu = act;
+        L.conv_tc(c);
+    };
+    linear(hid, 3 * vit::PATCH * vit::PATCH, v.patch_w, W + v.patch_b, nullptr, D, 0, att, P);
+    if (stop_here(att, (size_t)P * D)) return;
+    L.vit_layernorm(true, att, W + v.pos, W + v.lnpre_g, W + v.lnpre_b, T, X);
+    if (stop_here(X, (size_t)T * D)) return;
+    for (const VitLayer& l : v.layer) {
+        L.vit_layernorm(false, X, nullptr, W + l.ln1g, W + l.ln1b, T, Xn);
+        linear(Xn, D, l.win, W + l.bin, nullptr, 3 * D, 0, qkv, T);
+        L.vit_attention(qkv, T, att);
+        linear(att, D, l.wout, W + l.bout, X, D, 0, X, T);
+        L.vit_layernorm(false, X, nullptr, W + l.ln2g, W + l.ln2b, T, Xn);
+        linear(Xn, D, l.wfc, W + l.bfc, nullptr, 4 * D, 2, hid, T);
+        linear(hid, 4 * D, l.wproj, W + l.bproj, X, D, 0, X, T);
+        if (stop_here(X, (size_t)T * D)) return;
+    }
+    const bool tap = m->debug_stop == 3 + v.layers;
+    L.begin(CLS_HEAD);
+    vit::k_vit_head<<<L.upper, 256, 0, L.st>>>(X, T, W + v.head_g, W + v.head_b, W + v.head_w, W + v.head_pb, fi.crops,
+                                               L.d_n, L.off, L.cap, d_out, out_ld, tap ? Xn : nullptr);
+    L.end();
+    ++L.launches;
+    if (tap) stop_here(Xn, vit::FEAT);
+}
 }  // namespace
 
 }  // namespace bmb
@@ -2291,7 +2465,7 @@ int reid_forward(ReidModel* m, const uint8_t* d_images, size_t image_stride, int
             Launcher L{m, d_ncrops, off, upper, upper, st};
             L.begin(CLS_CROP);
             k_crop_resize_norm<<<upper, 256, 0, st>>>(d_images, image_stride, rows, cols, d_crops, d_ncrops, off, upper,
-                                                      m->blob, m->preprocess, IN_H);
+                                                      m->blob, m->preprocess, IN_H, IN_W, kImageNetNorm);
             L.end();
             ++L.launches;
             float* X = m->bufA;
@@ -2335,12 +2509,13 @@ int reid_forward(ReidModel* m, const uint8_t* d_images, size_t image_stride, int
         return launches;
     }
     const FrameIn fi{d_images, image_stride, rows, cols, d_crops};
-    if (m->arch == 3 || m->arch == 5) {
+    if (m->arch == 3 || m->arch == 5 || m->arch == 6) {
         for (int off = first_crop; off < last_crop; off += m->chunk) {
             const int upper = (last_crop - off) < m->chunk ? (last_crop - off) : m->chunk;
             Launcher L{m, d_ncrops, off, upper, upper, st};
             if (m->arch == 3) run_lmbn_chunk(L, fi, d_out, out_ld);
-            else run_resnet_chunk(L, fi, d_out, out_ld);
+            else if (m->arch == 5) run_resnet_chunk(L, fi, d_out, out_ld);
+            else run_clip_chunk(L, fi, d_out, out_ld);
             launches += L.launches;
         }
         RCUDA_OK(cudaGetLastError());
@@ -2518,8 +2693,9 @@ void standalone_resnet_conv(const float* in0, int n, int h0, int w0, int c0, int
                             int w1, int c1, int stride1, const float* w, int N, const float* bias, const float* residual,
                             int relu, float* out, float* elapsed_ms) {
     if (n <= 0 || h0 <= 0 || w0 <= 0 || c0 <= 0 || c0 % rn::KC || (k != 1 && k != 3) || stride < 1 || N <= 0 || N % 64 ||
-        c1 < 0 || c1 % rn::KC || (c1 && (!in1 || h1 <= 0 || w1 <= 0 || stride1 < 1)))
-        throw std::runtime_error("n, h0, w0 > 0, k in {1, 3}, c0 and c1 multiples of 32, N a multiple of 64 required");
+        c1 < 0 || c1 % rn::KC || (c1 && (!in1 || h1 <= 0 || w1 <= 0 || stride1 < 1)) || relu < 0 || relu > 2)
+        throw std::runtime_error("n, h0, w0 > 0, k in {1, 3}, c0 and c1 multiples of 32, N a multiple of 64, relu in "
+                                 "{0, 1, 2} required");
     const int pad = k / 2, Ho = (h0 + 2 * pad - k) / stride + 1, Wo = (w0 + 2 * pad - k) / stride + 1;
     if (c1 && ((Ho - 1) * stride1 >= h1 || (Wo - 1) * stride1 >= w1))
         throw std::runtime_error("the second operand does not cover the output grid");
@@ -2569,6 +2745,61 @@ void standalone_resnet_conv(const float* in0, int n, int h0, int w0, int c0, int
         if (elapsed_ms) *elapsed_ms = ms / 10.f;
         cudaEventDestroy(e0); cudaEventDestroy(e1);
         RCUDA_OK(cudaMemcpy(out, dO, sizeof(float) * n_out, cudaMemcpyDeviceToHost));
+    } catch (...) {
+        cleanup();
+        throw;
+    }
+    cleanup();
+}
+
+// Standalone CLIP LayerNorm (vit::k_vit_layernorm) on host arrays: out[r] = LN(x[r]) * gamma + beta over rows of 768.
+void standalone_vit_layernorm(const float* x, int rows, const float* gamma, const float* beta, float* out) {
+    if (rows <= 0) throw std::runtime_error("rows > 0 required");
+    const size_t n = (size_t)rows * vit::D;
+    float *dx = nullptr, *dg = nullptr, *db = nullptr, *dO = nullptr;
+    int* dn = nullptr;
+    auto cleanup = [&] { cudaFree(dx); cudaFree(dg); cudaFree(db); cudaFree(dO); cudaFree(dn); };
+    try {
+        RCUDA_OK(cudaMalloc(&dx, sizeof(float) * n));
+        RCUDA_OK(cudaMalloc(&dO, sizeof(float) * n));
+        RCUDA_OK(cudaMalloc(&dg, sizeof(float) * vit::D));
+        RCUDA_OK(cudaMalloc(&db, sizeof(float) * vit::D));
+        RCUDA_OK(cudaMalloc(&dn, sizeof(int)));
+        RCUDA_OK(cudaMemcpy(dx, x, sizeof(float) * n, cudaMemcpyHostToDevice));
+        RCUDA_OK(cudaMemcpy(dg, gamma, sizeof(float) * vit::D, cudaMemcpyHostToDevice));
+        RCUDA_OK(cudaMemcpy(db, beta, sizeof(float) * vit::D, cudaMemcpyHostToDevice));
+        RCUDA_OK(cudaMemcpy(dn, &rows, sizeof(int), cudaMemcpyHostToDevice));
+        ReidModel fake;
+        Launcher L{&fake, dn, 0, rows, rows, nullptr};
+        L.vit_layernorm(false, dx, nullptr, dg, db, 1, dO);
+        RCUDA_OK(cudaGetLastError());
+        RCUDA_OK(cudaMemcpy(out, dO, sizeof(float) * n, cudaMemcpyDeviceToHost));
+    } catch (...) {
+        cleanup();
+        throw;
+    }
+    cleanup();
+}
+
+// Standalone CLIP attention (vit::k_vit_attention) on host arrays: qkv [n][tokens][3 * 768] (q already scaled by 1/8)
+// -> out [n][tokens][768].
+void standalone_vit_attention(const float* qkv, int n, int tokens, float* out) {
+    if (n <= 0 || tokens < 1 || tokens > vit::MAX_T) throw std::runtime_error("n > 0 and 1 <= tokens <= 288 required");
+    const size_t nin = (size_t)n * tokens * 3 * vit::D, nout = (size_t)n * tokens * vit::D;
+    float *dq = nullptr, *dO = nullptr;
+    int* dn = nullptr;
+    auto cleanup = [&] { cudaFree(dq); cudaFree(dO); cudaFree(dn); };
+    try {
+        RCUDA_OK(cudaMalloc(&dq, sizeof(float) * nin));
+        RCUDA_OK(cudaMalloc(&dO, sizeof(float) * nout));
+        RCUDA_OK(cudaMalloc(&dn, sizeof(int)));
+        RCUDA_OK(cudaMemcpy(dq, qkv, sizeof(float) * nin, cudaMemcpyHostToDevice));
+        RCUDA_OK(cudaMemcpy(dn, &n, sizeof(int), cudaMemcpyHostToDevice));
+        ReidModel fake;
+        Launcher L{&fake, dn, 0, n, n, nullptr};
+        L.vit_attention(dq, tokens, dO);
+        RCUDA_OK(cudaGetLastError());
+        RCUDA_OK(cudaMemcpy(out, dO, sizeof(float) * nout, cudaMemcpyDeviceToHost));
     } catch (...) {
         cleanup();
         throw;

@@ -17,7 +17,7 @@
 //     (cp.async.bulk, completing on the stage's mbarrier) brings a chunk's hi and lo halves;
 //   * chunk k + 1 is in flight while the MMAs of chunk k (and the tail of chunk k - 1) run; every wgmma is issued
 //     unconditionally, with BN a template parameter.
-// Epilogue: bias, optional residual, optional ReLU, float2 stores into NHWC [M][N].
+// Epilogue: bias, optional residual, then relu = 0 none / 1 ReLU / 2 QuickGELU, float2 stores into NHWC [M][N].
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -43,7 +43,7 @@ struct ConvArgs {
     float* out;              // [M][N]
     int H0, W0, C0, k0, s0;  // k0 in {1, 3} (pad k0 / 2), stride s0
     int H1, W1, C1, s1;
-    int Ho, Wo, N, relu;
+    int Ho, Wo, N, relu;     // relu: 0 none, 1 ReLU, 2 QuickGELU
 };
 
 // canonical (no swizzle, K-major) offset in floats of element (row, k) in a block whose K extent is KC
@@ -190,7 +190,11 @@ __global__ void __launch_bounds__(THREADS, 1) k_conv_tc(const ConvArgs a, const 
                 const float2 r = *reinterpret_cast<const float2*>(res + c);
                 o.x += r.x; o.y += r.y;
             }
-            if (a.relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); }
+            if (a.relu == 1) {
+                o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f);
+            } else if (a.relu == 2) {   // QuickGELU x * sigmoid(1.702 x) (CLIP's MLP)
+                o.x = o.x / (1.f + expf(-1.702f * o.x)); o.y = o.y / (1.f + expf(-1.702f * o.y));
+            }
             *reinterpret_cast<float2*>(dst + c) = o;
         }
     }

@@ -16,7 +16,7 @@ import numpy as np
 
 from . import _lib
 from ._lib import B200Error
-from .weights import ARCH_LMBN_N, export_blob, read_blob
+from .weights import ARCH_CLIP, ARCH_LMBN_N, export_blob, read_blob
 
 
 class _StagedCrops:
@@ -51,6 +51,11 @@ class B200ReID:
         self.feature_dim = int(header[7])
         if header[2] == ARCH_LMBN_N:
             self.input_shape = (int(header[9]), 128)   # LMBN_n runs on 384x128 crops (base_backend.py:59-60)
+        if header[2] == ARCH_CLIP:
+            # CLIP: 256x128, or 256x256 for the vehicle models; mean = std = 0.5 (base_backend.py:52-58)
+            self.input_shape = (int(header[9]), int(header[10]))
+            self.mean_array = np.array([0.5, 0.5, 0.5], dtype=np.float32)
+            self.std_array = np.array([0.5, 0.5, 0.5], dtype=np.float32)
         self.half = bool(half)
         self.device = "cuda:0"
         self.handle = ctypes.c_void_p()
@@ -137,7 +142,8 @@ class B200ReID:
         boxes = self._boxes(xyxys)
         img = np.ascontiguousarray(img, dtype=np.uint8)
         per = ctypes.c_int(0)
-        cap = len(boxes) * (self.input_shape[0] // 2) * 64 * 64   # the largest tap: the stem output
+        # the largest tap: the stem output of the CNNs; CLIP's token maps (at most 257 x 768) are smaller
+        cap = len(boxes) * max((self.input_shape[0] // 2) * 64 * 64, 257 * 768)
         out = np.empty(cap, np.float32)
         ok = self.lib.boxmot_b200_reid_debug_stage(self.handle, boxes.ctypes.data, len(boxes), img.ctypes.data,
                                                    img.shape[0], img.shape[1], stage, out.ctypes.data, cap,

@@ -302,6 +302,62 @@ def make_resnet_state(depth: int = 50, seed: int = 0, with_fc512: bool = False, 
     return sd
 
 
+def make_clip_state(seed: int = 0, vehicle: bool = False, num_classes: int = 751, extras: bool = True):
+    """Seeded state dict with the key set of the reference's CLIP-ReID `build_transformer` (ViT-B/16: image_encoder.*,
+    bottleneck.*, bottleneck_proj.*, classifier.*, classifier_proj.*); vehicle=True gives the 257-row positional table
+    of 256x256 crops (clip_veri / clip_vehicleid), otherwise 129 rows (256x128).  extras adds a few keys of CLIP-ReID
+    training checkpoints that the reference's loader discards (prompt_learner.*, text_encoder.*).
+    Not trivial on purpose: BatchNorm statistics and LayerNorm gammas / betas are randomised, and in_proj is scaled so
+    that q.k / 8 has a spread of a few units and attention rows are far from uniform; c_proj and out_proj start small
+    so the residual stream stays O(1) through the 12 blocks."""
+    import torch
+
+    g = torch.Generator().manual_seed(seed)
+    d, tokens = 768, (257 if vehicle else 129)
+    e = "image_encoder."
+
+    def randn(*shape, std=1.0):
+        return torch.randn(*shape, generator=g) * std
+
+    def ln(name):
+        sd[name + ".weight"] = 0.5 + torch.rand(d, generator=g)
+        sd[name + ".bias"] = randn(d, std=0.1)
+
+    def bn(name, c):
+        sd[name + ".weight"] = 0.5 + torch.rand(c, generator=g)
+        sd[name + ".bias"] = randn(c, std=0.1)
+        sd[name + ".running_mean"] = randn(c, std=0.1)
+        sd[name + ".running_var"] = 0.5 + torch.rand(c, generator=g)
+        sd[name + ".num_batches_tracked"] = torch.tensor(0)
+
+    sd = {"classifier.weight": randn(num_classes, d, std=0.001)}
+    sd["classifier_proj.weight"] = randn(num_classes, 512, std=0.001)
+    sd[e + "class_embedding"] = randn(d, std=0.1)
+    sd[e + "positional_embedding"] = randn(tokens, d, std=0.1)
+    sd[e + "proj"] = randn(d, 512, std=d ** -0.5)
+    sd[e + "conv1.weight"] = randn(d, 3, 16, 16, std=0.02)
+    ln(e + "ln_pre")
+    for i in range(12):
+        b = f"{e}transformer.resblocks.{i}."
+        sd[b + "attn.in_proj_weight"] = randn(3 * d, d, std=0.06)
+        sd[b + "attn.in_proj_bias"] = randn(3 * d, std=0.05)
+        sd[b + "attn.out_proj.weight"] = randn(d, d, std=0.02)
+        sd[b + "attn.out_proj.bias"] = randn(d, std=0.02)
+        ln(b + "ln_1")
+        sd[b + "mlp.c_fc.weight"] = randn(4 * d, d, std=0.04)
+        sd[b + "mlp.c_fc.bias"] = randn(4 * d, std=0.05)
+        sd[b + "mlp.c_proj.weight"] = randn(d, 4 * d, std=0.01)
+        sd[b + "mlp.c_proj.bias"] = randn(d, std=0.02)
+        ln(b + "ln_2")
+    ln(e + "ln_post")
+    bn("bottleneck", d)
+    bn("bottleneck_proj", 512)
+    if extras:
+        sd["prompt_learner.cls_ctx"] = randn(num_classes, 4, 512, std=0.02)
+        sd["text_encoder.positional_embedding"] = randn(77, 512, std=0.01)
+    return sd
+
+
 MOBILENETV2_LAYERS = ((1, 16, 1, 1), (6, 24, 2, 2), (6, 32, 3, 2), (6, 64, 4, 2), (6, 96, 3, 1), (6, 160, 3, 2),
                       (6, 320, 1, 1))  # (expansion t, base channels c, repeats n, first stride s), mobilenetv2.py:91-99
 

@@ -23,6 +23,9 @@ stem's instance norm and words 10-15 hold each block's IN placement (0 none, 1 b
 with the gamma / beta arrays stored right after the tensors of the stem or block they belong to.
 Arch 5 (Bottleneck ResNet50 / ResNet101, `fold_resnet`) records the Bottleneck counts of layer1..4 in words 3-6 and
 the 2048-d feature in word 7; its layout is listed above `fold_resnet`.
+Arch 6 (CLIP-ReID ViT-B/16, `fold_clip`) records width, layers, heads, the 512-d projection and the 1280-d feature
+in words 3-7, the input height / width in words 9-10 and the patch grid in words 11-12; its layout is listed above
+`fold_clip`.
 All 1x1 weights are stored K-major ([cin][cout]) so a thread owning consecutive output channels loads
 consecutive floats; every tensor is zero-padded to a multiple of 4 floats (16-byte aligned float4 loads).
 """
@@ -43,6 +46,7 @@ ARCH_LMBN_N = 3
 ARCH_OSNET_IN = 4
 ARCH_RESNET = 5
 RESNET_FEAT = 2048
+ARCH_CLIP = 6
 BRANCHES = (("conv2a", 1), ("conv2b", 2), ("conv2c", 3), ("conv2d", 4))
 EPS = 1e-5
 
@@ -354,6 +358,103 @@ def fold_resnet(sd):
     return list(RESNET_BLOCKS[depth]), out
 
 
+# CLIP-ReID ViT-B/16 (arch 6): build_transformer of reid/backbones/clip/make_model.py with cfg MODEL.NAME "ViT-B-16",
+# NECK_FEAT "after", SIE off.  Every linear weight is stored K-major ([in][out]); the arrays are
+#     patch     W[768][768] (k = (ky*16 + kx)*3 + ci), b[768] (zero: conv1 has no bias)
+#     pos       [T][768]  positional_embedding, class_embedding added to row 0
+#     ln_pre    gamma[768], beta[768]
+#     per block ln_1 gamma, beta; in_proj W[768][2304] (q | k | v; the q third and its bias scaled by 1/8, exact),
+#               b[2304]; out_proj W[768][768], b; ln_2 gamma, beta; c_fc W[768][3072], b; c_proj W[3072][768], b
+#     head      g[768], b[768]: ln_post's affine folded into bottleneck;  W[768][512], b[512]: ln_post's affine, proj
+#               and bottleneck_proj folded  (the head normalises token 0 without an affine, then applies both)
+CLIP_WIDTH, CLIP_LAYERS, CLIP_HEADS, CLIP_PROJ = 768, 12, 12, 512
+CLIP_FEAT = CLIP_WIDTH + CLIP_PROJ
+CLIP_GRIDS = {129: (16, 8), 257: (16, 16)}   # positional rows -> patch grid (256x128 and 256x256 crops)
+
+
+def _clip_ignored(k: str) -> bool:
+    """Keys registry.load_pretrained_weights drops for a CLIP model: anything outside build_transformer's state."""
+    return k.startswith(("classifier.", "classifier_proj.", "prompt_learner.", "text_encoder.")) or \
+        k.endswith("num_batches_tracked")
+
+
+def is_clip(sd) -> bool:
+    return "image_encoder.conv1.weight" in sd and "image_encoder.proj" in sd
+
+
+def clip_vehicle_name(name: str) -> bool:
+    """The reference runs 256x256 crops when the weights file name contains `veri` or `vehicleid` (registry.py:231,
+    base_backend.py:57)."""
+    return "veri" in name or "vehicleid" in name
+
+
+def clip_layout(tokens: int = 129):
+    """{key: shape} of build_transformer's state dict (ViT-B/16), without the classifiers and num_batches_tracked."""
+    d = CLIP_WIDTH
+    e = "image_encoder."
+    want = {e + "class_embedding": (d,), e + "positional_embedding": (tokens, d), e + "proj": (d, CLIP_PROJ),
+            e + "conv1.weight": (d, 3, 16, 16)}
+    for ln in ("ln_pre", "ln_post"):
+        want[f"{e}{ln}.weight"] = want[f"{e}{ln}.bias"] = (d,)
+    for i in range(CLIP_LAYERS):
+        b = f"{e}transformer.resblocks.{i}."
+        want.update({b + "attn.in_proj_weight": (3 * d, d), b + "attn.in_proj_bias": (3 * d,),
+                     b + "attn.out_proj.weight": (d, d), b + "attn.out_proj.bias": (d,),
+                     b + "ln_1.weight": (d,), b + "ln_1.bias": (d,), b + "ln_2.weight": (d,), b + "ln_2.bias": (d,),
+                     b + "mlp.c_fc.weight": (4 * d, d), b + "mlp.c_fc.bias": (4 * d,),
+                     b + "mlp.c_proj.weight": (d, 4 * d), b + "mlp.c_proj.bias": (d,)})
+    for bn, n in (("bottleneck", d), ("bottleneck_proj", CLIP_PROJ)):
+        for p in ("weight", "bias", "running_mean", "running_var"):
+            want[f"{bn}.{p}"] = (n,)
+    return want
+
+
+def fold_clip(sd, name=None):
+    """CLIP-ReID state dict -> (header dims, input hw, grid, arrays) of the arch-6 blob.  Only ViT-B/16 is supported:
+    any key or shape that differs from build_transformer's (another width or depth, CLIP-RN50's attnpool, a missing
+    key), apart from the keys the reference discards, raises a ValueError naming the keys.  `name` is the weights
+    file name: a `veri` / `vehicleid` name needs the 257-row positional table of 256x256 crops and any other name the
+    129-row one of 256x128, as the reference builds the model for that name."""
+    keys = {k for k in sd if not _clip_ignored(k)}
+    pos_key = "image_encoder.positional_embedding"
+    tokens = tuple(sd[pos_key].shape)[0] if pos_key in sd else 129
+    want = clip_layout(tokens if tokens in CLIP_GRIDS else 129)
+    bad_shape = sorted(k for k in keys & set(want) if tuple(sd[k].shape) != want[k])[:4]
+    if keys != set(want) or bad_shape:
+        extra, missing = sorted(keys - set(want))[:4], sorted(set(want) - keys)[:4]
+        raise ValueError(f"not a CLIP-ReID ViT-B/16 state dict (unexpected keys {extra}, missing keys {missing}, "
+                         f"unexpected shapes {bad_shape}); CLIP-RN50 and other widths or depths are not supported")
+    if name is not None and clip_vehicle_name(name) != (tokens == 257):
+        raise ValueError(f"CLIP weights '{name}' have a {tokens}-row positional table, but the reference runs "
+                         f"{'256x256' if clip_vehicle_name(name) else '256x128'} crops for that file name "
+                         f"({257 if clip_vehicle_name(name) else 129} rows) and would discard the table")
+    gh, gw = CLIP_GRIDS[tokens]
+    e = "image_encoder."
+    d = CLIP_WIDTH
+    w = _np(sd[e + "conv1.weight"])   # [768][3][16][16]
+    pos = _np(sd[e + "positional_embedding"]).copy()
+    pos[0] += _np(sd[e + "class_embedding"])
+    out: List[np.ndarray] = [w.transpose(2, 3, 1, 0).reshape(-1, d), np.zeros(d), pos,
+                             _np(sd[e + "ln_pre.weight"]), _np(sd[e + "ln_pre.bias"])]
+    qscale = np.ones(3 * d)
+    qscale[:d] = 1.0 / 8.0   # head_dim ** -0.5
+    for i in range(CLIP_LAYERS):
+        b = f"{e}transformer.resblocks.{i}."
+        out += [_np(sd[b + "ln_1.weight"]), _np(sd[b + "ln_1.bias"]),
+                (_np(sd[b + "attn.in_proj_weight"]) * qscale[:, None]).T, _np(sd[b + "attn.in_proj_bias"]) * qscale,
+                _np(sd[b + "attn.out_proj.weight"]).T, _np(sd[b + "attn.out_proj.bias"]),
+                _np(sd[b + "ln_2.weight"]), _np(sd[b + "ln_2.bias"]),
+                _np(sd[b + "mlp.c_fc.weight"]).T, _np(sd[b + "mlp.c_fc.bias"]),
+                _np(sd[b + "mlp.c_proj.weight"]).T, _np(sd[b + "mlp.c_proj.bias"])]
+    g, beta = _np(sd[e + "ln_post.weight"]), _np(sd[e + "ln_post.bias"])
+    sc, sh = _bn_fold(sd, "bottleneck")
+    scp, shp = _bn_fold(sd, "bottleneck_proj")
+    proj = _np(sd[e + "proj"])   # [768][512]
+    out += [sc * g, sc * beta + sh, (g[:, None] * proj) * scp[None, :], (beta @ proj) * scp + shp]
+    dims = [d, CLIP_LAYERS, CLIP_HEADS, CLIP_PROJ, CLIP_FEAT]
+    return dims, (16 * gh, 16 * gw), (gh, gw), out
+
+
 def _pad4(n: int) -> int:
     return (n + 3) // 4 * 4
 
@@ -412,19 +513,24 @@ def fold_mobilenetv2(sd):
 
 def export_blob(weights, out_path=None) -> Path:
     """`weights`: path to a .pt checkpoint or an in-memory state dict.  Returns the blob path."""
+    name = None
     if isinstance(weights, (str, Path)):
         src = Path(weights)
         if src.suffix == ".b200reid":
             return src
         sd = load_state_dict(src)
+        name = src.name
         if out_path is None:
             out_path = src.with_suffix(".b200reid")
     else:
         sd = weights
         if out_path is None:
             raise ValueError("out_path is required when exporting an in-memory state dict")
-    table, in_modes = [], []
-    if "conv9.conv.weight" in sd:
+    table, in_modes, extra = [], [], []
+    if is_clip(sd):
+        dims, input_hw, grid, arrays = fold_clip(sd, name)
+        arch, extra = ARCH_CLIP, [*input_hw, *grid]
+    elif "conv9.conv.weight" in sd:
         stem_c, feat, table, arrays = fold_mobilenetv2(sd)
         arch, dims = ARCH_MOBILENETV2, [stem_c, len(table), 0, 0, feat]
     elif _osnet_in_variant(sd) is not None:
@@ -440,8 +546,8 @@ def export_blob(weights, out_path=None) -> Path:
         blocks, arrays = fold_resnet(sd)
         arch, dims = ARCH_RESNET, blocks + [RESNET_FEAT]
     else:
-        raise ValueError("only OSNet, OSNet-AIN, OSNet-IBN, MobileNetV2, LMBN_n and ResNet50 / ResNet101 state dicts are "
-                         "implemented on the B200 ReID path")
+        raise ValueError("only OSNet, OSNet-AIN, OSNet-IBN, MobileNetV2, LMBN_n, ResNet50 / ResNet101 and CLIP-ReID "
+                         "ViT-B/16 state dicts are implemented on the B200 ReID path")
     # every tensor starts on a 16-byte boundary (the kernels read weights as float4)
     padded = []
     for a in arrays:
@@ -453,6 +559,8 @@ def export_blob(weights, out_path=None) -> Path:
         header[9] = LMBN_INPUT_H
     if arch == ARCH_OSNET_IN:
         header[9:16] = in_modes
+    if arch == ARCH_CLIP:
+        header[9:13] = extra
     out_path = Path(out_path)
     tmp = out_path.with_suffix(out_path.suffix + ".tmp")
     with open(tmp, "wb") as f:

@@ -414,8 +414,9 @@ BOXMOT_B200_API int boxmot_b200_pointwise_gemm(const float* a, int m, int k, con
 BOXMOT_B200_API int boxmot_b200_instance_norm(const float* x, int n, int h, int w, int c, const float* gamma,
                                               const float* beta, const float* residual, int relu, int pool, float* out);
 /* One convolution of the ResNet50 / ResNet101 path (wgmma tf32x3 implicit GEMM) on host arrays, NHWC float32:
- * out (n,Ho,Wo,out_c) = act(conv(in0) + conv1x1(in1) + bias (+ residual, optional)), act = ReLU when relu = 1.
- * in0 (n,h0,w0,c0) is read by a k x k kernel (k 1 or 3, pad k/2) at `stride`; in1 (n,h1,w1,c1), optional (c1 = 0
+ * out (n,Ho,Wo,out_c) = act(conv(in0) + conv1x1(in1) + bias (+ residual, optional)), act = none when relu = 0, ReLU
+ * when relu = 1, QuickGELU x * sigmoid(1.702 x) when relu = 2 (CLIP's MLP; a CLIP linear layer is a 1x1 convolution
+ * over h0 = tokens, w0 = 1).  in0 (n,h0,w0,c0) is read by a k x k kernel (k 1 or 3, pad k/2) at `stride`; in1 (n,h1,w1,c1), optional (c1 = 0
  * for none), by a 1x1 kernel at `stride1` over the same output grid (the fused conv3 + downsample of a stage's first
  * Bottleneck).  w is (k*k*c0 + c1, out_c) K-major, k index (kh*k + kw)*c0 + ci then the c1 channels; c0 and c1
  * multiples of 32, out_c a multiple of 64.  elapsed_ms (optional) receives the average device time of 10 launches. */
@@ -423,11 +424,20 @@ BOXMOT_B200_API int boxmot_b200_resnet_conv(const float* in0, int n, int h0, int
                                             const float* in1, int h1, int w1, int c1, int stride1, const float* w,
                                             int out_c, const float* bias, const float* residual, int relu, float* out,
                                             float* elapsed_ms);
+/* LayerNorm of the CLIP ViT-B/16 path on host arrays: out (rows,768) = LN(x) * gamma + beta, eps 1e-5, float32. */
+BOXMOT_B200_API int boxmot_b200_vit_layernorm(const float* x, int rows, const float* gamma, const float* beta,
+                                              float* out);
+/* Multi-head attention of the CLIP ViT-B/16 path on host arrays: qkv (n,tokens,2304) holds q | k | v, head h at
+ * columns 64h..64h+63 of each, with q already scaled by 1/8; out (n,tokens,768) = softmax(q k^T) v per head, heads
+ * interleaved.  1 <= tokens <= 288. */
+BOXMOT_B200_API int boxmot_b200_vit_attention(const float* qkv, int n, int tokens, float* out);
 BOXMOT_B200_API int boxmot_b200_device_count(void);
 /* Diagnostics for the ReID kernels: run the forward up to `stage` (0 input blob, 1 stem, 2 max-pool, 3..10 the
  * six OSBlocks and two transitions in order, 11 conv5) and copy that NHWC float32 tensor of the n crops out.  For
  * OSNet-AIN / OSNet-IBN the stem tap is the map after the instance norm and the ReLU.  For ResNet50 / ResNet101: 0 input
- * blob, 1 stem, 2 max-pool, 3 + i the output of Bottleneck i (layer1.0 first). */
+ * blob, 1 stem, 2 max-pool, 3 + i the output of Bottleneck i (layer1.0 first).  For CLIP ViT-B/16: 0 input blob
+ * (256 x 128 or 256 x 256), 1 patch embedding (patches x 768), 2 ln_pre (tokens x 768), 3 + l the output of residual
+ * block l, 15 the head row before the L2 normalisation (1280). */
 BOXMOT_B200_API int boxmot_b200_reid_debug_stage(void* reid_handle, const float* boxes_xyxy, int n_boxes,
                                                  const uint8_t* image_data, int image_rows, int image_cols,
                                                  int stage, float* out, int out_capacity_floats,
