@@ -1334,9 +1334,15 @@ enum { IN_NONE = 0, IN_BEFORE_RESIDUAL = 1, IN_AFTER_RESIDUAL = 2 };
 
 namespace tcx { struct Plan; }
 
+// MobileNetV2 (arch 2): the stem (stem channels, padded to 4), the inverted-residual blocks and conv9
 struct MbBlock {
     int cin, cout, t, stride, cinp, midp, coutp;
     size_t we, be, wd, bd, wp, bp;
+};
+struct MbW {
+    int stem = 0, stemp = 0, last = 0;   // last: padded output width of the last block
+    size_t stem_w = 0, stem_b = 0, c9w = 0, c9b = 0;
+    std::vector<MbBlock> blocks;
 };
 
 // LMBN_n (arch 3): OSNet_x1_0 trunk up to conv3[0], three branches (global, partial, channel) of conv3[1:] + conv4 +
@@ -1367,9 +1373,18 @@ struct VitW {
     std::vector<VitLayer> layer;
 };
 
+// Backbone of a blob: header word 2, numbered as in weights.py
+enum ReidArch {
+    ARCH_OSNET = 1,
+    ARCH_MOBILENETV2 = 2,
+    ARCH_LMBN_N = 3,
+    ARCH_OSNET_IN = 4,   // OSNet with instance norms (AIN / IBN)
+    ARCH_RESNET = 5,
+    ARCH_CLIP = 6,       // CLIP-ReID ViT-B/16
+};
+
 struct ReidModel {
-    int arch = 1;                 // 1 OSNet, 2 MobileNetV2, 3 LMBN_n, 4 OSNet with instance norms (AIN / IBN), 5 ResNet,
-                                  // 6 CLIP-ReID ViT-B/16
+    ReidArch arch = ARCH_OSNET;
     int in_h = IN_H;              // crop height
     int in_w = IN_W;              // crop width (256 only for CLIP's vehicle models)
     CropNorm norm = kImageNetNorm;
@@ -1378,11 +1393,9 @@ struct ReidModel {
     size_t stem_beta = 0;
     float* in_tmp = nullptr;      // arch 4: conv3 output of an IN_BEFORE_RESIDUAL block with a downsample
     LmbnW lm;
-    std::vector<MbBlock> mb;      // MobileNetV2 bottlenecks
+    MbW mb;
     std::vector<RnBlock> rn;      // ResNet Bottlenecks, layer1.0 .. layer4.last
-    float* d_wrn = nullptr;       // ResNet: every convolution's weights packed by rn::pack_conv_weights
-    int mb_stem = 0, mb_stemp = 0, mb_last = 0;
-    size_t mb_stem_w = 0, mb_stem_b = 0, mb_c9w = 0, mb_c9b = 0;
+    float* d_wrn = nullptr;       // ResNet / CLIP: every GEMM's weights packed by rn::pack_conv_weights
     int c[4] = {0, 0, 0, 0};
     int feat = 0;
     float* d_w = nullptr;
@@ -1439,407 +1452,417 @@ Plan* plan_build(ReidModel* m, const float* host_w);
 bool plan_supported(const ReidModel* m);
 }
 
-ReidModel* reid_load(const char* path) {
-    std::ifstream f(path, std::ios::binary);
-    if (!f) throw std::runtime_error(std::string("cannot open ReID blob: ") + path);
-    int32_t hdr[16];
-    f.read(reinterpret_cast<char*>(hdr), sizeof(hdr));
-    if (!f || (uint32_t)hdr[0] != BLOB_MAGIC || hdr[1] != 1 || hdr[2] < 1 || hdr[2] > 6)
-        throw std::runtime_error("not a version-1 .b200reid blob (export it with boxmot_b200.weights.export_blob)");
-    ReidModel* m = new ReidModel();
-    if (hdr[2] == 6) {
-        // ---- CLIP-ReID ViT-B/16 (reid/backbones/clip): patch embedding, ln_pre, 12 residual attention blocks, head ----
-        try {
-            m->arch = 6;
-            constexpr int D = vit::D;
-            if (hdr[3] != D || hdr[4] < 1 || hdr[4] > 64 || hdr[5] != vit::HEADS || hdr[6] != vit::PROJ ||
+namespace {
+// Offsets of the tensors in the blob payload, in walk order; every tensor starts 16-byte aligned
+struct BlobCursor {
+    size_t o = 0;
+    size_t operator()(size_t n) { const size_t r = o; o += (n + 3) / 4 * 4; return r; }
+};
+
+// Layers whose K-major [K][N] weights rn::k_conv_tc reads pre-split (rn::pack_conv_weights): ResNet's convolutions and
+// CLIP's linear layers.  The layout queues them; after the upload each `dst` points at its packing in m->d_wrn.
+struct WgmmaPack {
+    struct Todo { const float** dst; size_t w; int K, N; size_t at; };
+    std::vector<Todo> todo;
+    size_t n = 0;
+    void add(const float*& dst, size_t w, int K, int N) {
+        todo.push_back({&dst, w, K, N, n});
+        n += 2 * (size_t)K * N;
+    }
+};
+
+// Per-crop float counts of the workspace buffers a chunk runner uses (0: not allocated)
+struct Workspace {
+    size_t blob = 0, bufA = 0, bufB = 0, x1 = 0, Y[4][2] = {}, sums[4] = {}, gates = 0, trunk = 0, pooled = 0, in_tmp = 0;
+    size_t total() const {
+        size_t t = blob + bufA + bufB + x1 + gates + trunk + pooled + in_tmp;
+        for (int b = 0; b < 4; ++b) t += Y[b][0] + Y[b][1] + sums[b];
+        return t;
+    }
+};
+
+// The arch-specific header words: the model's geometry, checked before the payload is read
+void read_header(ReidModel* m, const int32_t* hdr) {
+    m->arch = (ReidArch)hdr[2];
+    m->feat = hdr[7];
+    switch (m->arch) {
+        case ARCH_CLIP:
+            if (hdr[3] != vit::D || hdr[4] < 1 || hdr[4] > 64 || hdr[5] != vit::HEADS || hdr[6] != vit::PROJ ||
                 hdr[7] != vit::FEAT)
                 throw std::runtime_error("bad CLIP blob header (only ViT-B/16: width 768, 12 heads, 512-d projection)");
-            m->feat = hdr[7];
             m->in_h = hdr[9];
             m->in_w = hdr[10];
             if (m->in_h != 256 || (m->in_w != 128 && m->in_w != 256) || hdr[11] != m->in_h / vit::PATCH ||
                 hdr[12] != m->in_w / vit::PATCH)
                 throw std::runtime_error("bad CLIP blob header (input 256x128 or 256x256, 16x16 patches)");
             m->norm = CropNorm{{0.5f, 0.5f, 0.5f}, {0.5f, 0.5f, 0.5f}};
-            VitW& v = m->vit;
-            v.layers = hdr[4];
-            v.tokens = 1 + hdr[11] * hdr[12];
-            const size_t n_floats = (size_t)hdr[8];
-            std::vector<float> host(n_floats);
-            f.read(reinterpret_cast<char*>(host.data()), sizeof(float) * n_floats);
-            if (!f) throw std::runtime_error("truncated ReID blob");
-            size_t o = 0;
-            auto take = [&](size_t n) { size_t r = o; o += (n + 3) / 4 * 4; return r; };
-            struct Todo { const float** dst; size_t w; int K, N; size_t at; };
-            std::vector<Todo> todo;
-            size_t packed_n = 0;
-            auto linear = [&](const float*& dst, int K, int N) {
-                todo.push_back({&dst, take((size_t)K * N), K, N, packed_n});
-                packed_n += 2 * (size_t)K * N;
-            };
-            linear(v.patch_w, 3 * vit::PATCH * vit::PATCH, D);
-            v.patch_b = take(D);
-            v.pos = take((size_t)v.tokens * D);
-            v.lnpre_g = take(D); v.lnpre_b = take(D);
-            v.layer.resize(v.layers);   // `todo` keeps pointers into the layers
-            for (VitLayer& l : v.layer) {
-                l.ln1g = take(D); l.ln1b = take(D);
-                linear(l.win, D, 3 * D); l.bin = take(3 * D);
-                linear(l.wout, D, D); l.bout = take(D);
-                l.ln2g = take(D); l.ln2b = take(D);
-                linear(l.wfc, D, 4 * D); l.bfc = take(4 * D);
-                linear(l.wproj, 4 * D, D); l.bproj = take(D);
-            }
-            v.head_g = take(D); v.head_b = take(D);
-            v.head_w = take((size_t)D * vit::PROJ); v.head_pb = take(vit::PROJ);
-            if (o != n_floats) throw std::runtime_error("ReID blob size does not match its header");
-            std::vector<float> packed(packed_n);
-            for (auto& t : todo) rn::pack_conv_weights(host.data() + t.w, t.K, t.N, packed.data() + t.at);
-            RCUDA_OK(cudaMalloc(&m->d_w, sizeof(float) * n_floats));
-            RCUDA_OK(cudaMemcpy(m->d_w, host.data(), sizeof(float) * n_floats, cudaMemcpyHostToDevice));
-            RCUDA_OK(cudaMalloc(&m->d_wrn, sizeof(float) * packed_n));
-            RCUDA_OK(cudaMemcpy(m->d_wrn, packed.data(), sizeof(float) * packed_n, cudaMemcpyHostToDevice));
-            for (auto& t : todo) *t.dst = m->d_wrn + t.at;
-            if (const char* ce = getenv("BOXMOT_B200_REID_CHUNK")) {
-                const int c = atoi(ce);
-                if (c >= 8 && c <= 1024) m->chunk = c;
-            }
-            // per crop: the staged crop, the residual stream, the LayerNorm output and the attention output
-            // ([T][768] each), q | k | v ([T][2304]) and the MLP hidden layer ([T][3072], which also holds the patch
-            // rows): 1.09 M floats at 129 tokens, 2.17 M at 257, both below the 2.36 M an OSNet_x1_0 chunk takes per
-            // crop, so the chunk keeps its size
-            const size_t CH = m->chunk, T = v.tokens;
-            RCUDA_OK(cudaMalloc(&m->blob, sizeof(float) * CH * m->in_h * m->in_w * 3));
-            RCUDA_OK(cudaMalloc(&m->bufA, sizeof(float) * CH * T * D));
-            RCUDA_OK(cudaMalloc(&m->bufB, sizeof(float) * CH * T * D));
-            RCUDA_OK(cudaMalloc(&m->Y[0][0], sizeof(float) * CH * T * D));
-            RCUDA_OK(cudaMalloc(&m->x1, sizeof(float) * CH * T * 3 * D));
-            RCUDA_OK(cudaMalloc(&m->Y[0][1], sizeof(float) * CH * T * 4 * D));
-        } catch (...) {
-            reid_free(m);
-            throw;
-        }
-        return m;
-    }
-    if (hdr[2] == 5) {
-        // ---- Bottleneck ResNet (reid/backbones/resnet.py resnet50 / resnet101): stem, layer1..4, GAP ----
-        try {
-            m->arch = 5;
+            m->vit.layers = hdr[4];
+            m->vit.tokens = 1 + hdr[11] * hdr[12];
+            return;
+        case ARCH_RESNET:
             m->c[0] = 64;
-            m->feat = hdr[7];
-            const size_t n_floats = (size_t)hdr[8];
             for (int l = 0; l < 4; ++l)
                 if (hdr[3 + l] < 1 || hdr[3 + l] > 64) throw std::runtime_error("bad ResNet blob header (block counts)");
             if (m->feat != 2048) throw std::runtime_error("bad ResNet blob header (feature dim)");
-            std::vector<float> host(n_floats);
-            f.read(reinterpret_cast<char*>(host.data()), sizeof(float) * n_floats);
-            if (!f) throw std::runtime_error("truncated ReID blob");
-            size_t o = 0;
-            auto take = [&](size_t n) { size_t r = o; o += (n + 3) / 4 * 4; return r; };
-            m->stem_w = take((size_t)147 * 64);
-            m->stem_b = take(64);
-            struct Todo { RnConv* dst; size_t w; int K, N; size_t at; };
-            std::vector<Todo> todo;
-            size_t packed_n = 0;
-            auto conv = [&](RnConv& c, int K, int N) {
-                const size_t w = take((size_t)K * N);
-                c.b = take(N);
-                todo.push_back({&c, w, K, N, packed_n});
-                packed_n += 2 * (size_t)K * N;
-            };
-            int cin = 64;
-            m->rn.reserve((size_t)hdr[3] + hdr[4] + hdr[5] + hdr[6]);   // `todo` keeps pointers into the blocks
-            for (int l = 0; l < 4; ++l)
-                for (int j = 0; j < hdr[3 + l]; ++j) {
-                    RnBlock b{};
-                    b.cin = cin; b.width = 64 << l; b.cout = 4 * b.width; b.stride = (j == 0 && l > 0) ? 2 : 1;
-                    m->rn.push_back(b);
-                    RnBlock& r = m->rn.back();
-                    conv(r.c1, r.cin, r.width);
-                    conv(r.c2, 9 * r.width, r.width);
-                    conv(r.c3, r.width + (j == 0 ? r.cin : 0), r.cout);
-                    cin = r.cout;
-                }
-            if (o != n_floats || cin != m->feat) throw std::runtime_error("ReID blob size does not match its header");
-            std::vector<float> packed(packed_n);
-            for (auto& t : todo) rn::pack_conv_weights(host.data() + t.w, t.K, t.N, packed.data() + t.at);
-            RCUDA_OK(cudaMalloc(&m->d_w, sizeof(float) * n_floats));
-            RCUDA_OK(cudaMemcpy(m->d_w, host.data(), sizeof(float) * n_floats, cudaMemcpyHostToDevice));
-            RCUDA_OK(cudaMalloc(&m->d_wrn, sizeof(float) * packed_n));
-            RCUDA_OK(cudaMemcpy(m->d_wrn, packed.data(), sizeof(float) * packed_n, cudaMemcpyHostToDevice));
-            for (auto& t : todo) t.dst->w = m->d_wrn + t.at;
-            if (const char* ce = getenv("BOXMOT_B200_REID_CHUNK")) {
-                const int v = atoi(ce);
-                if (v >= 8 && v <= 1024) m->chunk = v;
+            return;
+        case ARCH_MOBILENETV2:   // hdr[4] blocks: it sizes the block table that follows the header
+            m->mb.stem = hdr[3];
+            m->mb.stemp = (hdr[3] + 3) / 4 * 4;
+            if (hdr[4] < 1 || hdr[4] > 64 || m->feat < 1) throw std::runtime_error("bad MobileNetV2 blob header");
+            return;
+        case ARCH_OSNET:
+        case ARCH_LMBN_N:
+        case ARCH_OSNET_IN:
+            for (int i = 0; i < 4; ++i) m->c[i] = hdr[3 + i];
+            if (m->c[0] % 16 != 0 || m->feat < 1) throw std::runtime_error("unsupported OSNet width (stem channels)");
+            if (m->arch == ARCH_LMBN_N) {
+                if (hdr[9] != 384 || m->c[0] != 64 || m->c[1] != 256 || m->c[2] != 384 || m->c[3] != LMBN_C ||
+                    m->feat != LMBN_VECS * LMBN_C)
+                    throw std::runtime_error("unsupported LMBN_n blob header (expected 384x128 input, widths 64/256/384/512, 3584-d)");
+                m->in_h = hdr[9];
             }
-            // per crop: the staged crop, two block maps as large as the stem output / layer1's 64x32x256, layer2.0's
-            // conv1 output (64x32x128) and layer1's conv2 output (64x32x64): 1.54 M floats, below the 2.36 M an
-            // OSNet_x1_0 chunk takes per crop, so the chunk keeps its size
-            const size_t CH = m->chunk, big = (size_t)128 * 64 * 64;
-            RCUDA_OK(cudaMalloc(&m->blob, sizeof(float) * CH * IN_H * IN_W * 3));
-            RCUDA_OK(cudaMalloc(&m->bufA, sizeof(float) * CH * big));
-            RCUDA_OK(cudaMalloc(&m->bufB, sizeof(float) * CH * big));
-            RCUDA_OK(cudaMalloc(&m->x1, sizeof(float) * CH * 64 * 32 * 128));
-            RCUDA_OK(cudaMalloc(&m->Y[0][0], sizeof(float) * CH * 64 * 32 * 64));
-        } catch (...) {
-            reid_free(m);
-            throw;
-        }
-        return m;
+            if (m->arch == ARCH_OSNET_IN) {   // header word 9: stem IN flag; words 10-15: per-block IN placement
+                m->stem_in = hdr[9] != 0;
+                for (int i = 0; i < 6; ++i)
+                    if (hdr[10 + i] < IN_NONE || hdr[10 + i] > IN_AFTER_RESIDUAL)
+                        throw std::runtime_error("bad instance-norm placement in an arch-4 ReID blob header");
+            }
+            return;
     }
-    if (hdr[2] == 2) {
-        // ---- MobileNetV2 (reid/backbones/mobilenetv2.py): stem, 17 inverted-residual blocks, conv9, GAP ----
-        try {
-            m->arch = 2;
-            m->mb_stem = hdr[3];
-            m->mb_stemp = (hdr[3] + 3) / 4 * 4;
-            const int n_blocks = hdr[4];
-            m->feat = hdr[7];
-            const size_t n_floats = (size_t)hdr[8];
-            if (n_blocks < 1 || n_blocks > 64 || m->feat < 1) throw std::runtime_error("bad MobileNetV2 blob header");
-            std::vector<int32_t> table((size_t)n_blocks * 4);
-            f.read(reinterpret_cast<char*>(table.data()), sizeof(int32_t) * table.size());
-            std::vector<float> host(n_floats);
-            f.read(reinterpret_cast<char*>(host.data()), sizeof(float) * n_floats);
-            if (!f) throw std::runtime_error("truncated ReID blob");
-            size_t o = 0;
-            auto take = [&](size_t n) { size_t r = o; o += (n + 3) / 4 * 4; return r; };
-            auto p4 = [](int n) { return (n + 3) / 4 * 4; };
-            m->mb_stem_w = take((size_t)27 * m->mb_stemp);
-            m->mb_stem_b = take(m->mb_stemp);
-            int H = 128, Wd = 64;
-            size_t max_x = (size_t)H * Wd * m->mb_stemp, max_e = 0, max_d = 0;
-            for (int i = 0; i < n_blocks; ++i) {
-                MbBlock b{};
-                b.cin = table[i * 4]; b.cout = table[i * 4 + 1]; b.t = table[i * 4 + 2]; b.stride = table[i * 4 + 3];
-                if (b.stride != 1 && b.stride != 2) throw std::runtime_error("bad MobileNetV2 stride");
-                b.cinp = p4(b.cin); b.midp = p4(b.cin * b.t); b.coutp = p4(b.cout);
-                b.we = take((size_t)b.cinp * b.midp); b.be = take(b.midp);
-                b.wd = take((size_t)9 * b.midp); b.bd = take(b.midp);
-                b.wp = take((size_t)b.midp * b.coutp); b.bp = take(b.coutp);
-                max_e = std::max(max_e, (size_t)H * Wd * b.midp);
-                H /= b.stride; Wd /= b.stride;
-                max_d = std::max(max_d, (size_t)H * Wd * b.midp);
-                max_x = std::max(max_x, (size_t)H * Wd * b.coutp);
-                m->mb.push_back(b);
-            }
-            m->mb_last = m->mb.back().coutp;
-            const int featp = p4(m->feat);
-            m->mb_c9w = take((size_t)m->mb_last * featp);
-            m->mb_c9b = take(featp);
-            if (o != n_floats || featp != m->feat) throw std::runtime_error("ReID blob size does not match its header");
-            max_x = std::max(max_x, (size_t)H * Wd * featp);
-            RCUDA_OK(cudaMalloc(&m->d_w, sizeof(float) * n_floats));
-            RCUDA_OK(cudaMemcpy(m->d_w, host.data(), sizeof(float) * n_floats, cudaMemcpyHostToDevice));
-            m->chunk = 256;
-            if (const char* ce = getenv("BOXMOT_B200_REID_CHUNK")) {
-                const int v = atoi(ce);
-                if (v >= 8 && v <= 1024) m->chunk = v;
-            }
-            const size_t CH = m->chunk;
-            RCUDA_OK(cudaMalloc(&m->blob, sizeof(float) * CH * IN_H * IN_W * 3));
-            RCUDA_OK(cudaMalloc(&m->bufA, sizeof(float) * CH * max_x));
-            RCUDA_OK(cudaMalloc(&m->bufB, sizeof(float) * CH * max_x));
-            RCUDA_OK(cudaMalloc(&m->x1, sizeof(float) * CH * max_e));
-            RCUDA_OK(cudaMalloc(&m->Y[0][0], sizeof(float) * CH * max_d));
-        } catch (...) {
-            reid_free(m);
-            throw;
-        }
-        return m;
+}
+
+// OSNet-family workspace per crop at crop height in_h: the crop, two block maps as large as the stem output
+// (in_h/2 x 64 x c0) or the stage-2 maps (in_h/4 x 32 x c1), whichever is larger, the conv1 output and the eight
+// LightConv maps of a stage-2 block, the branch sums and gates, and for LMBN_n the trunk output and the head poolings
+Workspace osnet_workspace(const ReidModel* m, int in_h, bool lmbn) {
+    Workspace ws;
+    const size_t big = std::max((size_t)(in_h / 2) * 64 * m->c[0], (size_t)(in_h / 4) * 32 * m->c[1]);
+    const size_t mid = (size_t)(in_h / 4) * 32 * (m->c[1] / 4);
+    ws.blob = (size_t)in_h * IN_W * 3;
+    ws.bufA = ws.bufB = big;
+    ws.x1 = mid;
+    for (int b = 0; b < 4; ++b) {
+        ws.Y[b][0] = ws.Y[b][1] = mid;
+        ws.sums[b] = 64 * (size_t)(m->c[3] / 4);
     }
+    ws.gates = 4 * (size_t)(m->c[3] / 4);
+    if (lmbn) {
+        ws.trunk = (size_t)(in_h / 8) * 16 * m->c[2];
+        ws.pooled = (size_t)LMBN_POOLS * LMBN_C;
+    }
+    return ws;
+}
+
+// ---- OSNet, LMBN_n and OSNet-AIN / IBN (arch 1, 3, 4): stem, OSBlocks, transitions, conv5 and fc (or LMBN_n's
+// branches and neck) ----
+Workspace layout_osnet(ReidModel* m, const int32_t* hdr, BlobCursor& take) {
+    auto take_block = [&](BlockW& b, int cin, int cout, int in_mode = IN_NONE) {
+        b.in_mode = in_mode;
+        b.cin = cin;
+        b.cout = cout;
+        b.mid = b.cout / 4;
+        b.hid = b.mid / 16;
+        b.has_ds = b.cin != b.cout;
+        if (b.mid % 8 != 0 || b.hid < 1) throw std::runtime_error("unsupported OSNet width (mid channels)");
+        b.c1w = take((size_t)b.cin * b.mid);
+        b.c1b = take(b.mid);
+        for (int l = 0; l < 10; ++l) {
+            b.light[l].pw = take((size_t)b.mid * b.mid);
+            b.light[l].dw = take((size_t)9 * b.mid);
+            b.light[l].b = take(b.mid);
+        }
+        b.g1w = take((size_t)b.mid * b.hid);
+        b.g1b = take(b.hid);
+        b.g2w = take((size_t)b.hid * b.mid);
+        b.g2b = take(b.mid);
+        if (in_mode == IN_BEFORE_RESIDUAL) {   // conv3 alone (zero bias), then the downsample on its own
+            b.cw = take((size_t)b.mid * b.cout);
+            b.cb = take(b.cout);
+            if (b.has_ds) {
+                b.dsw = take((size_t)b.cin * b.cout);
+                b.dsb = take(b.cout);
+            }
+        } else {
+            b.cw = take((size_t)(b.mid + (b.has_ds ? b.cin : 0)) * b.cout);
+            b.cb = take(b.cout);
+        }
+        if (in_mode != IN_NONE) {
+            if (b.cout % 4) throw std::runtime_error("unsupported OSNet width (instance-norm channels)");
+            b.ing = take(b.cout);
+            b.inb = take(b.cout);
+        }
+    };
+    m->stem_w = take((size_t)147 * m->c[0]);
+    m->stem_b = take(m->c[0]);
+    if (m->stem_in) m->stem_beta = take(m->c[0]);
+    if (m->arch == ARCH_LMBN_N) {   // weights.fold_lmbn_n walk order
+        LmbnW& lm = m->lm;
+        take_block(lm.trunk[0], 64, 256);
+        take_block(lm.trunk[1], 256, 256);
+        lm.trunk_tw = take((size_t)256 * 256);
+        lm.trunk_tb = take(256);
+        take_block(lm.trunk[2], 256, 384);
+        for (int br = 0; br < 3; ++br) {
+            take_block(lm.br[br][0], 384, 384);
+            lm.br_tw[br] = take((size_t)384 * 384);
+            lm.br_tb[br] = take(384);
+            take_block(lm.br[br][1], 384, 512);
+            take_block(lm.br[br][2], 512, 512);
+            lm.br_c5w[br] = take((size_t)512 * 512);
+            lm.br_c5b[br] = take(512);
+        }
+        take_block(lm.bottleneck, 512, 512);
+        for (int k = 0; k < 5; ++k) {
+            lm.neck_w[k] = take((size_t)LMBN_C * LMBN_C);
+            lm.neck_b[k] = take(LMBN_C);
+        }
+        lm.sh_w = take((size_t)(LMBN_C / 2) * LMBN_C);
+        lm.sh_b = take(LMBN_C);
+        lm.ch_st = take((size_t)4 * LMBN_C);
+        return osnet_workspace(m, m->in_h, true);
+    }
+    for (int s = 0; s < 3; ++s) {
+        for (int j = 0; j < 2; ++j)
+            take_block(m->blocks[s * 2 + j], j == 0 ? m->c[s] : m->c[s + 1], m->c[s + 1],
+                       m->arch == ARCH_OSNET_IN ? hdr[10 + s * 2 + j] : IN_NONE);
+        if (s < 2) {
+            m->trans_w[s] = take((size_t)m->c[s + 1] * m->c[s + 1]);
+            m->trans_b[s] = take(m->c[s + 1]);
+        }
+    }
+    m->c5w = take((size_t)m->c[3] * m->c[3]);
+    m->c5b = take(m->c[3]);
+    m->fcw = take((size_t)m->c[3] * m->feat);
+    m->fcb = take(m->feat);
+    Workspace ws = osnet_workspace(m, m->in_h, false);
+    // arch 4: the instance-norm statistics ({mean, rstd} per crop and channel, 4 floats) live in sums[0], which
+    // holds 16 * c3 >= 4 * C floats per crop and is free whenever they are needed (the stem runs before any block;
+    // a block's norm follows its gates kernel, the last reader of the branch sums).  The one extra buffer is the
+    // conv3 output of an IN_BEFORE_RESIDUAL block whose downsample GEMM writes the block output.
+    for (const BlockW& b : m->blocks)
+        if (b.in_mode == IN_BEFORE_RESIDUAL && b.has_ds) ws.in_tmp = ws.bufA;
+    return ws;
+}
+
+// ---- MobileNetV2 (reid/backbones/mobilenetv2.py): stem, 17 inverted-residual blocks, conv9, GAP ----
+// table: cin, cout, expansion, stride of every block
+Workspace layout_mobilenetv2(ReidModel* m, const std::vector<int32_t>& table, BlobCursor& take) {
+    MbW& mb = m->mb;
+    auto p4 = [](int n) { return (n + 3) / 4 * 4; };
+    mb.stem_w = take((size_t)27 * mb.stemp);
+    mb.stem_b = take(mb.stemp);
+    int H = 128, Wd = 64;
+    size_t max_x = (size_t)H * Wd * mb.stemp, max_e = 0, max_d = 0;
+    for (size_t i = 0; i < table.size(); i += 4) {
+        MbBlock b{};
+        b.cin = table[i]; b.cout = table[i + 1]; b.t = table[i + 2]; b.stride = table[i + 3];
+        if (b.stride != 1 && b.stride != 2) throw std::runtime_error("bad MobileNetV2 stride");
+        b.cinp = p4(b.cin); b.midp = p4(b.cin * b.t); b.coutp = p4(b.cout);
+        b.we = take((size_t)b.cinp * b.midp); b.be = take(b.midp);
+        b.wd = take((size_t)9 * b.midp); b.bd = take(b.midp);
+        b.wp = take((size_t)b.midp * b.coutp); b.bp = take(b.coutp);
+        max_e = std::max(max_e, (size_t)H * Wd * b.midp);
+        H /= b.stride; Wd /= b.stride;
+        max_d = std::max(max_d, (size_t)H * Wd * b.midp);
+        max_x = std::max(max_x, (size_t)H * Wd * b.coutp);
+        mb.blocks.push_back(b);
+    }
+    mb.last = mb.blocks.back().coutp;
+    const int featp = p4(m->feat);
+    mb.c9w = take((size_t)mb.last * featp);
+    mb.c9b = take(featp);
+    if (featp != m->feat) throw std::runtime_error("ReID blob size does not match its header");
+    // per crop: the crop, two block maps, the expansion output and the depthwise output, each at its largest
+    Workspace ws;
+    ws.blob = (size_t)m->in_h * m->in_w * 3;
+    ws.bufA = ws.bufB = std::max(max_x, (size_t)H * Wd * featp);
+    ws.x1 = max_e;
+    ws.Y[0][0] = max_d;
+    return ws;
+}
+
+// ---- Bottleneck ResNet (reid/backbones/resnet.py resnet50 / resnet101): stem, layer1..4, GAP ----
+Workspace layout_resnet(ReidModel* m, const int32_t* hdr, BlobCursor& take, WgmmaPack& pack) {
+    m->stem_w = take((size_t)147 * 64);
+    m->stem_b = take(64);
+    auto conv = [&](RnConv& c, int K, int N) {
+        const size_t w = take((size_t)K * N);
+        c.b = take(N);
+        pack.add(c.w, w, K, N);
+    };
+    int cin = 64;
+    m->rn.reserve((size_t)hdr[3] + hdr[4] + hdr[5] + hdr[6]);   // `pack` keeps pointers into the blocks
+    for (int l = 0; l < 4; ++l)
+        for (int j = 0; j < hdr[3 + l]; ++j) {
+            RnBlock b{};
+            b.cin = cin; b.width = 64 << l; b.cout = 4 * b.width; b.stride = (j == 0 && l > 0) ? 2 : 1;
+            m->rn.push_back(b);
+            RnBlock& r = m->rn.back();
+            conv(r.c1, r.cin, r.width);
+            conv(r.c2, 9 * r.width, r.width);
+            conv(r.c3, r.width + (j == 0 ? r.cin : 0), r.cout);
+            cin = r.cout;
+        }
+    if (cin != m->feat) throw std::runtime_error("ReID blob size does not match its header");
+    // per crop: the staged crop, two block maps as large as the stem output / layer1's 64x32x256, layer2.0's
+    // conv1 output (64x32x128) and layer1's conv2 output (64x32x64): 1.54 M floats, below the 2.36 M an
+    // OSNet_x1_0 chunk takes per crop, so the chunk keeps its size
+    Workspace ws;
+    ws.blob = (size_t)m->in_h * m->in_w * 3;
+    ws.bufA = ws.bufB = (size_t)128 * 64 * 64;
+    ws.x1 = (size_t)64 * 32 * 128;
+    ws.Y[0][0] = (size_t)64 * 32 * 64;
+    return ws;
+}
+
+// ---- CLIP-ReID ViT-B/16 (reid/backbones/clip): patch embedding, ln_pre, 12 residual attention blocks, head ----
+Workspace layout_clip(ReidModel* m, BlobCursor& take, WgmmaPack& pack) {
+    constexpr int D = vit::D;
+    VitW& v = m->vit;
+    auto linear = [&](const float*& dst, int K, int N) { pack.add(dst, take((size_t)K * N), K, N); };
+    linear(v.patch_w, 3 * vit::PATCH * vit::PATCH, D);
+    v.patch_b = take(D);
+    v.pos = take((size_t)v.tokens * D);
+    v.lnpre_g = take(D); v.lnpre_b = take(D);
+    v.layer.resize(v.layers);   // `pack` keeps pointers into the layers
+    for (VitLayer& l : v.layer) {
+        l.ln1g = take(D); l.ln1b = take(D);
+        linear(l.win, D, 3 * D); l.bin = take(3 * D);
+        linear(l.wout, D, D); l.bout = take(D);
+        l.ln2g = take(D); l.ln2b = take(D);
+        linear(l.wfc, D, 4 * D); l.bfc = take(4 * D);
+        linear(l.wproj, 4 * D, D); l.bproj = take(D);
+    }
+    v.head_g = take(D); v.head_b = take(D);
+    v.head_w = take((size_t)D * vit::PROJ); v.head_pb = take(vit::PROJ);
+    // per crop: the staged crop, the residual stream, the LayerNorm output and the attention output
+    // ([T][768] each), q | k | v ([T][2304]) and the MLP hidden layer ([T][3072], which also holds the patch
+    // rows): 1.09 M floats at 129 tokens, 2.17 M at 257, both below the 2.36 M an OSNet_x1_0 chunk takes per
+    // crop, so the chunk keeps its size
+    const size_t T = v.tokens;
+    Workspace ws;
+    ws.blob = (size_t)m->in_h * m->in_w * 3;
+    ws.bufA = ws.bufB = ws.Y[0][0] = T * D;
+    ws.x1 = T * 3 * D;
+    ws.Y[0][1] = T * 4 * D;
+    return ws;
+}
+
+// The A/B kernel switches of the OSNet family, and for OSNet (arch 1) the tensor-core copies of every 1x1 weight that
+// fits the tensor-core kernel's accumulators and shared memory
+void setup_osnet_kernels(ReidModel* m, const float* host) {
+    const char* env = getenv("BOXMOT_B200_REID_TC");
+    // At OSNet_x0_25's K,N <= 128 every 1x1 layer is bandwidth-bound, and on an H100 this unpipelined kernel is
+    // 1.1-2.4x slower than the float32 CUDA-core GEMM (tests/test_gpu_pointwise_tc.py prints both), so the
+    // standalone tensor-core GEMM is opt-in.
+    m->use_tc = env && env[0] == '1' && m->arch == ARCH_OSNET;   // LMBN_n runs the float32 CUDA-core kernels only
+    const char* lv = getenv("BOXMOT_B200_LIGHT_V1");
+    m->light_v2 = !(lv && lv[0] == '1');
+    if (const char* cv = getenv("BOXMOT_B200_LIGHT_CHAIN")) m->light_chain = !(cv[0] == '0');
+    if (const char* cv = getenv("BOXMOT_B200_LIGHT_TC")) m->light_tc = cv[0] == '1';
+    if (const char* cv = getenv("BOXMOT_B200_LIGHT_SMALL")) m->light_small = cv[0] == '1';
+    if (const char* cv = getenv("BOXMOT_B200_CHAIN_VAR")) m->chain_var = atoi(cv);
+    const char* pv = getenv("BOXMOT_B200_PW_V1");
+    m->pw_v2 = !(pv && pv[0] == '1');
+    if (const char* cv = getenv("BOXMOT_B200_PW_SMALL")) m->pw_small = !(cv[0] == '0');
+    if (m->arch != ARCH_OSNET) return;
+    std::vector<float> packed;
+    struct Todo { TcW* dst; size_t w; int K, N; size_t at; };
+    std::vector<Todo> todo;
+    auto add = [&](TcW* dst, size_t w, int K, int N) {
+        const int Kpad = (K + 7) / 8 * 8, Npad = (N + 15) / 16 * 16;
+        if (Npad > tc::NPAD_MAX || tc::smem_bytes(Kpad, Npad) > 200 * 1024) return;
+        dst->Kpad = Kpad; dst->Npad = Npad;
+        todo.push_back({dst, w, K, N, packed.size()});
+        packed.resize(packed.size() + 2 * (size_t)Npad * Kpad);
+    };
+    for (BlockW& b : m->blocks) {
+        add(&b.tc_c1, b.c1w, b.cin, b.mid);
+        add(&b.tc_c, b.cw, b.mid + (b.has_ds ? b.cin : 0), b.cout);
+        if (b.mid % 16 == 0)
+            for (int l = 0; l < 10; ++l) add(&b.light_tc[l], b.light[l].pw, b.mid, b.mid);
+    }
+    for (int s = 0; s < 2; ++s) add(&m->tc_trans[s], m->trans_w[s], m->c[s + 1], m->c[s + 1]);
+    add(&m->tc_c5, m->c5w, m->c[3], m->c[3]);
+    for (auto& t : todo) tc::pack_weights(host + t.w, t.K, t.N, t.dst->Kpad, t.dst->Npad, packed.data() + t.at);
+    if (!packed.empty()) {
+        RCUDA_OK(cudaMalloc(&m->d_wtc, sizeof(float) * packed.size()));
+        RCUDA_OK(cudaMemcpy(m->d_wtc, packed.data(), sizeof(float) * packed.size(), cudaMemcpyHostToDevice));
+        for (auto& t : todo) t.dst->w = m->d_wtc + t.at;
+    }
+}
+}  // namespace
+
+ReidModel* reid_load(const char* path) {
+    std::ifstream f(path, std::ios::binary);
+    if (!f) throw std::runtime_error(std::string("cannot open ReID blob: ") + path);
+    int32_t hdr[16];
+    f.read(reinterpret_cast<char*>(hdr), sizeof(hdr));
+    if (!f || (uint32_t)hdr[0] != BLOB_MAGIC || hdr[1] != 1 || hdr[2] < ARCH_OSNET || hdr[2] > ARCH_CLIP)
+        throw std::runtime_error("not a version-1 .b200reid blob (export it with boxmot_b200.weights.export_blob)");
+    ReidModel* m = new ReidModel();
     try {
-        for (int i = 0; i < 4; ++i) m->c[i] = hdr[3 + i];
-        m->feat = hdr[7];
-        m->arch = hdr[2];
+        read_header(m, hdr);
+        std::vector<int32_t> table;   // MobileNetV2's block table sits between the header and the payload
+        if (m->arch == ARCH_MOBILENETV2) {
+            table.resize((size_t)hdr[4] * 4);
+            f.read(reinterpret_cast<char*>(table.data()), sizeof(int32_t) * table.size());
+        }
         const size_t n_floats = (size_t)hdr[8];
-        if (m->c[0] % 16 != 0 || m->feat < 1) throw std::runtime_error("unsupported OSNet width (stem channels)");
-        if (m->arch == 3) {
-            if (hdr[9] != 384 || m->c[0] != 64 || m->c[1] != 256 || m->c[2] != 384 || m->c[3] != LMBN_C ||
-                m->feat != LMBN_VECS * LMBN_C)
-                throw std::runtime_error("unsupported LMBN_n blob header (expected 384x128 input, widths 64/256/384/512, 3584-d)");
-            m->in_h = hdr[9];
-        }
-        int in_modes[6] = {0, 0, 0, 0, 0, 0};
-        if (m->arch == 4) {   // header word 9: stem IN flag; words 10-15: per-block IN placement
-            m->stem_in = hdr[9] != 0;
-            for (int i = 0; i < 6; ++i) {
-                in_modes[i] = hdr[10 + i];
-                if (in_modes[i] < IN_NONE || in_modes[i] > IN_AFTER_RESIDUAL)
-                    throw std::runtime_error("bad instance-norm placement in an arch-4 ReID blob header");
-            }
-        }
         std::vector<float> host(n_floats);
         f.read(reinterpret_cast<char*>(host.data()), sizeof(float) * n_floats);
         if (!f) throw std::runtime_error("truncated ReID blob");
-        size_t o = 0;
-        auto take = [&](size_t n) { size_t r = o; o += (n + 3) / 4 * 4; return r; };  // 16-byte aligned tensors
-        auto take_block = [&](BlockW& b, int cin, int cout, int in_mode = IN_NONE) {
-            b.in_mode = in_mode;
-            b.cin = cin;
-            b.cout = cout;
-            b.mid = b.cout / 4;
-            b.hid = b.mid / 16;
-            b.has_ds = b.cin != b.cout;
-            if (b.mid % 8 != 0 || b.hid < 1) throw std::runtime_error("unsupported OSNet width (mid channels)");
-            b.c1w = take((size_t)b.cin * b.mid);
-            b.c1b = take(b.mid);
-            for (int l = 0; l < 10; ++l) {
-                b.light[l].pw = take((size_t)b.mid * b.mid);
-                b.light[l].dw = take((size_t)9 * b.mid);
-                b.light[l].b = take(b.mid);
-            }
-            b.g1w = take((size_t)b.mid * b.hid);
-            b.g1b = take(b.hid);
-            b.g2w = take((size_t)b.hid * b.mid);
-            b.g2b = take(b.mid);
-            if (in_mode == IN_BEFORE_RESIDUAL) {   // conv3 alone (zero bias), then the downsample on its own
-                b.cw = take((size_t)b.mid * b.cout);
-                b.cb = take(b.cout);
-                if (b.has_ds) {
-                    b.dsw = take((size_t)b.cin * b.cout);
-                    b.dsb = take(b.cout);
-                }
-            } else {
-                b.cw = take((size_t)(b.mid + (b.has_ds ? b.cin : 0)) * b.cout);
-                b.cb = take(b.cout);
-            }
-            if (in_mode != IN_NONE) {
-                if (b.cout % 4) throw std::runtime_error("unsupported OSNet width (instance-norm channels)");
-                b.ing = take(b.cout);
-                b.inb = take(b.cout);
-            }
-        };
-        m->stem_w = take((size_t)147 * m->c[0]);
-        m->stem_b = take(m->c[0]);
-        if (m->stem_in) m->stem_beta = take(m->c[0]);
-        if (m->arch == 3) {   // weights.fold_lmbn_n walk order
-            LmbnW& lm = m->lm;
-            take_block(lm.trunk[0], 64, 256);
-            take_block(lm.trunk[1], 256, 256);
-            lm.trunk_tw = take((size_t)256 * 256);
-            lm.trunk_tb = take(256);
-            take_block(lm.trunk[2], 256, 384);
-            for (int br = 0; br < 3; ++br) {
-                take_block(lm.br[br][0], 384, 384);
-                lm.br_tw[br] = take((size_t)384 * 384);
-                lm.br_tb[br] = take(384);
-                take_block(lm.br[br][1], 384, 512);
-                take_block(lm.br[br][2], 512, 512);
-                lm.br_c5w[br] = take((size_t)512 * 512);
-                lm.br_c5b[br] = take(512);
-            }
-            take_block(lm.bottleneck, 512, 512);
-            for (int k = 0; k < 5; ++k) {
-                lm.neck_w[k] = take((size_t)LMBN_C * LMBN_C);
-                lm.neck_b[k] = take(LMBN_C);
-            }
-            lm.sh_w = take((size_t)(LMBN_C / 2) * LMBN_C);
-            lm.sh_b = take(LMBN_C);
-            lm.ch_st = take((size_t)4 * LMBN_C);
-        } else {
-            for (int s = 0; s < 3; ++s) {
-                for (int j = 0; j < 2; ++j)
-                    take_block(m->blocks[s * 2 + j], j == 0 ? m->c[s] : m->c[s + 1], m->c[s + 1], in_modes[s * 2 + j]);
-                if (s < 2) {
-                    m->trans_w[s] = take((size_t)m->c[s + 1] * m->c[s + 1]);
-                    m->trans_b[s] = take(m->c[s + 1]);
-                }
-            }
-            m->c5w = take((size_t)m->c[3] * m->c[3]);
-            m->c5b = take(m->c[3]);
-            m->fcw = take((size_t)m->c[3] * m->feat);
-            m->fcb = take(m->feat);
+        BlobCursor take;
+        WgmmaPack pack;
+        Workspace ws;
+        switch (m->arch) {
+            case ARCH_MOBILENETV2: ws = layout_mobilenetv2(m, table, take); break;
+            case ARCH_RESNET: ws = layout_resnet(m, hdr, take, pack); break;
+            case ARCH_CLIP: ws = layout_clip(m, take, pack); break;
+            default: ws = layout_osnet(m, hdr, take); break;
         }
-        if (o != n_floats) throw std::runtime_error("ReID blob size does not match its header");
+        if (take.o != n_floats) throw std::runtime_error("ReID blob size does not match its header");
+
         RCUDA_OK(cudaMalloc(&m->d_w, sizeof(float) * n_floats));
         RCUDA_OK(cudaMemcpy(m->d_w, host.data(), sizeof(float) * n_floats, cudaMemcpyHostToDevice));
-        {   // tensor-core copies of every 1x1 weight that fits the tensor-core kernel's accumulators and shared memory
-            const char* env = getenv("BOXMOT_B200_REID_TC");
-            // At OSNet_x0_25's K,N <= 128 every 1x1 layer is bandwidth-bound, and on an H100 this unpipelined kernel is
-            // 1.1-2.4x slower than the float32 CUDA-core GEMM (tests/test_gpu_pointwise_tc.py prints both), so the
-            // standalone tensor-core GEMM is opt-in.
-            m->use_tc = env && env[0] == '1' && m->arch == 1;   // LMBN_n runs the float32 CUDA-core kernels only
-            const char* lv = getenv("BOXMOT_B200_LIGHT_V1");
-            m->light_v2 = !(lv && lv[0] == '1');
-            if (const char* cv = getenv("BOXMOT_B200_LIGHT_CHAIN")) m->light_chain = !(cv[0] == '0');
-            if (const char* cv = getenv("BOXMOT_B200_LIGHT_TC")) m->light_tc = cv[0] == '1';
-            if (const char* cv = getenv("BOXMOT_B200_LIGHT_SMALL")) m->light_small = cv[0] == '1';
-            if (const char* cv = getenv("BOXMOT_B200_CHAIN_VAR")) m->chain_var = atoi(cv);
-            const char* pv = getenv("BOXMOT_B200_PW_V1");
-            m->pw_v2 = !(pv && pv[0] == '1');
-            if (const char* cv = getenv("BOXMOT_B200_PW_SMALL")) m->pw_small = !(cv[0] == '0');
-            std::vector<float> packed;
-            struct Todo { TcW* dst; size_t w; int K, N; size_t at; };
-            std::vector<Todo> todo;
-            auto add = [&](TcW* dst, size_t w, int K, int N) {
-                const int Kpad = (K + 7) / 8 * 8, Npad = (N + 15) / 16 * 16;
-                if (Npad > tc::NPAD_MAX || tc::smem_bytes(Kpad, Npad) > 200 * 1024) return;
-                dst->Kpad = Kpad; dst->Npad = Npad;
-                todo.push_back({dst, w, K, N, packed.size()});
-                packed.resize(packed.size() + 2 * (size_t)Npad * Kpad);
-            };
-            for (int bi = 0; bi < (m->arch == 1 ? 6 : 0); ++bi) {
-                BlockW& b = m->blocks[bi];
-                add(&b.tc_c1, b.c1w, b.cin, b.mid);
-                add(&b.tc_c, b.cw, b.mid + (b.has_ds ? b.cin : 0), b.cout);
-                if (b.mid % 16 == 0)
-                    for (int l = 0; l < 10; ++l) add(&b.light_tc[l], b.light[l].pw, b.mid, b.mid);
-            }
-            if (m->arch == 1) {
-                for (int s = 0; s < 2; ++s) add(&m->tc_trans[s], m->trans_w[s], m->c[s + 1], m->c[s + 1]);
-                add(&m->tc_c5, m->c5w, m->c[3], m->c[3]);
-            }
-            for (auto& t : todo) tc::pack_weights(host.data() + t.w, t.K, t.N, t.dst->Kpad, t.dst->Npad, packed.data() + t.at);
-            if (!packed.empty()) {
-                RCUDA_OK(cudaMalloc(&m->d_wtc, sizeof(float) * packed.size()));
-                RCUDA_OK(cudaMemcpy(m->d_wtc, packed.data(), sizeof(float) * packed.size(), cudaMemcpyHostToDevice));
-                for (auto& t : todo) t.dst->w = m->d_wtc + t.at;
-            }
+        if (!pack.todo.empty()) {
+            std::vector<float> packed(pack.n);
+            for (auto& t : pack.todo) rn::pack_conv_weights(host.data() + t.w, t.K, t.N, packed.data() + t.at);
+            RCUDA_OK(cudaMalloc(&m->d_wrn, sizeof(float) * pack.n));
+            RCUDA_OK(cudaMemcpy(m->d_wrn, packed.data(), sizeof(float) * pack.n, cudaMemcpyHostToDevice));
+            for (auto& t : pack.todo) *t.dst = m->d_wrn + t.at;
         }
-        // workspace
+        const bool osnet_family = m->arch == ARCH_OSNET || m->arch == ARCH_LMBN_N || m->arch == ARCH_OSNET_IN;
+        if (osnet_family) setup_osnet_kernels(m, host.data());
+
+        // workspace for one chunk of crops
         if (const char* ce = getenv("BOXMOT_B200_REID_CHUNK")) {
             const int v = atoi(ce);
             if (v >= 8 && v <= 1024) m->chunk = v;
         }
-        // per-crop activations: the stem output (in_h/2 x 64 x c0) or the stage-2 maps (in_h/4 x 32 x c1), whichever is larger
-        auto big_of = [&](int in_h) { return std::max((size_t)(in_h / 2) * 64 * m->c[0], (size_t)(in_h / 4) * 32 * m->c[1]); };
-        auto mid_of = [&](int in_h) { return (size_t)(in_h / 4) * 32 * (m->c[1] / 4); };
-        auto workspace_floats = [&](int in_h, bool lmbn) {   // per crop, every buffer allocated below
-            return (size_t)in_h * IN_W * 3 + 2 * big_of(in_h) + 9 * mid_of(in_h) + 4 * 64 * (size_t)(m->c[3] / 4) +
-                   4 * (size_t)(m->c[3] / 4) + (lmbn ? (size_t)(in_h / 8) * 16 * m->c[2] + (size_t)LMBN_POOLS * LMBN_C : 0);
-        };
         // LMBN_n's maps are 1.5x taller and it keeps the trunk output: fewer crops per chunk, so that a chunk's
         // workspace stays within what an OSNet of the same widths at 256x128 takes for the configured chunk
-        if (m->arch == 3)
-            m->chunk = std::max(8, (int)((size_t)m->chunk * workspace_floats(IN_H, false) / workspace_floats(m->in_h, true)));
+        if (m->arch == ARCH_LMBN_N)
+            m->chunk = std::max(8, (int)((size_t)m->chunk * osnet_workspace(m, IN_H, false).total() / ws.total()));
         const size_t CH = m->chunk;
-        const size_t big = big_of(m->in_h);
-        const size_t mid_max = mid_of(m->in_h);
-        RCUDA_OK(cudaMalloc(&m->blob, sizeof(float) * CH * m->in_h * IN_W * 3));
-        RCUDA_OK(cudaMalloc(&m->bufA, sizeof(float) * CH * big));
-        RCUDA_OK(cudaMalloc(&m->bufB, sizeof(float) * CH * big));
-        RCUDA_OK(cudaMalloc(&m->x1, sizeof(float) * CH * mid_max));
+        auto alloc = [&](float*& p, size_t per_crop) {
+            if (per_crop) RCUDA_OK(cudaMalloc(&p, sizeof(float) * CH * per_crop));
+        };
+        alloc(m->blob, ws.blob);
+        alloc(m->bufA, ws.bufA);
+        alloc(m->bufB, ws.bufB);
+        alloc(m->x1, ws.x1);
         for (int b = 0; b < 4; ++b) {
-            for (int k = 0; k < 2; ++k) RCUDA_OK(cudaMalloc(&m->Y[b][k], sizeof(float) * CH * mid_max));
-            RCUDA_OK(cudaMalloc(&m->sums[b], sizeof(float) * CH * 64 * (m->c[3] / 4)));
+            for (int k = 0; k < 2; ++k) alloc(m->Y[b][k], ws.Y[b][k]);
+            alloc(m->sums[b], ws.sums[b]);
         }
-        RCUDA_OK(cudaMalloc(&m->gates, sizeof(float) * CH * 4 * (m->c[3] / 4)));
-        // arch 4: the instance-norm statistics ({mean, rstd} per crop and channel, 4 floats) live in sums[0], which
-        // holds 16 * c3 >= 4 * C floats per crop and is free whenever they are needed (the stem runs before any block;
-        // a block's norm follows its gates kernel, the last reader of the branch sums).  The one extra buffer is the
-        // conv3 output of an IN_BEFORE_RESIDUAL block whose downsample GEMM writes the block output.
-        if (m->arch == 4)
-            for (const BlockW& b : m->blocks)
-                if (b.in_mode == IN_BEFORE_RESIDUAL && b.has_ds && !m->in_tmp)
-                    RCUDA_OK(cudaMalloc(&m->in_tmp, sizeof(float) * CH * big));
-        if (m->arch == 3) {
-            RCUDA_OK(cudaMalloc(&m->trunk, sizeof(float) * CH * (m->in_h / 8) * 16 * m->c[2]));
-            RCUDA_OK(cudaMalloc(&m->pooled, sizeof(float) * CH * LMBN_POOLS * LMBN_C));
-        }
-        {   // tensor-core path: the default wherever its kernel instances cover the widths (BOXMOT_B200_REID_FP32=1
-            // keeps the float32 CUDA-core kernels of round 1, e.g. for A/B runs)
+        alloc(m->gates, ws.gates);
+        alloc(m->in_tmp, ws.in_tmp);
+        alloc(m->trunk, ws.trunk);
+        alloc(m->pooled, ws.pooled);
+        // tensor-core path: the default wherever its kernel instances cover the widths (BOXMOT_B200_REID_FP32=1
+        // keeps the float32 CUDA-core kernels of round 1, e.g. for A/B runs)
+        if (osnet_family) {
             const char* fe = getenv("BOXMOT_B200_REID_FP32");
             if (!(fe && fe[0] == '1') && tcx::plan_supported(m)) m->tc = tcx::plan_build(m, host.data());
         }
@@ -1906,7 +1929,9 @@ struct Launcher {
         m->prof_cls.push_back(cls);
         RCUDA_OK(cudaEventRecord(e0, st));
     }
+    // counts every launch, so that reid_forward's count and the profile's per-class counts agree
     void end() {
+        ++launches;
         if (!m->profile) return;
         RCUDA_OK(cudaEventRecord(m->prof_ev.back(), st));
     }
@@ -1931,7 +1956,6 @@ struct Launcher {
             tc::k_pointwise_tc<false><<<grid, tc::THREADS, smem, st>>>(t, d_n, off, cap);
         }
         end();
-        ++launches;
     }
     void pointwise(const PwArgs& a) {
         if (m->use_tc && a.w_tc && a.HW % tc::TILE_M == 0) { pointwise_tc(a); return; }
@@ -1953,7 +1977,6 @@ struct Launcher {
             if (a.gates) k_pointwise2<BN, true, 128><<<g, 128, smem, st>>>(a, d_n, off, cap);
             else k_pointwise2<BN, false, 128><<<g, 128, smem, st>>>(a, d_n, off, cap);
             end();
-            ++launches;
             return;
         }
         if (m->pw_v2) {
@@ -1969,14 +1992,12 @@ struct Launcher {
                 k_pointwise2<BN, false><<<grid, 256, smem, st>>>(a, d_n, off, cap);
             }
             end();
-            ++launches;
             return;
         }
         begin(CLS_POINTWISE);
         if (a.gates) k_pointwise<BN, true><<<grid, 256, 0, st>>>(a, d_n, off, cap);
         else k_pointwise<BN, false><<<grid, 256, 0, st>>>(a, d_n, off, cap);
         end();
-        ++launches;
     }
     template <int C, int W, int R, int PPL = 4, int MINB = 2, bool TC = false, int NT = 256>
     void launch_light2(const LightArgs& a, int n_branches) {
@@ -1987,7 +2008,6 @@ struct Launcher {
         begin(CLS_LIGHTCONV);
         k_lightconv2<C, W, R, PPL, MINB, TC, NT><<<dim3(tiles, n_branches, upper), NT, smem, st>>>(a, d_n, off, cap);
         end();
-        ++launches;
     }
     template <int C, int W, int R, int NT>
     void launch_chain(const ChainArgs& a) {
@@ -1997,7 +2017,6 @@ struct Launcher {
         begin(CLS_LIGHTCONV);
         k_lightchain<C, W, R, NT><<<dim3(tiles, 4, upper), NT, smem, st>>>(a, d_n, off, cap);
         end();
-        ++launches;
     }
     // whole-branch LightConv chains for the osnet_x0_25 stage shapes; returns the tile rows used (0 = not covered)
     int light_chain(const ChainArgs& a, int C, int W) {
@@ -2033,14 +2052,12 @@ struct Launcher {
         k_in_stats<<<dim3((C + INS_LANES - 1) / INS_LANES, upper), INS_LANES * INS_STRIPES, 0, st>>>(x, HW, C, d_n, off,
                                                                                                        cap, stats);
         end();
-        ++launches;
     }
     void in_apply(const float* x, const float* residual, float* out, int HW, int C, const float* gamma,
                   const float* beta, const double2* stats, int relu, int cls) {
         begin(cls);
         k_in_apply<<<m->sms * 8, 256, 0, st>>>(x, residual, out, HW, C, gamma, beta, stats, relu, d_n, off, cap);
         end();
-        ++launches;
     }
     // one ResNet convolution (rn::k_conv_tc) over the output pixels of at most `upper` crops
     void conv_tc(const rn::ConvArgs& a) {
@@ -2055,7 +2072,6 @@ struct Launcher {
             rn::k_conv_tc<64><<<grid, rn::THREADS, rn::smem_bytes<64>(), st>>>(a, d_n, off, cap);
         }
         end();
-        ++launches;
     }
     // CLIP: LayerNorm of T token rows per crop (EMBED: token assembly + ln_pre), timed under `gates`
     void vit_layernorm(bool embed, const float* in, const float* pos, const float* g, const float* b, int T, float* out) {
@@ -2064,7 +2080,6 @@ struct Launcher {
         if (embed) vit::k_vit_layernorm<true><<<grid, 256, 0, st>>>(in, pos, g, b, T, d_n, off, cap, out);
         else vit::k_vit_layernorm<false><<<grid, 256, 0, st>>>(in, pos, g, b, T, d_n, off, cap, out);
         end();
-        ++launches;
     }
     // CLIP: multi-head attention of every (crop, head, query block), timed under `lightconv`
     void vit_attention(const float* qkv, int T, float* out) {
@@ -2074,7 +2089,6 @@ struct Launcher {
         vit::k_vit_attention<<<dim3((T + vit::ATT_QB - 1) / vit::ATT_QB, vit::HEADS, upper), vit::ATT_THREADS, smem, st>>>(
             qkv, T, d_n, off, cap, out);
         end();
-        ++launches;
     }
     void light(const LightArgs& a, int n_branches, int threads) {
         if (m->light_v2 && light2(a, n_branches)) return;
@@ -2087,7 +2101,6 @@ struct Launcher {
         begin(CLS_LIGHTCONV);
         k_lightconv<<<dim3(tiles, n_branches, upper), threads, smem, st>>>(a, d_n, off, cap);
         end();
-        ++launches;
     }
 };
 
@@ -2128,16 +2141,21 @@ struct FrameIn {
     const CropDesc* crops;
 };
 
+// Crop staging of one chunk: every crop resized (or letterboxed) to in_h x in_w and normalised into m->blob
+void stage_crops(Launcher& L, const FrameIn& fi) {
+    ReidModel* m = L.m;
+    L.begin(CLS_CROP);
+    k_crop_resize_norm<<<L.upper, 256, 0, L.st>>>(fi.images, fi.image_stride, fi.rows, fi.cols, fi.crops, L.d_n, L.off,
+                                                  L.cap, m->blob, m->preprocess, m->in_h, m->in_w, m->norm);
+    L.end();
+}
+
 // Crop staging, 7x7 stem and 3x3 max pool of one chunk (taps 0-2): the pooled map (in_h/4 x 32 x c0) ends in m->bufB.
 // Returns true when a debug tap stopped the chunk.
 bool run_front(Launcher& L, const FrameIn& fi, StageTaps& stop_here) {
     ReidModel* m = L.m;
     const float* W = m->d_w;
-    L.begin(CLS_CROP);
-    k_crop_resize_norm<<<L.upper, 256, 0, L.st>>>(fi.images, fi.image_stride, fi.rows, fi.cols, fi.crops, L.d_n, L.off,
-                                                  L.cap, m->blob, m->preprocess, m->in_h, IN_W, kImageNetNorm);
-    L.end();
-    ++L.launches;
+    stage_crops(L, fi);
     if (stop_here(m->blob, (size_t)m->in_h * IN_W * 3)) return true;
     if (m->stem_in) {   // conv 7x7 -> IN -> ReLU -> max pool: the norm and the ReLU are applied inside the pool
         const size_t smem = sizeof(float) * ((size_t)((ST_IR * ST_IC * 3 + 3) & ~3) + 147 * 16);
@@ -2146,7 +2164,6 @@ bool run_front(Launcher& L, const FrameIn& fi, StageTaps& stop_here) {
         k_stem<true><<<dim3(m->in_h / 2 / ST_R, L.upper), 256, smem, L.st>>>(m->blob, W + m->stem_w, nullptr, m->c[0],
                                                                              L.d_n, L.off, L.cap, m->bufA, m->in_h);
         L.end();
-        ++L.launches;
         const int HW = (m->in_h / 2) * 64;
         double2* stats = reinterpret_cast<double2*>(m->sums[0]);
         L.in_stats(m->bufA, HW, m->c[0], stats, CLS_MAXPOOL);
@@ -2159,7 +2176,6 @@ bool run_front(Launcher& L, const FrameIn& fi, StageTaps& stop_here) {
         k_maxpool3s2_in<<<m->sms * 8, 256, 0, L.st>>>(m->bufA, m->in_h / 2, 64, m->c[0], W + m->stem_b, W + m->stem_beta,
                                                       stats, L.d_n, L.off, L.cap, m->bufB);
         L.end();
-        ++L.launches;
         return stop_here(m->bufB, (size_t)(m->in_h / 4) * 32 * m->c[0]);
     }
     {
@@ -2169,13 +2185,11 @@ bool run_front(Launcher& L, const FrameIn& fi, StageTaps& stop_here) {
         k_stem<false><<<dim3(m->in_h / 2 / ST_R, L.upper), 256, smem, L.st>>>(m->blob, W + m->stem_w, W + m->stem_b, m->c[0],
                                                                        L.d_n, L.off, L.cap, m->bufA, m->in_h);
         L.end();
-        ++L.launches;
     }
     if (stop_here(m->bufA, (size_t)(m->in_h / 2) * 64 * m->c[0])) return true;
     L.begin(CLS_MAXPOOL);
     k_maxpool3s2<<<m->sms * 8, 256, 0, L.st>>>(m->bufA, m->in_h / 2, 64, m->c[0], L.d_n, L.off, L.cap, m->bufB);
     L.end();
-    ++L.launches;
     return stop_here(m->bufB, (size_t)(m->in_h / 4) * 32 * m->c[0]);
 }
 
@@ -2232,7 +2246,6 @@ void run_osblock(Launcher& L, const BlockW& b, const float* X, float* Xo, int H,
     L.begin(CLS_GATES);
     k_gates<<<L.upper, 128, sizeof(float) * (4 * b.mid + 4 * b.hid), L.st>>>(ga, L.d_n, L.off, L.cap);
     L.end();
-    ++L.launches;
     PwArgs c{};
     for (int br = 0; br < 4; ++br) c.branch[br] = m->Y[br][kDepth[br] & 1];
     c.gates = m->gates; c.mid = b.mid;
@@ -2281,7 +2294,6 @@ void run_transition(Launcher& L, const float* X, float* tmp, float* out, int H, 
     L.begin(CLS_AVGPOOL);
     k_avgpool2<<<m->sms * 4, 256, 0, L.st>>>(tmp, H, Wd, C, L.d_n, L.off, L.cap, out);
     L.end();
-    ++L.launches;
 }
 
 // LMBN_n, one chunk (lmbn_n.py:83-146 in eval).  Taps: 0 crop, 1 stem, 2 pool, 3 backone.2.0, 4 backone.2.1,
@@ -2328,7 +2340,6 @@ void run_lmbn_chunk(Launcher& L, const FrameIn& fi, float* d_out, int out_ld) {
         L.begin(CLS_HEAD);
         k_lmbn_pool<<<L.upper, 256, 0, L.st>>>(pool_src, bh, bw, LMBN_C, br, m->pooled, L.d_n, L.off, L.cap);
         L.end();
-        ++L.launches;
     }
     NeckArgs na{};
     for (int k = 0; k < 5; ++k) { na.w[k] = m->d_w + lm.neck_w[k]; na.b[k] = m->d_w + lm.neck_b[k]; }
@@ -2338,11 +2349,9 @@ void run_lmbn_chunk(Launcher& L, const FrameIn& fi, float* d_out, int out_ld) {
     k_lmbn_neck<<<dim3(LMBN_C / NECK_COLS, 6), 256, NECK_SMEM, L.st>>>(na, m->pooled, fi.crops, L.d_n, L.off, L.cap,
                                                                          d_out, out_ld);
     L.end();
-    ++L.launches;
     L.begin(CLS_HEAD);
     k_l2_normalise<<<L.upper, 256, 0, L.st>>>(fi.crops, L.d_n, L.off, L.cap, d_out, out_ld, m->feat);
     L.end();
-    ++L.launches;
 }
 
 // Bottleneck ResNet, one chunk (resnet.py featuremaps + global average pool).  Taps: 0 crop, 1 stem, 2 pool, then
@@ -2384,7 +2393,6 @@ void run_resnet_chunk(Launcher& L, const FrameIn& fi, float* d_out, int out_ld) 
     k_head<<<L.upper, 256, sizeof(float) * (2 * m->feat + 32), L.st>>>(X, H * Wd, m->feat, nullptr, nullptr, m->feat,
                                                                        fi.crops, L.d_n, L.off, L.cap, d_out, out_ld);
     L.end();
-    ++L.launches;
 }
 
 // CLIP-ReID ViT-B/16, one chunk (clip/model.py VisionTransformer.forward + make_model.py build_transformer, eval,
@@ -2400,11 +2408,7 @@ void run_clip_chunk(Launcher& L, const FrameIn& fi, float* d_out, int out_ld) {
     constexpr int D = vit::D;
     const int T = v.tokens, P = T - 1;
     StageTaps stop_here{m};
-    L.begin(CLS_CROP);
-    k_crop_resize_norm<<<L.upper, 256, 0, L.st>>>(fi.images, fi.image_stride, fi.rows, fi.cols, fi.crops, L.d_n, L.off,
-                                                  L.cap, m->blob, m->preprocess, m->in_h, m->in_w, m->norm);
-    L.end();
-    ++L.launches;
+    stage_crops(L, fi);
     if (stop_here(m->blob, (size_t)m->in_h * m->in_w * 3)) return;
     float* X = m->bufA;          // residual stream [T][768]
     float* Xn = m->bufB;         // LayerNorm output
@@ -2414,7 +2418,6 @@ void run_clip_chunk(Launcher& L, const FrameIn& fi, float* d_out, int out_ld) {
     L.begin(CLS_STEM);
     vit::k_vit_patchify<<<m->sms * 8, 256, 0, L.st>>>(m->blob, m->in_h, m->in_w, L.d_n, L.off, L.cap, hid);
     L.end();
-    ++L.launches;
     auto linear = [&](const float* in, int K, const float* w, const float* bias, const float* residual, int N, int act,
                       float* out, int rows) {
         rn::ConvArgs c{};
@@ -2441,8 +2444,47 @@ void run_clip_chunk(Launcher& L, const FrameIn& fi, float* d_out, int out_ld) {
     vit::k_vit_head<<<L.upper, 256, 0, L.st>>>(X, T, W + v.head_g, W + v.head_b, W + v.head_w, W + v.head_pb, fi.crops,
                                                L.d_n, L.off, L.cap, d_out, out_ld, tap ? Xn : nullptr);
     L.end();
-    ++L.launches;
     if (tap) stop_here(Xn, vit::FEAT);
+}
+
+// MobileNetV2, one chunk: stem -> [expand 1x1 + ReLU6 -> depthwise 3x3 + ReLU6 -> project 1x1 (+ residual)] x 17 ->
+// conv9 -> GAP.  No debug taps.
+void run_mobilenetv2_chunk(Launcher& L, const FrameIn& fi, float* d_out, int out_ld) {
+    ReidModel* m = L.m;
+    const float* W = m->d_w;
+    const MbW& mb = m->mb;
+    stage_crops(L, fi);
+    float* X = m->bufA;
+    float* Xo = m->bufB;
+    L.begin(CLS_STEM);
+    k_stem3<<<m->sms * 8, 256, 0, L.st>>>(m->blob, W + mb.stem_w, W + mb.stem_b, mb.stemp, L.d_n, L.off, L.cap, X);
+    L.end();
+    int H = 128, Wd = 64;
+    for (const MbBlock& b : mb.blocks) {
+        PwArgs e{};
+        e.in = X; e.w = W + b.we; e.bias = W + b.be; e.out = m->x1;
+        e.K = b.cinp; e.N = b.midp; e.HW = H * Wd; e.relu = 2;
+        L.pointwise(e);
+        L.begin(CLS_LIGHTCONV);
+        k_dwconv3<<<m->sms * 8, 256, 0, L.st>>>(m->x1, H, Wd, b.midp, b.stride, W + b.wd, W + b.bd, L.d_n, L.off, L.cap,
+                                                m->Y[0][0]);
+        L.end();
+        H /= b.stride; Wd /= b.stride;
+        PwArgs p{};
+        p.in = m->Y[0][0]; p.w = W + b.wp; p.bias = W + b.bp; p.out = Xo;
+        p.residual = (b.stride == 1 && b.cin == b.cout) ? X : nullptr;
+        p.K = b.midp; p.N = b.coutp; p.HW = H * Wd; p.relu = 0;
+        L.pointwise(p);
+        std::swap(X, Xo);
+    }
+    PwArgs c9{};
+    c9.in = X; c9.w = W + mb.c9w; c9.bias = W + mb.c9b; c9.out = Xo;
+    c9.K = mb.last; c9.N = m->feat; c9.HW = H * Wd; c9.relu = 2;
+    L.pointwise(c9);
+    L.begin(CLS_HEAD);
+    k_head<<<L.upper, 256, sizeof(float) * (2 * m->feat + 32), L.st>>>(Xo, H * Wd, m->feat, nullptr, nullptr, m->feat,
+                                                                       fi.crops, L.d_n, L.off, L.cap, d_out, out_ld);
+    L.end();
 }
 }  // namespace
 
@@ -2450,133 +2492,82 @@ void run_clip_chunk(Launcher& L, const FrameIn& fi, float* d_out, int out_ld) {
 #include "reid_tc_plan.cuh"
 namespace bmb {
 
+namespace {
+// OSNet head: global average pool of x [crops][HW][c3], fc + folded BatchNorm1d, L2 norm into the caller's rows
+void run_osnet_head(Launcher& L, const FrameIn& fi, const float* x, int HW, float* d_out, int out_ld) {
+    ReidModel* m = L.m;
+    const int C = m->c[3];
+    L.begin(CLS_HEAD);
+    k_head<<<L.upper, 256, sizeof(float) * (C + 32 + (256 / C > 0 ? 256 / C : 1) * C), L.st>>>(
+        x, HW, C, m->d_w + m->fcw, m->d_w + m->fcb, m->feat, fi.crops, L.d_n, L.off, L.cap, d_out, out_ld);
+    L.end();
+}
+
+// OSNet and OSNet-AIN / IBN, one chunk (osnet.py:380-405).  Taps: 0 crop, 1 stem, 2 pool, then every OSBlock and
+// transition output in order, conv5 last.
+void run_osnet_chunk(Launcher& L, const FrameIn& fi, float* d_out, int out_ld) {
+    ReidModel* m = L.m;
+    if (m->tc && m->debug_stop != 0 && m->debug_stop != 1) {
+        // tensor-core path: crop staging, stem and max pool are one fused kernel (k_front_tc); diagnostic stops at the
+        // blob / stem tensors (0, 1) run the float32 kernels below instead
+        const tcx::FrontInput tfi{fi.images, fi.image_stride, fi.rows, fi.cols, fi.crops, d_out, out_ld};
+        if (tcx::plan_run(m, tfi, L.d_n, L.off, L.upper, L.st, L)) return;
+        if (!(m->tc->head_fused && m->debug_stop < 0)) run_osnet_head(L, fi, m->tc->c5, 128, d_out, out_ld);
+        return;
+    }
+    StageTaps stop_here{m};
+    if (run_front(L, fi, stop_here)) return;
+    float* X = m->bufB;
+    float* Xo = m->bufA;
+    int H = 64, Wd = 32;
+    for (int s = 0; s < 3; ++s) {
+        for (int j = 0; j < 2; ++j) {
+            const BlockW& b = m->blocks[s * 2 + j];
+            run_osblock(L, b, X, Xo, H, Wd);
+            std::swap(X, Xo);
+            if (stop_here(X, (size_t)H * Wd * b.cout)) return;
+        }
+        if (s < 2) {
+            const int C = m->c[s + 1];
+            run_transition(L, X, Xo, X, H, Wd, C, m->trans_w[s], m->trans_b[s], m->tc_trans[s]);
+            H /= 2; Wd /= 2;
+            if (stop_here(X, (size_t)H * Wd * C)) return;
+        }
+    }
+    const int C = m->c[3];
+    PwArgs p{};
+    p.in = X; p.w = m->d_w + m->c5w; p.bias = m->d_w + m->c5b; p.out = Xo;
+    p.K = C; p.N = C; p.HW = H * Wd; p.relu = 1;
+    p.w_tc = m->tc_c5.w; p.Kpad = m->tc_c5.Kpad; p.Npad = m->tc_c5.Npad;
+    L.pointwise(p);
+    if (stop_here(Xo, (size_t)H * Wd * C)) return;
+    run_osnet_head(L, fi, Xo, H * Wd, d_out, out_ld);
+}
+
+void run_chunk(Launcher& L, const FrameIn& fi, float* d_out, int out_ld) {
+    switch (L.m->arch) {
+        case ARCH_OSNET:
+        case ARCH_OSNET_IN: run_osnet_chunk(L, fi, d_out, out_ld); return;
+        case ARCH_MOBILENETV2: run_mobilenetv2_chunk(L, fi, d_out, out_ld); return;
+        case ARCH_LMBN_N: run_lmbn_chunk(L, fi, d_out, out_ld); return;
+        case ARCH_RESNET: run_resnet_chunk(L, fi, d_out, out_ld); return;
+        case ARCH_CLIP: run_clip_chunk(L, fi, d_out, out_ld); return;
+    }
+}
+}  // namespace
+
 int reid_forward(ReidModel* m, const uint8_t* d_images, size_t image_stride, int rows, int cols,
                  const CropDesc* d_crops, const int* d_ncrops, int max_crops, float* d_out, int out_ld,
                  cudaStream_t st, int first_crop, int last_crop) {
     // [first_crop, last_crop) restricts the call to a slice of the crop list (two models on two streams split a frame)
     if (last_crop < 0 || last_crop > max_crops) last_crop = max_crops;
-    int launches = 0;
-    const float* W = m->d_w;
     m->debug_ptr = nullptr;
-    if (m->arch == 2) {
-        // MobileNetV2: stem -> [expand 1x1 + ReLU6 -> depthwise 3x3 + ReLU6 -> project 1x1 (+ residual)] x 17 -> conv9 -> GAP
-        for (int off = first_crop; off < last_crop; off += m->chunk) {
-            const int upper = (last_crop - off) < m->chunk ? (last_crop - off) : m->chunk;
-            Launcher L{m, d_ncrops, off, upper, upper, st};
-            L.begin(CLS_CROP);
-            k_crop_resize_norm<<<upper, 256, 0, st>>>(d_images, image_stride, rows, cols, d_crops, d_ncrops, off, upper,
-                                                      m->blob, m->preprocess, IN_H, IN_W, kImageNetNorm);
-            L.end();
-            ++L.launches;
-            float* X = m->bufA;
-            float* Xo = m->bufB;
-            L.begin(CLS_STEM);
-            k_stem3<<<m->sms * 8, 256, 0, st>>>(m->blob, W + m->mb_stem_w, W + m->mb_stem_b, m->mb_stemp, d_ncrops, off,
-                                              upper, X);
-            L.end();
-            ++L.launches;
-            int H = 128, Wd = 64;
-            for (const MbBlock& b : m->mb) {
-                PwArgs e{};
-                e.in = X; e.w = W + b.we; e.bias = W + b.be; e.out = m->x1;
-                e.K = b.cinp; e.N = b.midp; e.HW = H * Wd; e.relu = 2;
-                L.pointwise(e);
-                L.begin(CLS_LIGHTCONV);
-                k_dwconv3<<<m->sms * 8, 256, 0, st>>>(m->x1, H, Wd, b.midp, b.stride, W + b.wd, W + b.bd, d_ncrops, off,
-                                                    upper, m->Y[0][0]);
-                L.end();
-                ++L.launches;
-                H /= b.stride; Wd /= b.stride;
-                PwArgs p{};
-                p.in = m->Y[0][0]; p.w = W + b.wp; p.bias = W + b.bp; p.out = Xo;
-                p.residual = (b.stride == 1 && b.cin == b.cout) ? X : nullptr;
-                p.K = b.midp; p.N = b.coutp; p.HW = H * Wd; p.relu = 0;
-                L.pointwise(p);
-                float* t = X; X = Xo; Xo = t;
-            }
-            PwArgs c9{};
-            c9.in = X; c9.w = W + m->mb_c9w; c9.bias = W + m->mb_c9b; c9.out = Xo;
-            c9.K = m->mb_last; c9.N = m->feat; c9.HW = H * Wd; c9.relu = 2;
-            L.pointwise(c9);
-            L.begin(CLS_HEAD);
-            k_head<<<upper, 256, sizeof(float) * (2 * m->feat + 32), st>>>(Xo, H * Wd, m->feat, nullptr, nullptr, m->feat,
-                                                                           d_crops, d_ncrops, off, upper, d_out, out_ld);
-            L.end();
-            ++L.launches;
-            launches += L.launches;
-        }
-        RCUDA_OK(cudaGetLastError());
-        return launches;
-    }
     const FrameIn fi{d_images, image_stride, rows, cols, d_crops};
-    if (m->arch == 3 || m->arch == 5 || m->arch == 6) {
-        for (int off = first_crop; off < last_crop; off += m->chunk) {
-            const int upper = (last_crop - off) < m->chunk ? (last_crop - off) : m->chunk;
-            Launcher L{m, d_ncrops, off, upper, upper, st};
-            if (m->arch == 3) run_lmbn_chunk(L, fi, d_out, out_ld);
-            else if (m->arch == 5) run_resnet_chunk(L, fi, d_out, out_ld);
-            else run_clip_chunk(L, fi, d_out, out_ld);
-            launches += L.launches;
-        }
-        RCUDA_OK(cudaGetLastError());
-        return launches;
-    }
+    int launches = 0;
     for (int off = first_crop; off < last_crop; off += m->chunk) {
         const int upper = (last_crop - off) < m->chunk ? (last_crop - off) : m->chunk;
         Launcher L{m, d_ncrops, off, upper, upper, st};
-        StageTaps stop_here{m};
-        if (m->tc && m->debug_stop != 0 && m->debug_stop != 1) {
-            // tensor-core path: crop staging, stem and max pool are one fused kernel (k_front_tc); diagnostic stops at the
-            // blob / stem tensors (0, 1) run the float32 kernels below instead
-            bool tc_stopped = false;
-            const tcx::FrontInput tfi{d_images, image_stride, rows, cols, d_crops, d_out, out_ld};
-            L.launches += tcx::plan_run(m, tfi, d_ncrops, off, upper, st, &tc_stopped, L);
-            if (!tc_stopped && !(m->tc->head_fused && m->debug_stop < 0)) {
-                const int C = m->c[3];
-                L.begin(CLS_HEAD);
-                k_head<<<upper, 256, sizeof(float) * (C + 32 + (256 / C > 0 ? 256 / C : 1) * C), st>>>(
-                    m->tc->c5, 128, C, W + m->fcw, W + m->fcb, m->feat, d_crops, d_ncrops, off, upper, d_out, out_ld);
-                L.end();
-                ++L.launches;
-            }
-            launches += L.launches;
-            continue;
-        }
-        if (run_front(L, fi, stop_here)) { launches += L.launches; continue; }
-        float* X = m->bufB;
-        float* Xo = m->bufA;
-        int H = 64, Wd = 32;
-        bool stopped = false;
-        for (int s = 0; s < 3 && !stopped; ++s) {
-            for (int j = 0; j < 2 && !stopped; ++j) {
-                const BlockW& b = m->blocks[s * 2 + j];
-                run_osblock(L, b, X, Xo, H, Wd);
-                float* t = X; X = Xo; Xo = t;
-                if (stop_here(X, (size_t)H * Wd * b.cout)) { stopped = true; break; }
-            }
-            if (stopped) break;
-            if (s < 2) {
-                const int C = m->c[s + 1];
-                run_transition(L, X, Xo, X, H, Wd, C, m->trans_w[s], m->trans_b[s], m->tc_trans[s]);
-                H /= 2; Wd /= 2;
-                if (stop_here(X, (size_t)H * Wd * C)) { stopped = true; break; }
-            }
-        }
-        if (!stopped) {
-            const int C = m->c[3];
-            PwArgs p{};
-            p.in = X; p.w = W + m->c5w; p.bias = W + m->c5b; p.out = Xo;
-            p.K = C; p.N = C; p.HW = H * Wd; p.relu = 1;
-            p.w_tc = m->tc_c5.w; p.Kpad = m->tc_c5.Kpad; p.Npad = m->tc_c5.Npad;
-            L.pointwise(p);
-            if (!stop_here(Xo, (size_t)H * Wd * C)) {
-                L.begin(CLS_HEAD);
-                k_head<<<upper, 256, sizeof(float) * (C + 32 + (256 / C > 0 ? 256 / C : 1) * C), st>>>(Xo, H * Wd, C, W + m->fcw, W + m->fcb, m->feat,
-                                                                     d_crops, d_ncrops, off, upper, d_out, out_ld);
-                L.end();
-                ++L.launches;
-            }
-        }
+        run_chunk(L, fi, d_out, out_ld);
         launches += L.launches;
     }
     RCUDA_OK(cudaGetLastError());

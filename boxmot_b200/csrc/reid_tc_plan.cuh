@@ -11,7 +11,7 @@ static const ChainShape kChainShapes[3] = {{16, 16, 32, 64, chain_rows<BMB_CHAIN
                                            {32, 32, 8, 16, chain_rows<BMB_CHAIN_S4>(), LK_CHAIN_S4}};
 
 inline bool plan_supported(const ReidModel* m) {
-    return m->arch == 1 && m->c[0] == 16 && m->c[1] == 64 && m->c[2] == 96 && m->c[3] == 128;
+    return m->arch == ARCH_OSNET && m->c[0] == 16 && m->c[1] == 64 && m->c[2] == 96 && m->c[3] == 128;
 }
 
 Plan* plan_build(ReidModel* m, const float* hw) {
@@ -365,13 +365,13 @@ Plan* plan_build(ReidModel* m, const float* hw) {
     return P;
 }
 
-// Replays the plan for one chunk of crops (the stem output of that chunk is in m->bufA).  Returns launches made.
+// Replays the plan for one chunk of crops (the stem output of that chunk is in m->bufA).  Returns true when a debug tap
+// stopped the chunk.
 struct FrontInput { const uint8_t* images; size_t image_stride; int rows, cols; const CropDesc* crops; float* out; int out_ld; };
 
 template <class Prof>
-int plan_run(ReidModel* m, const FrontInput& fi, const int* d_n, int off, int upper, cudaStream_t st, bool* stopped, Prof& prof) {
+bool plan_run(ReidModel* m, const FrontInput& fi, const int* d_n, int off, int upper, cudaStream_t st, Prof& prof) {
     Plan* P = m->tc;
-    int launches = 0;
     for (const Launch& L : (m->debug_stop >= 0 ? P->launches_dbg : P->launches)) {
         prof.begin(L.cls);
         switch (L.kind) {
@@ -403,12 +403,10 @@ int plan_run(ReidModel* m, const FrontInput& fi, const int* d_n, int off, int up
                 break;
         }
         prof.end();
-        ++launches;
         if (m->debug_stop == 50 && L.kind == LK_FRONT) {
             m->debug_ptr = P->dbg_crop;
             m->debug_floats_per_crop = (size_t)256 * 128 * 3;
-            *stopped = true;
-            return launches;
+            return true;
         }
         if (m->debug_stop >= 0 && L.stage_after == m->debug_stop) {
             if (L.stage_after == 11) {
@@ -419,11 +417,10 @@ int plan_run(ReidModel* m, const FrontInput& fi, const int* d_n, int off, int up
                 m->debug_ptr = P->dbg;
                 m->debug_floats_per_crop = (size_t)L.dbg_HW * L.dbg_C;
             }
-            *stopped = true;
-            return launches;
+            return true;
         }
     }
-    return launches;
+    return false;
 }
 
 }  // namespace tcx
