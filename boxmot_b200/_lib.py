@@ -158,6 +158,10 @@ SYMBOLS = {
                                         POINTER(c_float)]),
     "boxmot_b200_vit_layernorm": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
     "boxmot_b200_vit_attention": (c_int, [c_void_p, c_int, c_int, c_void_p]),
+    "boxmot_b200_mlfn_group_conv": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
+                                            c_void_p, c_void_p]),
+    "boxmot_b200_mlfn_fsm": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p,
+                                     c_int, c_void_p, c_void_p, c_void_p]),
     "boxmot_b200_device_count": (c_int, []),
     "boxmot_b200_reid_debug_stage": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_void_p,
                                              c_int, POINTER(c_int)]),

@@ -404,6 +404,14 @@ int boxmot_b200_vit_layernorm(const float* x, int rows, const float* gamma, cons
 int boxmot_b200_vit_attention(const float* qkv, int n, int tokens, float* out) {
     return guard([&] { standalone_vit_attention(qkv, n, tokens, out); });
 }
+int boxmot_b200_mlfn_group_conv(const float* in, int n, int h, int w, int c, int gw, int stride, const float* weight,
+                                const float* bias, const float* gates, float* out) {
+    return guard([&] { standalone_mlfn_group_conv(in, n, h, w, c, gw, stride, weight, bias, gates, out); });
+}
+int boxmot_b200_mlfn_fsm(const float* x, int n, int h, int w, int c, const float* w1, const float* b1, int f0,
+                         const float* w2, const float* b2, int f1, const float* w3, const float* b3, float* out) {
+    return guard([&] { standalone_mlfn_fsm(x, n, h, w, c, w1, b1, f0, w2, b2, f1, w3, b3, out); });
+}
 int boxmot_b200_cosine_cost(const float* a, int rows, const float* b, int cols, int dim, double* out) {
     return guard([&] { standalone_cosine(a, rows, b, cols, dim, out); });
 }

@@ -250,5 +250,9 @@ void standalone_resnet_conv(const float* in0, int n, int h0, int w0, int c0, int
                             int relu, float* out, float* elapsed_ms);
 void standalone_vit_layernorm(const float* x, int rows, const float* gamma, const float* beta, float* out);
 void standalone_vit_attention(const float* qkv, int n, int tokens, float* out);
+void standalone_mlfn_group_conv(const float* in, int n, int h, int w, int c, int gw, int stride, const float* weight,
+                                const float* bias, const float* gates, float* out);
+void standalone_mlfn_fsm(const float* x, int n, int h, int w, int c, const float* w1, const float* b1, int f0,
+                         const float* w2, const float* b2, int f1, const float* w3, const float* b3, float* out);
 
 }  // namespace bmb

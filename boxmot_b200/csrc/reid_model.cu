@@ -24,6 +24,7 @@
 
 #include "engine.h"
 #include "pointwise_tc.cuh"
+#include "mlfn_kernels.cuh"
 #include "resnet_tc.cuh"
 #include "vit_tc.cuh"
 
@@ -1360,6 +1361,18 @@ struct LmbnW {
 struct RnConv { size_t b = 0; const float* w = nullptr; };
 struct RnBlock { int cin, width, cout, stride; RnConv c1, c2, c3; };
 
+// MLFN (arch 7): per MLFNBlock the shapes, the tensor-core packings of its dense 1x1 convolutions (FSM layers 1 and 2,
+// fm_conv1, fm_conv3, the downsample), and the offsets in d_w of the FSM's last layer and of the grouped 3x3
+struct MlfnBlock {
+    int cin, cout, mid, gw, f0, f1, stride, ds;
+    RnConv fsm1, fsm2, c1, c3, down;
+    size_t fsm3w = 0, fsm3b = 0, gcw = 0, gcb = 0;
+};
+struct MlfnW {
+    std::vector<MlfnBlock> blocks;
+    RnConv fc_x, fc_s;
+};
+
 // CLIP-ReID ViT-B/16 (arch 6): per residual block the offsets in d_w of its LayerNorm parameters and biases, and the
 // tensor-core packings of its four linear layers
 struct VitLayer {
@@ -1381,6 +1394,7 @@ enum ReidArch {
     ARCH_OSNET_IN = 4,   // OSNet with instance norms (AIN / IBN)
     ARCH_RESNET = 5,
     ARCH_CLIP = 6,       // CLIP-ReID ViT-B/16
+    ARCH_MLFN = 7,
 };
 
 struct ReidModel {
@@ -1395,7 +1409,8 @@ struct ReidModel {
     LmbnW lm;
     MbW mb;
     std::vector<RnBlock> rn;      // ResNet Bottlenecks, layer1.0 .. layer4.last
-    float* d_wrn = nullptr;       // ResNet / CLIP: every GEMM's weights packed by rn::pack_conv_weights
+    MlfnW ml;
+    float* d_wrn = nullptr;       // ResNet / CLIP / MLFN: every GEMM's weights packed by rn::pack_conv_weights
     int c[4] = {0, 0, 0, 0};
     int feat = 0;
     float* d_w = nullptr;
@@ -1498,6 +1513,11 @@ void read_header(ReidModel* m, const int32_t* hdr) {
             m->norm = CropNorm{{0.5f, 0.5f, 0.5f}, {0.5f, 0.5f, 0.5f}};
             m->vit.layers = hdr[4];
             m->vit.tokens = 1 + hdr[11] * hdr[12];
+            return;
+        case ARCH_MLFN:
+            if (hdr[3] != 64 || hdr[4] != 2048 || hdr[5] != mlfn::GROUPS || hdr[6] != mlfn::BLOCKS || m->feat != mlfn::FEAT)
+                throw std::runtime_error("bad MLFN blob header (only groups 32, channels 64-2048, 16 blocks, 1024-d)");
+            m->c[0] = 64;
             return;
         case ARCH_RESNET:
             m->c[0] = 64;
@@ -1715,6 +1735,59 @@ Workspace layout_resnet(ReidModel* m, const int32_t* hdr, BlobCursor& take, Wgmm
     return ws;
 }
 
+// ---- MLFN (reid/backbones/mlfn.py): stem, 16 MLFNBlocks, fc_x / fc_s head ----
+Workspace layout_mlfn(ReidModel* m, BlobCursor& take, WgmmaPack& pack) {
+    static const int kStages[4][4] = {{3, 256, 128, 64}, {4, 512, 256, 128}, {6, 1024, 512, 128}, {3, 2048, 512, 128}};
+    m->stem_w = take((size_t)147 * 64);
+    m->stem_b = take(64);
+    auto conv = [&](RnConv& c, int K, int N) {
+        const size_t w = take((size_t)K * N);
+        c.b = take(N);
+        pack.add(c.w, w, K, N);
+    };
+    MlfnW& ml = m->ml;
+    ml.blocks.reserve(mlfn::BLOCKS);   // `pack` keeps pointers into the blocks
+    int cin = 64;
+    for (int s = 0; s < 4; ++s)
+        for (int j = 0; j < kStages[s][0]; ++j) {
+            MlfnBlock b{};
+            b.cin = cin; b.cout = kStages[s][1]; b.mid = b.cout / 2; b.gw = b.mid / mlfn::GROUPS;
+            b.f0 = kStages[s][2]; b.f1 = kStages[s][3];
+            b.stride = (j == 0 && s > 0) ? 2 : 1;
+            b.ds = b.cin != b.cout || b.stride > 1;
+            ml.blocks.push_back(b);
+            MlfnBlock& r = ml.blocks.back();
+            conv(r.fsm1, r.cin, r.f0);
+            conv(r.fsm2, r.f0, r.f1);
+            r.fsm3w = take((size_t)r.f1 * mlfn::GROUPS);
+            r.fsm3b = take(mlfn::GROUPS);
+            conv(r.c1, r.cin, r.mid);
+            r.gcw = take((size_t)9 * r.gw * r.mid);
+            r.gcb = take(r.mid);
+            conv(r.c3, r.mid, r.cout);
+            if (r.ds) conv(r.down, r.cin, r.cout);
+            cin = r.cout;
+        }
+    conv(ml.fc_x, 2048, mlfn::FEAT);
+    conv(ml.fc_s, mlfn::SHAT, mlfn::FEAT);
+    // per crop: the staged crop, two block maps as large as the stem output / stage 1's 64x32x256, fm_conv1's output
+    // (at most 64x32x256, the first block of stage 2), fm_conv2's (at most 64x32x128), and rows for the pooled map
+    // (2048), s_hat (512), the FSM hidden layers (512, 128), fc_x and x + s (1024 each): 1.94 M floats, below the
+    // 2.36 M an OSNet_x1_0 chunk takes per crop, so the chunk keeps its size.  The downsample writes the block output
+    // buffer, which fm_conv3 then reads as its residual and overwrites in place.
+    Workspace ws;
+    ws.blob = (size_t)m->in_h * m->in_w * 3;
+    ws.bufA = ws.bufB = (size_t)128 * 64 * 64;
+    ws.x1 = (size_t)64 * 32 * 256;
+    ws.Y[0][0] = (size_t)64 * 32 * 128;
+    ws.pooled = 2048;
+    ws.gates = mlfn::SHAT;
+    ws.sums[0] = 512;
+    ws.sums[1] = 128;
+    ws.sums[2] = ws.sums[3] = mlfn::FEAT;
+    return ws;
+}
+
 // ---- CLIP-ReID ViT-B/16 (reid/backbones/clip): patch embedding, ln_pre, 12 residual attention blocks, head ----
 Workspace layout_clip(ReidModel* m, BlobCursor& take, WgmmaPack& pack) {
     constexpr int D = vit::D;
@@ -1798,7 +1871,7 @@ ReidModel* reid_load(const char* path) {
     if (!f) throw std::runtime_error(std::string("cannot open ReID blob: ") + path);
     int32_t hdr[16];
     f.read(reinterpret_cast<char*>(hdr), sizeof(hdr));
-    if (!f || (uint32_t)hdr[0] != BLOB_MAGIC || hdr[1] != 1 || hdr[2] < ARCH_OSNET || hdr[2] > ARCH_CLIP)
+    if (!f || (uint32_t)hdr[0] != BLOB_MAGIC || hdr[1] != 1 || hdr[2] < ARCH_OSNET || hdr[2] > ARCH_MLFN)
         throw std::runtime_error("not a version-1 .b200reid blob (export it with boxmot_b200.weights.export_blob)");
     ReidModel* m = new ReidModel();
     try {
@@ -1819,6 +1892,7 @@ ReidModel* reid_load(const char* path) {
             case ARCH_MOBILENETV2: ws = layout_mobilenetv2(m, table, take); break;
             case ARCH_RESNET: ws = layout_resnet(m, hdr, take, pack); break;
             case ARCH_CLIP: ws = layout_clip(m, take, pack); break;
+            case ARCH_MLFN: ws = layout_mlfn(m, take, pack); break;
             default: ws = layout_osnet(m, hdr, take); break;
         }
         if (take.o != n_floats) throw std::runtime_error("ReID blob size does not match its header");
@@ -2064,13 +2138,49 @@ struct Launcher {
         const int BN = rn::tile_n(a.N);
         const dim3 grid((unsigned)(((size_t)upper * a.Ho * a.Wo + rn::BM - 1) / rn::BM), (unsigned)(a.N / BN));
         begin(a.k0 == 3 ? CLS_LIGHTCONV : CLS_POINTWISE);
-        if (BN == 128) {
+        if (a.relu == 3) {   // relu(residual + relu(acc + bias)): MLFN's fm_conv3
+            if (BN == 128) {
+                RCUDA_OK(cudaFuncSetAttribute(rn::k_conv_tc<128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rn::smem_bytes<128>()));
+                rn::k_conv_tc<128, true><<<grid, rn::THREADS, rn::smem_bytes<128>(), st>>>(a, d_n, off, cap);
+            } else {
+                RCUDA_OK(cudaFuncSetAttribute(rn::k_conv_tc<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rn::smem_bytes<64>()));
+                rn::k_conv_tc<64, true><<<grid, rn::THREADS, rn::smem_bytes<64>(), st>>>(a, d_n, off, cap);
+            }
+        } else if (BN == 128) {
             RCUDA_OK(cudaFuncSetAttribute(rn::k_conv_tc<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rn::smem_bytes<128>()));
             rn::k_conv_tc<128><<<grid, rn::THREADS, rn::smem_bytes<128>(), st>>>(a, d_n, off, cap);
         } else {
             RCUDA_OK(cudaFuncSetAttribute(rn::k_conv_tc<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rn::smem_bytes<64>()));
             rn::k_conv_tc<64><<<grid, rn::THREADS, rn::smem_bytes<64>(), st>>>(a, d_n, off, cap);
         }
+        end();
+    }
+    // MLFN: grouped 3x3 (+ bias, ReLU, gate) of x [crops][H][Wd][C], group width gw, timed under `lightconv`
+    void group_conv(const float* x, int H, int Wd, int C, int gw, int stride, const float* w, const float* bias,
+                    const float* gates, float* out) {
+        const int Ho = (H - 1) / stride + 1, Wo = (Wd - 1) / stride + 1;
+        const size_t items = (size_t)upper * Ho * (Wo / 4) * (C / 4);
+        const unsigned grid = (unsigned)((items + 255) / 256);
+        begin(CLS_LIGHTCONV);
+        switch (gw) {
+            case 4: mlfn::k_group_conv<4><<<grid, 256, 0, st>>>(x, H, Wd, C, stride, w, bias, gates, mlfn::SHAT, d_n, off, cap, out); break;
+            case 8: mlfn::k_group_conv<8><<<grid, 256, 0, st>>>(x, H, Wd, C, stride, w, bias, gates, mlfn::SHAT, d_n, off, cap, out); break;
+            case 16: mlfn::k_group_conv<16><<<grid, 256, 0, st>>>(x, H, Wd, C, stride, w, bias, gates, mlfn::SHAT, d_n, off, cap, out); break;
+            case 32: mlfn::k_group_conv<32><<<grid, 256, 0, st>>>(x, H, Wd, C, stride, w, bias, gates, mlfn::SHAT, d_n, off, cap, out); break;
+            default: throw std::runtime_error("MLFN grouped convolution: group width must be 4, 8, 16 or 32");
+        }
+        end();
+    }
+    // MLFN: average pool of x [crops][HW][C] into rows [crops][C], timed under `gates`
+    void mlfn_gap(const float* x, int HW, int C, float* out) {
+        begin(CLS_GATES);
+        mlfn::k_mlfn_gap<<<dim3(C / 64, upper), 256, 0, st>>>(x, HW, C, d_n, off, cap, out);
+        end();
+    }
+    // MLFN: the FSM's last layer + sigmoid into columns col .. col + 31 of s_hat, timed under `gates`
+    void mlfn_gate(const float* h, int F1, const float* w, const float* b, float* s_hat, int col) {
+        begin(CLS_GATES);
+        mlfn::k_mlfn_gate<<<(upper + 7) / 8, 256, 0, st>>>(h, F1, w, b, d_n, off, cap, s_hat, col);
         end();
     }
     // CLIP: LayerNorm of T token rows per crop (EMBED: token assembly + ln_pre), timed under `gates`
@@ -2447,6 +2557,57 @@ void run_clip_chunk(Launcher& L, const FrameIn& fi, float* d_out, int out_ld) {
     if (tap) stop_here(Xn, vit::FEAT);
 }
 
+// MLFN, one chunk (mlfn.py MLFN.forward, eval).  Taps: 0 crop, 1 stem, 2 pool, 3 + i after MLFNBlock i, 19 s_hat
+// ([512]), 20 the head row v = 0.5 (x + s) before the L2 norm ([1024]).  Per block: the FSM (average pool of x, two
+// 1x1 layers + ReLU on k_conv_tc over a [crops] x 1 map, the last layer + sigmoid into s_hat), fm_conv1 (+ ReLU), the
+// grouped 3x3 with the block's gates, the strided downsample (first block of a stage) into the output buffer, and
+// fm_conv3 with the relu(residual + relu(.)) epilogue.  The head pools the last map, runs fc_x (+ ReLU), and fc_s with
+// the same epilogue and fc_x's output as the residual (x >= 0, so the outer ReLU leaves x + s), then halves,
+// L2-normalises and scatters.  Timing classes as for ResNet: 1x1 convolutions `pointwise_gemm`, the grouped 3x3
+// `lightconv`, pools and gates `gates`, the head's last kernel `head`.
+void run_mlfn_chunk(Launcher& L, const FrameIn& fi, float* d_out, int out_ld) {
+    ReidModel* m = L.m;
+    const float* W = m->d_w;
+    const MlfnW& ml = m->ml;
+    StageTaps stop_here{m};
+    if (run_front(L, fi, stop_here)) return;
+    auto conv1x1 = [&](const float* in, int h, int w, int cin, int stride, const RnConv& cv, int N, const float* res,
+                       int act, float* out) {
+        rn::ConvArgs c{};
+        c.in0 = in; c.H0 = h; c.W0 = w; c.C0 = cin; c.k0 = 1; c.s0 = stride;
+        c.w = cv.w; c.bias = W + cv.b; c.residual = res; c.out = out;
+        c.Ho = (h - 1) / stride + 1; c.Wo = (w - 1) / stride + 1; c.N = N; c.relu = act;
+        L.conv_tc(c);
+    };
+    float* X = m->bufB;
+    float* Xo = m->bufA;
+    int H = IN_H / 4, Wd = IN_W / 4, col = 0;
+    for (const MlfnBlock& b : ml.blocks) {
+        L.mlfn_gap(X, H * Wd, b.cin, m->pooled);
+        conv1x1(m->pooled, 1, 1, b.cin, 1, b.fsm1, b.f0, nullptr, 1, m->sums[0]);
+        conv1x1(m->sums[0], 1, 1, b.f0, 1, b.fsm2, b.f1, nullptr, 1, m->sums[1]);
+        L.mlfn_gate(m->sums[1], b.f1, W + b.fsm3w, W + b.fsm3b, m->gates, col);
+        conv1x1(X, H, Wd, b.cin, 1, b.c1, b.mid, nullptr, 1, m->x1);
+        L.group_conv(m->x1, H, Wd, b.mid, b.gw, b.stride, W + b.gcw, W + b.gcb, m->gates + col, m->Y[0][0]);
+        const int Ho = H / b.stride, Wo = Wd / b.stride;
+        if (b.ds) conv1x1(X, H, Wd, b.cin, b.stride, b.down, b.cout, nullptr, 0, Xo);
+        conv1x1(m->Y[0][0], Ho, Wo, b.mid, 1, b.c3, b.cout, b.ds ? Xo : X, 3, Xo);
+        std::swap(X, Xo);
+        H = Ho; Wd = Wo; col += mlfn::GROUPS;
+        if (stop_here(X, (size_t)H * Wd * b.cout)) return;
+    }
+    if (stop_here(m->gates, mlfn::SHAT)) return;
+    L.mlfn_gap(X, H * Wd, 2048, m->pooled);
+    conv1x1(m->pooled, 1, 1, 2048, 1, ml.fc_x, mlfn::FEAT, nullptr, 1, m->sums[2]);
+    conv1x1(m->gates, 1, 1, mlfn::SHAT, 1, ml.fc_s, mlfn::FEAT, m->sums[2], 3, m->sums[3]);
+    const bool tap = m->debug_stop == stop_here.idx;
+    L.begin(CLS_HEAD);
+    mlfn::k_mlfn_head<<<L.upper, 256, 0, L.st>>>(m->sums[3], fi.crops, L.d_n, L.off, L.cap, d_out, out_ld,
+                                                 tap ? m->sums[2] : nullptr);
+    L.end();
+    if (tap) stop_here(m->sums[2], mlfn::FEAT);
+}
+
 // MobileNetV2, one chunk: stem -> [expand 1x1 + ReLU6 -> depthwise 3x3 + ReLU6 -> project 1x1 (+ residual)] x 17 ->
 // conv9 -> GAP.  No debug taps.
 void run_mobilenetv2_chunk(Launcher& L, const FrameIn& fi, float* d_out, int out_ld) {
@@ -2552,6 +2713,7 @@ void run_chunk(Launcher& L, const FrameIn& fi, float* d_out, int out_ld) {
         case ARCH_LMBN_N: run_lmbn_chunk(L, fi, d_out, out_ld); return;
         case ARCH_RESNET: run_resnet_chunk(L, fi, d_out, out_ld); return;
         case ARCH_CLIP: run_clip_chunk(L, fi, d_out, out_ld); return;
+        case ARCH_MLFN: run_mlfn_chunk(L, fi, d_out, out_ld); return;
     }
 }
 }  // namespace
@@ -2684,9 +2846,10 @@ void standalone_resnet_conv(const float* in0, int n, int h0, int w0, int c0, int
                             int w1, int c1, int stride1, const float* w, int N, const float* bias, const float* residual,
                             int relu, float* out, float* elapsed_ms) {
     if (n <= 0 || h0 <= 0 || w0 <= 0 || c0 <= 0 || c0 % rn::KC || (k != 1 && k != 3) || stride < 1 || N <= 0 || N % 64 ||
-        c1 < 0 || c1 % rn::KC || (c1 && (!in1 || h1 <= 0 || w1 <= 0 || stride1 < 1)) || relu < 0 || relu > 2)
+        c1 < 0 || c1 % rn::KC || (c1 && (!in1 || h1 <= 0 || w1 <= 0 || stride1 < 1)) || relu < 0 || relu > 3 ||
+        (relu == 3 && !residual))
         throw std::runtime_error("n, h0, w0 > 0, k in {1, 3}, c0 and c1 multiples of 32, N a multiple of 64, relu in "
-                                 "{0, 1, 2} required");
+                                 "{0, 1, 2, 3} (3 with a residual) required");
     const int pad = k / 2, Ho = (h0 + 2 * pad - k) / stride + 1, Wo = (w0 + 2 * pad - k) / stride + 1;
     if (c1 && ((Ho - 1) * stride1 >= h1 || (Wo - 1) * stride1 >= w1))
         throw std::runtime_error("the second operand does not cover the output grid");
@@ -2791,6 +2954,102 @@ void standalone_vit_attention(const float* qkv, int n, int tokens, float* out) {
         L.vit_attention(dq, tokens, dO);
         RCUDA_OK(cudaGetLastError());
         RCUDA_OK(cudaMemcpy(out, dO, sizeof(float) * nout, cudaMemcpyDeviceToHost));
+    } catch (...) {
+        cleanup();
+        throw;
+    }
+    cleanup();
+}
+
+// Standalone MLFN grouped 3x3 (mlfn::k_group_conv) on host arrays: in (n,h,w,c) NHWC, w [9][gw][c], bias [c],
+// gates (n,32) -> out (n,Ho,Wo,c) = relu(conv + bias) * gates[n][channel / gw].
+void standalone_mlfn_group_conv(const float* in, int n, int h, int w, int c, int gw, int stride, const float* weight,
+                                const float* bias, const float* gates, float* out) {
+    const int Ho = h > 0 && stride > 0 ? (h - 1) / stride + 1 : 0, Wo = w > 0 && stride > 0 ? (w - 1) / stride + 1 : 0;
+    if (n <= 0 || h <= 0 || w <= 0 || (stride != 1 && stride != 2) || Wo % 4 || (gw != 4 && gw != 8 && gw != 16 && gw != 32) ||
+        c != gw * mlfn::GROUPS)
+        throw std::runtime_error("n, h, w > 0, stride 1 or 2, output width a multiple of 4, gw in {4, 8, 16, 32} and "
+                                 "c = 32 gw required");
+    const size_t n_in = (size_t)n * h * w * c, n_out = (size_t)n * Ho * Wo * c, n_w = (size_t)9 * gw * c;
+    float *dx = nullptr, *dw = nullptr, *db = nullptr, *dg = nullptr, *dO = nullptr;
+    int* dn = nullptr;
+    auto cleanup = [&] { cudaFree(dx); cudaFree(dw); cudaFree(db); cudaFree(dg); cudaFree(dO); cudaFree(dn); };
+    try {
+        std::vector<float> g((size_t)n * mlfn::SHAT, 0.f);   // the kernel reads gate rows of s_hat's width
+        for (int i = 0; i < n; ++i) std::memcpy(&g[(size_t)i * mlfn::SHAT], gates + (size_t)i * mlfn::GROUPS, sizeof(float) * mlfn::GROUPS);
+        RCUDA_OK(cudaMalloc(&dx, sizeof(float) * n_in));
+        RCUDA_OK(cudaMalloc(&dw, sizeof(float) * n_w));
+        RCUDA_OK(cudaMalloc(&db, sizeof(float) * c));
+        RCUDA_OK(cudaMalloc(&dg, sizeof(float) * g.size()));
+        RCUDA_OK(cudaMalloc(&dO, sizeof(float) * n_out));
+        RCUDA_OK(cudaMalloc(&dn, sizeof(int)));
+        RCUDA_OK(cudaMemcpy(dx, in, sizeof(float) * n_in, cudaMemcpyHostToDevice));
+        RCUDA_OK(cudaMemcpy(dw, weight, sizeof(float) * n_w, cudaMemcpyHostToDevice));
+        RCUDA_OK(cudaMemcpy(db, bias, sizeof(float) * c, cudaMemcpyHostToDevice));
+        RCUDA_OK(cudaMemcpy(dg, g.data(), sizeof(float) * g.size(), cudaMemcpyHostToDevice));
+        RCUDA_OK(cudaMemcpy(dn, &n, sizeof(int), cudaMemcpyHostToDevice));
+        ReidModel fake;
+        Launcher L{&fake, dn, 0, n, n, nullptr};
+        L.group_conv(dx, h, w, c, gw, stride, dw, db, dg, dO);
+        RCUDA_OK(cudaGetLastError());
+        RCUDA_OK(cudaMemcpy(out, dO, sizeof(float) * n_out, cudaMemcpyDeviceToHost));
+    } catch (...) {
+        cleanup();
+        throw;
+    }
+    cleanup();
+}
+
+// Standalone MLFN factor-selection module on host arrays, as run_mlfn_chunk launches it: x (n,h,w,c) NHWC ->
+// out (n,32) = sigmoid(relu(relu(GAP(x) w1 + b1) w2 + b2) w3 + b3), w1 [c][f0], w2 [f0][f1], w3 [f1][32] K-major.
+void standalone_mlfn_fsm(const float* x, int n, int h, int w, int c, const float* w1, const float* b1, int f0,
+                         const float* w2, const float* b2, int f1, const float* w3, const float* b3, float* out) {
+    if (n <= 0 || h <= 0 || w <= 0 || c <= 0 || c % 64 || f0 <= 0 || f0 % 64 || f1 <= 0 || f1 % 64)
+        throw std::runtime_error("n, h, w > 0 and c, f0, f1 positive multiples of 64 required");
+    const size_t n_x = (size_t)n * h * w * c;
+    std::vector<float*> bufs;
+    int* dn = nullptr;
+    auto cleanup = [&] { for (float* p : bufs) cudaFree(p); cudaFree(dn); };
+    auto upload = [&](const float* src, size_t count) {
+        float* d = nullptr;
+        RCUDA_OK(cudaMalloc(&d, sizeof(float) * count));
+        bufs.push_back(d);
+        if (src) RCUDA_OK(cudaMemcpy(d, src, sizeof(float) * count, cudaMemcpyHostToDevice));
+        return d;
+    };
+    try {
+        std::vector<float> p1(2 * (size_t)c * f0), p2(2 * (size_t)f0 * f1);
+        rn::pack_conv_weights(w1, c, f0, p1.data());
+        rn::pack_conv_weights(w2, f0, f1, p2.data());
+        float* dx = upload(x, n_x);
+        float* dp1 = upload(p1.data(), p1.size());
+        float* db1 = upload(b1, f0);
+        float* dp2 = upload(p2.data(), p2.size());
+        float* db2 = upload(b2, f1);
+        float* dw3 = upload(w3, (size_t)f1 * mlfn::GROUPS);
+        float* db3 = upload(b3, mlfn::GROUPS);
+        float* pooled = upload(nullptr, (size_t)n * c);
+        float* h1 = upload(nullptr, (size_t)n * f0);
+        float* h2 = upload(nullptr, (size_t)n * f1);
+        float* s_hat = upload(nullptr, (size_t)n * mlfn::SHAT);
+        RCUDA_OK(cudaMalloc(&dn, sizeof(int)));
+        RCUDA_OK(cudaMemcpy(dn, &n, sizeof(int), cudaMemcpyHostToDevice));
+        ReidModel fake;
+        Launcher L{&fake, dn, 0, n, n, nullptr};
+        auto dense = [&](const float* in, int K, const float* pw, const float* b, int N, float* o) {
+            rn::ConvArgs a{};
+            a.in0 = in; a.H0 = 1; a.W0 = 1; a.C0 = K; a.k0 = 1; a.s0 = 1;
+            a.w = pw; a.bias = b; a.out = o; a.Ho = 1; a.Wo = 1; a.N = N; a.relu = 1;
+            L.conv_tc(a);
+        };
+        L.mlfn_gap(dx, h * w, c, pooled);
+        dense(pooled, c, dp1, db1, f0, h1);
+        dense(h1, f0, dp2, db2, f1, h2);
+        L.mlfn_gate(h2, f1, dw3, db3, s_hat, 0);
+        RCUDA_OK(cudaGetLastError());
+        std::vector<float> s((size_t)n * mlfn::SHAT);
+        RCUDA_OK(cudaMemcpy(s.data(), s_hat, sizeof(float) * s.size(), cudaMemcpyDeviceToHost));
+        for (int i = 0; i < n; ++i) std::memcpy(out + (size_t)i * mlfn::GROUPS, &s[(size_t)i * mlfn::SHAT], sizeof(float) * mlfn::GROUPS);
     } catch (...) {
         cleanup();
         throw;

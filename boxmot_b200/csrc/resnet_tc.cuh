@@ -17,7 +17,9 @@
 //     (cp.async.bulk, completing on the stage's mbarrier) brings a chunk's hi and lo halves;
 //   * chunk k + 1 is in flight while the MMAs of chunk k (and the tail of chunk k - 1) run; every wgmma is issued
 //     unconditionally, with BN a template parameter.
-// Epilogue: bias, optional residual, then relu = 0 none / 1 ReLU / 2 QuickGELU, float2 stores into NHWC [M][N].
+// Epilogue: bias, optional residual, then relu = 0 none / 1 ReLU / 2 QuickGELU, float2 stores into NHWC [M][N].  The
+// RELU_RES instances (relu = 3) compute relu(residual + relu(acc + bias)) instead: MLFN's fm_conv3, whose ReLU comes
+// before the residual add.  They are separate instances so that the default ones keep their code.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -43,7 +45,7 @@ struct ConvArgs {
     float* out;              // [M][N]
     int H0, W0, C0, k0, s0;  // k0 in {1, 3} (pad k0 / 2), stride s0
     int H1, W1, C1, s1;
-    int Ho, Wo, N, relu;     // relu: 0 none, 1 ReLU, 2 QuickGELU
+    int Ho, Wo, N, relu;     // relu: 0 none, 1 ReLU, 2 QuickGELU, 3 relu(residual + relu(.)) (RELU_RES instances)
 };
 
 // canonical (no swizzle, K-major) offset in floats of element (row, k) in a block whose K extent is KC
@@ -60,7 +62,7 @@ constexpr size_t smem_bytes() {
     return sizeof(float) * (size_t)STAGES * (2 * BM * KC + 2 * BN * KC) + 128;
 }
 
-template <int BN>
+template <int BN, bool RELU_RES = false>
 __global__ void __launch_bounds__(THREADS, 1) k_conv_tc(const ConvArgs a, const int* __restrict__ d_n, int off, int cap) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     __shared__ __align__(8) uint64_t bar[STAGES];
@@ -186,6 +188,12 @@ __global__ void __launch_bounds__(THREADS, 1) k_conv_tc(const ConvArgs a, const 
             const int c = 8 * i + cq;
             const float2 b = *reinterpret_cast<const float2*>(a.bias + n0 + c);
             float2 o = make_float2(acc[4 * i + 2 * h] + b.x, acc[4 * i + 2 * h + 1] + b.y);
+            if constexpr (RELU_RES) {
+                const float2 r = *reinterpret_cast<const float2*>(res + c);
+                o.x = fmaxf(r.x + fmaxf(o.x, 0.f), 0.f); o.y = fmaxf(r.y + fmaxf(o.y, 0.f), 0.f);
+                *reinterpret_cast<float2*>(dst + c) = o;
+                continue;
+            }
             if (res) {
                 const float2 r = *reinterpret_cast<const float2*>(res + c);
                 o.x += r.x; o.y += r.y;

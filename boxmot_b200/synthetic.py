@@ -302,6 +302,66 @@ def make_resnet_state(depth: int = 50, seed: int = 0, with_fc512: bool = False, 
     return sd
 
 
+# MLFN (reid/backbones/mlfn.py, groups 32, channels 64 / 256 / 512 / 1024 / 2048, embed_dim 1024): per stage the
+# MLFNBlock count, the output width and the FSM widths; the stride-2 grouped 3x3 sits on the first block of stages 2-4
+MLFN_STAGES = ((3, 256, (128, 64)), (4, 512, (256, 128)), (6, 1024, (512, 128)), (3, 2048, (512, 128)))
+MLFN_GROUPS = 32
+MLFN_FEAT = 1024
+
+
+def mlfn_blocks():
+    """[(cin, cout, stride, (fsm0, fsm1), has_downsample)] of the 16 MLFNBlocks in `feature` order."""
+    out, cin = [], 64
+    for s, (n, cout, fsm) in enumerate(MLFN_STAGES):
+        for j in range(n):
+            stride = 2 if (j == 0 and s > 0) else 1
+            out.append((cin, cout, stride, fsm, cin != cout or stride > 1))
+            cin = cout
+    return out
+
+
+def mlfn_layout():
+    """[(parameter prefix, kind, shape)] of the reference's `mlfn` in module order, kind "conv" (weight only), "convb"
+    (weight and bias) or "bn" (BatchNorm2d of `shape[0]` channels).  `classifier` is not listed."""
+    g = MLFN_GROUPS
+    out = [("conv1", "convb", (64, 3, 7, 7)), ("bn1", "bn", (64,))]
+    for i, (cin, cout, _, (f0, f1), ds) in enumerate(mlfn_blocks()):
+        b, mid = f"feature.{i}", cout // 2
+        out += [(b + ".fm_conv1", "conv", (mid, cin, 1, 1)), (b + ".fm_bn1", "bn", (mid,)),
+                (b + ".fm_conv2", "conv", (mid, mid // g, 3, 3)), (b + ".fm_bn2", "bn", (mid,)),
+                (b + ".fm_conv3", "conv", (cout, mid, 1, 1)), (b + ".fm_bn3", "bn", (cout,)),
+                (b + ".fsm.1", "convb", (f0, cin, 1, 1)), (b + ".fsm.2", "bn", (f0,)),
+                (b + ".fsm.4", "convb", (f1, f0, 1, 1)), (b + ".fsm.5", "bn", (f1,)),
+                (b + ".fsm.7", "convb", (g, f1, 1, 1)), (b + ".fsm.8", "bn", (g,))]
+        if ds:
+            out += [(b + ".downsample.0", "conv", (cout, cin, 1, 1)), (b + ".downsample.1", "bn", (cout,))]
+    out += [("fc_x.0", "conv", (MLFN_FEAT, 2048, 1, 1)), ("fc_x.1", "bn", (MLFN_FEAT,)),
+            ("fc_s.0", "conv", (MLFN_FEAT, 16 * g, 1, 1)), ("fc_s.1", "bn", (MLFN_FEAT,))]
+    return out
+
+
+def make_mlfn_state(seed: int = 0, num_classes: int = 751):
+    """Seeded state dict with the parameter names of the reference's `mlfn(num_classes)` (loads with strict=True).
+    BatchNorm statistics are randomised so folding is exercised, the convolution biases of the stem and the FSM are
+    non-zero, and fm_conv3 starts small so the residual stream stays O(1-10) through the 16 blocks."""
+    import torch
+
+    g = torch.Generator().manual_seed(seed)
+    sd = {}
+    conv, bn, _ = _osnet_makers(g, sd)
+    for name, kind, shape in mlfn_layout():
+        if kind == "bn":
+            bn(name, shape[0])
+            continue
+        groups = MLFN_GROUPS if name.endswith("fm_conv2") else 1
+        conv(name, shape[0], shape[1] * groups, shape[2], groups=groups, gain=0.1 if name.endswith("fm_conv3") else 1.0)
+        if kind == "convb":
+            sd[name + ".bias"] = 0.1 * torch.randn(shape[0], generator=g)
+    sd["classifier.weight"] = 0.01 * torch.randn(num_classes, MLFN_FEAT, generator=g)
+    sd["classifier.bias"] = torch.zeros(num_classes)
+    return sd
+
+
 def make_clip_state(seed: int = 0, vehicle: bool = False, num_classes: int = 751, extras: bool = True):
     """Seeded state dict with the key set of the reference's CLIP-ReID `build_transformer` (ViT-B/16: image_encoder.*,
     bottleneck.*, bottleneck_proj.*, classifier.*, classifier_proj.*); vehicle=True gives the 257-row positional table

@@ -26,6 +26,8 @@ the 2048-d feature in word 7; its layout is listed above `fold_resnet`.
 Arch 6 (CLIP-ReID ViT-B/16, `fold_clip`) records width, layers, heads, the 512-d projection and the 1280-d feature
 in words 3-7, the input height / width in words 9-10 and the patch grid in words 11-12; its layout is listed above
 `fold_clip`.
+Arch 7 (MLFN, `fold_mlfn`) records the stem width, the last block width, the groups, the block count and the 1024-d
+feature in words 3-7; its layout is listed above `fold_mlfn`.
 All 1x1 weights are stored K-major ([cin][cout]) so a thread owning consecutive output channels loads
 consecutive floats; every tensor is zero-padded to a multiple of 4 floats (16-byte aligned float4 loads).
 """
@@ -47,6 +49,8 @@ ARCH_OSNET_IN = 4
 ARCH_RESNET = 5
 RESNET_FEAT = 2048
 ARCH_CLIP = 6
+ARCH_MLFN = 7
+MLFN_FEAT = 1024
 BRANCHES = (("conv2a", 1), ("conv2b", 2), ("conv2c", 3), ("conv2d", 4))
 EPS = 1e-5
 
@@ -455,6 +459,67 @@ def fold_clip(sd, name=None):
     return dims, (16 * gh, 16 * gw), (gh, gw), out
 
 
+# MLFN (arch 7): mlfn of reid/backbones/mlfn.py (groups 32, channels 64 / 256 / 512 / 1024 / 2048, embed_dim 1024).
+# Header words 3-7 hold the stem width 64, the last block width 2048, the 32 groups, the 16 blocks and the 1024-d
+# feature.  Every 1x1 weight is K-major ([cin][cout]) with its BatchNorm (and conv bias) folded; the arrays are
+#     stem      W[147][64] (k = (kh*7+kw)*3 + ci), b[64]          (bn1 folded, conv1's bias included)
+#     per MLFNBlock i (cin, cout, mid = cout / 2, group width gw = mid / 32, fsm widths f0, f1):
+#         fsm       W[cin][f0], b[f0]; W[f0][f1], b[f1]; W[f1][32], b[32]   (fsm.1 / .4 / .7 with .2 / .5 / .8 folded)
+#         fm_conv1  W[cin][mid], b[mid]
+#         fm_conv2  W[9][gw][mid] (element (tap, i, c) weighs input channel (c / gw) gw + i), b[mid]
+#         fm_conv3  W[mid][cout], b[cout]
+#         downsample (first block of a stage) W[cin][cout], b[cout]
+#     fc_x      W[2048][1024], b[1024];   fc_s  W[512][1024], b[1024]
+def _mlfn_ignored(k: str) -> bool:
+    return k.startswith("classifier.") or k.endswith("num_batches_tracked")
+
+
+def is_mlfn(sd) -> bool:
+    return "feature.0.fm_conv1.weight" in sd
+
+
+def fold_mlfn(sd) -> List[np.ndarray]:
+    """MLFN state dict -> arrays of the arch-7 blob.  Only the reference's `mlfn` with its default groups, channels and
+    embed_dim is supported: any key or shape that differs from it, apart from `classifier.*` and
+    `num_batches_tracked`, raises a ValueError naming the keys."""
+    from .synthetic import MLFN_GROUPS, mlfn_blocks, mlfn_layout
+
+    keys = {k for k in sd if not _mlfn_ignored(k)}
+    want = {}
+    for name, kind, shape in mlfn_layout():
+        if kind == "bn":
+            for p in ("weight", "bias", "running_mean", "running_var"):
+                want[f"{name}.{p}"] = shape
+        else:
+            want[name + ".weight"] = shape
+            if kind == "convb":
+                want[name + ".bias"] = shape[:1]
+    bad_shape = sorted(k for k in keys & set(want) if tuple(sd[k].shape) != want[k])[:4]
+    if keys != set(want) or bad_shape:
+        extra, missing = sorted(keys - set(want))[:4], sorted(set(want) - keys)[:4]
+        raise ValueError(f"not an MLFN state dict (unexpected keys {extra}, missing keys {missing}, unexpected shapes "
+                         f"{bad_shape}); only mlfn with groups 32, channels 64-2048 and embed_dim 1024 is supported")
+    w = _np(sd["conv1.weight"])   # [64][3][7][7]
+    scale, shift = _bn_fold(sd, "bn1")
+    out: List[np.ndarray] = [(w * scale[:, None, None, None]).transpose(2, 3, 1, 0).reshape(147, 64),
+                             _np(sd["conv1.bias"]) * scale + shift]
+    for i, (cin, cout, _, _, ds) in enumerate(mlfn_blocks()):
+        b, mid = f"feature.{i}", cout // 2
+        gw = mid // MLFN_GROUPS
+        for conv, bn in (("fsm.1", "fsm.2"), ("fsm.4", "fsm.5"), ("fsm.7", "fsm.8")):
+            out += list(_pw(sd, f"{b}.{conv}", f"{b}.{bn}"))
+        out += list(_pw(sd, b + ".fm_conv1", b + ".fm_bn1"))
+        w2 = _np(sd[b + ".fm_conv2.weight"])   # [mid][gw][3][3]
+        sc, sh = _bn_fold(sd, b + ".fm_bn2")
+        out += [(w2 * sc[:, None, None, None]).transpose(2, 3, 1, 0).reshape(9 * gw, mid), sh]
+        out += list(_pw(sd, b + ".fm_conv3", b + ".fm_bn3"))
+        if ds:
+            out += list(_pw(sd, b + ".downsample.0", b + ".downsample.1"))
+    out += list(_pw(sd, "fc_x.0", "fc_x.1"))
+    out += list(_pw(sd, "fc_s.0", "fc_s.1"))
+    return out
+
+
 def _pad4(n: int) -> int:
     return (n + 3) // 4 * 4
 
@@ -545,9 +610,12 @@ def export_blob(weights, out_path=None) -> Path:
     elif is_resnet(sd):
         blocks, arrays = fold_resnet(sd)
         arch, dims = ARCH_RESNET, blocks + [RESNET_FEAT]
+    elif is_mlfn(sd):
+        arrays = fold_mlfn(sd)
+        arch, dims = ARCH_MLFN, [64, 2048, 32, 16, MLFN_FEAT]
     else:
-        raise ValueError("only OSNet, OSNet-AIN, OSNet-IBN, MobileNetV2, LMBN_n, ResNet50 / ResNet101 and CLIP-ReID "
-                         "ViT-B/16 state dicts are implemented on the B200 ReID path")
+        raise ValueError("only OSNet, OSNet-AIN, OSNet-IBN, MobileNetV2, LMBN_n, ResNet50 / ResNet101, CLIP-ReID "
+                         "ViT-B/16 and MLFN state dicts are implemented on the B200 ReID path")
     # every tensor starts on a 16-byte boundary (the kernels read weights as float4)
     padded = []
     for a in arrays:

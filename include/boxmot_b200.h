@@ -416,7 +416,8 @@ BOXMOT_B200_API int boxmot_b200_instance_norm(const float* x, int n, int h, int 
 /* One convolution of the ResNet50 / ResNet101 path (wgmma tf32x3 implicit GEMM) on host arrays, NHWC float32:
  * out (n,Ho,Wo,out_c) = act(conv(in0) + conv1x1(in1) + bias (+ residual, optional)), act = none when relu = 0, ReLU
  * when relu = 1, QuickGELU x * sigmoid(1.702 x) when relu = 2 (CLIP's MLP; a CLIP linear layer is a 1x1 convolution
- * over h0 = tokens, w0 = 1).  in0 (n,h0,w0,c0) is read by a k x k kernel (k 1 or 3, pad k/2) at `stride`; in1 (n,h1,w1,c1), optional (c1 = 0
+ * over h0 = tokens, w0 = 1). relu = 3 gives relu(residual + relu(conv(in0) + conv1x1(in1) + bias)) (MLFN's fm_conv3, whose
+ * ReLU precedes the residual add; the residual is then required).  in0 (n,h0,w0,c0) is read by a k x k kernel (k 1 or 3, pad k/2) at `stride`; in1 (n,h1,w1,c1), optional (c1 = 0
  * for none), by a 1x1 kernel at `stride1` over the same output grid (the fused conv3 + downsample of a stage's first
  * Bottleneck).  w is (k*k*c0 + c1, out_c) K-major, k index (kh*k + kw)*c0 + ci then the c1 channels; c0 and c1
  * multiples of 32, out_c a multiple of 64.  elapsed_ms (optional) receives the average device time of 10 launches. */
@@ -431,13 +432,26 @@ BOXMOT_B200_API int boxmot_b200_vit_layernorm(const float* x, int rows, const fl
  * columns 64h..64h+63 of each, with q already scaled by 1/8; out (n,tokens,768) = softmax(q k^T) v per head, heads
  * interleaved.  1 <= tokens <= 288. */
 BOXMOT_B200_API int boxmot_b200_vit_attention(const float* qkv, int n, int tokens, float* out);
+/* Grouped 3x3 convolution of the MLFN path (fm_conv2, 32 groups, pad 1) on host arrays, NHWC float32: in (n,h,w,c)
+ * with c = 32 gw, group width gw in {4, 8, 16, 32}, stride 1 or 2, output width a multiple of 4; weight (9,gw,c),
+ * element (kh*3 + kw, i, co) weighing input channel (co / gw) gw + i; out (n,Ho,Wo,c) = relu(conv + bias) *
+ * gates[n][co / gw] with gates (n,32). */
+BOXMOT_B200_API int boxmot_b200_mlfn_group_conv(const float* in, int n, int h, int w, int c, int gw, int stride,
+                                                const float* weight, const float* bias, const float* gates, float* out);
+/* Factor-selection module of the MLFN path on host arrays: x (n,h,w,c) NHWC float32 -> out (n,32) = sigmoid(relu(
+ * relu(mean_hw(x) w1 + b1) w2 + b2) w3 + b3), w1 (c,f0), w2 (f0,f1), w3 (f1,32) K-major; c, f0, f1 multiples of 64. */
+BOXMOT_B200_API int boxmot_b200_mlfn_fsm(const float* x, int n, int h, int w, int c, const float* w1, const float* b1,
+                                         int f0, const float* w2, const float* b2, int f1, const float* w3,
+                                         const float* b3, float* out);
 BOXMOT_B200_API int boxmot_b200_device_count(void);
 /* Diagnostics for the ReID kernels: run the forward up to `stage` (0 input blob, 1 stem, 2 max-pool, 3..10 the
  * six OSBlocks and two transitions in order, 11 conv5) and copy that NHWC float32 tensor of the n crops out.  For
  * OSNet-AIN / OSNet-IBN the stem tap is the map after the instance norm and the ReLU.  For ResNet50 / ResNet101: 0 input
  * blob, 1 stem, 2 max-pool, 3 + i the output of Bottleneck i (layer1.0 first).  For CLIP ViT-B/16: 0 input blob
  * (256 x 128 or 256 x 256), 1 patch embedding (patches x 768), 2 ln_pre (tokens x 768), 3 + l the output of residual
- * block l, 15 the head row before the L2 normalisation (1280). */
+ * block l, 15 the head row before the L2 normalisation (1280).  For MLFN: 0 input blob, 1 stem, 2 max-pool, 3 + i the
+ * output of MLFNBlock i (i = 0 .. 15), 19 s_hat (the 16 blocks' gates, 512), 20 the head row v = 0.5 (x + s) before
+ * the L2 normalisation (1024). */
 BOXMOT_B200_API int boxmot_b200_reid_debug_stage(void* reid_handle, const float* boxes_xyxy, int n_boxes,
                                                  const uint8_t* image_data, int image_rows, int image_cols,
                                                  int stage, float* out, int out_capacity_floats,
