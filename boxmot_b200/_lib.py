@@ -162,6 +162,20 @@ SYMBOLS = {
                                             c_void_p, c_void_p]),
     "boxmot_b200_mlfn_fsm": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p,
                                      c_int, c_void_p, c_void_p, c_void_p]),
+    "boxmot_b200_f32_pointwise": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int,
+                                          c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_void_p]),
+    "boxmot_b200_f32_lightconv": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
+                                          c_int, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p]),
+    "boxmot_b200_f32_lightchain": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int,
+                                           c_int, c_void_p, c_int, c_void_p, c_int, c_void_p]),
+    "boxmot_b200_f32_gates": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
+                                      c_void_p, c_int, c_int, c_void_p, c_int]),
+    "boxmot_b200_f32_head": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int,
+                                     c_void_p, c_int, c_int]),
+    "boxmot_b200_f32_map": (c_int, [c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int,
+                                    c_int, c_void_p, c_int]),
+    "boxmot_b200_f32_lmbn_head": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p,
+                                          c_int, c_void_p, c_int, c_int]),
     "boxmot_b200_device_count": (c_int, []),
     "boxmot_b200_reid_debug_stage": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_void_p,
                                              c_int, POINTER(c_int)]),

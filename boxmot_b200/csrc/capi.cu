@@ -412,6 +412,47 @@ int boxmot_b200_mlfn_fsm(const float* x, int n, int h, int w, int c, const float
                          const float* w2, const float* b2, int f1, const float* w3, const float* b3, float* out) {
     return guard([&] { standalone_mlfn_fsm(x, n, h, w, c, w1, b1, f0, w2, b2, f1, w3, b3, out); });
 }
+int boxmot_b200_f32_pointwise(const float* a, const float* branches, const float* gates, int n, int hw, int k, int mid,
+                              const float* w, int nout, const float* bias, const float* residual, int relu, int off,
+                              int count, float* out, int out_floats, int* instance) {
+    return guard([&] {
+        standalone_f32_pointwise(a, branches, gates, n, hw, k, mid, w, nout, bias, residual, relu, off, count, out, out_floats, instance);
+    });
+}
+int boxmot_b200_f32_lightconv(const float* in, int nb, int n, int h, int w, int c, const float* wpw, const float* wdw,
+                              const float* bias, int off, int count, float* out, int out_stride, float* sums,
+                              int sums_stride, int* instance) {
+    return guard([&] {
+        standalone_f32_lightconv(in, nb, n, h, w, c, wpw, wdw, bias, off, count, out, out_stride, sums, sums_stride, instance);
+    });
+}
+int boxmot_b200_f32_lightchain(const float* in, int n, int h, int w, int c, const float* wpw, const float* wdw,
+                               const float* bias, int off, int count, float* out, int out_stride, float* sums,
+                               int sums_stride, int* instance) {
+    return guard([&] {
+        standalone_f32_lightchain(in, n, h, w, c, wpw, wdw, bias, off, count, out, out_stride, sums, sums_stride, instance);
+    });
+}
+int boxmot_b200_f32_gates(const float* sums, int n, int tiles, int c, int hid, int hw, const float* w1, const float* b1,
+                          const float* w2, const float* b2, int off, int count, float* gates, int gates_floats) {
+    return guard([&] {
+        standalone_f32_gates(sums, n, tiles, c, hid, hw, w1, b1, w2, b2, off, count, gates, gates_floats);
+    });
+}
+int boxmot_b200_f32_head(const float* x, int n, int hw, int c, const float* wfc, const float* bfc, int feat,
+                         const int* rows, int off, int count, float* out, int out_floats, int out_ld) {
+    return guard([&] { standalone_f32_head(x, n, hw, c, wfc, bfc, feat, rows, off, count, out, out_floats, out_ld); });
+}
+int boxmot_b200_f32_map(int op, const float* in, int n, int h, int w, int c, int stride, const float* weight,
+                        const float* bias, int off, int count, float* out, int out_floats) {
+    return guard([&] { standalone_f32_map(op, in, n, h, w, c, stride, weight, bias, off, count, out, out_floats); });
+}
+int boxmot_b200_f32_lmbn_head(const float* x, int n, int h, int w, const float* neck, const int* rows, int off,
+                              int count, float* pooled, int pooled_floats, float* out, int out_floats, int out_ld) {
+    return guard([&] {
+        standalone_f32_lmbn_head(x, n, h, w, neck, rows, off, count, pooled, pooled_floats, out, out_floats, out_ld);
+    });
+}
 int boxmot_b200_cosine_cost(const float* a, int rows, const float* b, int cols, int dim, double* out) {
     return guard([&] { standalone_cosine(a, rows, b, cols, dim, out); });
 }

@@ -254,5 +254,22 @@ void standalone_mlfn_group_conv(const float* in, int n, int h, int w, int c, int
                                 const float* bias, const float* gates, float* out);
 void standalone_mlfn_fsm(const float* x, int n, int h, int w, int c, const float* w1, const float* b1, int f0,
                          const float* w2, const float* b2, int f1, const float* w3, const float* b3, float* out);
+void standalone_f32_pointwise(const float* a, const float* branches, const float* gates, int n, int hw, int k, int mid,
+                              const float* w, int nout, const float* bias, const float* residual, int relu, int off,
+                              int count, float* out, int out_floats, int* instance);
+void standalone_f32_lightconv(const float* in, int nb, int n, int h, int w, int c, const float* wpw, const float* wdw,
+                              const float* bias, int off, int count, float* out, int out_stride, float* sums,
+                              int sums_stride, int* instance);
+void standalone_f32_lightchain(const float* in, int n, int h, int w, int c, const float* wpw, const float* wdw,
+                               const float* bias, int off, int count, float* out, int out_stride, float* sums,
+                               int sums_stride, int* instance);
+void standalone_f32_gates(const float* sums, int n, int tiles, int c, int hid, int hw, const float* w1, const float* b1,
+                          const float* w2, const float* b2, int off, int count, float* gates, int gates_floats);
+void standalone_f32_head(const float* x, int n, int hw, int c, const float* wfc, const float* bfc, int feat,
+                         const int* rows, int off, int count, float* out, int out_floats, int out_ld);
+void standalone_f32_map(int op, const float* in, int n, int h, int w, int c, int stride, const float* weight,
+                        const float* bias, int off, int count, float* out, int out_floats);
+void standalone_f32_lmbn_head(const float* x, int n, int h, int w, const float* neck, const int* rows, int off,
+                              int count, float* pooled, int pooled_floats, float* out, int out_floats, int out_ld);
 
 }  // namespace bmb

@@ -1992,6 +1992,10 @@ struct Launcher {
     int off, cap, upper;  // upper = host-side bound on crops in this chunk (grid sizing)
     cudaStream_t st;
     int launches = 0;
+    // the kernel instance of the last pointwise / LightConv launch (standalone entry points report it):
+    // pointwise {BN, threads, gated, 0}; LightConv {kind, C, W, R} with kind 1 k_lightconv, 2 k_lightconv2,
+    // 3 k_lightchain (R = chain tile rows)
+    int inst[4] = {0, 0, 0, 0};
 
     void begin(int cls) {
         if (!m->profile) return;
@@ -2048,11 +2052,13 @@ struct Launcher {
             constexpr size_t smem = 2 * sizeof(float4) * (4 * (BMs + 2) + 16 * BN / 4);
             dim3 g((unsigned)((Mmax + BMs - 1) / BMs), (unsigned)((a.N + BN - 1) / BN));
             begin(CLS_POINTWISE);
+            inst[0] = BN; inst[1] = 128; inst[2] = a.gates != nullptr; inst[3] = 0;
             if (a.gates) k_pointwise2<BN, true, 128><<<g, 128, smem, st>>>(a, d_n, off, cap);
             else k_pointwise2<BN, false, 128><<<g, 128, smem, st>>>(a, d_n, off, cap);
             end();
             return;
         }
+        inst[0] = BN; inst[1] = 256; inst[2] = a.gates != nullptr; inst[3] = 0;
         if (m->pw_v2) {
             constexpr size_t smem = 2 * sizeof(float4) * (4 * (BM + 2) + 16 * BN / 4);
             begin(CLS_POINTWISE);
@@ -2080,6 +2086,7 @@ struct Launcher {
         if (smem > 48 * 1024)
             RCUDA_OK(cudaFuncSetAttribute(k_lightconv2<C, W, R, PPL, MINB, TC, NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         begin(CLS_LIGHTCONV);
+        inst[0] = 2; inst[1] = C; inst[2] = W; inst[3] = R;
         k_lightconv2<C, W, R, PPL, MINB, TC, NT><<<dim3(tiles, n_branches, upper), NT, smem, st>>>(a, d_n, off, cap);
         end();
     }
@@ -2089,6 +2096,7 @@ struct Launcher {
         constexpr size_t smem = chain_smem_bytes<C, W, R, NT>();
         RCUDA_OK(cudaFuncSetAttribute(k_lightchain<C, W, R, NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         begin(CLS_LIGHTCONV);
+        inst[0] = 3; inst[1] = C; inst[2] = W; inst[3] = R;
         k_lightchain<C, W, R, NT><<<dim3(tiles, 4, upper), NT, smem, st>>>(a, d_n, off, cap);
         end();
     }
@@ -2200,8 +2208,77 @@ struct Launcher {
             qkv, T, d_n, off, cap, out);
         end();
     }
+    // ChannelGate of an OSBlock: one CTA per crop
+    void gates(const GateArgs& a) {
+        begin(CLS_GATES);
+        k_gates<<<upper, 128, sizeof(float) * (4 * a.C + 4 * a.hid), st>>>(a, d_n, off, cap);
+        end();
+    }
+    // head of OSNet (fc + ReLU) and of ResNet / MobileNetV2 (wfc null: the pooled map is the embedding), L2-normalised
+    // into the caller's rows
+    void head(const float* x, int HW, int C, const float* wfc, const float* bfc, int feat, const CropDesc* crops,
+              float* out, int out_ld) {
+        const int groups = 256 / C > 0 ? 256 / C : 1;
+        begin(CLS_HEAD);
+        k_head<<<upper, 256, sizeof(float) * (C + 32 + (size_t)groups * C), st>>>(x, HW, C, wfc, bfc, feat, crops, d_n,
+                                                                                   off, cap, out, out_ld);
+        end();
+    }
+    // 7x7 stride-2 stem of the OSNet family (raw: the instance-norm stem's bare convolution)
+    void stem(bool raw, const float* blob, const float* w, const float* bias, int C0, float* out, int in_h) {
+        const size_t smem = sizeof(float) * ((size_t)((ST_IR * ST_IC * 3 + 3) & ~3) + 147 * 16);
+        const dim3 grid(in_h / 2 / ST_R, upper);
+        begin(CLS_STEM);
+        if (raw) {
+            RCUDA_OK(cudaFuncSetAttribute(k_stem<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            k_stem<true><<<grid, 256, smem, st>>>(blob, w, nullptr, C0, d_n, off, cap, out, in_h);
+        } else {
+            RCUDA_OK(cudaFuncSetAttribute(k_stem<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            k_stem<false><<<grid, 256, smem, st>>>(blob, w, bias, C0, d_n, off, cap, out, in_h);
+        }
+        end();
+    }
+    void maxpool(const float* in, int H, int W, int C, float* out) {
+        begin(CLS_MAXPOOL);
+        k_maxpool3s2<<<m->sms * 8, 256, 0, st>>>(in, H, W, C, d_n, off, cap, out);
+        end();
+    }
+    void avgpool(const float* in, int H, int W, int C, float* out) {
+        begin(CLS_AVGPOOL);
+        k_avgpool2<<<m->sms * 4, 256, 0, st>>>(in, H, W, C, d_n, off, cap, out);
+        end();
+    }
+    // MobileNetV2: 3x3 stride-2 stem and the depthwise 3x3 of an inverted-residual block
+    void stem3(const float* blob, const float* w, const float* bias, int C0, float* out) {
+        begin(CLS_STEM);
+        k_stem3<<<m->sms * 8, 256, 0, st>>>(blob, w, bias, C0, d_n, off, cap, out);
+        end();
+    }
+    void dwconv3(const float* in, int H, int W, int C, int stride, const float* w9c, const float* bias, float* out) {
+        begin(CLS_LIGHTCONV);
+        k_dwconv3<<<m->sms * 8, 256, 0, st>>>(in, H, W, C, stride, w9c, bias, d_n, off, cap, out);
+        end();
+    }
+    // LMBN_n head: the poolings of one branch output, the neck GEMMs of the chunk, the row L2 normalisation
+    void lmbn_pool(const float* x, int H, int W, int which, float* pooled) {
+        begin(CLS_HEAD);
+        k_lmbn_pool<<<upper, 256, 0, st>>>(x, H, W, LMBN_C, which, pooled, d_n, off, cap);
+        end();
+    }
+    void lmbn_neck(const NeckArgs& na, const float* pooled, const CropDesc* crops, float* out, int out_ld) {
+        RCUDA_OK(cudaFuncSetAttribute(k_lmbn_neck, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)NECK_SMEM));
+        begin(CLS_HEAD);
+        k_lmbn_neck<<<dim3(LMBN_C / NECK_COLS, 6), 256, NECK_SMEM, st>>>(na, pooled, crops, d_n, off, cap, out, out_ld);
+        end();
+    }
+    void l2_normalise(const CropDesc* crops, float* out, int out_ld, int feat) {
+        begin(CLS_HEAD);
+        k_l2_normalise<<<upper, 256, 0, st>>>(crops, d_n, off, cap, out, out_ld, feat);
+        end();
+    }
     void light(const LightArgs& a, int n_branches, int threads) {
         if (m->light_v2 && light2(a, n_branches)) return;
+        inst[0] = 1; inst[1] = a.C; inst[2] = a.W; inst[3] = a.R;
         const int tiles = (a.H + a.R - 1) / a.R;
         const int n_grp = threads / (a.C / 4);
         const size_t smem = sizeof(float) * ((size_t)(a.R + 2) * (a.W + 2) * a.C + (size_t)a.C * a.C + 9 * a.C +
@@ -2268,12 +2345,7 @@ bool run_front(Launcher& L, const FrameIn& fi, StageTaps& stop_here) {
     stage_crops(L, fi);
     if (stop_here(m->blob, (size_t)m->in_h * IN_W * 3)) return true;
     if (m->stem_in) {   // conv 7x7 -> IN -> ReLU -> max pool: the norm and the ReLU are applied inside the pool
-        const size_t smem = sizeof(float) * ((size_t)((ST_IR * ST_IC * 3 + 3) & ~3) + 147 * 16);
-        RCUDA_OK(cudaFuncSetAttribute(k_stem<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        L.begin(CLS_STEM);
-        k_stem<true><<<dim3(m->in_h / 2 / ST_R, L.upper), 256, smem, L.st>>>(m->blob, W + m->stem_w, nullptr, m->c[0],
-                                                                             L.d_n, L.off, L.cap, m->bufA, m->in_h);
-        L.end();
+        L.stem(true, m->blob, W + m->stem_w, nullptr, m->c[0], m->bufA, m->in_h);
         const int HW = (m->in_h / 2) * 64;
         double2* stats = reinterpret_cast<double2*>(m->sums[0]);
         L.in_stats(m->bufA, HW, m->c[0], stats, CLS_MAXPOOL);
@@ -2288,18 +2360,9 @@ bool run_front(Launcher& L, const FrameIn& fi, StageTaps& stop_here) {
         L.end();
         return stop_here(m->bufB, (size_t)(m->in_h / 4) * 32 * m->c[0]);
     }
-    {
-        const size_t smem = sizeof(float) * ((size_t)((ST_IR * ST_IC * 3 + 3) & ~3) + 147 * 16);
-        RCUDA_OK(cudaFuncSetAttribute(k_stem<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        L.begin(CLS_STEM);
-        k_stem<false><<<dim3(m->in_h / 2 / ST_R, L.upper), 256, smem, L.st>>>(m->blob, W + m->stem_w, W + m->stem_b, m->c[0],
-                                                                       L.d_n, L.off, L.cap, m->bufA, m->in_h);
-        L.end();
-    }
+    L.stem(false, m->blob, W + m->stem_w, W + m->stem_b, m->c[0], m->bufA, m->in_h);
     if (stop_here(m->bufA, (size_t)(m->in_h / 2) * 64 * m->c[0])) return true;
-    L.begin(CLS_MAXPOOL);
-    k_maxpool3s2<<<m->sms * 8, 256, 0, L.st>>>(m->bufA, m->in_h / 2, 64, m->c[0], L.d_n, L.off, L.cap, m->bufB);
-    L.end();
+    L.maxpool(m->bufA, m->in_h / 2, 64, m->c[0], m->bufB);
     return stop_here(m->bufB, (size_t)(m->in_h / 4) * 32 * m->c[0]);
 }
 
@@ -2353,9 +2416,7 @@ void run_osblock(Launcher& L, const BlockW& b, const float* X, float* Xo, int H,
     for (int br = 0; br < 4; ++br) ga.sums[br] = m->sums[br];
     ga.w1 = W + b.g1w; ga.b1 = W + b.g1b; ga.w2 = W + b.g2w; ga.b2 = W + b.g2b;
     ga.gates = m->gates; ga.C = b.mid; ga.hid = b.hid; ga.tiles = tiles; ga.HW = HW;
-    L.begin(CLS_GATES);
-    k_gates<<<L.upper, 128, sizeof(float) * (4 * b.mid + 4 * b.hid), L.st>>>(ga, L.d_n, L.off, L.cap);
-    L.end();
+    L.gates(ga);
     PwArgs c{};
     for (int br = 0; br < 4; ++br) c.branch[br] = m->Y[br][kDepth[br] & 1];
     c.gates = m->gates; c.mid = b.mid;
@@ -2401,9 +2462,7 @@ void run_transition(Launcher& L, const float* X, float* tmp, float* out, int H, 
     p.K = C; p.N = C; p.HW = H * Wd; p.relu = 1;
     p.w_tc = tc.w; p.Kpad = tc.Kpad; p.Npad = tc.Npad;
     L.pointwise(p);
-    L.begin(CLS_AVGPOOL);
-    k_avgpool2<<<m->sms * 4, 256, 0, L.st>>>(tmp, H, Wd, C, L.d_n, L.off, L.cap, out);
-    L.end();
+    L.avgpool(tmp, H, Wd, C, out);
 }
 
 // LMBN_n, one chunk (lmbn_n.py:83-146 in eval).  Taps: 0 crop, 1 stem, 2 pool, 3 backone.2.0, 4 backone.2.1,
@@ -2447,21 +2506,13 @@ void run_lmbn_chunk(Launcher& L, const FrameIn& fi, float* d_out, int out_ld) {
             if (stop_here(A, (size_t)bh * bw * LMBN_C)) return;
             pool_src = A;
         }
-        L.begin(CLS_HEAD);
-        k_lmbn_pool<<<L.upper, 256, 0, L.st>>>(pool_src, bh, bw, LMBN_C, br, m->pooled, L.d_n, L.off, L.cap);
-        L.end();
+        L.lmbn_pool(pool_src, bh, bw, br, m->pooled);
     }
     NeckArgs na{};
     for (int k = 0; k < 5; ++k) { na.w[k] = m->d_w + lm.neck_w[k]; na.b[k] = m->d_w + lm.neck_b[k]; }
     na.wsh = m->d_w + lm.sh_w; na.bsh = m->d_w + lm.sh_b; na.chst = m->d_w + lm.ch_st;
-    RCUDA_OK(cudaFuncSetAttribute(k_lmbn_neck, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)NECK_SMEM));
-    L.begin(CLS_HEAD);
-    k_lmbn_neck<<<dim3(LMBN_C / NECK_COLS, 6), 256, NECK_SMEM, L.st>>>(na, m->pooled, fi.crops, L.d_n, L.off, L.cap,
-                                                                         d_out, out_ld);
-    L.end();
-    L.begin(CLS_HEAD);
-    k_l2_normalise<<<L.upper, 256, 0, L.st>>>(fi.crops, L.d_n, L.off, L.cap, d_out, out_ld, m->feat);
-    L.end();
+    L.lmbn_neck(na, m->pooled, fi.crops, d_out, out_ld);
+    L.l2_normalise(fi.crops, d_out, out_ld, m->feat);
 }
 
 // Bottleneck ResNet, one chunk (resnet.py featuremaps + global average pool).  Taps: 0 crop, 1 stem, 2 pool, then
@@ -2499,10 +2550,7 @@ void run_resnet_chunk(Launcher& L, const FrameIn& fi, float* d_out, int out_ld) 
         H = Ho; Wd = Wo;
         if (stop_here(X, (size_t)H * Wd * b.cout)) return;
     }
-    L.begin(CLS_HEAD);
-    k_head<<<L.upper, 256, sizeof(float) * (2 * m->feat + 32), L.st>>>(X, H * Wd, m->feat, nullptr, nullptr, m->feat,
-                                                                       fi.crops, L.d_n, L.off, L.cap, d_out, out_ld);
-    L.end();
+    L.head(X, H * Wd, m->feat, nullptr, nullptr, m->feat, fi.crops, d_out, out_ld);
 }
 
 // CLIP-ReID ViT-B/16, one chunk (clip/model.py VisionTransformer.forward + make_model.py build_transformer, eval,
@@ -2617,19 +2665,14 @@ void run_mobilenetv2_chunk(Launcher& L, const FrameIn& fi, float* d_out, int out
     stage_crops(L, fi);
     float* X = m->bufA;
     float* Xo = m->bufB;
-    L.begin(CLS_STEM);
-    k_stem3<<<m->sms * 8, 256, 0, L.st>>>(m->blob, W + mb.stem_w, W + mb.stem_b, mb.stemp, L.d_n, L.off, L.cap, X);
-    L.end();
+    L.stem3(m->blob, W + mb.stem_w, W + mb.stem_b, mb.stemp, X);
     int H = 128, Wd = 64;
     for (const MbBlock& b : mb.blocks) {
         PwArgs e{};
         e.in = X; e.w = W + b.we; e.bias = W + b.be; e.out = m->x1;
         e.K = b.cinp; e.N = b.midp; e.HW = H * Wd; e.relu = 2;
         L.pointwise(e);
-        L.begin(CLS_LIGHTCONV);
-        k_dwconv3<<<m->sms * 8, 256, 0, L.st>>>(m->x1, H, Wd, b.midp, b.stride, W + b.wd, W + b.bd, L.d_n, L.off, L.cap,
-                                                m->Y[0][0]);
-        L.end();
+        L.dwconv3(m->x1, H, Wd, b.midp, b.stride, W + b.wd, W + b.bd, m->Y[0][0]);
         H /= b.stride; Wd /= b.stride;
         PwArgs p{};
         p.in = m->Y[0][0]; p.w = W + b.wp; p.bias = W + b.bp; p.out = Xo;
@@ -2642,10 +2685,7 @@ void run_mobilenetv2_chunk(Launcher& L, const FrameIn& fi, float* d_out, int out
     c9.in = X; c9.w = W + mb.c9w; c9.bias = W + mb.c9b; c9.out = Xo;
     c9.K = mb.last; c9.N = m->feat; c9.HW = H * Wd; c9.relu = 2;
     L.pointwise(c9);
-    L.begin(CLS_HEAD);
-    k_head<<<L.upper, 256, sizeof(float) * (2 * m->feat + 32), L.st>>>(Xo, H * Wd, m->feat, nullptr, nullptr, m->feat,
-                                                                       fi.crops, L.d_n, L.off, L.cap, d_out, out_ld);
-    L.end();
+    L.head(Xo, H * Wd, m->feat, nullptr, nullptr, m->feat, fi.crops, d_out, out_ld);
 }
 }  // namespace
 
@@ -2657,11 +2697,7 @@ namespace {
 // OSNet head: global average pool of x [crops][HW][c3], fc + folded BatchNorm1d, L2 norm into the caller's rows
 void run_osnet_head(Launcher& L, const FrameIn& fi, const float* x, int HW, float* d_out, int out_ld) {
     ReidModel* m = L.m;
-    const int C = m->c[3];
-    L.begin(CLS_HEAD);
-    k_head<<<L.upper, 256, sizeof(float) * (C + 32 + (256 / C > 0 ? 256 / C : 1) * C), L.st>>>(
-        x, HW, C, m->d_w + m->fcw, m->d_w + m->fcb, m->feat, fi.crops, L.d_n, L.off, L.cap, d_out, out_ld);
-    L.end();
+    L.head(x, HW, m->c[3], m->d_w + m->fcw, m->d_w + m->fcb, m->feat, fi.crops, d_out, out_ld);
 }
 
 // OSNet and OSNet-AIN / IBN, one chunk (osnet.py:380-405).  Taps: 0 crop, 1 stem, 2 pool, then every OSBlock and
@@ -3055,6 +3091,256 @@ void standalone_mlfn_fsm(const float* x, int n, int h, int w, int c, const float
         throw;
     }
     cleanup();
+}
+
+// ---- float32 CUDA-core kernels of the OSNet family, MobileNetV2 and LMBN_n on their own (parity tests) ----------------
+// Each entry runs one kernel family through the Launcher method a loaded model calls, on a default-constructed
+// ReidModel (so the template instance is the one a shipped model gets), over a crop window: the host arrays hold
+// n crops, the device crop count is `count` and the chunk starts at crop `off`, so the kernels see
+// clamp(count - off, 0, n) crops (chunk_count).  Every output array is uploaded as given and read back whole, so
+// the caller's canaries after each tensor and in the crops outside the window come back untouched unless a kernel
+// writes there.
+namespace {
+struct StandaloneRun {
+    std::vector<void*> bufs;
+    int* dn = nullptr;
+    ReidModel fake;
+    Launcher L;
+    StandaloneRun(int n, int off, int count) : L{&fake, nullptr, off, n, n, nullptr} {
+        if (n <= 0 || off < 0 || count < 0) throw std::runtime_error("n > 0, off >= 0 and count >= 0 required");
+        dn = up(&count, 1);
+        L.d_n = dn;
+    }
+    ~StandaloneRun() {
+        for (void* p : bufs) cudaFree(p);
+    }
+    template <typename T>
+    T* up(const T* src, size_t count) {
+        if (!src) return nullptr;
+        T* d = nullptr;
+        RCUDA_OK(cudaMalloc(&d, sizeof(T) * std::max<size_t>(count, 1)));
+        bufs.push_back(d);
+        RCUDA_OK(cudaMemcpy(d, src, sizeof(T) * count, cudaMemcpyHostToDevice));
+        return d;
+    }
+    void down(float* dst, const float* src, size_t count) {
+        RCUDA_OK(cudaGetLastError());
+        RCUDA_OK(cudaMemcpy(dst, src, sizeof(float) * count, cudaMemcpyDeviceToHost));
+    }
+    // crop descriptors whose out_row fields are rows[0 .. n_rows)
+    const CropDesc* crops(const int* rows, int n_rows) {
+        std::vector<CropDesc> cd((size_t)n_rows);
+        for (int i = 0; i < n_rows; ++i) cd[i] = CropDesc{0.f, 0.f, 0.f, 0.f, 0, rows[i]};
+        return up(cd.data(), cd.size());
+    }
+    void report(int* instance) {
+        if (instance) std::memcpy(instance, L.inst, sizeof(L.inst));
+    }
+};
+void need(bool ok, const char* what) {
+    if (!ok) throw std::runtime_error(what);
+}
+}  // namespace
+
+// 1x1 GEMM (k_pointwise2): out [n][hw][nout] = act(A W + bias (+ residual)).  branches (4 x [n][hw][mid]) selects the
+// gated prologue, A[m][k] = sum_b gates[crop][b][k] branch_b[m][k] for k < mid and a[m][k - mid] (downsample rows
+// [n][hw][k - mid], null when k == mid) above; otherwise a is [n][hw][k].  instance: {BN, threads, gated, 0}.
+void standalone_f32_pointwise(const float* a, const float* branches, const float* gates, int n, int hw, int k, int mid,
+                              const float* w, int nout, const float* bias, const float* residual, int relu, int off,
+                              int count, float* out, int out_floats, int* instance) {
+    const bool gated = branches != nullptr;
+    need(hw > 0 && k > 0 && nout > 0 && k % 4 == 0 && nout % 4 == 0 && relu >= 0 && relu <= 2 &&
+             (!gated || (gates && mid > 0 && mid % 4 == 0 && mid <= k)) && (a || (gated && k == mid)) &&
+             out_floats >= n * hw * nout,
+         "hw, k, nout > 0, k and nout multiples of 4, relu 0-2, gated: 0 < mid <= k, mid a multiple of 4; out large enough");
+    StandaloneRun r(n, off, count);
+    const size_t M = (size_t)n * hw;
+    PwArgs p{};
+    if (gated) {
+        p.in = r.up(a, M * (k - mid));
+        const float* br = r.up(branches, 4 * M * mid);
+        for (int b = 0; b < 4; ++b) p.branch[b] = br + b * M * mid;
+        p.gates = r.up(gates, (size_t)n * 4 * mid);
+        p.mid = mid;
+    } else {
+        p.in = r.up(a, M * k);
+    }
+    p.w = r.up(w, (size_t)k * nout);
+    p.bias = r.up(bias, nout);
+    p.residual = r.up(residual, M * nout);
+    float* d_out = r.up(out, out_floats);
+    p.out = d_out;
+    p.K = k; p.N = nout; p.HW = hw; p.relu = relu;
+    r.L.pointwise(p);
+    r.down(out, d_out, out_floats);
+    r.report(instance);
+}
+
+// One LightConv3x3 level of nb branches (k_lightconv2 or the generic k_lightconv), tile rows picked as run_osblock
+// picks them: in nb x [n][H][W][C], wpw nb x [C][C] (K-major), wdw nb x [9][C], bias nb x [C].  Branch b writes out
+// + b * out_stride ([n][H][W][C]) and, when sums is given, its per-tile channel sums to sums + b * sums_stride
+// ([n][H / R][C]).  instance: {kind (1 k_lightconv, 2 k_lightconv2), C, W, R}.
+void standalone_f32_lightconv(const float* in, int nb, int n, int H, int W, int C, const float* wpw, const float* wdw,
+                              const float* bias, int off, int count, float* out, int out_stride, float* sums,
+                              int sums_stride, int* instance) {
+    need(nb >= 1 && nb <= 4 && H > 0 && W > 0 && C >= 8 && C % 8 == 0 && out_stride >= n * H * W * C &&
+             out_stride % 4 == 0 && (!sums || (sums_stride >= n * H * C && sums_stride % 4 == 0)),
+         "1 <= nb <= 4, H, W > 0, C a positive multiple of 8; out_stride >= n H W C, sums_stride >= n H C, both "
+         "multiples of 4 (float4 stores)");
+    StandaloneRun r(n, off, count);
+    const size_t map = (size_t)n * H * W * C;
+    const float* d_in = r.up(in, nb * map);
+    const float* d_pw = r.up(wpw, (size_t)nb * C * C);
+    const float* d_dw = r.up(wdw, (size_t)nb * 9 * C);
+    const float* d_b = r.up(bias, (size_t)nb * C);
+    float* d_out = r.up(out, (size_t)nb * out_stride);
+    float* d_sums = r.up(sums, (size_t)nb * sums_stride);
+    LightArgs la{};
+    la.H = H; la.W = W; la.C = C; la.R = pick_tile_rows2(H, W, C);
+    for (int b = 0; b < nb; ++b) {
+        la.in[b] = d_in + b * map;
+        la.out[b] = d_out + (size_t)b * out_stride;
+        la.wpw[b] = d_pw + (size_t)b * C * C;
+        la.wdw[b] = d_dw + (size_t)b * 9 * C;
+        la.bias[b] = d_b + (size_t)b * C;
+        la.sums[b] = d_sums ? d_sums + (size_t)b * sums_stride : nullptr;
+    }
+    r.L.light(la, nb, (256 / (C / 4)) * (C / 4));
+    r.down(out, d_out, (size_t)nb * out_stride);
+    if (sums) r.down(sums, d_sums, (size_t)nb * sums_stride);
+    r.report(instance);
+}
+
+// The four LightConv branches of an OSBlock as whole-branch CTAs (k_lightchain): in [n][H][W][C] (the conv1 output),
+// per LightConv l (branch b, level v: l = b (b + 1) / 2 + v - 1) wpw [10][C][C], wdw [10][9][C], bias [10][C].  Branch b
+// writes out + b * out_stride and its per-tile channel sums to sums + b * sums_stride ([n][H / R][C]).  Shapes the
+// model does not chain are an error.  instance: {3, C, W, R}.
+void standalone_f32_lightchain(const float* in, int n, int H, int W, int C, const float* wpw, const float* wdw,
+                               const float* bias, int off, int count, float* out, int out_stride, float* sums,
+                               int sums_stride, int* instance) {
+    need(H > 0 && W > 0 && C > 0 && out_stride >= n * H * W * C && sums_stride >= n * H * C && out_stride % 4 == 0 &&
+             sums_stride % 4 == 0,
+         "H, W, C > 0, out_stride >= n H W C and sums_stride >= n H C, both multiples of 4 (float4 stores), required");
+    StandaloneRun r(n, off, count);
+    const float* d_in = r.up(in, (size_t)n * H * W * C);
+    const float* d_pw = r.up(wpw, (size_t)10 * C * C);
+    const float* d_dw = r.up(wdw, (size_t)10 * 9 * C);
+    const float* d_b = r.up(bias, (size_t)10 * C);
+    float* d_out = r.up(out, (size_t)4 * out_stride);
+    float* d_sums = r.up(sums, (size_t)4 * sums_stride);
+    ChainArgs ca{};
+    ca.in = d_in; ca.H = H;
+    for (int b = 0; b < 4; ++b) { ca.out[b] = d_out + (size_t)b * out_stride; ca.sums[b] = d_sums + (size_t)b * sums_stride; }
+    for (int l = 0; l < 10; ++l) {
+        ca.wpw[l] = d_pw + (size_t)l * C * C; ca.wdw[l] = d_dw + (size_t)l * 9 * C; ca.bias[l] = d_b + (size_t)l * C;
+    }
+    need(r.L.light_chain(ca, C, W) > 0, "no LightConv chain kernel for this (C, W)");
+    r.down(out, d_out, (size_t)4 * out_stride);
+    r.down(sums, d_sums, (size_t)4 * sums_stride);
+    r.report(instance);
+}
+
+// ChannelGate of an OSBlock (k_gates): sums 4 x [n][tiles][C] (branch b at b * n * tiles * C), w1 [C][hid], b1 [hid],
+// w2 [hid][C], b2 [C] -> gates [n][4][C] = sigmoid(relu(mean w1 + b1) w2 + b2), mean = (sum over tiles) / hw.
+void standalone_f32_gates(const float* sums, int n, int tiles, int C, int hid, int hw, const float* w1, const float* b1,
+                          const float* w2, const float* b2, int off, int count, float* gates, int gates_floats) {
+    need(tiles > 0 && C > 0 && hid > 0 && hw > 0 && gates_floats >= n * 4 * C,
+         "tiles, C, hid, hw > 0 and gates_floats >= 4 n C required");
+    StandaloneRun r(n, off, count);
+    const size_t per = (size_t)n * tiles * C;
+    const float* d_s = r.up(sums, 4 * per);
+    float* d_g = r.up(gates, gates_floats);
+    GateArgs ga{};
+    for (int b = 0; b < 4; ++b) ga.sums[b] = d_s + b * per;
+    ga.w1 = r.up(w1, (size_t)C * hid); ga.b1 = r.up(b1, hid); ga.w2 = r.up(w2, (size_t)hid * C); ga.b2 = r.up(b2, C);
+    ga.gates = d_g; ga.C = C; ga.hid = hid; ga.tiles = tiles; ga.HW = hw;
+    r.L.gates(ga);
+    r.down(gates, d_g, gates_floats);
+}
+
+// Head (k_head): x [n][hw][C] -> average pool, fc + ReLU when wfc ([C][feat]) is given (else feat == C and the pooled
+// row is the embedding), L2 normalisation, into row rows[off + i] of out (out_ld floats per row) for window crop i.
+// rows holds off + n entries.
+void standalone_f32_head(const float* x, int n, int hw, int C, const float* wfc, const float* bfc, int feat,
+                         const int* rows, int off, int count, float* out, int out_floats, int out_ld) {
+    need(hw > 0 && C > 0 && feat > 0 && (wfc ? bfc != nullptr : feat == C) && out_ld >= feat,
+         "hw, C, feat > 0, a bias with the fc (feat == C without), out_ld >= feat required");
+    for (int i = 0; i < off + n; ++i)
+        need(rows[i] >= 0 && (size_t)rows[i] * out_ld + feat <= (size_t)out_floats, "an output row lies outside out");
+    StandaloneRun r(n, off, count);
+    const float* d_x = r.up(x, (size_t)n * hw * C);
+    const float* d_w = r.up(wfc, (size_t)C * feat);
+    const float* d_b = r.up(bfc, wfc ? feat : 0);
+    const CropDesc* d_c = r.crops(rows, off + n);
+    float* d_out = r.up(out, out_floats);
+    r.L.head(d_x, hw, C, d_w, d_b, feat, d_c, d_out, out_ld);
+    r.down(out, d_out, out_floats);
+}
+
+// Stems, pools and the MobileNetV2 depthwise convolution, NHWC float32, `in` [n][h][w][c_in]:
+//   op 0 k_stem<false>  7x7/2 conv + bias + ReLU, in [n][h][128][3] (h 256 or 384), weight [147][c], out [n][h/2][64][c]
+//   op 1 k_stem<true>   the same convolution without bias and ReLU (the instance-norm stem)
+//   op 2 k_maxpool3s2   3x3/2 pad 1 max, out [n][h/2][w/2][c]
+//   op 3 k_avgpool2     2x2/2 average, out [n][h/2][w/2][c]
+//   op 4 k_stem3        3x3/2 pad 1 conv + bias + ReLU6, in [n][256][128][3], weight [27][c], out [n][128][64][c]
+//   op 5 k_dwconv3      depthwise 3x3 pad 1 at `stride` + bias + ReLU6, weight [9][c], out [n][h/s][w/s][c]
+void standalone_f32_map(int op, const float* in, int n, int h, int w, int c, int stride, const float* weight,
+                        const float* bias, int off, int count, float* out, int out_floats) {
+    need(op >= 0 && op <= 5 && h > 0 && w > 0 && c > 0 && c % 4 == 0, "op 0-5, h, w > 0, c a multiple of 4 required");
+    if (op <= 1) need(w == IN_W && (h == IN_H || h == IN_H_MAX) && c % 16 == 0, "stem: 256 or 384 x 128 crops, c % 16 == 0");
+    if (op == 4) need(w == IN_W && h == IN_H, "MobileNetV2 stem: 256 x 128 crops");
+    if (op == 2 || op == 3) need(h % 2 == 0 && w % 2 == 0, "pools: even h and w");
+    if (op == 5) need((stride == 1 || stride == 2) && h % stride == 0 && w % stride == 0, "depthwise: stride 1 or 2 dividing h, w");
+    const int cin = (op <= 1 || op == 4) ? 3 : c;
+    const int oh = op == 5 ? h / stride : h / 2, ow = op == 5 ? w / stride : (op <= 1 ? 64 : w / 2);
+    need(out_floats >= n * oh * ow * c, "out too small");
+    const size_t wk = op <= 1 ? 147 : (op == 4 ? 27 : 9);
+    StandaloneRun r(n, off, count);
+    const float* d_in = r.up(in, (size_t)n * h * w * cin);
+    const float* d_w = (op == 2 || op == 3) ? nullptr : r.up(weight, wk * c);
+    const float* d_b = (op == 0 || op == 4 || op == 5) ? r.up(bias, c) : nullptr;
+    float* d_out = r.up(out, out_floats);
+    switch (op) {
+        case 0:
+        case 1: r.L.stem(op == 1, d_in, d_w, d_b, c, d_out, h); break;
+        case 2: r.L.maxpool(d_in, h, w, c, d_out); break;
+        case 3: r.L.avgpool(d_in, h, w, c, d_out); break;
+        case 4: r.L.stem3(d_in, d_w, d_b, c, d_out); break;
+        case 5: r.L.dwconv3(d_in, h, w, c, stride, d_w, d_b, d_out); break;
+    }
+    r.down(out, d_out, out_floats);
+}
+
+// LMBN_n head: k_lmbn_pool of the bottleneck, partial and channel branch maps (x [3][n][h][w][512]) into pooled
+// ([n][6][512], read back), the neck GEMMs (neck = the five reduction matrices [5][512][512], their biases [5][512],
+// shared [256][512], its bias [512], reduction_ch scale / shift [4][512], concatenated in that order) and the L2
+// normalisation of the 3584-d rows, written to row rows[off + i] of out as run_lmbn_chunk does.
+void standalone_f32_lmbn_head(const float* x, int n, int h, int w, const float* neck, const int* rows, int off, int count,
+                              float* pooled, int pooled_floats, float* out, int out_floats, int out_ld) {
+    constexpr int C = LMBN_C;
+    need(h > 0 && h % 2 == 0 && w > 0 && pooled_floats >= n * LMBN_POOLS * C && out_ld >= LMBN_VECS * C,
+         "h even, w > 0, pooled_floats >= 6 n 512, out_ld >= 3584 required");
+    for (int i = 0; i < off + n; ++i)
+        need(rows[i] >= 0 && (size_t)rows[i] * out_ld + LMBN_VECS * C <= (size_t)out_floats, "an output row lies outside out");
+    StandaloneRun r(n, off, count);
+    const size_t map = (size_t)n * h * w * C;
+    const float* d_x = r.up(x, 3 * map);
+    const float* d_neck = r.up(neck, (size_t)5 * C * C + 5 * C + (size_t)(C / 2) * C + C + 4 * C);
+    float* d_p = r.up(pooled, pooled_floats);
+    float* d_out = r.up(out, out_floats);
+    const CropDesc* d_c = r.crops(rows, off + n);
+    NeckArgs na{};
+    const float* q = d_neck;
+    for (int k = 0; k < 5; ++k) { na.w[k] = q; q += (size_t)C * C; }
+    for (int k = 0; k < 5; ++k) { na.b[k] = q; q += C; }
+    na.wsh = q; q += (size_t)(C / 2) * C;
+    na.bsh = q; q += C;
+    na.chst = q;
+    for (int which = 0; which < 3; ++which) r.L.lmbn_pool(d_x + which * map, h, w, which, d_p);
+    r.L.lmbn_neck(na, d_p, d_c, d_out, out_ld);
+    r.L.l2_normalise(d_c, d_out, out_ld, LMBN_VECS * C);
+    r.down(pooled, d_p, pooled_floats);
+    r.down(out, d_out, out_floats);
 }
 
 }  // namespace bmb

@@ -443,6 +443,53 @@ BOXMOT_B200_API int boxmot_b200_mlfn_group_conv(const float* in, int n, int h, i
 BOXMOT_B200_API int boxmot_b200_mlfn_fsm(const float* x, int n, int h, int w, int c, const float* w1, const float* b1,
                                          int f0, const float* w2, const float* b2, int f1, const float* w3,
                                          const float* b3, float* out);
+/* The float32 CUDA-core kernels of the OSNet family, MobileNetV2 and LMBN_n, one family per entry, launched as a loaded
+ * model launches them, on host arrays (NHWC float32) over a crop window: the arrays hold n crops, the device crop count
+ * is `count` and the window starts at crop `off`, so the kernels process crops 0 .. clamp(count - off, 0, n) - 1 of the
+ * arrays (head entries: with output rows rows[off + i], rows holding off + n entries).  Every output array is uploaded
+ * as given and read back whole (out_floats / *_stride floats per tensor), so values the kernels must not write come
+ * back unchanged.  `instance` (optional, 4 ints) receives the kernel instance that ran.
+ *   f32_pointwise: out (n,hw,nout) = act(A W + bias (+ residual)), act 0 none, 1 ReLU, 2 ReLU6; branches (4,n,hw,mid)
+ *     and gates (n,4,mid) select the gated prologue A = [sum_b gates[crop][b] * branch_b | a (n,hw,k-mid), null when
+ *     k == mid], else A = a (n,hw,k).  instance {BN, threads, gated, 0}.
+ *   f32_lightconv: nb <= 4 LightConv3x3 branches of one level (1x1 wpw (C,C) -> depthwise 3x3 wdw (9,C) + bias + ReLU),
+ *     in (nb,n,h,w,c); branch b writes out + b out_stride and, with sums, its per-tile channel sums (n,h/R,c) at
+ *     sums + b sums_stride (strides multiples of 4).  instance {1 generic / 2 shape-specialised kernel, C, W, R (tile rows)}.
+ *   f32_lightchain: the four branches of an OSBlock in whole-branch CTAs, in (n,h,w,c), weights of LightConv
+ *     l = b (b + 1) / 2 + level - 1 at wpw (10,c,c), wdw (10,9,c), bias (10,c); outputs and sums as f32_lightconv.
+ *     instance {3, C, W, R}.
+ *   f32_gates: gates (n,4,c) = sigmoid(relu(mean w1 + b1) w2 + b2), mean = sum over tiles of sums (4,n,tiles,c) / hw,
+ *     w1 (c,hid), w2 (hid,c).
+ *   f32_head: average pool of x (n,hw,c), fc (c,feat) + bias + ReLU (wfc null: feat == c, no fc), L2 norm, into the
+ *     rows of out (out_ld floats per row).
+ *   f32_map: op 0 7x7/2 stem + bias + ReLU of (n,h,128,3) crops, h 256 or 384, weight (147,c); 1 the same without
+ *     bias and ReLU; 2 3x3/2 max pool; 3 2x2/2 average pool; 4 MobileNetV2's 3x3/2 stem + bias + ReLU6 of (n,256,128,3)
+ *     crops, weight (27,c); 5 depthwise 3x3 pad 1 at stride 1 or 2 + bias + ReLU6, weight (9,c).
+ *   f32_lmbn_head: LMBN_n's poolings of the bottleneck, partial and channel branch maps x (3,n,h,w,512) into pooled
+ *     (n,6,512), the neck (neck = reduction weights (5,512,512), biases (5,512), shared (256,512), its bias (512),
+ *     reduction_ch scale / shift (4,512)) and the L2 norm of the 3584-d rows. */
+BOXMOT_B200_API int boxmot_b200_f32_pointwise(const float* a, const float* branches, const float* gates, int n, int hw,
+                                              int k, int mid, const float* w, int nout, const float* bias,
+                                              const float* residual, int relu, int off, int count, float* out,
+                                              int out_floats, int* instance);
+BOXMOT_B200_API int boxmot_b200_f32_lightconv(const float* in, int nb, int n, int h, int w, int c, const float* wpw,
+                                              const float* wdw, const float* bias, int off, int count, float* out,
+                                              int out_stride, float* sums, int sums_stride, int* instance);
+BOXMOT_B200_API int boxmot_b200_f32_lightchain(const float* in, int n, int h, int w, int c, const float* wpw,
+                                               const float* wdw, const float* bias, int off, int count, float* out,
+                                               int out_stride, float* sums, int sums_stride, int* instance);
+BOXMOT_B200_API int boxmot_b200_f32_gates(const float* sums, int n, int tiles, int c, int hid, int hw, const float* w1,
+                                          const float* b1, const float* w2, const float* b2, int off, int count,
+                                          float* gates, int gates_floats);
+BOXMOT_B200_API int boxmot_b200_f32_head(const float* x, int n, int hw, int c, const float* wfc, const float* bfc,
+                                         int feat, const int* rows, int off, int count, float* out, int out_floats,
+                                         int out_ld);
+BOXMOT_B200_API int boxmot_b200_f32_map(int op, const float* in, int n, int h, int w, int c, int stride,
+                                        const float* weight, const float* bias, int off, int count, float* out,
+                                        int out_floats);
+BOXMOT_B200_API int boxmot_b200_f32_lmbn_head(const float* x, int n, int h, int w, const float* neck, const int* rows,
+                                              int off, int count, float* pooled, int pooled_floats, float* out,
+                                              int out_floats, int out_ld);
 BOXMOT_B200_API int boxmot_b200_device_count(void);
 /* Diagnostics for the ReID kernels: run the forward up to `stage` (0 input blob, 1 stem, 2 max-pool, 3..10 the
  * six OSBlocks and two transitions in order, 11 conv5) and copy that NHWC float32 tensor of the n crops out.  For
