@@ -176,6 +176,16 @@ SYMBOLS = {
                                     c_int, c_void_p, c_int]),
     "boxmot_b200_f32_lmbn_head": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p,
                                           c_int, c_void_p, c_int, c_int]),
+    "boxmot_b200_hacnn_conv": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int,
+                                       c_void_p, c_void_p, c_int, c_int]),
+    "boxmot_b200_hacnn_map": (c_int, [c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
+                                      c_void_p]),
+    "boxmot_b200_hacnn_attention": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p,
+                                            c_void_p, c_void_p, c_void_p, c_void_p]),
+    "boxmot_b200_hacnn_stn": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p,
+                                      c_int, c_int, c_void_p]),
+    "boxmot_b200_hacnn_head": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p,
+                                       c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
     "boxmot_b200_device_count": (c_int, []),
     "boxmot_b200_reid_debug_stage": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_void_p,
                                              c_int, POINTER(c_int)]),

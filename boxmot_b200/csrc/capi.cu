@@ -453,6 +453,27 @@ int boxmot_b200_f32_lmbn_head(const float* x, int n, int h, int w, const float* 
         standalone_f32_lmbn_head(x, n, h, w, neck, rows, off, count, pooled, pooled_floats, out, out_floats, out_ld);
     });
 }
+int boxmot_b200_hacnn_conv(const float* in, int n, int off, int count, int h, int w, int c0, int k, int stride,
+                           const float* weight, int N, const float* bias, float* out, int out_ld, int out_off) {
+    return guard([&] { standalone_hacnn_conv(in, n, off, count, h, w, c0, k, stride, weight, N, bias, out, out_ld, out_off); });
+}
+int boxmot_b200_hacnn_map(int op, const float* in, int n, int off, int count, int h, int w, int c, const float* weight,
+                          const float* bias, float* out) {
+    return guard([&] { standalone_hacnn_map(op, in, n, off, count, h, w, c, weight, bias, out); });
+}
+int boxmot_b200_hacnn_attention(const float* x, int n, int off, int count, int h, int w, int c, int level,
+                                const float* params, float* out, float* s, float* v, float* theta) {
+    return guard([&] { standalone_hacnn_attention(x, n, off, count, h, w, c, level, params, out, s, v, theta); });
+}
+int boxmot_b200_hacnn_stn(const float* src, int n, int off, int count, int H, int W, int C, const float* theta,
+                          int level, const float* prev, int lh, int lw, float* out) {
+    return guard([&] { standalone_hacnn_stn(src, n, off, count, H, W, C, theta, level, prev, lh, lw, out); });
+}
+int boxmot_b200_hacnn_head(const float* x3, int n, int off, int count, int hw3, const float* loc, int hwl,
+                           const float* wg, const float* bg, const float* wl, const float* bl, const int* rows,
+                           int out_rows, float* out, float* v) {
+    return guard([&] { standalone_hacnn_head(x3, n, off, count, hw3, loc, hwl, wg, bg, wl, bl, rows, out_rows, out, v); });
+}
 int boxmot_b200_cosine_cost(const float* a, int rows, const float* b, int cols, int dim, double* out) {
     return guard([&] { standalone_cosine(a, rows, b, cols, dim, out); });
 }

@@ -272,4 +272,16 @@ void standalone_f32_map(int op, const float* in, int n, int h, int w, int c, int
 void standalone_f32_lmbn_head(const float* x, int n, int h, int w, const float* neck, const int* rows, int off,
                               int count, float* pooled, int pooled_floats, float* out, int out_floats, int out_ld);
 
+void standalone_hacnn_conv(const float* in, int n, int off, int count, int h, int w, int c0, int k, int stride,
+                           const float* weight, int N, const float* bias, float* out, int out_ld, int out_off);
+void standalone_hacnn_map(int op, const float* in, int n, int off, int count, int h, int w, int c, const float* weight,
+                          const float* bias, float* out);
+void standalone_hacnn_attention(const float* x, int n, int off, int count, int h, int w, int c, int level,
+                                const float* params, float* out, float* s, float* v, float* theta);
+void standalone_hacnn_stn(const float* src, int n, int off, int count, int H, int W, int C, const float* theta,
+                          int level, const float* prev, int lh, int lw, float* out);
+void standalone_hacnn_head(const float* x3, int n, int off, int count, int hw3, const float* loc, int hwl,
+                           const float* wg, const float* bg, const float* wl, const float* bl, const int* rows,
+                           int out_rows, float* out, float* v);
+
 }  // namespace bmb

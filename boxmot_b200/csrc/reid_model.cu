@@ -24,6 +24,7 @@
 
 #include "engine.h"
 #include "pointwise_tc.cuh"
+#include "hacnn_kernels.cuh"
 #include "mlfn_kernels.cuh"
 #include "resnet_tc.cuh"
 #include "vit_tc.cuh"
@@ -1373,6 +1374,14 @@ struct MlfnW {
     RnConv fc_x, fc_s;
 };
 
+// HACNN (arch 8): the tensor-core packings of every ConvBlock after the stem (per level the InceptionA's seven, the
+// InceptionB's six and the local branch's InceptionB's six, in fold_hacnn's stream order) and of the two heads, and
+// the offsets in d_w of each level's attention parameters (sp, w1, b1, w2, b2, wv, bv, wfc, bfc)
+struct HacnnW {
+    RnConv ia[3][7], ib[3][6], lb[3][6], fcg, fcl;
+    size_t att[3][9] = {};
+};
+
 // CLIP-ReID ViT-B/16 (arch 6): per residual block the offsets in d_w of its LayerNorm parameters and biases, and the
 // tensor-core packings of its four linear layers
 struct VitLayer {
@@ -1395,6 +1404,7 @@ enum ReidArch {
     ARCH_RESNET = 5,
     ARCH_CLIP = 6,       // CLIP-ReID ViT-B/16
     ARCH_MLFN = 7,
+    ARCH_HACNN = 8,
 };
 
 struct ReidModel {
@@ -1410,7 +1420,9 @@ struct ReidModel {
     MbW mb;
     std::vector<RnBlock> rn;      // ResNet Bottlenecks, layer1.0 .. layer4.last
     MlfnW ml;
-    float* d_wrn = nullptr;       // ResNet / CLIP / MLFN: every GEMM's weights packed by rn::pack_conv_weights
+    HacnnW ha;
+    int* d_n4 = nullptr;          // HACNN: 4 x the crop count, the image count of the [crop][region] local branch
+    float* d_wrn = nullptr;       // ResNet / CLIP / MLFN / HACNN: every GEMM's weights packed by rn::pack_conv_weights
     int c[4] = {0, 0, 0, 0};
     int feat = 0;
     float* d_w = nullptr;
@@ -1518,6 +1530,13 @@ void read_header(ReidModel* m, const int32_t* hdr) {
             if (hdr[3] != 64 || hdr[4] != 2048 || hdr[5] != mlfn::GROUPS || hdr[6] != mlfn::BLOCKS || m->feat != mlfn::FEAT)
                 throw std::runtime_error("bad MLFN blob header (only groups 32, channels 64-2048, 16 blocks, 1024-d)");
             m->c[0] = 64;
+            return;
+        case ARCH_HACNN:
+            if (hdr[3] != hacnn::STEM_C || hdr[4] != 128 || hdr[5] != 256 || hdr[6] != hacnn::C3 ||
+                m->feat != hacnn::FEAT || hdr[9] != hacnn::IN_H || hdr[10] != hacnn::IN_W)
+                throw std::runtime_error("bad HACNN blob header (only nchannels 128/256/384, 1024-d, 160x64 input)");
+            m->in_h = hacnn::IN_H;
+            m->in_w = hacnn::IN_W;
             return;
         case ARCH_RESNET:
             m->c[0] = 64;
@@ -1788,6 +1807,60 @@ Workspace layout_mlfn(ReidModel* m, BlobCursor& take, WgmmaPack& pack) {
     return ws;
 }
 
+// ---- HACNN (reid/backbones/hacnn.py): stem, three Inception + HarmAttn levels, the local branch, two heads ----
+Workspace layout_hacnn(ReidModel* m, BlobCursor& take, WgmmaPack& pack) {
+    static const int kC[4] = {hacnn::STEM_C, 128, 256, hacnn::C3};
+    m->stem_w = take((size_t)27 * hacnn::STEM_C);
+    m->stem_b = take(hacnn::STEM_C);
+    auto conv = [&](RnConv& c, int K, int N) {
+        const size_t w = take((size_t)K * N);
+        c.b = take(N);
+        pack.add(c.w, w, K, N);
+    };
+    auto inception_b = [&](RnConv* cv, int cin, int cout) {
+        const int mid = cout / 4;
+        conv(cv[0], cin, mid);
+        conv(cv[1], 9 * mid, mid);
+        conv(cv[2], cin, mid);
+        conv(cv[3], 9 * mid, mid);
+        conv(cv[4], 9 * mid, mid);
+        conv(cv[5], cin, 2 * mid);
+    };
+    HacnnW& h = m->ha;
+    for (int i = 0; i < 3; ++i) {
+        const int cin = kC[i], c = kC[i + 1], mid = c / 4, r = c / 16;
+        for (int s = 0; s < 3; ++s) {
+            conv(h.ia[i][2 * s], cin, mid);
+            conv(h.ia[i][2 * s + 1], 9 * mid, mid);
+        }
+        conv(h.ia[i][6], cin, mid);
+        inception_b(h.ib[i], c, c);
+        const size_t sizes[9] = {12, (size_t)c * r, (size_t)r, (size_t)r * c, (size_t)c, (size_t)c * c, (size_t)c,
+                                 (size_t)c * 8, 8};
+        for (int k = 0; k < 9; ++k) h.att[i][k] = take(sizes[k]);
+    }
+    for (int i = 0; i < 3; ++i) inception_b(h.lb[i], kC[i], kC[i + 1]);
+    conv(h.fcg, hacnn::C3, hacnn::HALF);
+    conv(h.fcl, 4 * hacnn::C3, hacnn::HALF);
+    // per crop: the crop; two maps as large as the stem output (80x32x32, also x1_out 40x16x128) for the previous and
+    // the current level; InceptionA's output (at most 80x32x128); three stream scratch maps and the local branch's
+    // STN map and local map (each at most 4 x 24x28x32); the attention's s (40x16) and v (384), theta (24), the two
+    // heads' pools (384 + 1536) and the head row (1024): 0.96 M floats, below OSNet_x1_0's 2.36 M, so the chunk keeps
+    // its size.
+    constexpr size_t kLocal = (size_t)4 * 24 * 28 * 32;
+    Workspace ws;
+    ws.blob = (size_t)hacnn::IN_H * hacnn::IN_W * 3;
+    ws.bufA = ws.bufB = (size_t)80 * 32 * 32;
+    ws.x1 = (size_t)80 * 32 * 128;
+    ws.Y[0][0] = ws.Y[0][1] = ws.Y[1][0] = ws.Y[1][1] = ws.Y[2][0] = kLocal;
+    ws.sums[0] = hacnn::MAX_HW;
+    ws.sums[1] = hacnn::MAX_C;
+    ws.sums[2] = hacnn::FEAT;
+    ws.gates = hacnn::THETA;
+    ws.pooled = 5 * hacnn::C3;
+    return ws;
+}
+
 // ---- CLIP-ReID ViT-B/16 (reid/backbones/clip): patch embedding, ln_pre, 12 residual attention blocks, head ----
 Workspace layout_clip(ReidModel* m, BlobCursor& take, WgmmaPack& pack) {
     constexpr int D = vit::D;
@@ -1871,7 +1944,7 @@ ReidModel* reid_load(const char* path) {
     if (!f) throw std::runtime_error(std::string("cannot open ReID blob: ") + path);
     int32_t hdr[16];
     f.read(reinterpret_cast<char*>(hdr), sizeof(hdr));
-    if (!f || (uint32_t)hdr[0] != BLOB_MAGIC || hdr[1] != 1 || hdr[2] < ARCH_OSNET || hdr[2] > ARCH_MLFN)
+    if (!f || (uint32_t)hdr[0] != BLOB_MAGIC || hdr[1] != 1 || hdr[2] < ARCH_OSNET || hdr[2] > ARCH_HACNN)
         throw std::runtime_error("not a version-1 .b200reid blob (export it with boxmot_b200.weights.export_blob)");
     ReidModel* m = new ReidModel();
     try {
@@ -1893,6 +1966,7 @@ ReidModel* reid_load(const char* path) {
             case ARCH_RESNET: ws = layout_resnet(m, hdr, take, pack); break;
             case ARCH_CLIP: ws = layout_clip(m, take, pack); break;
             case ARCH_MLFN: ws = layout_mlfn(m, take, pack); break;
+            case ARCH_HACNN: ws = layout_hacnn(m, take, pack); break;
             default: ws = layout_osnet(m, hdr, take); break;
         }
         if (take.o != n_floats) throw std::runtime_error("ReID blob size does not match its header");
@@ -1934,6 +2008,7 @@ ReidModel* reid_load(const char* path) {
         alloc(m->in_tmp, ws.in_tmp);
         alloc(m->trunk, ws.trunk);
         alloc(m->pooled, ws.pooled);
+        if (m->arch == ARCH_HACNN) RCUDA_OK(cudaMalloc(&m->d_n4, sizeof(int)));
         // tensor-core path: the default wherever its kernel instances cover the widths (BOXMOT_B200_REID_FP32=1
         // keeps the float32 CUDA-core kernels of round 1, e.g. for A/B runs)
         if (osnet_family) {
@@ -1952,6 +2027,7 @@ void reid_free(ReidModel* m) {
     cudaFree(m->d_w); cudaFree(m->d_wtc); cudaFree(m->blob); cudaFree(m->bufA); cudaFree(m->bufB); cudaFree(m->x1);
     for (int b = 0; b < 4; ++b) { cudaFree(m->Y[b][0]); cudaFree(m->Y[b][1]); cudaFree(m->sums[b]); }
     cudaFree(m->gates); cudaFree(m->trunk); cudaFree(m->pooled); cudaFree(m->in_tmp); cudaFree(m->d_wrn);
+    cudaFree(m->d_n4);
     tcx::plan_free(m->tc);
     delete m;
 }
@@ -2146,7 +2222,11 @@ struct Launcher {
         const int BN = rn::tile_n(a.N);
         const dim3 grid((unsigned)(((size_t)upper * a.Ho * a.Wo + rn::BM - 1) / rn::BM), (unsigned)(a.N / BN));
         begin(a.k0 == 3 ? CLS_LIGHTCONV : CLS_POINTWISE);
-        if (a.relu == 3) {   // relu(residual + relu(acc + bias)): MLFN's fm_conv3
+        if (a.out_ld) {   // a stream's channel slice of a concatenated map (HACNN)
+            if (BN == 128) conv_tc_slice<128>(a, grid);
+            else if (BN == 64) conv_tc_slice<64>(a, grid);
+            else conv_tc_slice<32>(a, grid);
+        } else if (a.relu == 3) {   // relu(residual + relu(acc + bias)): MLFN's fm_conv3
             if (BN == 128) {
                 RCUDA_OK(cudaFuncSetAttribute(rn::k_conv_tc<128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rn::smem_bytes<128>()));
                 rn::k_conv_tc<128, true><<<grid, rn::THREADS, rn::smem_bytes<128>(), st>>>(a, d_n, off, cap);
@@ -2161,6 +2241,53 @@ struct Launcher {
             RCUDA_OK(cudaFuncSetAttribute(rn::k_conv_tc<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rn::smem_bytes<64>()));
             rn::k_conv_tc<64><<<grid, rn::THREADS, rn::smem_bytes<64>(), st>>>(a, d_n, off, cap);
         }
+        end();
+    }
+    template <int BN>
+    void conv_tc_slice(const rn::ConvArgs& a, dim3 grid) {
+        RCUDA_OK(cudaFuncSetAttribute(rn::k_conv_tc<BN, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rn::smem_bytes<BN>()));
+        rn::k_conv_tc<BN, false, true><<<grid, rn::THREADS, rn::smem_bytes<BN>(), st>>>(a, d_n, off, cap);
+    }
+    // HACNN: the 3x3 stride-2 stem of the 160x64 crop, timed under `stem`
+    void hacnn_stem(const float* blob, const float* w, const float* b, float* out) {
+        begin(CLS_STEM);
+        hacnn::k_stem<<<m->sms * 8, 256, 0, st>>>(blob, w, b, d_n, off, cap, out);
+        end();
+    }
+    // HACNN: 3x3 pad-1 pool of x [imgs][H][Wd][C], the max at stride 2 or the average (/ 9) at stride 1
+    void hacnn_pool(bool max, const float* x, int H, int Wd, int C, float* out) {
+        begin(max ? CLS_MAXPOOL : CLS_AVGPOOL);
+        if (max) hacnn::k_pool3<true><<<m->sms * 8, 256, 0, st>>>(x, H, Wd, C, 2, d_n, off, cap, out);
+        else hacnn::k_pool3<false><<<m->sms * 8, 256, 0, st>>>(x, H, Wd, C, 1, d_n, off, cap, out);
+        end();
+    }
+    // HACNN: the soft attention's s and v and the hard attention's theta of x [crops][H][Wd][C], timed under `gates`
+    void hacnn_attn(const float* x, int H, int Wd, int C, const hacnn::AttnW& a, int level, float* s, float* v,
+                    float* theta) {
+        begin(CLS_GATES);
+        hacnn::k_attn<<<upper, 256, 0, st>>>(x, H, Wd, C, a, level, d_n, off, cap, s, v, theta);
+        end();
+    }
+    void hacnn_attn_apply(float* x, int HW, int C, const float* s, const float* v, const float* b) {
+        begin(CLS_GATES);
+        hacnn::k_attn_apply<<<m->sms * 8, 256, 0, st>>>(x, HW, C, s, v, b, d_n, off, cap);
+        end();
+    }
+    // HACNN: the four regions' STN samples of src, resized to h x w (+ prev) into [crops][4][h][w][C], under `gates`
+    void hacnn_stn(const float* src, int H, int Wd, int C, const float* theta, const float* prev, int h, int w,
+                   float* out) {
+        begin(CLS_GATES);
+        hacnn::k_stn<<<m->sms * 8, 256, 0, st>>>(src, H, Wd, C, theta, prev, h, w, d_n, off, cap, out);
+        end();
+    }
+    void hacnn_head_pool(const float* x3, int HW3, const float* loc, int HWl, float* pg, float* pl) {
+        begin(CLS_HEAD);
+        hacnn::k_head_pool<<<upper, 256, 0, st>>>(x3, HW3, loc, HWl, d_n, off, cap, pg, pl);
+        end();
+    }
+    void hacnn_head(const float* v, const CropDesc* crops, float* out, int out_ld) {
+        begin(CLS_HEAD);
+        hacnn::k_head<<<upper, 256, 0, st>>>(v, crops, d_n, off, cap, out, out_ld);
         end();
     }
     // MLFN: grouped 3x3 (+ bias, ReLU, gate) of x [crops][H][Wd][C], group width gw, timed under `lightconv`
@@ -2656,6 +2783,92 @@ void run_mlfn_chunk(Launcher& L, const FrameIn& fi, float* d_out, int out_ld) {
     if (tap) stop_here(m->sums[2], mlfn::FEAT);
 }
 
+hacnn::AttnW hacnn_attn_w(const float* W, const size_t* o) {
+    return hacnn::AttnW{W + o[0], W + o[1], W + o[2], W + o[3], W + o[4], W + o[5], W + o[6], W + o[7], W + o[8]};
+}
+
+// HACNN, one chunk (hacnn.py HACNN.forward, eval).  Taps: 0 crop (160x64x3), 1 stem (80x32x32), 2 + i x_{i+1}_out
+// (i = 0 .. 2: 40x16x128, 20x8x256, 10x4x384), 5 + i the local map of level i + 1 ([region][h][w][C]: 4 x 12x14x128,
+// 4 x 6x7x256, 4 x 3x4x384), 8 theta ([level][region][tx, ty], 24), 9 the head row [fc_global | fc_local] before the
+// normalisations (1024).  Per level: InceptionA and InceptionB on k_conv_tc, every stream storing its slice of the
+// concatenated map; the attention (s, v, theta) of the InceptionB output; the STN of the previous level's output
+// (the stem for level 1) resized and added to the previous local map; the local InceptionB over the chunk's
+// 4 x crops regions (a second Launcher whose device count is 4 x the crop count); then x *= attention.  The head
+// pools both branches, runs fc_global / fc_local (BatchNorm1d folded, ReLU) on k_conv_tc over a [crops] x 1 map into
+// the two halves of the head row, and normalises.  Timing classes: 1x1 `pointwise_gemm`, 3x3 `lightconv`, pools
+// `maxpool` / `avgpool`, attention and STN `gates`, the head `head`.
+void run_hacnn_chunk(Launcher& L, const FrameIn& fi, float* d_out, int out_ld) {
+    ReidModel* m = L.m;
+    const float* W = m->d_w;
+    const HacnnW& h = m->ha;
+    auto tap = [&](int idx, const float* p, size_t per_crop) {
+        if (m->debug_stop != idx) return false;
+        m->debug_ptr = p;
+        m->debug_floats_per_crop = per_crop;
+        return true;
+    };
+    stage_crops(L, fi);
+    if (tap(0, m->blob, (size_t)hacnn::IN_H * hacnn::IN_W * 3)) return;
+    L.hacnn_stem(m->blob, W + m->stem_w, W + m->stem_b, m->bufA);
+    if (tap(1, m->bufA, (size_t)80 * 32 * hacnn::STEM_C)) return;
+    L.begin(CLS_GATES);
+    hacnn::k_count4<<<1, 1, 0, L.st>>>(L.d_n, m->d_n4);
+    L.end();
+    Launcher R{m, m->d_n4, 4 * L.off, 4 * L.cap, 4 * L.upper, L.st};   // the local branch: [crop][region] images
+    auto conv = [&](Launcher& La, const float* in, int H, int Wd, int cin, int k, int stride, const RnConv& cv, int N,
+                    float* out, int ld) {
+        rn::ConvArgs c{};
+        c.in0 = in; c.H0 = H; c.W0 = Wd; c.C0 = cin; c.k0 = k; c.s0 = stride;
+        c.w = cv.w; c.bias = W + cv.b; c.out = out;
+        c.Ho = (H - 1) / stride + 1; c.Wo = (Wd - 1) / stride + 1; c.N = N; c.relu = 1; c.out_ld = ld;
+        La.conv_tc(c);
+    };
+    auto inception_b = [&](Launcher& La, const RnConv* cv, const float* x, int H, int Wd, int cin, int cout, float* out) {
+        const int mid = cout / 4;
+        conv(La, x, H, Wd, cin, 1, 1, cv[0], mid, m->Y[0][0], mid);
+        conv(La, m->Y[0][0], H, Wd, mid, 3, 2, cv[1], mid, out, cout);
+        conv(La, x, H, Wd, cin, 1, 1, cv[2], mid, m->Y[0][0], mid);
+        conv(La, m->Y[0][0], H, Wd, mid, 3, 1, cv[3], mid, m->Y[0][1], mid);
+        conv(La, m->Y[0][1], H, Wd, mid, 3, 2, cv[4], mid, out + mid, cout);
+        La.hacnn_pool(true, x, H, Wd, cin, m->Y[1][0]);
+        conv(La, m->Y[1][0], (H - 1) / 2 + 1, (Wd - 1) / 2 + 1, cin, 1, 1, cv[5], 2 * mid, out + 2 * mid, cout);
+    };
+    static const int kC[4] = {hacnn::STEM_C, 128, 256, hacnn::C3};
+    static const int kLocal[3][2] = {{24, 28}, {12, 14}, {6, 7}};
+    float *prev = m->bufA, *cur = m->bufB, *T = m->Y[1][1], *Lc = m->Y[2][0];
+    int H = 80, Wd = 32;
+    for (int i = 0; i < 3; ++i) {
+        const int cin = kC[i], c = kC[i + 1], mid = c / 4, Hc = H / 2, Wc = Wd / 2;
+        for (int s = 0; s < 3; ++s) {   // InceptionA into x1, then InceptionB into cur
+            conv(L, prev, H, Wd, cin, 1, 1, h.ia[i][2 * s], mid, m->Y[0][0], mid);
+            conv(L, m->Y[0][0], H, Wd, mid, 3, 1, h.ia[i][2 * s + 1], mid, m->x1 + s * mid, c);
+        }
+        L.hacnn_pool(false, prev, H, Wd, cin, m->Y[1][0]);
+        conv(L, m->Y[1][0], H, Wd, cin, 1, 1, h.ia[i][6], mid, m->x1 + 3 * mid, c);
+        inception_b(L, h.ib[i], m->x1, H, Wd, c, c, cur);
+        L.hacnn_attn(cur, Hc, Wc, c, hacnn_attn_w(W, h.att[i]), i, m->sums[0], m->sums[1], m->gates);
+        const int lh = kLocal[i][0], lw = kLocal[i][1];
+        L.hacnn_stn(prev, H, Wd, cin, m->gates + 8 * i, i ? Lc : nullptr, lh, lw, T);
+        inception_b(R, h.lb[i], T, lh, lw, cin, c, Lc);
+        L.hacnn_attn_apply(cur, Hc * Wc, c, m->sums[0], m->sums[1], W + h.att[i][6]);
+        L.launches += R.launches;
+        R.launches = 0;
+        if (tap(2 + i, cur, (size_t)Hc * Wc * c) ||
+            tap(5 + i, Lc, (size_t)4 * ((lh - 1) / 2 + 1) * ((lw - 1) / 2 + 1) * c))
+            return;
+        std::swap(prev, cur);
+        H = Hc; Wd = Wc;
+    }
+    if (tap(8, m->gates, hacnn::THETA)) return;
+    float* pg = m->pooled;
+    float* pl = m->pooled + (size_t)m->chunk * hacnn::C3;
+    L.hacnn_head_pool(prev, H * Wd, Lc, 3 * 4, pg, pl);
+    conv(L, pg, 1, 1, hacnn::C3, 1, 1, h.fcg, hacnn::HALF, m->sums[2], hacnn::FEAT);
+    conv(L, pl, 1, 1, 4 * hacnn::C3, 1, 1, h.fcl, hacnn::HALF, m->sums[2] + hacnn::HALF, hacnn::FEAT);
+    if (tap(9, m->sums[2], hacnn::FEAT)) return;
+    L.hacnn_head(m->sums[2], fi.crops, d_out, out_ld);
+}
+
 // MobileNetV2, one chunk: stem -> [expand 1x1 + ReLU6 -> depthwise 3x3 + ReLU6 -> project 1x1 (+ residual)] x 17 ->
 // conv9 -> GAP.  No debug taps.
 void run_mobilenetv2_chunk(Launcher& L, const FrameIn& fi, float* d_out, int out_ld) {
@@ -2750,6 +2963,7 @@ void run_chunk(Launcher& L, const FrameIn& fi, float* d_out, int out_ld) {
         case ARCH_RESNET: run_resnet_chunk(L, fi, d_out, out_ld); return;
         case ARCH_CLIP: run_clip_chunk(L, fi, d_out, out_ld); return;
         case ARCH_MLFN: run_mlfn_chunk(L, fi, d_out, out_ld); return;
+        case ARCH_HACNN: run_hacnn_chunk(L, fi, d_out, out_ld); return;
     }
 }
 }  // namespace
@@ -3341,6 +3555,121 @@ void standalone_f32_lmbn_head(const float* x, int n, int h, int w, const float* 
     r.L.l2_normalise(d_c, d_out, out_ld, LMBN_VECS * C);
     r.down(pooled, d_p, pooled_floats);
     r.down(out, d_out, out_floats);
+}
+
+// ---- HACNN kernels on their own (parity tests), with the crop window and whole-array round trip described above ----
+// One ConvBlock on k_conv_tc's SLICE instances: in (n,h,w,c0), weight (k*k*c0, N) K-major, out (n,Ho,Wo,out_ld) with
+// columns out_off .. out_off + N - 1 = relu(conv(in) + bias); the other columns come back as given.
+void standalone_hacnn_conv(const float* in, int n, int off, int count, int h, int w, int c0, int k, int stride,
+                           const float* weight, int N, const float* bias, float* out, int out_ld, int out_off) {
+    need(h > 0 && w > 0 && c0 > 0 && c0 % rn::KC == 0 && (k == 1 || k == 3) && (stride == 1 || stride == 2) && N > 0 &&
+             N % 32 == 0 && out_off >= 0 && out_off % 2 == 0 && out_ld % 2 == 0 && out_off + N <= out_ld,
+         "h, w > 0, c0 a multiple of 32, k 1 or 3, stride 1 or 2, N a multiple of 32, even out_off and out_ld, "
+         "out_off + N <= out_ld required");
+    StandaloneRun r(n, off, count);
+    const int Ho = (h - 1) / stride + 1, Wo = (w - 1) / stride + 1, K = k * k * c0;
+    std::vector<float> packed(2 * (size_t)K * N);
+    rn::pack_conv_weights(weight, K, N, packed.data());
+    const size_t out_floats = (size_t)n * Ho * Wo * out_ld;
+    float* d_out = r.up(out, out_floats);
+    rn::ConvArgs c{};
+    c.in0 = r.up(in, (size_t)n * h * w * c0); c.H0 = h; c.W0 = w; c.C0 = c0; c.k0 = k; c.s0 = stride;
+    c.w = r.up(packed.data(), packed.size()); c.bias = r.up(bias, N); c.out = d_out + out_off;
+    c.Ho = Ho; c.Wo = Wo; c.N = N; c.relu = 1; c.out_ld = out_ld;
+    r.L.conv_tc(c);
+    r.down(out, d_out, out_floats);
+}
+
+// op 0: the 3x3 stride-2 stem, in (n,160,64,3), weight (27,32), bias (32) -> out (n,80,32,32);
+// op 1: 3x3 stride-1 pad-1 average (/ 9), op 2: 3x3 stride-2 pad-1 max, in (n,h,w,c) -> out (n,Ho,Wo,c)
+void standalone_hacnn_map(int op, const float* in, int n, int off, int count, int h, int w, int c, const float* weight,
+                          const float* bias, float* out) {
+    need(op >= 0 && op <= 2, "op 0 (stem), 1 (average pool) or 2 (max pool) required");
+    if (op == 0) need(h == hacnn::IN_H && w == hacnn::IN_W && c == 3, "stem: 160 x 64 x 3 crops");
+    else need(h > 0 && w > 0 && c > 0 && c % 4 == 0, "pools: h, w > 0 and c a multiple of 4");
+    StandaloneRun r(n, off, count);
+    const int s = op == 2 ? 2 : (op == 0 ? 2 : 1), co = op == 0 ? hacnn::STEM_C : c;
+    const size_t out_floats = (size_t)n * ((h - 1) / s + 1) * ((w - 1) / s + 1) * co;
+    const float* d_in = r.up(in, (size_t)n * h * w * c);
+    float* d_out = r.up(out, out_floats);
+    if (op == 0) r.L.hacnn_stem(d_in, r.up(weight, (size_t)27 * hacnn::STEM_C), r.up(bias, hacnn::STEM_C), d_out);
+    else r.L.hacnn_pool(op == 2, d_in, h, w, c, d_out);
+    r.down(out, d_out, out_floats);
+}
+
+// The attention of one level as run_hacnn_chunk launches it: x (n,h,w,c) -> out (n,h,w,c) = x * sigmoid(relu(
+// s[p] v[o] + b[o])), s (n,h*w), v (n,c), and columns 8 level .. 8 level + 7 of theta (n,24); params holds the level's
+// arrays in blob order (sp[12], w1[c][c/16], b1, w2[c/16][c], b2, wv[c][c], bv, wfc[c][8], bfc), each padded to 4.
+void standalone_hacnn_attention(const float* x, int n, int off, int count, int h, int w, int c, int level,
+                                const float* params, float* out, float* s, float* v, float* theta) {
+    need(h > 1 && w > 1 && h % 2 == 0 && w % 2 == 0 && h * w <= hacnn::MAX_HW && c > 0 && c % 16 == 0 &&
+             c <= hacnn::MAX_C && level >= 0 && level < 3,
+         "even h, w > 1 with h w <= 640, c a multiple of 16 up to 384, level 0..2 required");
+    StandaloneRun r(n, off, count);
+    const int R = c / 16;
+    const size_t sizes[9] = {12, (size_t)c * R, (size_t)R, (size_t)R * c, (size_t)c, (size_t)c * c, (size_t)c,
+                             (size_t)c * 8, 8};
+    size_t o[9], total = 0;
+    for (int k = 0; k < 9; ++k) { o[k] = total; total += (sizes[k] + 3) / 4 * 4; }
+    const float* d_p = r.up(params, total);
+    const size_t nx = (size_t)n * h * w * c;
+    float* d_out = r.up(out, nx);
+    float* d_s = r.up(s, (size_t)n * h * w);
+    float* d_v = r.up(v, (size_t)n * c);
+    float* d_t = r.up(theta, (size_t)n * hacnn::THETA);
+    RCUDA_OK(cudaMemcpy(d_out, x, sizeof(float) * nx, cudaMemcpyHostToDevice));   // the apply runs in place
+    const hacnn::AttnW a = hacnn_attn_w(d_p, o);
+    r.L.hacnn_attn(d_out, h, w, c, a, level, d_s, d_v, d_t);
+    r.L.hacnn_attn_apply(d_out, h * w, c, d_s, d_v, a.bv);
+    r.down(out, d_out, nx);
+    r.down(s, d_s, (size_t)n * h * w);
+    r.down(v, d_v, (size_t)n * c);
+    r.down(theta, d_t, (size_t)n * hacnn::THETA);
+}
+
+// The STN resample of one level: src (n,H,W,C), theta (n,24) (columns 8 level .. + 7), prev (n,4,lh,lw,C) or null
+// -> out (n,4,lh,lw,C)
+void standalone_hacnn_stn(const float* src, int n, int off, int count, int H, int W, int C, const float* theta,
+                          int level, const float* prev, int lh, int lw, float* out) {
+    need(H > 1 && W > 1 && C > 0 && C % 4 == 0 && lh > 1 && lw > 1 && level >= 0 && level < 3,
+         "H, W, lh, lw > 1, C a multiple of 4, level 0..2 required");
+    StandaloneRun r(n, off, count);
+    const size_t nl = (size_t)n * 4 * lh * lw * C;
+    const float* d_t = r.up(theta, (size_t)n * hacnn::THETA);
+    float* d_out = r.up(out, nl);
+    r.L.hacnn_stn(r.up(src, (size_t)n * H * W * C), H, W, C, d_t + 8 * level, r.up(prev, nl), lh, lw, d_out);
+    r.down(out, d_out, nl);
+}
+
+// The head: x3 (n,hw3,384) and loc (n,4,hwl,384) pooled, fc_global wg (384,512) + bg and fc_local wl (1536,512) + bl
+// (K-major, BatchNorm1d folded) with ReLU into v (n,1024), then the normalised row of window crop i into out row
+// rows[off + i] (rows has off + n entries; out (out_rows,1024)).
+void standalone_hacnn_head(const float* x3, int n, int off, int count, int hw3, const float* loc, int hwl,
+                           const float* wg, const float* bg, const float* wl, const float* bl, const int* rows,
+                           int out_rows, float* out, float* v) {
+    need(hw3 > 0 && hwl > 0 && out_rows > 0, "hw3, hwl, out_rows > 0 required");
+    for (int i = 0; i < off + n; ++i) need(rows[i] >= 0 && rows[i] < out_rows, "rows must lie in [0, out_rows)");
+    StandaloneRun r(n, off, count);
+    constexpr int C = hacnn::C3, F = hacnn::HALF;
+    std::vector<float> pg(2 * (size_t)C * F), pl(2 * (size_t)4 * C * F);
+    rn::pack_conv_weights(wg, C, F, pg.data());
+    rn::pack_conv_weights(wl, 4 * C, F, pl.data());
+    float* pooled = r.up(std::vector<float>((size_t)n * 5 * C, 0.f).data(), (size_t)n * 5 * C);
+    float* d_v = r.up(v, (size_t)n * hacnn::FEAT);
+    float* d_out = r.up(out, (size_t)out_rows * hacnn::FEAT);
+    r.L.hacnn_head_pool(r.up(x3, (size_t)n * hw3 * C), hw3, r.up(loc, (size_t)n * 4 * hwl * C), hwl, pooled,
+                        pooled + (size_t)n * C);
+    auto fc = [&](const float* in, int K, const float* w, const float* b, float* o) {
+        rn::ConvArgs a{};
+        a.in0 = in; a.H0 = 1; a.W0 = 1; a.C0 = K; a.k0 = 1; a.s0 = 1;
+        a.w = w; a.bias = b; a.out = o; a.Ho = 1; a.Wo = 1; a.N = F; a.relu = 1; a.out_ld = hacnn::FEAT;
+        r.L.conv_tc(a);
+    };
+    fc(pooled, C, r.up(pg.data(), pg.size()), r.up(bg, F), d_v);
+    fc(pooled + (size_t)n * C, 4 * C, r.up(pl.data(), pl.size()), r.up(bl, F), d_v + F);
+    r.L.hacnn_head(d_v, r.crops(rows, off + n), d_out, hacnn::FEAT);
+    r.down(v, d_v, (size_t)n * hacnn::FEAT);
+    r.down(out, d_out, (size_t)out_rows * hacnn::FEAT);
 }
 
 }  // namespace bmb

@@ -19,7 +19,10 @@
 //     unconditionally, with BN a template parameter.
 // Epilogue: bias, optional residual, then relu = 0 none / 1 ReLU / 2 QuickGELU, float2 stores into NHWC [M][N].  The
 // RELU_RES instances (relu = 3) compute relu(residual + relu(acc + bias)) instead: MLFN's fm_conv3, whose ReLU comes
-// before the residual add.  They are separate instances so that the default ones keep their code.
+// before the residual add.  They are separate instances so that the default ones keep their code.  The SLICE
+// instances (HACNN's Inception streams, BN 32 / 64 / 128) store row m at out + m * out_ld instead of out + m * N, so
+// that each stream writes its channel slice of the concatenated map in place (the caller offsets `out` by the slice's
+// first channel).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -46,6 +49,7 @@ struct ConvArgs {
     int H0, W0, C0, k0, s0;  // k0 in {1, 3} (pad k0 / 2), stride s0
     int H1, W1, C1, s1;
     int Ho, Wo, N, relu;     // relu: 0 none, 1 ReLU, 2 QuickGELU, 3 relu(residual + relu(.)) (RELU_RES instances)
+    int out_ld;              // SLICE instances: floats between output rows (0: the default [M][N] store)
 };
 
 // canonical (no swizzle, K-major) offset in floats of element (row, k) in a block whose K extent is KC
@@ -62,7 +66,7 @@ constexpr size_t smem_bytes() {
     return sizeof(float) * (size_t)STAGES * (2 * BM * KC + 2 * BN * KC) + 128;
 }
 
-template <int BN, bool RELU_RES = false>
+template <int BN, bool RELU_RES = false, bool SLICE = false>
 __global__ void __launch_bounds__(THREADS, 1) k_conv_tc(const ConvArgs a, const int* __restrict__ d_n, int off, int cap) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     __shared__ __align__(8) uint64_t bar[STAGES];
@@ -181,7 +185,7 @@ __global__ void __launch_bounds__(THREADS, 1) k_conv_tc(const ConvArgs a, const 
     for (int h = 0; h < 2; ++h) {
         const int m = m0 + row + 8 * h;
         if (m >= M) continue;
-        float* dst = a.out + (size_t)m * a.N + n0;
+        float* dst = a.out + (size_t)m * (SLICE ? a.out_ld : a.N) + n0;
         const float* res = a.residual ? a.residual + (size_t)m * a.N + n0 : nullptr;
 #pragma unroll
         for (int i = 0; i < BN / 8; ++i) {
@@ -208,8 +212,9 @@ __global__ void __launch_bounds__(THREADS, 1) k_conv_tc(const ConvArgs a, const 
     }
 }
 
-// output-channel tile of a layer: 64 for N = 64 (layer1's conv1 / conv2), 128 otherwise
-inline int tile_n(int N) { return N % 128 == 0 ? 128 : 64; }
+// output-channel tile of a layer: 128 when it divides N, else 64 (ResNet's layer1 conv1 / conv2), else 32 (HACNN's
+// 32- and 96-wide streams, SLICE instances only)
+inline int tile_n(int N) { return N % 128 == 0 ? 128 : (N % 64 == 0 ? 64 : 32); }
 
 // host: W [K][N] (K-major rows of N) -> [N / BN][K / KC][hi | lo][BN x KC canonical]; K % KC == 0, N % BN == 0
 inline void pack_conv_weights(const float* w, int K, int N, float* out) {

@@ -362,6 +362,79 @@ def make_mlfn_state(seed: int = 0, num_classes: int = 751):
     return sd
 
 
+# HACNN (reid/backbones/hacnn.py, nchannels 128 / 256 / 384, feat_dim 512, learn_region=True): 160x64 crops
+HACNN_CH = (128, 256, 384)
+HACNN_FEAT = 512
+HACNN_INPUT_HW = (160, 64)
+HACNN_HARD_BIAS = (0.0, -0.75, 0.0, -0.25, 0.0, 0.25, 0.0, 0.75)   # HardAttn.init_params
+
+
+def _inception_a(p, cin, cout):
+    mid = cout // 4
+    return [(f"{p}.stream{s}.{j}", "cb", (mid, cin if j == 0 else mid, 1 if j == 0 else 3, 1 if j == 0 else 3))
+            for s in (1, 2, 3) for j in (0, 1)] + [(f"{p}.stream4.1", "cb", (mid, cin, 1, 1))]
+
+
+def _inception_b(p, cin, cout):
+    mid = cout // 4
+    return [(f"{p}.stream1.0", "cb", (mid, cin, 1, 1)), (f"{p}.stream1.1", "cb", (mid, mid, 3, 3)),
+            (f"{p}.stream2.0", "cb", (mid, cin, 1, 1)), (f"{p}.stream2.1", "cb", (mid, mid, 3, 3)),
+            (f"{p}.stream2.2", "cb", (mid, mid, 3, 3)), (f"{p}.stream3.1", "cb", (2 * mid, cin, 1, 1))]
+
+
+def hacnn_layout():
+    """[(parameter prefix, kind, shape)] of the reference's HACNN in blob order: kind "cb" is a ConvBlock (conv weight
+    `shape` and bias, BatchNorm2d), "lin" an nn.Linear (weight `shape`, bias), "bn" a BatchNorm1d of shape[0].  The
+    classifiers are not listed."""
+    out = [("conv", "cb", (32, 3, 3, 3))]
+    cin = 32
+    for i, c in enumerate(HACNN_CH, 1):
+        out += _inception_a(f"inception{i}.0", cin, c) + _inception_b(f"inception{i}.1", c, c)
+        h = f"ha{i}"
+        out += [(h + ".soft_attn.spatial_attn.conv1", "cb", (1, 1, 3, 3)),
+                (h + ".soft_attn.spatial_attn.conv2", "cb", (1, 1, 1, 1)),
+                (h + ".soft_attn.channel_attn.conv1", "cb", (c // 16, c, 1, 1)),
+                (h + ".soft_attn.channel_attn.conv2", "cb", (c, c // 16, 1, 1)),
+                (h + ".soft_attn.conv", "cb", (c, c, 1, 1)),
+                (h + ".hard_attn.fc", "lin", (8, c))]
+        cin = c
+    cin = 32
+    for i, c in enumerate(HACNN_CH, 1):
+        out += _inception_b(f"local_conv{i}", cin, c)
+        cin = c
+    out += [("fc_global.0", "lin", (HACNN_FEAT, HACNN_CH[2])), ("fc_global.1", "bn", (HACNN_FEAT,)),
+            ("fc_local.0", "lin", (HACNN_FEAT, 4 * HACNN_CH[2])), ("fc_local.1", "bn", (HACNN_FEAT,))]
+    return out
+
+
+def make_hacnn_state(seed: int = 0, num_classes: int = 751):
+    """Seeded state dict with the parameter names of the reference's `HACNN(num_classes)` (loads with strict=True).
+    BatchNorm statistics are randomised so folding is exercised, every ConvBlock conv has a non-zero bias, and
+    `hard_attn.fc` has a non-zero weight, so the four regions move off centre and partly off the map."""
+    import torch
+
+    g = torch.Generator().manual_seed(seed)
+    sd = {}
+    conv, bn, _ = _osnet_makers(g, sd)
+    for name, kind, shape in hacnn_layout():
+        if kind == "cb":
+            conv(name + ".conv", shape[0], shape[1], shape[2], gain=2.0)
+            sd[name + ".conv.bias"] = 0.1 * torch.randn(shape[0], generator=g)
+            bn(name + ".bn", shape[0])
+        elif kind == "bn":
+            bn(name, shape[0])
+        elif name.endswith("hard_attn.fc"):
+            sd[name + ".weight"] = 2.0 * torch.randn(*shape, generator=g) / shape[1] ** 0.5
+            sd[name + ".bias"] = torch.tensor(HACNN_HARD_BIAS) + 0.2 * torch.randn(8, generator=g)
+        else:
+            sd[name + ".weight"] = torch.randn(*shape, generator=g) / shape[1] ** 0.5
+            sd[name + ".bias"] = 0.1 * torch.randn(shape[0], generator=g)
+    for name in ("classifier_global", "classifier_local"):
+        sd[name + ".weight"] = 0.01 * torch.randn(num_classes, HACNN_FEAT, generator=g)
+        sd[name + ".bias"] = torch.zeros(num_classes)
+    return sd
+
+
 def make_clip_state(seed: int = 0, vehicle: bool = False, num_classes: int = 751, extras: bool = True):
     """Seeded state dict with the key set of the reference's CLIP-ReID `build_transformer` (ViT-B/16: image_encoder.*,
     bottleneck.*, bottleneck_proj.*, classifier.*, classifier_proj.*); vehicle=True gives the 257-row positional table

@@ -28,6 +28,8 @@ in words 3-7, the input height / width in words 9-10 and the patch grid in words
 `fold_clip`.
 Arch 7 (MLFN, `fold_mlfn`) records the stem width, the last block width, the groups, the block count and the 1024-d
 feature in words 3-7; its layout is listed above `fold_mlfn`.
+Arch 8 (HACNN, `fold_hacnn`) records the stem width and the three Inception widths and the 1024-d feature in words
+3-7 and the 160x64 input in words 9-10; its layout is listed above `fold_hacnn`.
 All 1x1 weights are stored K-major ([cin][cout]) so a thread owning consecutive output channels loads
 consecutive floats; every tensor is zero-padded to a multiple of 4 floats (16-byte aligned float4 loads).
 """
@@ -51,6 +53,8 @@ RESNET_FEAT = 2048
 ARCH_CLIP = 6
 ARCH_MLFN = 7
 MLFN_FEAT = 1024
+ARCH_HACNN = 8
+HACNN_FEAT = 1024
 BRANCHES = (("conv2a", 1), ("conv2b", 2), ("conv2c", 3), ("conv2d", 4))
 EPS = 1e-5
 
@@ -520,6 +524,80 @@ def fold_mlfn(sd) -> List[np.ndarray]:
     return out
 
 
+# HACNN (arch 8): HACNN of reid/backbones/hacnn.py (nchannels 128 / 256 / 384, feat_dim 512, learn_region=True).
+# Header words 3-7 hold 32, 128, 256, 384 and the 1024-d feature, words 9-10 the 160x64 input.  Every ConvBlock has its
+# conv bias and BatchNorm folded; a k x k convolution is stored K-major W[k*k*cin][cout] with k index
+# (kh*k + kw)*cin + ci, then b[cout].  In `hacnn_layout` order:
+#     conv (stem)                          W[27][32], b[32]
+#     per level i = 1..3 (C = 128, 256, 384):
+#         inception{i}.0 (InceptionA)      stream1.0, stream1.1, stream2.0, stream2.1, stream3.0, stream3.1, stream4.1
+#         inception{i}.1 (InceptionB)      stream1.0, stream1.1, stream2.0, stream2.1, stream2.2, stream3.1
+#         ha{i} spatial                    [12]: conv1's 9 taps and bias, conv2's scale and shift (BN folded)
+#         ha{i} channel_attn conv1 / conv2 W[C][C/16], b[C/16]; W[C/16][C], b[C]
+#         ha{i} soft_attn.conv             W[C][C], b[C]
+#         ha{i} hard_attn.fc               W[C][8], b[8]
+#     local_conv1..3 (InceptionB)          as above
+#     fc_global                            W[384][512], b[512]  (BatchNorm1d folded)
+#     fc_local                             W[1536][512], b[512] (BatchNorm1d folded)
+def _hacnn_ignored(k: str) -> bool:
+    return k.startswith(("classifier_global.", "classifier_local.")) or k.endswith("num_batches_tracked")
+
+
+def is_hacnn(sd) -> bool:
+    return "ha1.hard_attn.fc.weight" in sd
+
+
+def _conv_block(sd, name) -> List[np.ndarray]:
+    w = _np(sd[name + ".conv.weight"])   # [co][ci][k][k]
+    scale, shift = _bn_fold(sd, name + ".bn")
+    co, ci, k, _ = w.shape
+    return [(w * scale[:, None, None, None]).transpose(2, 3, 1, 0).reshape(k * k * ci, co),
+            _np(sd[name + ".conv.bias"]) * scale + shift]
+
+
+def fold_hacnn(sd) -> List[np.ndarray]:
+    """HACNN state dict -> arrays of the arch-8 blob.  Only the reference's HACNN with its default nchannels, feat_dim
+    and learn_region=True is supported: any key or shape that differs from it, apart from the classifiers and
+    `num_batches_tracked`, raises a ValueError naming the keys."""
+    from .synthetic import hacnn_layout
+
+    keys = {k for k in sd if not _hacnn_ignored(k)}
+    want = {}
+    for name, kind, shape in hacnn_layout():
+        if kind == "cb":
+            want[name + ".conv.weight"], want[name + ".conv.bias"] = shape, shape[:1]
+            for p in ("weight", "bias", "running_mean", "running_var"):
+                want[f"{name}.bn.{p}"] = shape[:1]
+        elif kind == "bn":
+            for p in ("weight", "bias", "running_mean", "running_var"):
+                want[f"{name}.{p}"] = shape
+        else:
+            want[name + ".weight"], want[name + ".bias"] = shape, shape[:1]
+    bad_shape = sorted(k for k in keys & set(want) if tuple(sd[k].shape) != want[k])[:4]
+    if keys != set(want) or bad_shape:
+        extra, missing = sorted(keys - set(want))[:4], sorted(set(want) - keys)[:4]
+        raise ValueError(f"not a HACNN state dict (unexpected keys {extra}, missing keys {missing}, unexpected shapes "
+                         f"{bad_shape}); only HACNN with nchannels 128/256/384, feat_dim 512 and learn_region=True "
+                         "is supported")
+    out: List[np.ndarray] = []
+    spatial = None
+    for name, kind, shape in hacnn_layout():
+        if name.endswith("spatial_attn.conv1"):
+            spatial = _conv_block(sd, name)
+        elif name.endswith("spatial_attn.conv2"):
+            a, b = _conv_block(sd, name)
+            out.append(np.concatenate([spatial[0].ravel(), spatial[1], a.ravel(), b]))
+        elif kind == "cb":
+            out += _conv_block(sd, name)
+        elif kind == "lin":
+            w, b = _np(sd[name + ".weight"]), _np(sd[name + ".bias"])
+            if name.startswith("fc_"):
+                scale, shift = _bn_fold(sd, name[:-1] + "1")
+                w, b = w * scale[:, None], b * scale + shift
+            out += [w.T.copy(), b]
+    return out
+
+
 def _pad4(n: int) -> int:
     return (n + 3) // 4 * 4
 
@@ -613,9 +691,12 @@ def export_blob(weights, out_path=None) -> Path:
     elif is_mlfn(sd):
         arrays = fold_mlfn(sd)
         arch, dims = ARCH_MLFN, [64, 2048, 32, 16, MLFN_FEAT]
+    elif is_hacnn(sd):
+        arrays = fold_hacnn(sd)
+        arch, dims = ARCH_HACNN, [32, 128, 256, 384, HACNN_FEAT]
     else:
         raise ValueError("only OSNet, OSNet-AIN, OSNet-IBN, MobileNetV2, LMBN_n, ResNet50 / ResNet101, CLIP-ReID "
-                         "ViT-B/16 and MLFN state dicts are implemented on the B200 ReID path")
+                         "ViT-B/16, MLFN and HACNN state dicts are implemented on the B200 ReID path")
     # every tensor starts on a 16-byte boundary (the kernels read weights as float4)
     padded = []
     for a in arrays:
@@ -629,6 +710,8 @@ def export_blob(weights, out_path=None) -> Path:
         header[9:16] = in_modes
     if arch == ARCH_CLIP:
         header[9:13] = extra
+    if arch == ARCH_HACNN:
+        header[9:11] = [160, 64]
     out_path = Path(out_path)
     tmp = out_path.with_suffix(out_path.suffix + ".tmp")
     with open(tmp, "wb") as f:

@@ -443,6 +443,34 @@ BOXMOT_B200_API int boxmot_b200_mlfn_group_conv(const float* in, int n, int h, i
 BOXMOT_B200_API int boxmot_b200_mlfn_fsm(const float* x, int n, int h, int w, int c, const float* w1, const float* b1,
                                          int f0, const float* w2, const float* b2, int f1, const float* w3,
                                          const float* b3, float* out);
+/* The HACNN kernels on their own, over a crop window as for the float32 kernels below (n crops in the arrays, device
+ * count `count`, window start `off`; every output array uploaded as given and read back whole), NHWC float32.
+ * hacnn_conv: one ConvBlock on the tensor cores (the Inception streams' SLICE store): in (n,h,w,c0), c0 a multiple of
+ * 32, k 1 or 3 (pad k/2), stride 1 or 2, weight (k*k*c0, N) K-major with k index (kh*k + kw)*c0 + ci, N a multiple of
+ * 32; out (n,Ho,Wo,out_ld) columns out_off .. out_off + N - 1 = relu(conv + bias), Ho = (h - 1) / stride + 1.
+ * hacnn_map: op 0 the 3x3 stride-2 stem (in (n,160,64,3), weight (27,32) as above, bias (32) -> (n,80,32,32), ReLU),
+ * op 1 the 3x3 stride-1 pad-1 average pool (/ 9), op 2 the 3x3 stride-2 pad-1 max pool (odd sizes: Ho = (h - 1) / 2 + 1).
+ * hacnn_attention: x (n,h,w,c), even h, w with h w <= 640, c a multiple of 16 up to 384, params the level's attention
+ * arrays in blob order (each padded to 4 floats): out = x * sigmoid(relu(s[p] v[o] + bv[o])) with s (n,h*w) the
+ * spatial map and v (n,c) = W c, and theta (n,24) columns 8 level .. 8 level + 7 = tanh(fc(mean_hw(x))).
+ * hacnn_stn: src (n,H,W,C), theta (n,24) columns 8 level .., prev (n,4,lh,lw,C) or NULL -> out (n,4,lh,lw,C) = the four
+ * regions' affine_grid + grid_sample of src (align_corners=False, zero padding), resized to lh x lw with
+ * align_corners=True (+ prev).
+ * hacnn_head: x3 (n,hw3,384), loc (n,4,hwl,384) -> v (n,1024) = [relu(mean(x3) wg + bg) | relu(mean(loc) wl + bl)]
+ * (wg (384,512), wl (1536,512) K-major) and out row rows[off + i] = v_i with each half L2-normalised, then the row. */
+BOXMOT_B200_API int boxmot_b200_hacnn_conv(const float* in, int n, int off, int count, int h, int w, int c0, int k,
+                                           int stride, const float* weight, int N, const float* bias, float* out,
+                                           int out_ld, int out_off);
+BOXMOT_B200_API int boxmot_b200_hacnn_map(int op, const float* in, int n, int off, int count, int h, int w, int c,
+                                          const float* weight, const float* bias, float* out);
+BOXMOT_B200_API int boxmot_b200_hacnn_attention(const float* x, int n, int off, int count, int h, int w, int c,
+                                                int level, const float* params, float* out, float* s, float* v,
+                                                float* theta);
+BOXMOT_B200_API int boxmot_b200_hacnn_stn(const float* src, int n, int off, int count, int H, int W, int C,
+                                          const float* theta, int level, const float* prev, int lh, int lw, float* out);
+BOXMOT_B200_API int boxmot_b200_hacnn_head(const float* x3, int n, int off, int count, int hw3, const float* loc,
+                                           int hwl, const float* wg, const float* bg, const float* wl, const float* bl,
+                                           const int* rows, int out_rows, float* out, float* v);
 /* The float32 CUDA-core kernels of the OSNet family, MobileNetV2 and LMBN_n, one family per entry, launched as a loaded
  * model launches them, on host arrays (NHWC float32) over a crop window: the arrays hold n crops, the device crop count
  * is `count` and the window starts at crop `off`, so the kernels process crops 0 .. clamp(count - off, 0, n) - 1 of the
@@ -498,7 +526,9 @@ BOXMOT_B200_API int boxmot_b200_device_count(void);
  * (256 x 128 or 256 x 256), 1 patch embedding (patches x 768), 2 ln_pre (tokens x 768), 3 + l the output of residual
  * block l, 15 the head row before the L2 normalisation (1280).  For MLFN: 0 input blob, 1 stem, 2 max-pool, 3 + i the
  * output of MLFNBlock i (i = 0 .. 15), 19 s_hat (the 16 blocks' gates, 512), 20 the head row v = 0.5 (x + s) before
- * the L2 normalisation (1024). */
+ * the L2 normalisation (1024).  For HACNN: 0 input blob (160 x 64), 1 stem, 2 + i x_{i+1}_out (i = 0 .. 2), 5 + i the
+ * local map of level i + 1 ([region][h][w][c], 4 regions), 8 theta ([level][region][tx, ty], 24), 9 the head row
+ * [fc_global | fc_local] before the normalisations (1024). */
 BOXMOT_B200_API int boxmot_b200_reid_debug_stage(void* reid_handle, const float* boxes_xyxy, int n_boxes,
                                                  const uint8_t* image_data, int image_rows, int image_cols,
                                                  int stage, float* out, int out_capacity_floats,
