@@ -158,6 +158,10 @@ SYMBOLS = {
                                         POINTER(c_float)]),
     "boxmot_b200_vit_layernorm": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
     "boxmot_b200_vit_attention": (c_int, [c_void_p, c_int, c_int, c_void_p]),
+    "boxmot_b200_vit_attention_width": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p]),
+    "boxmot_b200_vits_layernorm": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
+    "boxmot_b200_vits_ain": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "boxmot_b200_vits_head": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int, c_int, c_void_p]),
     "boxmot_b200_mlfn_group_conv": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
                                             c_void_p, c_void_p]),
     "boxmot_b200_mlfn_fsm": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p,

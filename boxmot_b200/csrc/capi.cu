@@ -402,7 +402,20 @@ int boxmot_b200_vit_layernorm(const float* x, int rows, const float* gamma, cons
     return guard([&] { standalone_vit_layernorm(x, rows, gamma, beta, out); });
 }
 int boxmot_b200_vit_attention(const float* qkv, int n, int tokens, float* out) {
-    return guard([&] { standalone_vit_attention(qkv, n, tokens, out); });
+    return guard([&] { standalone_vit_attention(qkv, n, tokens, out, 768); });
+}
+int boxmot_b200_vit_attention_width(const float* qkv, int n, int tokens, int width, float* out) {
+    return guard([&] { standalone_vit_attention(qkv, n, tokens, out, width); });
+}
+int boxmot_b200_vits_layernorm(const float* x, int rows, const float* gamma, const float* beta, float* out) {
+    return guard([&] { standalone_vits_layernorm(x, rows, gamma, beta, out); });
+}
+int boxmot_b200_vits_ain(const float* x, int n, int tokens, const float* a, const float* b, const float* s, float* out) {
+    return guard([&] { standalone_vits_ain(x, n, tokens, a, b, s, out); });
+}
+int boxmot_b200_vits_head(const float* x, int n, int gh, int gw, int pool, int proj, const float* hw, int n_hw,
+                          int normalise, float* out) {
+    return guard([&] { standalone_vits_head(x, n, gh, gw, pool, proj, hw, n_hw, normalise, out); });
 }
 int boxmot_b200_mlfn_group_conv(const float* in, int n, int h, int w, int c, int gw, int stride, const float* weight,
                                 const float* bias, const float* gates, float* out) {

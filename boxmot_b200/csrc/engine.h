@@ -249,7 +249,11 @@ void standalone_resnet_conv(const float* in0, int n, int h0, int w0, int c0, int
                             int w1, int c1, int stride1, const float* w, int N, const float* bias, const float* residual,
                             int relu, float* out, float* elapsed_ms);
 void standalone_vit_layernorm(const float* x, int rows, const float* gamma, const float* beta, float* out);
-void standalone_vit_attention(const float* qkv, int n, int tokens, float* out);
+void standalone_vit_attention(const float* qkv, int n, int tokens, float* out, int width);
+void standalone_vits_layernorm(const float* x, int rows, const float* gamma, const float* beta, float* out);
+void standalone_vits_ain(const float* x, int n, int tokens, const float* a, const float* b, const float* s, float* out);
+void standalone_vits_head(const float* x, int n, int gh, int gw, int pool, int proj, const float* hw, int n_hw,
+                          int normalise, float* out);
 void standalone_mlfn_group_conv(const float* in, int n, int h, int w, int c, int gw, int stride, const float* weight,
                                 const float* bias, const float* gates, float* out);
 void standalone_mlfn_fsm(const float* x, int n, int h, int w, int c, const float* w1, const float* b1, int f0,

@@ -1311,6 +1311,7 @@ __global__ void k_head(const float* __restrict__ x, int HW, int C, const float* 
 
 }  // namespace bmb
 #include "lmbn_head.cuh"
+#include "vit_small.cuh"   // after every kernel above, whose line numbers (-lineinfo) it leaves unchanged
 namespace bmb {
 
 // ---------------------------------------------------------------------------------------------------
@@ -1395,6 +1396,20 @@ struct VitW {
     std::vector<VitLayer> layer;
 };
 
+// ViT-Nano / ViT-Tiny family (arch 9): per block the offsets in d_w of norm1 (LayerNorm gamma, beta; AIN: IN scale,
+// LN scale, shift), the biases and norm2, and the tensor-core packings of its four linear layers
+struct VitsLayer {
+    bool ain = false;
+    size_t n1a = 0, n1b = 0, n1c = 0, bqkv = 0, bproj = 0, n2g = 0, n2b = 0, bfc1 = 0, bfc2 = 0;
+    const float *wqkv = nullptr, *wproj = nullptr, *wfc1 = nullptr, *wfc2 = nullptr;
+};
+struct VitsW {
+    int tokens = 0, depth = 0, ain = 0, gh = 0, gw = 0, stride = 16, pool = 0, proj = 0;
+    size_t patch_b = 0, pos = 0, norm_g = 0, norm_b = 0, head = 0;
+    const float* patch_w = nullptr;
+    std::vector<VitsLayer> layer;
+};
+
 // Backbone of a blob: header word 2, numbered as in weights.py
 enum ReidArch {
     ARCH_OSNET = 1,
@@ -1405,6 +1420,7 @@ enum ReidArch {
     ARCH_CLIP = 6,       // CLIP-ReID ViT-B/16
     ARCH_MLFN = 7,
     ARCH_HACNN = 8,
+    ARCH_VIT = 9,        // ViT-Nano / ViT-Tiny (vit_nano*, vit_tiny*)
 };
 
 struct ReidModel {
@@ -1413,6 +1429,7 @@ struct ReidModel {
     int in_w = IN_W;              // crop width (256 only for CLIP's vehicle models)
     CropNorm norm = kImageNetNorm;
     VitW vit;
+    VitsW vs;
     bool stem_in = false;         // arch 4: conv 7x7 -> IN -> ReLU stem (stem_b is then gamma, stem_beta beta)
     size_t stem_beta = 0;
     float* in_tmp = nullptr;      // arch 4: conv3 output of an IN_BEFORE_RESIDUAL block with a downsample
@@ -1422,7 +1439,7 @@ struct ReidModel {
     MlfnW ml;
     HacnnW ha;
     int* d_n4 = nullptr;          // HACNN: 4 x the crop count, the image count of the [crop][region] local branch
-    float* d_wrn = nullptr;       // ResNet / CLIP / MLFN / HACNN: every GEMM's weights packed by rn::pack_conv_weights
+    float* d_wrn = nullptr;       // ResNet / CLIP / MLFN / HACNN / ViT: every GEMM's weights packed by rn::pack_conv_weights
     int c[4] = {0, 0, 0, 0};
     int feat = 0;
     float* d_w = nullptr;
@@ -1526,6 +1543,26 @@ void read_header(ReidModel* m, const int32_t* hdr) {
             m->vit.layers = hdr[4];
             m->vit.tokens = 1 + hdr[11] * hdr[12];
             return;
+        case ARCH_VIT: {
+            // words 3-7: width, depth, heads, AIN blocks, row width; 9-15: crop h, w, grid h, w, patch stride,
+            // pooling (0 class token, 1 omni-scale, P >= 2 class token + P strips), projection width (0 or 512)
+            VitsW& v = m->vs;
+            v.depth = hdr[4]; v.ain = hdr[6];
+            m->in_h = hdr[9]; m->in_w = hdr[10];
+            v.gh = hdr[11]; v.gw = hdr[12]; v.stride = hdr[13]; v.pool = hdr[14]; v.proj = hdr[15];
+            v.tokens = 1 + v.gh * v.gw;
+            const bool geom = m->in_h >= 16 && m->in_h <= IN_H_MAX && m->in_w == IN_W && (v.stride == 16 || v.stride == 12) &&
+                              v.gh == (m->in_h - vit::PATCH) / v.stride + 1 && v.gw == (m->in_w - vit::PATCH) / v.stride + 1 &&
+                              v.tokens <= vits::MAX_T;
+            const bool head = (v.proj == 0 || v.proj == vits::PROJ) && v.pool >= 0 && v.pool <= vits::MAX_PARTS &&
+                              (v.pool != 1 || (v.proj == 0 && v.gh % 8 == 0)) && (v.pool < 2 || (v.proj && v.pool <= v.gh)) &&
+                              m->feat == vits::head_feat(v.pool, v.proj);
+            if (hdr[3] != vits::D || hdr[5] != vits::HEADS || v.depth < 1 || v.depth > 64 || v.ain < 0 ||
+                v.ain > v.depth || !geom || !head || (v.ain && vits::ain_smem_bytes(v.tokens) > 200 * 1024))
+                throw std::runtime_error("bad ViT blob header (width 192, 3 heads, 16x16 patches at stride 16 or 12, "
+                                         "at most 320 tokens, a known pooling head)");
+            return;
+        }
         case ARCH_MLFN:
             if (hdr[3] != 64 || hdr[4] != 2048 || hdr[5] != mlfn::GROUPS || hdr[6] != mlfn::BLOCKS || m->feat != mlfn::FEAT)
                 throw std::runtime_error("bad MLFN blob header (only groups 32, channels 64-2048, 16 blocks, 1024-d)");
@@ -1894,6 +1931,40 @@ Workspace layout_clip(ReidModel* m, BlobCursor& take, WgmmaPack& pack) {
     return ws;
 }
 
+// ---- ViT-Nano / ViT-Tiny (reid/backbones/vit_nano.py, vit_tiny.py): patch embedding, tokens, blocks, norm, head ----
+Workspace layout_vits(ReidModel* m, BlobCursor& take, WgmmaPack& pack) {
+    constexpr int D = vits::D;
+    VitsW& v = m->vs;
+    auto linear = [&](const float*& dst, int K, int N) { pack.add(dst, take((size_t)K * N), K, N); };
+    linear(v.patch_w, 3 * vit::PATCH * vit::PATCH, D);
+    v.patch_b = take(D);
+    v.pos = take((size_t)v.tokens * D);
+    v.layer.resize(v.depth);   // `pack` keeps pointers into the layers
+    for (int i = 0; i < v.depth; ++i) {
+        VitsLayer& l = v.layer[i];
+        l.ain = i < v.ain;
+        l.n1a = take(D); l.n1b = take(D);
+        if (l.ain) l.n1c = take(D);
+        linear(l.wqkv, D, 3 * D); l.bqkv = take(3 * D);
+        linear(l.wproj, D, D); l.bproj = take(D);
+        l.n2g = take(D); l.n2b = take(D);
+        linear(l.wfc1, D, vits::MLP); l.bfc1 = take(vits::MLP);
+        linear(l.wfc2, vits::MLP, D); l.bfc2 = take(D);
+    }
+    v.norm_g = take(D); v.norm_b = take(D);
+    v.head = take(vits::head_floats(v.pool, v.proj));
+    // per crop: the staged crop, the residual stream, the norm output and the attention output ([T][192] each),
+    // q | k | v ([T][576], also the head tap) and the MLP hidden layer ([T][768], which also holds the patch rows):
+    // 0.74 M floats at vit_tiny's 311 tokens, below the 2.36 M an OSNet_x1_0 chunk takes per crop
+    const size_t T = v.tokens;
+    Workspace ws;
+    ws.blob = (size_t)m->in_h * m->in_w * 3;
+    ws.bufA = ws.bufB = ws.Y[0][0] = T * D;
+    ws.x1 = std::max(T * 3 * D, (size_t)vits::MAX_FEAT);
+    ws.Y[0][1] = T * vits::MLP;
+    return ws;
+}
+
 // The A/B kernel switches of the OSNet family, and for OSNet (arch 1) the tensor-core copies of every 1x1 weight that
 // fits the tensor-core kernel's accumulators and shared memory
 void setup_osnet_kernels(ReidModel* m, const float* host) {
@@ -1944,7 +2015,7 @@ ReidModel* reid_load(const char* path) {
     if (!f) throw std::runtime_error(std::string("cannot open ReID blob: ") + path);
     int32_t hdr[16];
     f.read(reinterpret_cast<char*>(hdr), sizeof(hdr));
-    if (!f || (uint32_t)hdr[0] != BLOB_MAGIC || hdr[1] != 1 || hdr[2] < ARCH_OSNET || hdr[2] > ARCH_HACNN)
+    if (!f || (uint32_t)hdr[0] != BLOB_MAGIC || hdr[1] != 1 || hdr[2] < ARCH_OSNET || hdr[2] > ARCH_VIT)
         throw std::runtime_error("not a version-1 .b200reid blob (export it with boxmot_b200.weights.export_blob)");
     ReidModel* m = new ReidModel();
     try {
@@ -1967,6 +2038,7 @@ ReidModel* reid_load(const char* path) {
             case ARCH_CLIP: ws = layout_clip(m, take, pack); break;
             case ARCH_MLFN: ws = layout_mlfn(m, take, pack); break;
             case ARCH_HACNN: ws = layout_hacnn(m, take, pack); break;
+            case ARCH_VIT: ws = layout_vits(m, take, pack); break;
             default: ws = layout_osnet(m, hdr, take); break;
         }
         if (take.o != n_floats) throw std::runtime_error("ReID blob size does not match its header");
@@ -2226,6 +2298,9 @@ struct Launcher {
             if (BN == 128) conv_tc_slice<128>(a, grid);
             else if (BN == 64) conv_tc_slice<64>(a, grid);
             else conv_tc_slice<32>(a, grid);
+        } else if (a.relu == 4) {   // exact GELU: the ViT-Nano / ViT-Tiny MLP's fc1
+            if (BN == 128) conv_tc_gelu<128>(a, grid);
+            else conv_tc_gelu<64>(a, grid);
         } else if (a.relu == 3) {   // relu(residual + relu(acc + bias)): MLFN's fm_conv3
             if (BN == 128) {
                 RCUDA_OK(cudaFuncSetAttribute(rn::k_conv_tc<128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rn::smem_bytes<128>()));
@@ -2242,6 +2317,11 @@ struct Launcher {
             rn::k_conv_tc<64><<<grid, rn::THREADS, rn::smem_bytes<64>(), st>>>(a, d_n, off, cap);
         }
         end();
+    }
+    template <int BN>
+    void conv_tc_gelu(const rn::ConvArgs& a, dim3 grid) {
+        RCUDA_OK(cudaFuncSetAttribute(rn::k_conv_tc<BN, false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rn::smem_bytes<BN>()));
+        rn::k_conv_tc<BN, false, false, true><<<grid, rn::THREADS, rn::smem_bytes<BN>(), st>>>(a, d_n, off, cap);
     }
     template <int BN>
     void conv_tc_slice(const rn::ConvArgs& a, dim3 grid) {
@@ -2326,13 +2406,42 @@ struct Launcher {
         else vit::k_vit_layernorm<false><<<grid, 256, 0, st>>>(in, pos, g, b, T, d_n, off, cap, out);
         end();
     }
-    // CLIP: multi-head attention of every (crop, head, query block), timed under `lightconv`
-    void vit_attention(const float* qkv, int T, float* out) {
+    // CLIP (width 768) and ViT-Nano / ViT-Tiny (width 192): multi-head attention of every (crop, head, query block),
+    // timed under `lightconv`
+    void vit_attention(const float* qkv, int T, float* out, int width = vit::D) {
         const size_t smem = vit::attention_smem_bytes(T);
-        RCUDA_OK(cudaFuncSetAttribute(vit::k_vit_attention, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        const dim3 grid((T + vit::ATT_QB - 1) / vit::ATT_QB, width / vit::HD, upper);
         begin(CLS_LIGHTCONV);
-        vit::k_vit_attention<<<dim3((T + vit::ATT_QB - 1) / vit::ATT_QB, vit::HEADS, upper), vit::ATT_THREADS, smem, st>>>(
-            qkv, T, d_n, off, cap, out);
+        if (width == vit::D) {
+            RCUDA_OK(cudaFuncSetAttribute(vit::k_vit_attention<vit::D, vit::MAX_T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            vit::k_vit_attention<vit::D, vit::MAX_T><<<grid, vit::ATT_THREADS, smem, st>>>(qkv, T, d_n, off, cap, out);
+        } else {
+            RCUDA_OK(cudaFuncSetAttribute(vit::k_vit_attention<vits::D, vits::MAX_T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            vit::k_vit_attention<vits::D, vits::MAX_T><<<grid, vit::ATT_THREADS, smem, st>>>(qkv, T, d_n, off, cap, out);
+        }
+        end();
+    }
+    // ViT-Nano / ViT-Tiny: LayerNorm of T 192-wide rows per crop, timed under `gates`
+    void vits_layernorm(const float* in, const float* g, const float* b, int T, float* out) {
+        const int grid = (int)std::min<size_t>(((size_t)upper * T + 7) / 8, (size_t)m->sms * 16);
+        begin(CLS_GATES);
+        vits::k_vits_layernorm<<<grid, 256, 0, st>>>(in, g, b, T, d_n, off, cap, out);
+        end();
+    }
+    // ViT-Nano AIN blocks: AdaptiveINLN of every crop (one CTA each), timed under `gates`
+    void vits_ain(const float* in, const float* a, const float* b, const float* s, int T, float* out) {
+        const size_t smem = vits::ain_smem_bytes(T);
+        RCUDA_OK(cudaFuncSetAttribute(vits::k_vits_ain, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        begin(CLS_GATES);
+        vits::k_vits_ain<<<upper, vits::AIN_THREADS, smem, st>>>(in, T, a, b, s, d_n, off, cap, out);
+        end();
+    }
+    // ViT-Nano / ViT-Tiny head (pooling, projections, BNNecks, L2 norm or the un-normalised tap), timed under `head`
+    void vits_head(const float* x, int T, int gh, int gw, int pool, int proj, const float* hw, const CropDesc* crops,
+                   float* out, int out_ld, float* tap) {
+        begin(CLS_HEAD);
+        vits::k_vits_head<<<upper, vits::HEAD_THREADS, 0, st>>>(x, T, gh, gw, pool, proj, hw, crops, d_n, off, cap, out,
+                                                                out_ld, tap);
         end();
     }
     // ChannelGate of an OSBlock: one CTA per crop
@@ -2701,7 +2810,7 @@ void run_clip_chunk(Launcher& L, const FrameIn& fi, float* d_out, int out_ld) {
     float* hid = m->Y[0][1];     // MLP hidden layer / patch rows
     float* qkv = m->x1;
     L.begin(CLS_STEM);
-    vit::k_vit_patchify<<<m->sms * 8, 256, 0, L.st>>>(m->blob, m->in_h, m->in_w, L.d_n, L.off, L.cap, hid);
+    vit::k_vit_patchify<<<m->sms * 8, 256, 0, L.st>>>(m->blob, m->in_h, m->in_w, vit::PATCH, L.d_n, L.off, L.cap, hid);
     L.end();
     auto linear = [&](const float* in, int K, const float* w, const float* bias, const float* residual, int N, int act,
                       float* out, int rows) {
@@ -2730,6 +2839,60 @@ void run_clip_chunk(Launcher& L, const FrameIn& fi, float* d_out, int out_ld) {
                                                L.d_n, L.off, L.cap, d_out, out_ld, tap ? Xn : nullptr);
     L.end();
     if (tap) stop_here(Xn, vit::FEAT);
+}
+
+// ViT-Nano / ViT-Tiny, one chunk (vit_nano.py ViTNano.forward / vit_tiny.py ViTTinyParts.forward, eval).  Taps: 0 crop,
+// 1 patch embedding ([P][192]), 2 tokens ([T][192]), 3 + l after block l, 3 + depth the final norm, 4 + depth the head
+// row before the L2 norm.  Per block: norm1 (LayerNorm, or AdaptiveINLN in the first `ain` blocks), qkv, attention,
+// proj + residual, norm2, fc1 + GELU, fc2 + residual; the linear layers are rn::k_conv_tc over a [crops x T] x 1 map
+// with the residual adds in place in the epilogue, as for CLIP.  Timing classes: crop, stem (patchify, patch GEMM,
+// tokens), gates (norms), pointwise_gemm (linear layers), lightconv (attention), head.
+void run_vits_chunk(Launcher& L, const FrameIn& fi, float* d_out, int out_ld) {
+    ReidModel* m = L.m;
+    const float* W = m->d_w;
+    const VitsW& v = m->vs;
+    constexpr int D = vits::D;
+    const int T = v.tokens, P = T - 1;
+    StageTaps stop_here{m};
+    stage_crops(L, fi);
+    if (stop_here(m->blob, (size_t)m->in_h * m->in_w * 3)) return;
+    float* X = m->bufA;          // residual stream [T][192]
+    float* Xn = m->bufB;         // norm output
+    float* att = m->Y[0][0];     // attention output / patch embedding
+    float* hid = m->Y[0][1];     // MLP hidden layer / patch rows
+    float* qkv = m->x1;
+    L.begin(CLS_STEM);
+    vit::k_vit_patchify<<<m->sms * 8, 256, 0, L.st>>>(m->blob, m->in_h, m->in_w, v.stride, L.d_n, L.off, L.cap, hid);
+    L.end();
+    auto linear = [&](const float* in, int K, const float* w, const float* bias, const float* residual, int N, int act,
+                      float* out, int rows) {
+        rn::ConvArgs c{};
+        c.in0 = in; c.H0 = rows; c.W0 = 1; c.C0 = K; c.k0 = 1; c.s0 = 1;
+        c.w = w; c.bias = bias; c.residual = residual; c.out = out; c.Ho = rows; c.Wo = 1; c.N = N; c.relu = act;
+        L.conv_tc(c);
+    };
+    linear(hid, 3 * vit::PATCH * vit::PATCH, v.patch_w, W + v.patch_b, nullptr, D, 0, att, P);
+    if (stop_here(att, (size_t)P * D)) return;
+    L.begin(CLS_STEM);
+    vits::k_vits_tokens<<<m->sms * 8, 256, 0, L.st>>>(att, W + v.pos, T, L.d_n, L.off, L.cap, X);
+    L.end();
+    if (stop_here(X, (size_t)T * D)) return;
+    for (const VitsLayer& l : v.layer) {
+        if (l.ain) L.vits_ain(X, W + l.n1a, W + l.n1b, W + l.n1c, T, Xn);
+        else L.vits_layernorm(X, W + l.n1a, W + l.n1b, T, Xn);
+        linear(Xn, D, l.wqkv, W + l.bqkv, nullptr, 3 * D, 0, qkv, T);
+        L.vit_attention(qkv, T, att, D);
+        linear(att, D, l.wproj, W + l.bproj, X, D, 0, X, T);
+        L.vits_layernorm(X, W + l.n2g, W + l.n2b, T, Xn);
+        linear(Xn, D, l.wfc1, W + l.bfc1, nullptr, vits::MLP, 4, hid, T);
+        linear(hid, vits::MLP, l.wfc2, W + l.bfc2, X, D, 0, X, T);
+        if (stop_here(X, (size_t)T * D)) return;
+    }
+    L.vits_layernorm(X, W + v.norm_g, W + v.norm_b, T, Xn);
+    if (stop_here(Xn, (size_t)T * D)) return;
+    const bool tap = m->debug_stop == stop_here.idx;
+    L.vits_head(Xn, T, v.gh, v.gw, v.pool, v.proj, W + v.head, fi.crops, d_out, out_ld, tap ? qkv : nullptr);
+    if (tap) stop_here(qkv, m->feat);
 }
 
 // MLFN, one chunk (mlfn.py MLFN.forward, eval).  Taps: 0 crop, 1 stem, 2 pool, 3 + i after MLFNBlock i, 19 s_hat
@@ -2964,6 +3127,7 @@ void run_chunk(Launcher& L, const FrameIn& fi, float* d_out, int out_ld) {
         case ARCH_CLIP: run_clip_chunk(L, fi, d_out, out_ld); return;
         case ARCH_MLFN: run_mlfn_chunk(L, fi, d_out, out_ld); return;
         case ARCH_HACNN: run_hacnn_chunk(L, fi, d_out, out_ld); return;
+        case ARCH_VIT: run_vits_chunk(L, fi, d_out, out_ld); return;
     }
 }
 }  // namespace
@@ -3096,10 +3260,10 @@ void standalone_resnet_conv(const float* in0, int n, int h0, int w0, int c0, int
                             int w1, int c1, int stride1, const float* w, int N, const float* bias, const float* residual,
                             int relu, float* out, float* elapsed_ms) {
     if (n <= 0 || h0 <= 0 || w0 <= 0 || c0 <= 0 || c0 % rn::KC || (k != 1 && k != 3) || stride < 1 || N <= 0 || N % 64 ||
-        c1 < 0 || c1 % rn::KC || (c1 && (!in1 || h1 <= 0 || w1 <= 0 || stride1 < 1)) || relu < 0 || relu > 3 ||
+        c1 < 0 || c1 % rn::KC || (c1 && (!in1 || h1 <= 0 || w1 <= 0 || stride1 < 1)) || relu < 0 || relu > 4 ||
         (relu == 3 && !residual))
         throw std::runtime_error("n, h0, w0 > 0, k in {1, 3}, c0 and c1 multiples of 32, N a multiple of 64, relu in "
-                                 "{0, 1, 2, 3} (3 with a residual) required");
+                                 "{0, 1, 2, 3, 4} (3 with a residual) required");
     const int pad = k / 2, Ho = (h0 + 2 * pad - k) / stride + 1, Wo = (w0 + 2 * pad - k) / stride + 1;
     if (c1 && ((Ho - 1) * stride1 >= h1 || (Wo - 1) * stride1 >= w1))
         throw std::runtime_error("the second operand does not cover the output grid");
@@ -3185,11 +3349,14 @@ void standalone_vit_layernorm(const float* x, int rows, const float* gamma, cons
     cleanup();
 }
 
-// Standalone CLIP attention (vit::k_vit_attention) on host arrays: qkv [n][tokens][3 * 768] (q already scaled by 1/8)
-// -> out [n][tokens][768].
-void standalone_vit_attention(const float* qkv, int n, int tokens, float* out) {
-    if (n <= 0 || tokens < 1 || tokens > vit::MAX_T) throw std::runtime_error("n > 0 and 1 <= tokens <= 288 required");
-    const size_t nin = (size_t)n * tokens * 3 * vit::D, nout = (size_t)n * tokens * vit::D;
+// Standalone attention (vit::k_vit_attention) on host arrays: qkv [n][tokens][3 * width] (q already scaled by 1/8)
+// -> out [n][tokens][width]; width 768 (CLIP, 12 heads, at most 288 tokens) or 192 (ViT-Nano / ViT-Tiny, 3 heads, at
+// most 320 tokens).
+void standalone_vit_attention(const float* qkv, int n, int tokens, float* out, int width) {
+    const int max_t = width == vit::D ? vit::MAX_T : vits::MAX_T;
+    if (n <= 0 || tokens < 1 || (width != vit::D && width != vits::D) || tokens > max_t)
+        throw std::runtime_error("n > 0, width 768 (1 <= tokens <= 288) or 192 (1 <= tokens <= 320) required");
+    const size_t nin = (size_t)n * tokens * 3 * width, nout = (size_t)n * tokens * width;
     float *dq = nullptr, *dO = nullptr;
     int* dn = nullptr;
     auto cleanup = [&] { cudaFree(dq); cudaFree(dO); cudaFree(dn); };
@@ -3201,7 +3368,7 @@ void standalone_vit_attention(const float* qkv, int n, int tokens, float* out) {
         RCUDA_OK(cudaMemcpy(dn, &n, sizeof(int), cudaMemcpyHostToDevice));
         ReidModel fake;
         Launcher L{&fake, dn, 0, n, n, nullptr};
-        L.vit_attention(dq, tokens, dO);
+        L.vit_attention(dq, tokens, dO, width);
         RCUDA_OK(cudaGetLastError());
         RCUDA_OK(cudaMemcpy(out, dO, sizeof(float) * nout, cudaMemcpyDeviceToHost));
     } catch (...) {
@@ -3209,6 +3376,78 @@ void standalone_vit_attention(const float* qkv, int n, int tokens, float* out) {
         throw;
     }
     cleanup();
+}
+
+namespace {
+// device copies of host arrays for the standalone entry points, freed together
+struct DevArrays {
+    std::vector<void*> p;
+    ~DevArrays() { for (void* q : p) cudaFree(q); }
+    template <typename T>
+    T* up(const T* host, size_t n) {
+        T* d = nullptr;
+        RCUDA_OK(cudaMalloc(&d, sizeof(T) * (n ? n : 1)));
+        p.push_back(d);
+        if (host && n) RCUDA_OK(cudaMemcpy(d, host, sizeof(T) * n, cudaMemcpyHostToDevice));
+        return d;
+    }
+};
+}  // namespace
+
+// Standalone ViT-Nano / ViT-Tiny LayerNorm (vits::k_vits_layernorm) on host arrays: rows of 192.
+void standalone_vits_layernorm(const float* x, int rows, const float* gamma, const float* beta, float* out) {
+    if (rows <= 0) throw std::runtime_error("rows > 0 required");
+    const size_t n = (size_t)rows * vits::D;
+    DevArrays d;
+    float *dx = d.up(x, n), *dg = d.up(gamma, vits::D), *db = d.up(beta, vits::D), *dO = d.up<float>(nullptr, n);
+    int* dn = d.up(&rows, 1);
+    ReidModel fake;
+    Launcher L{&fake, dn, 0, rows, rows, nullptr};
+    L.vits_layernorm(dx, dg, db, 1, dO);
+    RCUDA_OK(cudaGetLastError());
+    RCUDA_OK(cudaMemcpy(out, dO, sizeof(float) * n, cudaMemcpyDeviceToHost));
+}
+
+// Standalone AdaptiveINLN (vits::k_vits_ain) on host arrays: x [n][tokens][192] -> a IN(x) + b LN(x) + s.
+void standalone_vits_ain(const float* x, int n, int tokens, const float* a, const float* b, const float* s,
+                         float* out) {
+    if (n <= 0 || tokens < 1 || vits::ain_smem_bytes(tokens) > 200 * 1024)
+        throw std::runtime_error("n > 0 and 1 <= tokens <= 266 required");
+    const size_t nx = (size_t)n * tokens * vits::D;
+    DevArrays d;
+    float *dx = d.up(x, nx), *da = d.up(a, vits::D), *db = d.up(b, vits::D), *ds = d.up(s, vits::D);
+    float* dO = d.up<float>(nullptr, nx);
+    int* dn = d.up(&n, 1);
+    ReidModel fake;
+    Launcher L{&fake, dn, 0, n, n, nullptr};
+    L.vits_ain(dx, da, db, ds, tokens, dO);
+    RCUDA_OK(cudaGetLastError());
+    RCUDA_OK(cudaMemcpy(out, dO, sizeof(float) * nx, cudaMemcpyDeviceToHost));
+}
+
+// Standalone ViT-Nano / ViT-Tiny head (vits::k_vits_head) on host arrays: x [n][1 + gh gw][192] (the final norm's
+// output), hw the head weights of weights.fold_vit for `pool` / `proj` -> out [n][feat], L2-normalised when
+// `normalise`, else the row before the norm.
+void standalone_vits_head(const float* x, int n, int gh, int gw, int pool, int proj, const float* hw, int n_hw,
+                          int normalise, float* out) {
+    const bool ok = n > 0 && gh > 0 && gw > 0 && 1 + gh * gw <= vits::MAX_T && (proj == 0 || proj == vits::PROJ) &&
+                    pool >= 0 && pool <= vits::MAX_PARTS && (pool != 1 || proj == 0) && (pool < 2 || (proj && pool <= gh));
+    if (!ok || (size_t)n_hw != vits::head_floats(pool, proj))
+        throw std::runtime_error("n > 0, at most 320 tokens, pool 0 / 1 (no projection) / 2-3 (512-d projection) and "
+                                 "the head's weight count required");
+    const int T = 1 + gh * gw, feat = vits::head_feat(pool, proj);
+    DevArrays d;
+    float *dx = d.up(x, (size_t)n * T * vits::D), *dw = d.up(hw, (size_t)n_hw);
+    float* dO = d.up<float>(nullptr, (size_t)n * feat);
+    std::vector<CropDesc> crops(n);
+    for (int i = 0; i < n; ++i) { std::memset(&crops[i], 0, sizeof(CropDesc)); crops[i].out_row = i; }
+    CropDesc* dc = d.up(crops.data(), crops.size());
+    int* dn = d.up(&n, 1);
+    ReidModel fake;
+    Launcher L{&fake, dn, 0, n, n, nullptr};
+    L.vits_head(dx, T, gh, gw, pool, proj, dw, dc, dO, feat, normalise ? nullptr : dO);
+    RCUDA_OK(cudaGetLastError());
+    RCUDA_OK(cudaMemcpy(out, dO, sizeof(float) * n * feat, cudaMemcpyDeviceToHost));
 }
 
 // Standalone MLFN grouped 3x3 (mlfn::k_group_conv) on host arrays: in (n,h,w,c) NHWC, w [9][gw][c], bias [c],

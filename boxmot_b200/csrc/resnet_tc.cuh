@@ -22,7 +22,8 @@
 // before the residual add.  They are separate instances so that the default ones keep their code.  The SLICE
 // instances (HACNN's Inception streams, BN 32 / 64 / 128) store row m at out + m * out_ld instead of out + m * N, so
 // that each stream writes its channel slice of the concatenated map in place (the caller offsets `out` by the slice's
-// first channel).
+// first channel).  The GELU instances (relu = 4, BN 64 / 128) apply the exact erf GELU of the ViT-Nano / ViT-Tiny MLP,
+// x * 0.5 * (1 + erf(x / sqrt(2))), likewise separate so that no other instance's code changes.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -48,7 +49,8 @@ struct ConvArgs {
     float* out;              // [M][N]
     int H0, W0, C0, k0, s0;  // k0 in {1, 3} (pad k0 / 2), stride s0
     int H1, W1, C1, s1;
-    int Ho, Wo, N, relu;     // relu: 0 none, 1 ReLU, 2 QuickGELU, 3 relu(residual + relu(.)) (RELU_RES instances)
+    int Ho, Wo, N, relu;     // relu: 0 none, 1 ReLU, 2 QuickGELU, 3 relu(residual + relu(.)) (RELU_RES instances),
+                             // 4 exact GELU (GELU instances)
     int out_ld;              // SLICE instances: floats between output rows (0: the default [M][N] store)
 };
 
@@ -66,7 +68,7 @@ constexpr size_t smem_bytes() {
     return sizeof(float) * (size_t)STAGES * (2 * BM * KC + 2 * BN * KC) + 128;
 }
 
-template <int BN, bool RELU_RES = false, bool SLICE = false>
+template <int BN, bool RELU_RES = false, bool SLICE = false, bool GELU = false>
 __global__ void __launch_bounds__(THREADS, 1) k_conv_tc(const ConvArgs a, const int* __restrict__ d_n, int off, int cap) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     __shared__ __align__(8) uint64_t bar[STAGES];
@@ -202,7 +204,10 @@ __global__ void __launch_bounds__(THREADS, 1) k_conv_tc(const ConvArgs a, const 
                 const float2 r = *reinterpret_cast<const float2*>(res + c);
                 o.x += r.x; o.y += r.y;
             }
-            if (a.relu == 1) {
+            if constexpr (GELU) {
+                o.x = 0.5f * o.x * (1.f + erff(o.x * 0.70710678118654752f));
+                o.y = 0.5f * o.y * (1.f + erff(o.y * 0.70710678118654752f));
+            } else if (a.relu == 1) {
                 o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f);
             } else if (a.relu == 2) {   // QuickGELU x * sigmoid(1.702 x) (CLIP's MLP)
                 o.x = o.x / (1.f + expf(-1.702f * o.x)); o.y = o.y / (1.f + expf(-1.702f * o.y));

@@ -2,13 +2,15 @@
 // VisionTransformer + make_model.py build_transformer, eval mode).  The linear layers (patch embedding, in_proj,
 // out_proj, c_fc, c_proj) run on rn::k_conv_tc as 1x1 convolutions over a [crops x tokens] x 1 map; what is here:
 //
-//   k_vit_patchify    staged crop [H][W][3] -> patch rows [P][768], k = (ky * 16 + kx) * 3 + ci
+//   k_vit_patchify    staged crop [H][W][3] -> patch rows [P][768], k = (ky * 16 + kx) * 3 + ci, 16x16 patches at a
+//                     given stride (16 for CLIP; 12 for the overlapping patches of vit_tiny)
 //   k_vit_layernorm   one warp per 768-wide token row, float32, two-pass mean / variance (eps 1e-5); the EMBED form
 //                     builds the token first: row 0 is the class embedding, row t the patch row t - 1, plus the
 //                     positional table (which carries the class embedding in its row 0), then ln_pre
 //   k_vit_attention   fused multi-head attention of one (crop, head, query block): K and V of the head in shared
 //                     memory, scores, max-subtracted float32 softmax and P.V, written head-interleaved into
-//                     [tokens][768].  q arrives pre-scaled by 1/8 (folded into in_proj at export)
+//                     [tokens][width].  q arrives pre-scaled by 1/8 (folded into in_proj at export).  Instances:
+//                     <768, 288> (CLIP) and <192, 320> (the ViT-Nano / ViT-Tiny family, 3 heads, up to 311 tokens)
 //   k_vit_head        token 0 only: ln_post (its affine folded into the two BatchNorm1d), the 768x512 projection,
 //                     the concatenation [bottleneck | bottleneck_proj] and the L2 normalisation, into the caller's row
 #pragma once
@@ -29,12 +31,13 @@ constexpr int ATT_QB = 32;      // queries per attention CTA
 constexpr int ATT_THREADS = 256;
 constexpr float LN_EPS = 1e-5f;
 
-// staged crops [n][H][W][3] -> patch rows [n][(H/16) (W/16)][768]; one thread per float4 of output (768 = 192 x 4)
-__global__ void k_vit_patchify(const float* __restrict__ crop, int H, int W, const int* __restrict__ d_n, int off,
-                               int cap, float* __restrict__ out) {
+// staged crops [n][H][W][3] -> patch rows [n][gh gw][768], gh = (H - 16) / stride + 1 (likewise gw): the 16x16 window
+// of patch (py, px) starts at (py stride, px stride); one thread per float4 of output (768 = 192 x 4)
+__global__ void k_vit_patchify(const float* __restrict__ crop, int H, int W, int stride, const int* __restrict__ d_n,
+                               int off, int cap, float* __restrict__ out) {
     int n_crops = *d_n - off;
     n_crops = n_crops < 0 ? 0 : (n_crops > cap ? cap : n_crops);
-    const int gw = W / PATCH, P = (H / PATCH) * gw;
+    const int gw = (W - PATCH) / stride + 1, P = ((H - PATCH) / stride + 1) * gw;
     const size_t total = (size_t)n_crops * P * (D / 4);
     for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
         const int q = (int)(i % (D / 4));
@@ -45,7 +48,7 @@ __global__ void k_vit_patchify(const float* __restrict__ crop, int H, int W, con
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
             const int k = 4 * q + e, tap = k / 3, ci = k - 3 * tap, ky = tap / PATCH, kx = tap - ky * PATCH;
-            v[e] = crop[(((size_t)n * H + py * PATCH + ky) * W + px * PATCH + kx) * 3 + ci];
+            v[e] = crop[(((size_t)n * H + py * stride + ky) * W + px * stride + kx) * 3 + ci];
         }
         reinterpret_cast<float4*>(out)[i] = make_float4(v[0], v[1], v[2], v[3]);
     }
@@ -126,8 +129,9 @@ inline size_t attention_smem_bytes(int T) {
     return sizeof(float) * (k_block_floats(T) + (size_t)T * HD + (ATT_THREADS / 32) * ((size_t)T + HD));
 }
 
-// qkv [crops][T][3 * 768] (q | k | v, head h at columns 64 h .. 64 h + 63 of each), out [crops][T][768].
-// grid (ceil(T / ATT_QB), HEADS, crops); each warp walks its queries one at a time: lane j holds scores j, j + 32, ...
+// qkv [crops][T][3 * DM] (q | k | v, head h at columns 64 h .. 64 h + 63 of each), out [crops][T][DM], T <= MAXT.
+// grid (ceil(T / ATT_QB), DM / 64, crops); each warp walks its queries one at a time: lane j holds scores j, j + 32, ...
+template <int DM, int MAXT>
 __global__ void __launch_bounds__(ATT_THREADS) k_vit_attention(const float* __restrict__ qkv, int T,
                                                                const int* __restrict__ d_n, int off, int cap,
                                                                float* __restrict__ out) {
@@ -141,20 +145,20 @@ __global__ void __launch_bounds__(ATT_THREADS) k_vit_attention(const float* __re
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     float* sP = sV + (size_t)T * HD + (size_t)warp * (T + HD);   // this warp's probabilities [T] and query [64]
     float* sQ = sP + T;
-    const float* base = qkv + (size_t)n * T * 3 * D;
+    const float* base = qkv + (size_t)n * T * 3 * DM;
     for (int i = threadIdx.x; i < T * (HD / 4); i += blockDim.x) {
         const int t = i / (HD / 4), c = 4 * (i - t * (HD / 4));
-        const float4 k = *reinterpret_cast<const float4*>(base + (size_t)t * 3 * D + D + h * HD + c);
-        const float4 v = *reinterpret_cast<const float4*>(base + (size_t)t * 3 * D + 2 * D + h * HD + c);
+        const float4 k = *reinterpret_cast<const float4*>(base + (size_t)t * 3 * DM + DM + h * HD + c);
+        const float4 v = *reinterpret_cast<const float4*>(base + (size_t)t * 3 * DM + 2 * DM + h * HD + c);
         float* kr = sK + t * KPAD + c;
         kr[0] = k.x; kr[1] = k.y; kr[2] = k.z; kr[3] = k.w;
         *reinterpret_cast<float4*>(sV + t * HD + c) = v;
     }
     __syncthreads();
-    constexpr int NJ = MAX_T / 32;
+    constexpr int NJ = MAXT / 32;
     const int q_end = min(T, (int)(blockIdx.x + 1) * ATT_QB);
     for (int t = blockIdx.x * ATT_QB + warp; t < q_end; t += ATT_THREADS / 32) {
-        const float* qr = base + (size_t)t * 3 * D + h * HD;
+        const float* qr = base + (size_t)t * 3 * DM + h * HD;
         sQ[lane] = qr[lane];
         sQ[lane + 32] = qr[lane + 32];
         __syncwarp();
@@ -206,7 +210,7 @@ __global__ void __launch_bounds__(ATT_THREADS) k_vit_attention(const float* __re
             o0 = fmaf(sP[j], sV[j * HD + lane], o0);
             o1 = fmaf(sP[j], sV[j * HD + lane + 32], o1);
         }
-        float* orow = out + ((size_t)n * T + t) * D + h * HD;
+        float* orow = out + ((size_t)n * T + t) * DM + h * HD;
         orow[lane] = (o0 + o2) * inv;
         orow[lane + 32] = (o1 + o3) * inv;
         __syncwarp();   // sQ / sP are rewritten by this warp's next query

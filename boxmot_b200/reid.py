@@ -16,7 +16,7 @@ import numpy as np
 
 from . import _lib
 from ._lib import B200Error
-from .weights import ARCH_CLIP, ARCH_HACNN, ARCH_LMBN_N, export_blob, read_blob
+from .weights import ARCH_CLIP, ARCH_HACNN, ARCH_LMBN_N, ARCH_VIT, export_blob, read_blob
 
 
 class _StagedCrops:
@@ -53,6 +53,8 @@ class B200ReID:
             self.input_shape = (int(header[9]), 128)   # LMBN_n runs on 384x128 crops (base_backend.py:59-60)
         if header[2] == ARCH_HACNN:
             self.input_shape = (int(header[9]), int(header[10]))   # HACNN runs on 160x64 crops (base_backend.py:61-62)
+        if header[2] == ARCH_VIT:
+            self.input_shape = (int(header[9]), int(header[10]))   # vit_tiny*: 384x128, vit_nano*: 256x128 (base_backend.py:59-64)
         if header[2] == ARCH_CLIP:
             # CLIP: 256x128, or 256x256 for the vehicle models; mean = std = 0.5 (base_backend.py:52-58)
             self.input_shape = (int(header[9]), int(header[10]))

@@ -491,6 +491,51 @@ def make_clip_state(seed: int = 0, vehicle: bool = False, num_classes: int = 751
     return sd
 
 
+def make_vit_state(variant: str = "vit_tiny", seed: int = 0, num_classes: int = 751):
+    """Seeded state dict with the key set of the reference's ViT-Nano / ViT-Tiny model `variant` (vit_nano.py ViTNano,
+    vit_tiny.py ViTTinyParts), classifiers and num_batches_tracked included.
+    Not trivial on purpose: BatchNorm statistics, LayerNorm / InstanceNorm affines and the AIN gates (|gate| >= 1, far
+    from sigmoid's midpoint) are randomised, qkv is scaled so that q.k / 8 has a spread of a few units and attention
+    rows are far from uniform, and proj / fc2 start small so the residual stream stays O(1) through the blocks."""
+    import torch
+
+    from .weights import vit_layout
+
+    g = torch.Generator().manual_seed(seed)
+
+    def randn(*shape, std=1.0):
+        return torch.randn(*shape, generator=g) * std
+
+    sd = {}
+    for k, shape in vit_layout(variant, num_classes=num_classes).items():
+        name = k.rsplit(".", 1)[-1]
+        if k.endswith("norm1.gate"):
+            sd[k] = torch.sign(randn(*shape)) * (1.0 + 2.0 * torch.rand(*shape, generator=g))
+        elif name == "running_var":
+            sd[k] = 0.5 + torch.rand(*shape, generator=g)
+        elif name == "running_mean":
+            sd[k] = randn(*shape, std=0.1)
+        elif name == "weight" and len(shape) == 1:   # LayerNorm / InstanceNorm / BatchNorm scale
+            sd[k] = 0.5 + torch.rand(*shape, generator=g)
+        elif name == "bias" and len(shape) == 1:
+            sd[k] = randn(*shape, std=0.1 if "norm" in k or "bn" in k or "bottleneck" in k else 0.05)
+        elif k in ("cls_token", "pos_embed"):
+            sd[k] = randn(*shape, std=0.1)
+        elif k == "patch_embed.proj.weight":
+            sd[k] = randn(*shape, std=0.04)
+        elif k.endswith("attn.qkv.weight"):
+            sd[k] = randn(*shape, std=0.12)
+        elif k.endswith(("attn.proj.weight", "mlp.fc2.weight")):
+            sd[k] = randn(*shape, std=0.03)
+        elif "classifier" in k:
+            sd[k] = randn(*shape, std=0.001)
+        else:   # mlp.fc1, proj, part_projs, the omni-scale gate
+            sd[k] = randn(*shape, std=shape[-1] ** -0.5)
+    for k in [k for k in sd if k.endswith("running_var")]:
+        sd[k[: -len("running_var")] + "num_batches_tracked"] = torch.tensor(0)
+    return sd
+
+
 MOBILENETV2_LAYERS = ((1, 16, 1, 1), (6, 24, 2, 2), (6, 32, 3, 2), (6, 64, 4, 2), (6, 96, 3, 1), (6, 160, 3, 2),
                       (6, 320, 1, 1))  # (expansion t, base channels c, repeats n, first stride s), mobilenetv2.py:91-99
 

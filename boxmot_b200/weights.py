@@ -30,6 +30,10 @@ Arch 7 (MLFN, `fold_mlfn`) records the stem width, the last block width, the gro
 feature in words 3-7; its layout is listed above `fold_mlfn`.
 Arch 8 (HACNN, `fold_hacnn`) records the stem width and the three Inception widths and the 1024-d feature in words
 3-7 and the 160x64 input in words 9-10; its layout is listed above `fold_hacnn`.
+Arch 9 (ViT-Nano / ViT-Tiny, `fold_vit`) records width 192, depth, 3 heads, the AIN block count and the row width in
+words 3-7, the crop height / width in words 9-10, the patch grid in words 11-12, the patch stride in word 13, the
+pooling (0 class token, 1 omni-scale, P >= 2 class token + P strips) in word 14 and the projection width (0 or 512)
+in word 15; its layout is listed above `fold_vit`.
 All 1x1 weights are stored K-major ([cin][cout]) so a thread owning consecutive output channels loads
 consecutive floats; every tensor is zero-padded to a multiple of 4 floats (16-byte aligned float4 loads).
 """
@@ -55,6 +59,7 @@ ARCH_MLFN = 7
 MLFN_FEAT = 1024
 ARCH_HACNN = 8
 HACNN_FEAT = 1024
+ARCH_VIT = 9
 BRANCHES = (("conv2a", 1), ("conv2b", 2), ("conv2c", 3), ("conv2d", 4))
 EPS = 1e-5
 
@@ -66,11 +71,19 @@ def _np(t) -> np.ndarray:
 
 
 def load_state_dict(path) -> Dict[str, np.ndarray]:
+    return _load_checkpoint(path)[0]
+
+
+def _load_checkpoint(path):
+    """(state dict without `module.` prefixes, the top-level `model_name` a reference training checkpoint records or
+    None)."""
     import torch
 
     ckpt = torch.load(str(path), map_location="cpu", weights_only=False)
     sd = ckpt["state_dict"] if isinstance(ckpt, dict) and "state_dict" in ckpt else ckpt
-    return {(k[7:] if k.startswith("module.") else k): v for k, v in sd.items()}
+    name = ckpt.get("model_name") if isinstance(ckpt, dict) else None
+    sd = {(k[7:] if k.startswith("module.") else k): v for k, v in sd.items()}
+    return sd, (name if isinstance(name, str) and name else None)
 
 
 def _bn_fold(sd, name) -> Tuple[np.ndarray, np.ndarray]:
@@ -598,6 +611,188 @@ def fold_hacnn(sd) -> List[np.ndarray]:
     return out
 
 
+# ViT-Nano / ViT-Tiny (arch 9): ViTNano of reid/backbones/vit_nano.py (vit_nano, vit_nano_ain, vit_nano_ain_os,
+# vit_tiny) and ViTTinyParts of vit_tiny.py (vit_tiny_parts, vit_tiny_parts3), eval mode.  Every linear weight is stored
+# K-major ([in][out]); the arrays are
+#     patch     W[768][192] (k = (ky*16 + kx)*3 + ci), b[192]
+#     pos       [T][192]  pos_embed, cls_token added to row 0
+#     per block norm1: LayerNorm gamma, beta, or (AIN blocks) a = sigmoid(gate) in_norm.weight,
+#                      b = (1 - sigmoid(gate)) ln.weight, s = sigmoid(gate) in_norm.bias + (1 - sigmoid(gate)) ln.bias
+#               qkv W[192][576] (q | k | v; the q third and its bias scaled by 1/8, exact), b[576]
+#               proj W[192][192], b; norm2 gamma, beta; fc1 W[192][768], b; fc2 W[768][192], b
+#     norm      gamma[192], beta[192]
+#     head      class token:               bottleneck as scale[192], shift[192]
+#               class token + proj:        W[192][512] (proj with bottleneck's scale folded), b[512] (its shift)
+#               omni-scale:                per scale i: scale_norms[i] gamma, beta; gate W1[192][12], b1[12],
+#                                          W2[12][192], b2[192]; bottleneck scale[192], shift[192]
+#               class token + P strips:    the class token's W[192][512], b[512], then part_projs[i] with part_bns[i]
+#                                          folded, W[192][512], b[512], for each strip
+# (depth, AIN blocks, omni-scale, parts, crop h, crop w, patch stride) of each reference model name
+VIT_VARIANTS = {
+    "vit_nano": (6, 0, False, 0, 256, 128, 16),
+    "vit_nano_ain": (6, 3, False, 0, 256, 128, 16),
+    "vit_nano_ain_os": (6, 3, True, 0, 256, 128, 16),
+    "vit_tiny": (12, 0, False, 0, 384, 128, 12),
+    "vit_tiny_parts": (12, 0, False, 2, 384, 128, 12),
+    "vit_tiny_parts3": (12, 0, False, 3, 384, 128, 12),
+}
+VIT_WIDTH, VIT_HEADS, VIT_PROJ = 192, 3, 512
+# the reference's ReID model names (core/config.py MODEL_TYPES): a file name resolves to the longest one it contains
+REFERENCE_MODEL_TYPES = (
+    "resnet50", "resnet101", "mlfn", "hacnn", "mobilenetv2_x1_0", "mobilenetv2_x1_4", "osnet_x1_0", "osnet_x0_75",
+    "osnet_x0_5", "osnet_x0_25", "osnet_ibn_x1_0", "osnet_ain_x1_0", "lmbn_ain_n", "lmbn_n", "cspreid_n", "clip",
+    *VIT_VARIANTS, "csl_tinyvit_7m", "csl_tinyvit_7m_lmbn", "csl_tinyvit_11m", "csl_tinyvit_11m_lmbn",
+    "csl_tinyvit_23m", "csl_tinyvit_23m_lmbn", "csl_tinyvit_small", "csl_tinyvit_normal", "csl_tinyvit_large",
+    "csl_tinyvit_lmbn")
+
+
+def model_name_from_file(name: str):
+    """The reference's model name for a weights file name (registry.get_model_name without a checkpoint name)."""
+    low = name.lower()
+    return next((t for t in sorted(REFERENCE_MODEL_TYPES, key=len, reverse=True) if t in low), None)
+
+
+def vit_grid(variant):
+    """(crop h, crop w, stride, grid h, grid w, tokens) of a variant: PatchEmbed's (size - 16) // stride + 1."""
+    _, _, _, _, h, w, stride = VIT_VARIANTS[variant]
+    gh, gw = (h - 16) // stride + 1, (w - 16) // stride + 1
+    return h, w, stride, gh, gw, 1 + gh * gw
+
+
+def vit_layout(variant, num_classes=None):
+    """{key: shape} of the reference model's state dict for `variant`, without num_batches_tracked; with num_classes,
+    the classifiers too (the keys the reference's loader finds but the embedding never reads)."""
+    depth, ain, omni, parts, *_ = VIT_VARIANTS[variant]
+    d, mlp = VIT_WIDTH, 4 * VIT_WIDTH
+    tokens = vit_grid(variant)[5]
+    feat = VIT_PROJ if variant.startswith("vit_tiny") else d
+    want = {"cls_token": (1, 1, d), "pos_embed": (1, tokens, d), "patch_embed.proj.weight": (d, 3, 16, 16),
+            "patch_embed.proj.bias": (d,), "norm.weight": (d,), "norm.bias": (d,)}
+    for i in range(depth):
+        b = f"blocks.{i}."
+        if i < ain:
+            want.update({b + "norm1.ln.weight": (d,), b + "norm1.ln.bias": (d,), b + "norm1.in_norm.weight": (d,),
+                         b + "norm1.in_norm.bias": (d,), b + "norm1.gate": (d,)})
+        else:
+            want.update({b + "norm1.weight": (d,), b + "norm1.bias": (d,)})
+        want.update({b + "attn.qkv.weight": (3 * d, d), b + "attn.qkv.bias": (3 * d,), b + "attn.proj.weight": (d, d),
+                     b + "attn.proj.bias": (d,), b + "norm2.weight": (d,), b + "norm2.bias": (d,),
+                     b + "mlp.fc1.weight": (mlp, d), b + "mlp.fc1.bias": (mlp,), b + "mlp.fc2.weight": (d, mlp),
+                     b + "mlp.fc2.bias": (d,)})
+    if omni:
+        mid = d // 16
+        want.update({"os_agg.gate.fc.0.weight": (mid, d), "os_agg.gate.fc.0.bias": (mid,),
+                     "os_agg.gate.fc.2.weight": (d, mid), "os_agg.gate.fc.2.bias": (d,)})
+        for i in range(4):
+            want[f"os_agg.scale_norms.{i}.weight"] = want[f"os_agg.scale_norms.{i}.bias"] = (d,)
+    if feat != d:
+        want["proj.weight"] = (feat, d)
+    bns = ["bottleneck"] + [f"part_bns.{i}" for i in range(parts)]
+    for bn in bns:
+        for p in ("weight", "bias", "running_mean", "running_var"):
+            want[f"{bn}.{p}"] = (feat,)
+    for i in range(parts):
+        want[f"part_projs.{i}.weight"] = (feat, d)
+    if num_classes is not None:
+        want["classifier.weight"] = (num_classes, feat)
+        for i in range(parts):
+            want[f"part_classifiers.{i}.weight"] = (num_classes, feat)
+    return want
+
+
+def looks_like_vit(sd) -> bool:
+    return "cls_token" in sd and "patch_embed.proj.weight" in sd
+
+
+def vit_variant_from_keys(sd) -> str:
+    """The variant an unnamed state dict's keys suggest (the reference always has a name: file or checkpoint)."""
+    tiny = "proj.weight" in sd or "blocks.6.norm1.weight" in sd or "part_projs.0.weight" in sd
+    if tiny:
+        return "vit_tiny_parts3" if "part_projs.2.weight" in sd else (
+            "vit_tiny_parts" if "part_projs.0.weight" in sd else "vit_tiny")
+    if "os_agg.gate.fc.0.weight" in sd:
+        return "vit_nano_ain_os"
+    return "vit_nano_ain" if "blocks.0.norm1.gate" in sd else "vit_nano"
+
+
+def fold_vit(sd, variant):
+    """ViT-Nano / ViT-Tiny state dict -> (header dims, header words 9-15, arrays) of the arch-9 blob for the reference
+    model `variant`.  Every tensor of that model (apart from its classifiers) must be present with its shape: a missing
+    or mis-shaped key raises a ValueError naming the keys, where the reference would silently run that layer randomly
+    initialised.  Keys the model lacks are ignored, as the reference's loader discards them."""
+    if variant not in VIT_VARIANTS:
+        raise ValueError(f"unknown ViT variant {variant!r}; {', '.join(VIT_VARIANTS)} are supported")
+    want = vit_layout(variant)
+    missing = sorted(k for k in want if k not in sd)
+    bad_shape = sorted(k for k in want if k in sd and tuple(sd[k].shape) != want[k])
+    if missing or bad_shape:
+        raise ValueError(f"not a {variant} state dict (missing keys {missing[:4]}, unexpected shapes {bad_shape[:4]}); "
+                         "the reference would run these layers randomly initialised")
+    depth, ain, omni, parts, *_ = VIT_VARIANTS[variant]
+    h, w, stride, gh, gw, tokens = vit_grid(variant)
+    d = VIT_WIDTH
+    tiny = variant.startswith("vit_tiny")
+    proj = VIT_PROJ if tiny else 0
+    pw = _np(sd["patch_embed.proj.weight"])   # [192][3][16][16]
+    pos = _np(sd["pos_embed"])[0].copy()
+    pos[0] += _np(sd["cls_token"])[0, 0]
+    out: List[np.ndarray] = [pw.transpose(2, 3, 1, 0).reshape(-1, d), _np(sd["patch_embed.proj.bias"]), pos]
+    qscale = np.ones(3 * d)
+    qscale[:d] = 1.0 / 8.0   # head_dim ** -0.5
+    for i in range(depth):
+        b = f"blocks.{i}."
+        if i < ain:
+            g = 1.0 / (1.0 + np.exp(-_np(sd[b + "norm1.gate"])))
+            inw, inb = _np(sd[b + "norm1.in_norm.weight"]), _np(sd[b + "norm1.in_norm.bias"])
+            lnw, lnb = _np(sd[b + "norm1.ln.weight"]), _np(sd[b + "norm1.ln.bias"])
+            out += [g * inw, (1.0 - g) * lnw, g * inb + (1.0 - g) * lnb]
+        else:
+            out += [_np(sd[b + "norm1.weight"]), _np(sd[b + "norm1.bias"])]
+        out += [(_np(sd[b + "attn.qkv.weight"]) * qscale[:, None]).T, _np(sd[b + "attn.qkv.bias"]) * qscale,
+                _np(sd[b + "attn.proj.weight"]).T, _np(sd[b + "attn.proj.bias"]),
+                _np(sd[b + "norm2.weight"]), _np(sd[b + "norm2.bias"]),
+                _np(sd[b + "mlp.fc1.weight"]).T, _np(sd[b + "mlp.fc1.bias"]),
+                _np(sd[b + "mlp.fc2.weight"]).T, _np(sd[b + "mlp.fc2.bias"])]
+    out += [_np(sd["norm.weight"]), _np(sd["norm.bias"])]
+    sc, sh = _bn_fold(sd, "bottleneck")
+    if omni:
+        for i in range(4):
+            out += [_np(sd[f"os_agg.scale_norms.{i}.weight"]), _np(sd[f"os_agg.scale_norms.{i}.bias"])]
+        out += [_np(sd["os_agg.gate.fc.0.weight"]).T, _np(sd["os_agg.gate.fc.0.bias"]),
+                _np(sd["os_agg.gate.fc.2.weight"]).T, _np(sd["os_agg.gate.fc.2.bias"]), sc, sh]
+    elif not proj:
+        out += [sc, sh]
+    else:
+        out += [(_np(sd["proj.weight"]) * sc[:, None]).T, sh]
+        for i in range(parts):
+            psc, psh = _bn_fold(sd, f"part_bns.{i}")
+            out += [(_np(sd[f"part_projs.{i}.weight"]) * psc[:, None]).T, psh]
+    pool = 1 if omni else parts
+    feat = (1 + parts) * proj if proj else d
+    dims = [d, depth, VIT_HEADS, ain, feat]
+    return dims, [h, w, gh, gw, stride, pool, proj], out
+
+
+def resolve_vit(sd, file_name=None, model_name=None):
+    """The ViT variant the reference builds for these weights, or None when they are not a ViT-Nano / ViT-Tiny model.
+    The name is the checkpoint's `model_name`, else the longest reference model name in the file name; an unnamed
+    in-memory state dict falls back to its key set.  Raises ValueError for a `veri` / `vehicleid` file name (the
+    reference builds 256x256 crops there, which its positional table does not fit) and for ViT weights under a name
+    the reference builds another model for."""
+    name = model_name or (model_name_from_file(file_name) if file_name else None)
+    if name is None:
+        return vit_variant_from_keys(sd) if looks_like_vit(sd) else None
+    if name not in VIT_VARIANTS:
+        if looks_like_vit(sd) and not name.startswith(("csl_tinyvit", "cspreid")):
+            raise ValueError(f"ViT weights under the model name {name!r}: the reference would build {name} and run it "
+                             "randomly initialised")
+        return None
+    if file_name and clip_vehicle_name(file_name):
+        raise ValueError(f"ViT weights '{file_name}': the reference runs 256x256 crops for a veri / vehicleid file name, "
+                         f"which {name}'s positional table does not fit")
+    return name
+
+
 def _pad4(n: int) -> int:
     return (n + 3) // 4 * 4
 
@@ -656,12 +851,12 @@ def fold_mobilenetv2(sd):
 
 def export_blob(weights, out_path=None) -> Path:
     """`weights`: path to a .pt checkpoint or an in-memory state dict.  Returns the blob path."""
-    name = None
+    name = model_name = None
     if isinstance(weights, (str, Path)):
         src = Path(weights)
         if src.suffix == ".b200reid":
             return src
-        sd = load_state_dict(src)
+        sd, model_name = _load_checkpoint(src)
         name = src.name
         if out_path is None:
             out_path = src.with_suffix(".b200reid")
@@ -670,7 +865,11 @@ def export_blob(weights, out_path=None) -> Path:
         if out_path is None:
             raise ValueError("out_path is required when exporting an in-memory state dict")
     table, in_modes, extra = [], [], []
-    if is_clip(sd):
+    vit = resolve_vit(sd, name, model_name)
+    if vit is not None:
+        dims, extra, arrays = fold_vit(sd, vit)
+        arch = ARCH_VIT
+    elif is_clip(sd):
         dims, input_hw, grid, arrays = fold_clip(sd, name)
         arch, extra = ARCH_CLIP, [*input_hw, *grid]
     elif "conv9.conv.weight" in sd:
@@ -696,7 +895,7 @@ def export_blob(weights, out_path=None) -> Path:
         arch, dims = ARCH_HACNN, [32, 128, 256, 384, HACNN_FEAT]
     else:
         raise ValueError("only OSNet, OSNet-AIN, OSNet-IBN, MobileNetV2, LMBN_n, ResNet50 / ResNet101, CLIP-ReID "
-                         "ViT-B/16, MLFN and HACNN state dicts are implemented on the B200 ReID path")
+                         "ViT-B/16, MLFN, HACNN and ViT-Nano / ViT-Tiny state dicts are implemented on the B200 ReID path")
     # every tensor starts on a 16-byte boundary (the kernels read weights as float4)
     padded = []
     for a in arrays:
@@ -712,6 +911,8 @@ def export_blob(weights, out_path=None) -> Path:
         header[9:13] = extra
     if arch == ARCH_HACNN:
         header[9:11] = [160, 64]
+    if arch == ARCH_VIT:
+        header[9:16] = extra
     out_path = Path(out_path)
     tmp = out_path.with_suffix(out_path.suffix + ".tmp")
     with open(tmp, "wb") as f:

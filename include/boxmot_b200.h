@@ -416,7 +416,7 @@ BOXMOT_B200_API int boxmot_b200_instance_norm(const float* x, int n, int h, int 
 /* One convolution of the ResNet50 / ResNet101 path (wgmma tf32x3 implicit GEMM) on host arrays, NHWC float32:
  * out (n,Ho,Wo,out_c) = act(conv(in0) + conv1x1(in1) + bias (+ residual, optional)), act = none when relu = 0, ReLU
  * when relu = 1, QuickGELU x * sigmoid(1.702 x) when relu = 2 (CLIP's MLP; a CLIP linear layer is a 1x1 convolution
- * over h0 = tokens, w0 = 1). relu = 3 gives relu(residual + relu(conv(in0) + conv1x1(in1) + bias)) (MLFN's fm_conv3, whose
+ * over h0 = tokens, w0 = 1), exact GELU x * (1 + erf(x / sqrt 2)) / 2 when relu = 4 (the ViT-Nano / ViT-Tiny MLP). relu = 3 gives relu(residual + relu(conv(in0) + conv1x1(in1) + bias)) (MLFN's fm_conv3, whose
  * ReLU precedes the residual add; the residual is then required).  in0 (n,h0,w0,c0) is read by a k x k kernel (k 1 or 3, pad k/2) at `stride`; in1 (n,h1,w1,c1), optional (c1 = 0
  * for none), by a 1x1 kernel at `stride1` over the same output grid (the fused conv3 + downsample of a stage's first
  * Bottleneck).  w is (k*k*c0 + c1, out_c) K-major, k index (kh*k + kw)*c0 + ci then the c1 channels; c0 and c1
@@ -432,6 +432,23 @@ BOXMOT_B200_API int boxmot_b200_vit_layernorm(const float* x, int rows, const fl
  * columns 64h..64h+63 of each, with q already scaled by 1/8; out (n,tokens,768) = softmax(q k^T) v per head, heads
  * interleaved.  1 <= tokens <= 288. */
 BOXMOT_B200_API int boxmot_b200_vit_attention(const float* qkv, int n, int tokens, float* out);
+/* The same attention at width 768 (12 heads, 1 <= tokens <= 288) or 192 (the ViT-Nano / ViT-Tiny path: 3 heads,
+ * 1 <= tokens <= 320): qkv (n,tokens,3 width), out (n,tokens,width). */
+BOXMOT_B200_API int boxmot_b200_vit_attention_width(const float* qkv, int n, int tokens, int width, float* out);
+/* LayerNorm of the ViT-Nano / ViT-Tiny path on host arrays: out (rows,192) = LN(x) * gamma + beta, eps 1e-5. */
+BOXMOT_B200_API int boxmot_b200_vits_layernorm(const float* x, int rows, const float* gamma, const float* beta,
+                                               float* out);
+/* AdaptiveINLN of the ViT-Nano AIN blocks on host arrays: x (n,tokens,192) -> out = a * IN(x) + b * LN(x) + s per
+ * channel, IN over the tokens of each crop (biased variance), LN over the channels of each token, both eps 1e-5 and
+ * without affine (a, b, s fold the gate and both affines).  tokens * 192 floats must fit in 200 KB of shared memory. */
+BOXMOT_B200_API int boxmot_b200_vits_ain(const float* x, int n, int tokens, const float* a, const float* b,
+                                         const float* s, float* out);
+/* Head of the ViT-Nano / ViT-Tiny path on host arrays: x (n,1 + gh*gw,192) is the final norm's output; pool 0 takes
+ * the class token, 1 the omni-scale aggregation of the patch mean (proj 0), P = 2 or 3 the class token and P grid-row
+ * strips (proj 512); hw (n_hw floats) is the head block of the blob.  out (n,feat) is L2-normalised when `normalise`,
+ * else the row before the norm. */
+BOXMOT_B200_API int boxmot_b200_vits_head(const float* x, int n, int gh, int gw, int pool, int proj, const float* hw,
+                                          int n_hw, int normalise, float* out);
 /* Grouped 3x3 convolution of the MLFN path (fm_conv2, 32 groups, pad 1) on host arrays, NHWC float32: in (n,h,w,c)
  * with c = 32 gw, group width gw in {4, 8, 16, 32}, stride 1 or 2, output width a multiple of 4; weight (9,gw,c),
  * element (kh*3 + kw, i, co) weighing input channel (co / gw) gw + i; out (n,Ho,Wo,c) = relu(conv + bias) *
