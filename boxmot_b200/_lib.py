@@ -190,6 +190,14 @@ SYMBOLS = {
                                       c_int, c_int, c_void_p]),
     "boxmot_b200_hacnn_head": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p,
                                        c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
+    "boxmot_b200_cspreid_conv": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int,
+                                         c_int, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p, c_int,
+                                         c_int]),
+    "boxmot_b200_cspreid_map": (c_int, [c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
+                                        c_void_p]),
+    "boxmot_b200_cspreid_attention": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "boxmot_b200_cspreid_head": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int,
+                                         c_void_p, c_void_p]),
     "boxmot_b200_device_count": (c_int, []),
     "boxmot_b200_reid_debug_stage": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_void_p,
                                              c_int, POINTER(c_int)]),

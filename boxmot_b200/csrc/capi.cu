@@ -487,6 +487,26 @@ int boxmot_b200_hacnn_head(const float* x3, int n, int off, int count, int hw3, 
                            int out_rows, float* out, float* v) {
     return guard([&] { standalone_hacnn_head(x3, n, off, count, hw3, loc, hwl, wg, bg, wl, bl, rows, out_rows, out, v); });
 }
+int boxmot_b200_cspreid_conv(const float* in, int n, int off, int count, int h, int w, int c0, int in_ld, int in_off,
+                             int k, int stride, const float* weight, int N, const float* bias, const float* residual,
+                             int res_ld, int res_off, float* out, int out_ld, int out_off) {
+    return guard([&] {
+        standalone_cspreid_conv(in, n, off, count, h, w, c0, in_ld, in_off, k, stride, weight, N, bias, residual, res_ld,
+                                res_off, out, out_ld, out_off);
+    });
+}
+int boxmot_b200_cspreid_map(int op, const float* in, int n, int off, int count, int h, int w, int c,
+                            const float* weight, const float* bias, float* out) {
+    return guard([&] { standalone_cspreid_map(op, in, n, off, count, h, w, c, weight, bias, out); });
+}
+int boxmot_b200_cspreid_attention(const float* x, int n, int off, int count, int h, int w, const float* params,
+                                  float* out) {
+    return guard([&] { standalone_cspreid_attention(x, n, off, count, h, w, params, out); });
+}
+int boxmot_b200_cspreid_head(const float* x, int n, int off, int count, int h, int w, const float* params,
+                             const int* rows, int out_rows, float* out, float* raw) {
+    return guard([&] { standalone_cspreid_head(x, n, off, count, h, w, params, rows, out_rows, out, raw); });
+}
 int boxmot_b200_cosine_cost(const float* a, int rows, const float* b, int cols, int dim, double* out) {
     return guard([&] { standalone_cosine(a, rows, b, cols, dim, out); });
 }

@@ -288,4 +288,14 @@ void standalone_hacnn_head(const float* x3, int n, int off, int count, int hw3, 
                            const float* wg, const float* bg, const float* wl, const float* bl, const int* rows,
                            int out_rows, float* out, float* v);
 
+void standalone_cspreid_conv(const float* in, int n, int off, int count, int h, int w, int c0, int in_ld, int in_off,
+                             int k, int stride, const float* weight, int N, const float* bias, const float* residual,
+                             int res_ld, int res_off, float* out, int out_ld, int out_off);
+void standalone_cspreid_map(int op, const float* in, int n, int off, int count, int h, int w, int c,
+                            const float* weight, const float* bias, float* out);
+void standalone_cspreid_attention(const float* x, int n, int off, int count, int h, int w, const float* params,
+                                  float* out);
+void standalone_cspreid_head(const float* x, int n, int off, int count, int h, int w, const float* params,
+                             const int* rows, int out_rows, float* out, float* raw);
+
 }  // namespace bmb

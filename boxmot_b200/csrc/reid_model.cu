@@ -24,6 +24,7 @@
 
 #include "engine.h"
 #include "pointwise_tc.cuh"
+#include "cspreid_kernels.cuh"
 #include "hacnn_kernels.cuh"
 #include "mlfn_kernels.cuh"
 #include "resnet_tc.cuh"
@@ -1383,6 +1384,16 @@ struct HacnnW {
     size_t att[3][9] = {};
 };
 
+// CSPReID-n (arch 10): the tensor-core packings of every ConvBNSiLU after the first stem conv, in fold_cspreid's order
+// (stem.1; per stage cv1, each bottleneck's cv1 and cv2, cv2, the stride-2 downsample of stages 1-3; SPPF's cv1 and cv2),
+// and the offsets in d_w of the attention's parameters (fc.0, fc.2, depthwise weights, depthwise shift, spatial 1x1) and
+// of the three BNNeck3 heads (W, b each)
+struct CspW {
+    static constexpr int CONVS = 24;
+    RnConv conv[CONVS];
+    size_t attn[5] = {}, head[6] = {};
+};
+
 // CLIP-ReID ViT-B/16 (arch 6): per residual block the offsets in d_w of its LayerNorm parameters and biases, and the
 // tensor-core packings of its four linear layers
 struct VitLayer {
@@ -1421,6 +1432,7 @@ enum ReidArch {
     ARCH_MLFN = 7,
     ARCH_HACNN = 8,
     ARCH_VIT = 9,        // ViT-Nano / ViT-Tiny (vit_nano*, vit_tiny*)
+    ARCH_CSPREID = 10,   // CSPReID-n (cspreid_n)
 };
 
 struct ReidModel {
@@ -1438,6 +1450,7 @@ struct ReidModel {
     std::vector<RnBlock> rn;      // ResNet Bottlenecks, layer1.0 .. layer4.last
     MlfnW ml;
     HacnnW ha;
+    CspW cs;
     int* d_n4 = nullptr;          // HACNN: 4 x the crop count, the image count of the [crop][region] local branch
     float* d_wrn = nullptr;       // ResNet / CLIP / MLFN / HACNN / ViT: every GEMM's weights packed by rn::pack_conv_weights
     int c[4] = {0, 0, 0, 0};
@@ -1567,6 +1580,15 @@ void read_header(ReidModel* m, const int32_t* hdr) {
             if (hdr[3] != 64 || hdr[4] != 2048 || hdr[5] != mlfn::GROUPS || hdr[6] != mlfn::BLOCKS || m->feat != mlfn::FEAT)
                 throw std::runtime_error("bad MLFN blob header (only groups 32, channels 64-2048, 16 blocks, 1024-d)");
             m->c[0] = 64;
+            return;
+        case ARCH_CSPREID:
+            // words 3-7: stage widths 128, 256, 384, 512 and the 1536-d row; 9-10: crop h, w (256x128 or 256x256)
+            if (hdr[3] != 128 || hdr[4] != 256 || hdr[5] != 384 || hdr[6] != csp::C || m->feat != csp::FEAT ||
+                hdr[9] != 256 || (hdr[10] != 128 && hdr[10] != 256))
+                throw std::runtime_error("bad CSPReID-n blob header (only widths 128/256/384/512, 1536-d, 256x128 or "
+                                         "256x256 input)");
+            m->in_h = hdr[9];
+            m->in_w = hdr[10];
             return;
         case ARCH_HACNN:
             if (hdr[3] != hacnn::STEM_C || hdr[4] != 128 || hdr[5] != 256 || hdr[6] != hacnn::C3 ||
@@ -1965,6 +1987,53 @@ Workspace layout_vits(ReidModel* m, BlobCursor& take, WgmmaPack& pack) {
     return ws;
 }
 
+// ---- CSPReID-n (reid/backbones/cspreid_n.py): stem, four C3k2 stages, SPPF, LightSelfAttention, three BNNeck3 ----
+// The C3k2 shapes (in, out, bottlenecks) of stages 1-4
+static const int kCspStage[4][3] = {{64, 128, 1}, {128, 256, 1}, {256, 384, 2}, {384, 512, 1}};
+Workspace layout_cspreid(ReidModel* m, BlobCursor& take, WgmmaPack& pack) {
+    CspW& cs = m->cs;
+    m->stem_w = take((size_t)27 * csp::STEM_C);
+    m->stem_b = take(csp::STEM_C);
+    int i = 0;
+    auto conv = [&](int K, int N) {
+        RnConv& c = cs.conv[i++];
+        const size_t w = take((size_t)K * N);
+        c.b = take(N);
+        pack.add(c.w, w, K, N);
+    };
+    conv(9 * csp::STEM_C, 64);
+    for (int s = 0; s < 4; ++s) {
+        const int cin = kCspStage[s][0], cout = kCspStage[s][1], n = kCspStage[s][2], mid = cout / 2;
+        conv(cin, 2 * mid);
+        for (int b = 0; b < n; ++b) {
+            conv(mid, mid / 2);
+            conv(9 * (mid / 2), mid);
+        }
+        conv((2 + n) * mid, cout);
+        if (s < 3) conv(9 * cout, cout);
+    }
+    conv(csp::C, csp::SPPF_C);
+    conv(4 * csp::SPPF_C, csp::C);
+    const size_t attn[5] = {(size_t)csp::C * csp::HID, (size_t)csp::HID * csp::C, 9 * (size_t)csp::C, csp::C, csp::C};
+    for (int k = 0; k < 5; ++k) cs.attn[k] = take(attn[k]);
+    for (int h = 0; h < 3; ++h) {
+        cs.head[2 * h] = take((size_t)csp::C * csp::C);
+        cs.head[2 * h + 1] = take(csp::C);
+    }
+    // per crop (at H x W = 256 x 128; twice as much at 256 x 256): the crop; two maps as large as the first stem conv's
+    // output (H/2 x W/2 x 32, also stage 1's C3k2 output H/4 x W/4 x 128); stage 1's C3k2 concatenation
+    // (H/4 x W/4 x 192, the largest); a bottleneck's hidden map (H/4 x W/4 x 32); the head row: 1.1 M floats (2.2 M at
+    // 256 x 256), below the 2.36 M an OSNet_x1_0 chunk takes per crop, so the chunk keeps its size.
+    const size_t px = (size_t)(m->in_h / 4) * (m->in_w / 4);
+    Workspace ws;
+    ws.blob = (size_t)m->in_h * m->in_w * 3;
+    ws.bufA = ws.bufB = std::max((size_t)(m->in_h / 2) * (m->in_w / 2) * csp::STEM_C, px * 128);
+    ws.x1 = px * 192;
+    ws.Y[0][0] = px * 32;
+    ws.sums[0] = csp::FEAT;
+    return ws;
+}
+
 // The A/B kernel switches of the OSNet family, and for OSNet (arch 1) the tensor-core copies of every 1x1 weight that
 // fits the tensor-core kernel's accumulators and shared memory
 void setup_osnet_kernels(ReidModel* m, const float* host) {
@@ -2015,7 +2084,7 @@ ReidModel* reid_load(const char* path) {
     if (!f) throw std::runtime_error(std::string("cannot open ReID blob: ") + path);
     int32_t hdr[16];
     f.read(reinterpret_cast<char*>(hdr), sizeof(hdr));
-    if (!f || (uint32_t)hdr[0] != BLOB_MAGIC || hdr[1] != 1 || hdr[2] < ARCH_OSNET || hdr[2] > ARCH_VIT)
+    if (!f || (uint32_t)hdr[0] != BLOB_MAGIC || hdr[1] != 1 || hdr[2] < ARCH_OSNET || hdr[2] > ARCH_CSPREID)
         throw std::runtime_error("not a version-1 .b200reid blob (export it with boxmot_b200.weights.export_blob)");
     ReidModel* m = new ReidModel();
     try {
@@ -2039,6 +2108,7 @@ ReidModel* reid_load(const char* path) {
             case ARCH_MLFN: ws = layout_mlfn(m, take, pack); break;
             case ARCH_HACNN: ws = layout_hacnn(m, take, pack); break;
             case ARCH_VIT: ws = layout_vits(m, take, pack); break;
+            case ARCH_CSPREID: ws = layout_cspreid(m, take, pack); break;
             default: ws = layout_osnet(m, hdr, take); break;
         }
         if (take.o != n_floats) throw std::runtime_error("ReID blob size does not match its header");
@@ -2316,6 +2386,56 @@ struct Launcher {
             RCUDA_OK(cudaFuncSetAttribute(rn::k_conv_tc<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rn::smem_bytes<64>()));
             rn::k_conv_tc<64><<<grid, rn::THREADS, rn::smem_bytes<64>(), st>>>(a, d_n, off, cap);
         }
+        end();
+    }
+    // one ConvBNSiLU on k_conv_tc's SILU instances (CSPReID-n): a.relu 5 SiLU, 6 residual + SiLU; pitches in a.in_ld,
+    // a.res_ld, a.out_ld
+    void conv_tc_silu(const rn::ConvArgs& a) {
+        const int BN = rn::tile_n(a.N);
+        const dim3 grid((unsigned)(((size_t)upper * a.Ho * a.Wo + rn::BM - 1) / rn::BM), (unsigned)(a.N / BN));
+        begin(a.k0 == 3 ? CLS_LIGHTCONV : CLS_POINTWISE);
+        if (a.relu == 6) {
+            if (BN == 128) launch_silu<128, 2>(a, grid);
+            else if (BN == 64) launch_silu<64, 2>(a, grid);
+            else launch_silu<32, 2>(a, grid);
+        } else {
+            if (BN == 128) launch_silu<128, 1>(a, grid);
+            else if (BN == 64) launch_silu<64, 1>(a, grid);
+            else launch_silu<32, 1>(a, grid);
+        }
+        end();
+    }
+    template <int BN, int SILU>
+    void launch_silu(const rn::ConvArgs& a, dim3 grid) {
+        auto k = rn::k_conv_tc<BN, false, false, false, SILU>;
+        RCUDA_OK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rn::smem_bytes<BN>()));
+        k<<<grid, rn::THREADS, rn::smem_bytes<BN>(), st>>>(a, d_n, off, cap);
+    }
+    // CSPReID-n: the 3 -> 32 3x3 stride-2 stem of the H x Wd crop, timed under `stem`
+    void csp_stem(const float* blob, int H, int Wd, const float* w, const float* b, float* out) {
+        begin(CLS_STEM);
+        csp::k_stem<<<m->sms * 8, 256, 0, st>>>(blob, H, Wd, w, b, d_n, off, cap, out);
+        end();
+    }
+    // CSPReID-n: SPPF's three chained 3x3 max pools of slice 0 of buf [crops][H][Wd][4 c] into slices 1-3
+    void csp_sppf(float* buf, int H, int Wd, int c) {
+        begin(CLS_MAXPOOL);
+        csp::k_sppf<<<m->sms * 8, 256, 0, st>>>(buf, H, Wd, c, d_n, off, cap);
+        end();
+    }
+    // CSPReID-n: LightSelfAttention of x [crops][H][Wd][512] into out; p = fc.0, fc.2, dw, dw shift, spatial 1x1
+    void csp_attn(const float* x, int H, int Wd, const float* const* p, float* out) {
+        begin(CLS_GATES);
+        csp::k_attn<<<upper, csp::C, 0, st>>>(x, H, Wd, p[0], p[1], p[2], p[3], p[4], d_n, off, cap, out);
+        end();
+    }
+    // CSPReID-n: pools, three BNNeck3 GEMVs, interleave and L2 norm of x [crops][H][Wd][512] into the caller's rows;
+    // p = W, b of bn_global, bn_part0, bn_part1; raw (optional) gets the rows before the norm
+    void csp_head(const float* x, int H, int Wd, const float* const* p, const CropDesc* crops, float* out, int out_ld,
+                  float* raw) {
+        begin(CLS_HEAD);
+        csp::k_head<<<(upper + csp::HEAD_CROPS - 1) / csp::HEAD_CROPS, csp::C, 0, st>>>(
+            x, H, Wd, p[0], p[1], p[2], p[3], p[4], p[5], crops, d_n, off, cap, out, out_ld, raw);
         end();
     }
     template <int BN>
@@ -3032,6 +3152,70 @@ void run_hacnn_chunk(Launcher& L, const FrameIn& fi, float* d_out, int out_ld) {
     L.hacnn_head(m->sums[2], fi.crops, d_out, out_ld);
 }
 
+// CSPReID-n, one chunk (cspreid_n.py CSPReID_n.forward, eval).  Taps: 0 crop (H x W x 3), 1 stem (H/4 x W/4 x 64),
+// 2-4 stages 1-3 after their downsample (H/8 x W/8 x 128, H/16 x W/16 x 256, H/32 x W/32 x 384), 5 stage 4's C3k2,
+// 6 SPPF, 7 the attention (H/32 x W/32 x 512 each), 8 the interleaved head row before the L2 norm (1536).  Every
+// ConvBNSiLU after the first stem conv runs on k_conv_tc's SILU instances.  A C3k2's cv1 stores both halves into the
+// first 2 mid channels of its concatenation in m->x1; each bottleneck reads the previous slice in place (the chunk
+// is free), writes its hidden map to Y[0][0] and its output, residual + SiLU(.), into the next slice (the cat is free);
+// cv2 reads the whole concatenation.  SPPF's cv1 writes slice 0 of a 1024-wide concatenation and one launch fills
+// slices 1-3 with the chained pools.  Timing classes: 1x1 `pointwise_gemm`, 3x3 `lightconv`, SPPF `maxpool`, the
+// attention `gates`, the head `head`.
+void run_cspreid_chunk(Launcher& L, const FrameIn& fi, float* d_out, int out_ld) {
+    ReidModel* m = L.m;
+    const float* W = m->d_w;
+    const CspW& cs = m->cs;
+    StageTaps stop_here{m};
+    stage_crops(L, fi);
+    if (stop_here(m->blob, (size_t)m->in_h * m->in_w * 3)) return;
+    int i = 0;   // the next packed conv
+    auto conv = [&](const float* in, int H, int Wd, int cin, int in_ld, int k, int stride, int N, const float* res,
+                    int res_ld, float* out, int ld) {
+        const RnConv& cv = cs.conv[i++];
+        rn::ConvArgs c{};
+        c.in0 = in; c.H0 = H; c.W0 = Wd; c.C0 = cin; c.k0 = k; c.s0 = stride; c.in_ld = in_ld;
+        c.w = cv.w; c.bias = W + cv.b; c.residual = res; c.res_ld = res_ld; c.out = out; c.out_ld = ld;
+        c.Ho = (H - 1) / stride + 1; c.Wo = (Wd - 1) / stride + 1; c.N = N; c.relu = res ? 6 : 5;
+        L.conv_tc_silu(c);
+    };
+    L.csp_stem(m->blob, m->in_h, m->in_w, W + m->stem_w, W + m->stem_b, m->bufA);
+    int H = m->in_h / 2, Wd = m->in_w / 2;
+    conv(m->bufA, H, Wd, csp::STEM_C, csp::STEM_C, 3, 2, 64, nullptr, 0, m->bufB, 64);
+    H = (H - 1) / 2 + 1; Wd = (Wd - 1) / 2 + 1;
+    if (stop_here(m->bufB, (size_t)H * Wd * 64)) return;
+    float* X = m->bufB;
+    for (int s = 0; s < 4; ++s) {
+        const int cin = kCspStage[s][0], cout = kCspStage[s][1], n = kCspStage[s][2], mid = cout / 2;
+        const int ld = (2 + n) * mid;
+        float* cat = m->x1;
+        conv(X, H, Wd, cin, cin, 1, 1, 2 * mid, nullptr, 0, cat, ld);
+        for (int b = 0; b < n; ++b) {
+            float* src = cat + (1 + b) * mid;
+            conv(src, H, Wd, mid, ld, 1, 1, mid / 2, nullptr, 0, m->Y[0][0], mid / 2);
+            conv(m->Y[0][0], H, Wd, mid / 2, mid / 2, 3, 1, mid, src, ld, src + mid, ld);
+        }
+        conv(cat, H, Wd, ld, ld, 1, 1, cout, nullptr, 0, m->bufA, cout);
+        if (s == 3) break;
+        conv(m->bufA, H, Wd, cout, cout, 3, 2, cout, nullptr, 0, m->bufB, cout);
+        H = (H - 1) / 2 + 1; Wd = (Wd - 1) / 2 + 1;
+        if (stop_here(m->bufB, (size_t)H * Wd * cout)) return;
+    }
+    const size_t map = (size_t)H * Wd * csp::C;
+    if (stop_here(m->bufA, map)) return;
+    conv(m->bufA, H, Wd, csp::C, csp::C, 1, 1, csp::SPPF_C, nullptr, 0, m->x1, 4 * csp::SPPF_C);
+    L.csp_sppf(m->x1, H, Wd, csp::SPPF_C);
+    conv(m->x1, H, Wd, 4 * csp::SPPF_C, 4 * csp::SPPF_C, 1, 1, csp::C, nullptr, 0, m->bufB, csp::C);
+    if (stop_here(m->bufB, map)) return;
+    const float* attn[5] = {W + cs.attn[0], W + cs.attn[1], W + cs.attn[2], W + cs.attn[3], W + cs.attn[4]};
+    L.csp_attn(m->bufB, H, Wd, attn, m->bufA);
+    if (stop_here(m->bufA, map)) return;
+    const float* head[6] = {W + cs.head[0], W + cs.head[1], W + cs.head[2], W + cs.head[3], W + cs.head[4],
+                            W + cs.head[5]};
+    const bool tap = m->debug_stop == stop_here.idx;
+    L.csp_head(m->bufA, H, Wd, head, fi.crops, d_out, out_ld, tap ? m->sums[0] : nullptr);
+    if (tap) stop_here(m->sums[0], csp::FEAT);
+}
+
 // MobileNetV2, one chunk: stem -> [expand 1x1 + ReLU6 -> depthwise 3x3 + ReLU6 -> project 1x1 (+ residual)] x 17 ->
 // conv9 -> GAP.  No debug taps.
 void run_mobilenetv2_chunk(Launcher& L, const FrameIn& fi, float* d_out, int out_ld) {
@@ -3128,6 +3312,7 @@ void run_chunk(Launcher& L, const FrameIn& fi, float* d_out, int out_ld) {
         case ARCH_MLFN: run_mlfn_chunk(L, fi, d_out, out_ld); return;
         case ARCH_HACNN: run_hacnn_chunk(L, fi, d_out, out_ld); return;
         case ARCH_VIT: run_vits_chunk(L, fi, d_out, out_ld); return;
+        case ARCH_CSPREID: run_cspreid_chunk(L, fi, d_out, out_ld); return;
     }
 }
 }  // namespace
@@ -3909,6 +4094,99 @@ void standalone_hacnn_head(const float* x3, int n, int off, int count, int hw3, 
     r.L.hacnn_head(d_v, r.crops(rows, off + n), d_out, hacnn::FEAT);
     r.down(v, d_v, (size_t)n * hacnn::FEAT);
     r.down(out, d_out, (size_t)out_rows * hacnn::FEAT);
+}
+
+// ---- CSPReID-n kernels on their own (parity tests), with the crop window and whole-array round trip described above --
+// One ConvBNSiLU on k_conv_tc's SILU instances: in (n,h,w,in_ld) read at channels in_off .. in_off + c0 - 1, weight
+// (k*k*c0, N) K-major, residual (n,Ho,Wo,res_ld) at channels res_off .. (optional) -> out (n,Ho,Wo,out_ld) with columns
+// out_off .. out_off + N - 1 = silu(conv(in) + bias) (+ residual after the activation); the other columns come back as
+// given.
+void standalone_cspreid_conv(const float* in, int n, int off, int count, int h, int w, int c0, int in_ld, int in_off,
+                             int k, int stride, const float* weight, int N, const float* bias, const float* residual,
+                             int res_ld, int res_off, float* out, int out_ld, int out_off) {
+    need(h > 0 && w > 0 && c0 > 0 && (k * k * c0) % rn::KC == 0 && c0 % 4 == 0 && (k == 1 || k == 3) &&
+             (stride == 1 || stride == 2) && N > 0 && N % 32 == 0 && in_off >= 0 && in_off % 4 == 0 &&
+             in_ld % 4 == 0 && in_off + c0 <= in_ld && out_off >= 0 && out_off % 2 == 0 && out_ld % 2 == 0 &&
+             out_off + N <= out_ld && (!residual || (res_off >= 0 && res_off % 2 == 0 && res_ld % 2 == 0 &&
+                                                     res_off + N <= res_ld)),
+         "h, w > 0, c0 a multiple of 4 with k k c0 a multiple of 32, k 1 or 3, stride 1 or 2, N a multiple of 32, "
+         "in_off, in_ld multiples of 4 with in_off + c0 <= in_ld, even out_off / out_ld (res_off / res_ld) with "
+         "out_off + N <= out_ld (res_off + N <= res_ld) required");
+    StandaloneRun r(n, off, count);
+    const int Ho = (h - 1) / stride + 1, Wo = (w - 1) / stride + 1, K = k * k * c0;
+    std::vector<float> packed(2 * (size_t)K * N);
+    rn::pack_conv_weights(weight, K, N, packed.data());
+    const size_t out_floats = (size_t)n * Ho * Wo * out_ld;
+    float* d_out = r.up(out, out_floats);
+    rn::ConvArgs c{};
+    c.in0 = r.up(in, (size_t)n * h * w * in_ld) + in_off; c.H0 = h; c.W0 = w; c.C0 = c0; c.in_ld = in_ld;
+    c.k0 = k; c.s0 = stride;
+    c.w = r.up(packed.data(), packed.size()); c.bias = r.up(bias, N); c.out = d_out + out_off; c.out_ld = out_ld;
+    if (residual) {
+        c.residual = r.up(residual, (size_t)n * Ho * Wo * res_ld) + res_off;
+        c.res_ld = res_ld;
+    }
+    c.Ho = Ho; c.Wo = Wo; c.N = N; c.relu = residual ? 6 : 5;
+    r.L.conv_tc_silu(c);
+    r.down(out, d_out, out_floats);
+}
+
+// op 0: the 3x3 stride-2 stem, in (n,h,w,3), weight (27,32), bias (32) -> out (n,Ho,Wo,32) (SiLU);
+// op 1: SPPF's chained 3x3 max pools, in = out (n,h,w,4c): slices 1-3 of out from slice 0 (weight, bias unused)
+void standalone_cspreid_map(int op, const float* in, int n, int off, int count, int h, int w, int c,
+                            const float* weight, const float* bias, float* out) {
+    need(op == 0 || op == 1, "op 0 (stem) or 1 (SPPF pools) required");
+    need(h > 0 && w > 0 && (op == 0 ? c == 3 : c > 0 && c % 4 == 0), "h, w > 0; the stem takes c = 3, SPPF c % 4 == 0");
+    StandaloneRun r(n, off, count);
+    if (op == 0) {
+        const size_t out_floats = (size_t)n * ((h - 1) / 2 + 1) * ((w - 1) / 2 + 1) * csp::STEM_C;
+        float* d_out = r.up(out, out_floats);
+        r.L.csp_stem(r.up(in, (size_t)n * h * w * 3), h, w, r.up(weight, (size_t)27 * csp::STEM_C),
+                     r.up(bias, csp::STEM_C), d_out);
+        r.down(out, d_out, out_floats);
+        return;
+    }
+    const size_t floats = (size_t)n * h * w * 4 * c;
+    float* d_buf = r.up(in, floats);
+    r.L.csp_sppf(d_buf, h, w, c);
+    r.down(out, d_buf, floats);
+}
+
+// LightSelfAttention as run_cspreid_chunk launches it: x (n,h,w,512), h w <= 256, params in blob order (fc.0 (512,64),
+// fc.2 (64,512), depthwise (9,512), depthwise shift (512), spatial 1x1 (512)) -> out (n,h,w,512)
+void standalone_cspreid_attention(const float* x, int n, int off, int count, int h, int w, const float* params,
+                                  float* out) {
+    need(h > 0 && w > 0 && h * w <= csp::MAX_HW, "h, w > 0 with h w <= 256 required");
+    StandaloneRun r(n, off, count);
+    const size_t sizes[5] = {(size_t)csp::C * csp::HID, (size_t)csp::HID * csp::C, 9 * (size_t)csp::C, csp::C, csp::C};
+    size_t total = 0;
+    for (size_t z : sizes) total += z;
+    const float* d_p = r.up(params, total);
+    const float* p[5];
+    for (int k = 0, o = 0; k < 5; o += (int)sizes[k], ++k) p[k] = d_p + o;
+    const size_t nx = (size_t)n * h * w * csp::C;
+    float* d_out = r.up(out, nx);
+    r.L.csp_attn(r.up(x, nx), h, w, p, d_out);
+    r.down(out, d_out, nx);
+}
+
+// The head: x (n,h,w,512), h >= 2, h w <= 256; params = bn_global, bn_part0, bn_part1 each W (512,512) K-major and b
+// (512) -> row rows[off + i] of out (out_rows,1536) = the interleaved, L2-normalised row of crop i; raw (n,1536), the
+// rows before the norm
+void standalone_cspreid_head(const float* x, int n, int off, int count, int h, int w, const float* params,
+                             const int* rows, int out_rows, float* out, float* raw) {
+    need(h >= 2 && w > 0 && h * w <= csp::MAX_HW && out_rows > 0, "h >= 2, w > 0, h w <= 256, out_rows > 0 required");
+    for (int i = 0; i < off + n; ++i) need(rows[i] >= 0 && rows[i] < out_rows, "rows must lie in [0, out_rows)");
+    StandaloneRun r(n, off, count);
+    constexpr size_t WB = (size_t)csp::C * csp::C + csp::C;
+    const float* d_p = r.up(params, 3 * WB);
+    const float* p[6] = {d_p, d_p + csp::C * csp::C, d_p + WB, d_p + WB + csp::C * csp::C, d_p + 2 * WB,
+                         d_p + 2 * WB + csp::C * csp::C};
+    float* d_raw = r.up(raw, (size_t)n * csp::FEAT);
+    float* d_out = r.up(out, (size_t)out_rows * csp::FEAT);
+    r.L.csp_head(r.up(x, (size_t)n * h * w * csp::C), h, w, p, r.crops(rows, off + n), d_out, csp::FEAT, d_raw);
+    r.down(raw, d_raw, (size_t)n * csp::FEAT);
+    r.down(out, d_out, (size_t)out_rows * csp::FEAT);
 }
 
 }  // namespace bmb

@@ -23,7 +23,11 @@
 // instances (HACNN's Inception streams, BN 32 / 64 / 128) store row m at out + m * out_ld instead of out + m * N, so
 // that each stream writes its channel slice of the concatenated map in place (the caller offsets `out` by the slice's
 // first channel).  The GELU instances (relu = 4, BN 64 / 128) apply the exact erf GELU of the ViT-Nano / ViT-Tiny MLP,
-// x * 0.5 * (1 + erf(x / sqrt(2))), likewise separate so that no other instance's code changes.
+// x * 0.5 * (1 + erf(x / sqrt(2))), likewise separate so that no other instance's code changes.  The SILU instances
+// (CSPReID-n's ConvBNSiLU, BN 32 / 64 / 128) apply x * sigmoid(x) after the bias (SILU = 1), or residual + silu(.) with
+// the residual added after the activation (SILU = 2, a C3k2 bottleneck's shortcut).  They read the main operand, the
+// residual and the output with the pixel pitches in_ld, res_ld and out_ld, so that a bottleneck reads and writes its
+// channel slice of the C3k2 concatenation in place (the caller offsets each pointer by the slice's first channel).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -51,7 +55,8 @@ struct ConvArgs {
     int H1, W1, C1, s1;
     int Ho, Wo, N, relu;     // relu: 0 none, 1 ReLU, 2 QuickGELU, 3 relu(residual + relu(.)) (RELU_RES instances),
                              // 4 exact GELU (GELU instances)
-    int out_ld;              // SLICE instances: floats between output rows (0: the default [M][N] store)
+    int out_ld;              // SLICE / SILU instances: floats between output rows (0: the default [M][N] store)
+    int in_ld, res_ld;       // SILU instances: floats between the pixels of in0 and between the rows of residual
 };
 
 // canonical (no swizzle, K-major) offset in floats of element (row, k) in a block whose K extent is KC
@@ -68,7 +73,7 @@ constexpr size_t smem_bytes() {
     return sizeof(float) * (size_t)STAGES * (2 * BM * KC + 2 * BN * KC) + 128;
 }
 
-template <int BN, bool RELU_RES = false, bool SLICE = false, bool GELU = false>
+template <int BN, bool RELU_RES = false, bool SLICE = false, bool GELU = false, int SILU = 0>
 __global__ void __launch_bounds__(THREADS, 1) k_conv_tc(const ConvArgs a, const int* __restrict__ d_n, int off, int cap) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     __shared__ __align__(8) uint64_t bar[STAGES];
@@ -122,7 +127,7 @@ __global__ void __launch_bounds__(THREADS, 1) k_conv_tc(const ConvArgs a, const 
                 const int ky = tap / a.k0, kx = tap - ky * a.k0;
                 const int iy = ry[i] * a.s0 + ky - pad, ix = rx[i] * a.s0 + kx - pad;
                 ok = ok && iy >= 0 && iy < a.H0 && ix >= 0 && ix < a.W0;
-                if (ok) src = a.in0 + (((size_t)rn_[i] * a.H0 + iy) * a.W0 + ix) * a.C0 + ci;
+                if (ok) src = a.in0 + (((size_t)rn_[i] * a.H0 + iy) * a.W0 + ix) * (SILU ? a.in_ld : a.C0) + ci;
             } else {
                 const int ci = k - K0;
                 if (ok) src = a.in1 + (((size_t)rn_[i] * a.H1 + ry[i] * a.s1) * a.W1 + rx[i] * a.s1) * a.C1 + ci;
@@ -187,13 +192,22 @@ __global__ void __launch_bounds__(THREADS, 1) k_conv_tc(const ConvArgs a, const 
     for (int h = 0; h < 2; ++h) {
         const int m = m0 + row + 8 * h;
         if (m >= M) continue;
-        float* dst = a.out + (size_t)m * (SLICE ? a.out_ld : a.N) + n0;
-        const float* res = a.residual ? a.residual + (size_t)m * a.N + n0 : nullptr;
+        float* dst = a.out + (size_t)m * (SLICE || SILU ? a.out_ld : a.N) + n0;
+        const float* res = a.residual ? a.residual + (size_t)m * (SILU ? a.res_ld : a.N) + n0 : nullptr;
 #pragma unroll
         for (int i = 0; i < BN / 8; ++i) {
             const int c = 8 * i + cq;
             const float2 b = *reinterpret_cast<const float2*>(a.bias + n0 + c);
             float2 o = make_float2(acc[4 * i + 2 * h] + b.x, acc[4 * i + 2 * h + 1] + b.y);
+            if constexpr (SILU != 0) {
+                o.x = o.x / (1.f + expf(-o.x)); o.y = o.y / (1.f + expf(-o.y));
+                if constexpr (SILU == 2) {
+                    const float2 r = *reinterpret_cast<const float2*>(res + c);
+                    o.x += r.x; o.y += r.y;
+                }
+                *reinterpret_cast<float2*>(dst + c) = o;
+                continue;
+            }
             if constexpr (RELU_RES) {
                 const float2 r = *reinterpret_cast<const float2*>(res + c);
                 o.x = fmaxf(r.x + fmaxf(o.x, 0.f), 0.f); o.y = fmaxf(r.y + fmaxf(o.y, 0.f), 0.f);
@@ -218,7 +232,7 @@ __global__ void __launch_bounds__(THREADS, 1) k_conv_tc(const ConvArgs a, const 
 }
 
 // output-channel tile of a layer: 128 when it divides N, else 64 (ResNet's layer1 conv1 / conv2), else 32 (HACNN's
-// 32- and 96-wide streams, SLICE instances only)
+// 32- and 96-wide streams and CSPReID-n's 32- and 96-wide bottleneck convs, SLICE and SILU instances only)
 inline int tile_n(int N) { return N % 128 == 0 ? 128 : (N % 64 == 0 ? 64 : 32); }
 
 // host: W [K][N] (K-major rows of N) -> [N / BN][K / KC][hi | lo][BN x KC canonical]; K % KC == 0, N % BN == 0

@@ -435,6 +435,37 @@ def make_hacnn_state(seed: int = 0, num_classes: int = 751):
     return sd
 
 
+def make_cspreid_state(seed: int = 0, num_classes: int = 751):
+    """Seeded state dict with the parameter names of the reference's `CSPReID_n(num_classes)` (loads with strict=True).
+    Every BatchNorm's gamma, beta and running statistics are randomised, so folding is exercised and no bottleneck's
+    residual branch is the identity the reference's zero-gamma initialisation makes of it; the attention's gates are
+    spread over (0, 1) rather than saturated."""
+    import torch
+
+    from .weights import CSPREID_HEADS, cspreid_layout
+
+    g = torch.Generator().manual_seed(seed)
+    sd = {}
+    conv, bn, _ = _osnet_makers(g, sd)
+    for name, kind, shape in cspreid_layout():
+        if kind == "cbs":
+            conv(name + ".conv", shape[0], shape[1], shape[2], gain=2.0)
+            bn(name + ".bn", shape[0])
+        elif kind == "lsa":
+            c, hid = shape
+            conv(name + ".fc.0", hid, c, 1, gain=0.5)
+            conv(name + ".fc.2", c, hid, 1, gain=0.5)
+            conv(name + ".spatial.0", c, c, 3, groups=c, gain=2.0)
+            bn(name + ".spatial.1", c)
+            conv(name + ".spatial.3", 1, c, 1, gain=0.5)
+        else:
+            conv(name + ".reduction", shape[0], shape[1], 1)
+            bn(name + ".bn", shape[0])
+    for h in CSPREID_HEADS:
+        sd[f"head.{h}.classifier.weight"] = 0.001 * torch.randn(num_classes, 512, generator=g)
+    return sd
+
+
 def make_clip_state(seed: int = 0, vehicle: bool = False, num_classes: int = 751, extras: bool = True):
     """Seeded state dict with the key set of the reference's CLIP-ReID `build_transformer` (ViT-B/16: image_encoder.*,
     bottleneck.*, bottleneck_proj.*, classifier.*, classifier_proj.*); vehicle=True gives the 257-row positional table

@@ -34,6 +34,9 @@ Arch 9 (ViT-Nano / ViT-Tiny, `fold_vit`) records width 192, depth, 3 heads, the 
 words 3-7, the crop height / width in words 9-10, the patch grid in words 11-12, the patch stride in word 13, the
 pooling (0 class token, 1 omni-scale, P >= 2 class token + P strips) in word 14 and the projection width (0 or 512)
 in word 15; its layout is listed above `fold_vit`.
+Arch 10 (CSPReID-n, `fold_cspreid`) records the stage widths 128, 256, 384, 512 and the 1536-d row in words 3-7 and the
+crop height / width (256x128, or 256x256 for a vehicle file name) in words 9-10; its layout is listed above
+`cspreid_layout`.
 All 1x1 weights are stored K-major ([cin][cout]) so a thread owning consecutive output channels loads
 consecutive floats; every tensor is zero-padded to a multiple of 4 floats (16-byte aligned float4 loads).
 """
@@ -60,6 +63,7 @@ MLFN_FEAT = 1024
 ARCH_HACNN = 8
 HACNN_FEAT = 1024
 ARCH_VIT = 9
+ARCH_CSPREID = 10
 BRANCHES = (("conv2a", 1), ("conv2b", 2), ("conv2c", 3), ("conv2d", 4))
 EPS = 1e-5
 
@@ -793,6 +797,107 @@ def resolve_vit(sd, file_name=None, model_name=None):
     return name
 
 
+# CSPReID-n (arch 10): CSPReID_n of reid/backbones/cspreid_n.py.  Header words 3-7 hold the stage widths 128, 256, 384,
+# 512 and the 1536-d row, words 9-10 the crop (256x128, or 256x256 for a `veri` / `vehicleid` file name).  Every
+# ConvBNSiLU has its BatchNorm folded; a k x k convolution is stored K-major W[k*k*cin][cout] with k index
+# (kh*k + kw)*cin + ci, then b[cout].  In `cspreid_layout` order:
+#     stem.0, stem.1                       W[27][32], b[32]; W[288][64], b[64]
+#     stage{s}.0 (C3k2, mid = out / 2)     cv1 W[in][2 mid], b; per bottleneck: cv1 W[mid][mid/2], b; cv2 W[9 mid/2][mid],
+#                                          b; then cv2 W[(2 + n) mid][out], b
+#     stage{s}.1 (s = 1..3)                W[9 out][out], b (3x3 stride 2)
+#     stage4.1 (SPPF)                      cv1 W[512][256], b; cv2 W[1024][512], b
+#     stage4.2 (LightSelfAttention)        fc.0 W[512][64]; fc.2 W[64][512]; spatial depthwise W[9][512] (BN folded),
+#                                          b[512]; spatial.3 w[512]
+#     head.bn_global / bn_part0 / bn_part1 W[512][512] (BatchNorm1d folded), b[512]
+CSPREID_STAGES = ((64, 128, 1), (128, 256, 1), (256, 384, 2), (384, 512, 1))   # C3k2 (in, out, bottlenecks)
+CSPREID_FEAT = 1536
+CSPREID_HEADS = ("bn_global", "bn_part0", "bn_part1")
+
+
+def cspreid_layout():
+    """[(name, kind, shape)] of CSPReID_n in blob order: kind "cbs" (ConvBNSiLU: `name.conv.weight` of `shape` =
+    (cout, cin, k, k) and `name.bn.*`), "lsa" (LightSelfAttention at `name`, shape = (C, hidden)) or "neck" (a BNNeck3
+    at `name`, shape = (feat, C))."""
+    out = [("stem.0", "cbs", (32, 3, 3, 3)), ("stem.1", "cbs", (64, 32, 3, 3))]
+    for s, (cin, cout, n) in enumerate(CSPREID_STAGES, 1):
+        mid = cout // 2
+        p = f"stage{s}.0"
+        out.append((p + ".cv1", "cbs", (2 * mid, cin, 1, 1)))
+        for i in range(n):
+            out += [(f"{p}.bottlenecks.{i}.cv1", "cbs", (mid // 2, mid, 1, 1)),
+                    (f"{p}.bottlenecks.{i}.cv2", "cbs", (mid, mid // 2, 3, 3))]
+        out.append((p + ".cv2", "cbs", (cout, (2 + n) * mid, 1, 1)))
+        if s < 4:
+            out.append((f"stage{s}.1", "cbs", (cout, cout, 3, 3)))
+    out += [("stage4.1.cv1", "cbs", (256, 512, 1, 1)), ("stage4.1.cv2", "cbs", (512, 1024, 1, 1)),
+            ("stage4.2", "lsa", (512, 64))]
+    out += [(f"head.{h}", "neck", (512, 512)) for h in CSPREID_HEADS]
+    return out
+
+
+def cspreid_keys():
+    """{key: shape} of CSPReID_n's state dict without num_batches_tracked and the classifiers (the keys the embedding
+    reads)."""
+    want = {}
+
+    def bn(name, c):
+        for p in ("weight", "bias", "running_mean", "running_var"):
+            want[f"{name}.{p}"] = (c,)
+
+    for name, kind, shape in cspreid_layout():
+        if kind == "cbs":
+            want[name + ".conv.weight"] = shape
+            bn(name + ".bn", shape[0])
+        elif kind == "lsa":
+            c, hid = shape
+            want.update({name + ".fc.0.weight": (hid, c, 1, 1), name + ".fc.2.weight": (c, hid, 1, 1),
+                         name + ".spatial.0.weight": (c, 1, 3, 3), name + ".spatial.3.weight": (1, c, 1, 1)})
+            bn(name + ".spatial.1", c)
+        else:
+            want[name + ".reduction.weight"] = (shape[0], shape[1], 1, 1)
+            bn(name + ".bn", shape[0])
+    return want
+
+
+def is_cspreid(sd) -> bool:
+    return "stage4.2.spatial.0.weight" in sd or "head.bn_part1.reduction.weight" in sd
+
+
+def cspreid_input_hw(file_name=None):
+    """The reference's crop for cspreid_n weights: 256x256 for a `veri` / `vehicleid` file name, else 256x128
+    (base_backend.py:57-64)."""
+    return (256, 256) if file_name and clip_vehicle_name(file_name) else (256, 128)
+
+
+def fold_cspreid(sd) -> List[np.ndarray]:
+    """CSPReID_n state dict -> arrays of the arch-10 blob.  Every tensor of the reference model (apart from the
+    classifiers) must be present with its shape: a missing or mis-shaped key raises a ValueError naming the keys, where
+    the reference's loader would silently run that layer randomly initialised.  Extra keys are ignored, as that loader
+    discards them."""
+    want = cspreid_keys()
+    missing = sorted(k for k in want if k not in sd)
+    bad_shape = sorted(k for k in want if k in sd and tuple(sd[k].shape) != want[k])
+    if missing or bad_shape:
+        raise ValueError(f"not a cspreid_n state dict (missing keys {missing[:4]}, unexpected shapes {bad_shape[:4]}); "
+                         "the reference would run these layers randomly initialised")
+    out: List[np.ndarray] = []
+    for name, kind, shape in cspreid_layout():
+        if kind == "cbs":
+            w = _np(sd[name + ".conv.weight"])   # [co][ci][k][k]
+            scale, shift = _bn_fold(sd, name + ".bn")
+            co, ci, k, _ = w.shape
+            out += [(w * scale[:, None, None, None]).transpose(2, 3, 1, 0).reshape(k * k * ci, co), shift]
+        elif kind == "lsa":
+            scale, shift = _bn_fold(sd, name + ".spatial.1")
+            dw = _np(sd[name + ".spatial.0.weight"])[:, 0]   # [c][3][3]
+            out += [_np(sd[name + ".fc.0.weight"])[:, :, 0, 0].T, _np(sd[name + ".fc.2.weight"])[:, :, 0, 0].T,
+                    (dw * scale[:, None, None]).reshape(-1, 9).T, shift, _np(sd[name + ".spatial.3.weight"]).ravel()]
+        else:
+            scale, shift = _bn_fold(sd, name + ".bn")
+            out += [(_np(sd[name + ".reduction.weight"])[:, :, 0, 0] * scale[:, None]).T, shift]
+    return out
+
+
 def _pad4(n: int) -> int:
     return (n + 3) // 4 * 4
 
@@ -866,9 +971,16 @@ def export_blob(weights, out_path=None) -> Path:
             raise ValueError("out_path is required when exporting an in-memory state dict")
     table, in_modes, extra = [], [], []
     vit = resolve_vit(sd, name, model_name)
+    ref_name = model_name or (model_name_from_file(name) if name else None)
     if vit is not None:
         dims, extra, arrays = fold_vit(sd, vit)
         arch = ARCH_VIT
+    elif ref_name == "cspreid_n" or (ref_name is None and is_cspreid(sd)):
+        arrays = fold_cspreid(sd)
+        arch, dims, extra = ARCH_CSPREID, [128, 256, 384, 512, CSPREID_FEAT], list(cspreid_input_hw(name))
+    elif is_cspreid(sd):
+        raise ValueError(f"cspreid_n weights under the model name {ref_name!r}: the reference would build {ref_name} "
+                         "and run it randomly initialised")
     elif is_clip(sd):
         dims, input_hw, grid, arrays = fold_clip(sd, name)
         arch, extra = ARCH_CLIP, [*input_hw, *grid]
@@ -895,7 +1007,8 @@ def export_blob(weights, out_path=None) -> Path:
         arch, dims = ARCH_HACNN, [32, 128, 256, 384, HACNN_FEAT]
     else:
         raise ValueError("only OSNet, OSNet-AIN, OSNet-IBN, MobileNetV2, LMBN_n, ResNet50 / ResNet101, CLIP-ReID "
-                         "ViT-B/16, MLFN, HACNN and ViT-Nano / ViT-Tiny state dicts are implemented on the B200 ReID path")
+                         "ViT-B/16, MLFN, HACNN, ViT-Nano / ViT-Tiny and CSPReID-n state dicts are implemented on the "
+                         "B200 ReID path")
     # every tensor starts on a 16-byte boundary (the kernels read weights as float4)
     padded = []
     for a in arrays:
@@ -913,6 +1026,8 @@ def export_blob(weights, out_path=None) -> Path:
         header[9:11] = [160, 64]
     if arch == ARCH_VIT:
         header[9:16] = extra
+    if arch == ARCH_CSPREID:
+        header[9:11] = extra
     out_path = Path(out_path)
     tmp = out_path.with_suffix(out_path.suffix + ".tmp")
     with open(tmp, "wb") as f:

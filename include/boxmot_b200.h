@@ -488,6 +488,31 @@ BOXMOT_B200_API int boxmot_b200_hacnn_stn(const float* src, int n, int off, int 
 BOXMOT_B200_API int boxmot_b200_hacnn_head(const float* x3, int n, int off, int count, int hw3, const float* loc,
                                            int hwl, const float* wg, const float* bg, const float* wl, const float* bl,
                                            const int* rows, int out_rows, float* out, float* v);
+/* The CSPReID-n kernels on their own, over a crop window as for the HACNN kernels above, NHWC float32.
+ * cspreid_conv: one ConvBNSiLU on the tensor cores: in (n,h,w,in_ld) read at channels in_off .. in_off + c0 - 1 (c0 a
+ * multiple of 4, k*k*c0 of 32; in_off and in_ld multiples of 4), k 1 or 3 (pad k/2), stride 1 or 2, weight (k*k*c0, N)
+ * K-major with k index (kh*k + kw)*c0 + ci, N a multiple of 32; out (n,Ho,Wo,out_ld) columns out_off .. out_off + N - 1
+ * = silu(conv + bias), Ho = (h - 1) / stride + 1, plus, when residual (n,Ho,Wo,res_ld) is given, its columns
+ * res_off .. res_off + N - 1 after the activation (a C3k2 bottleneck's shortcut).
+ * cspreid_map: op 0 the 3x3 stride-2 stem (in (n,h,w,3), c = 3, weight (27,32) as above, bias (32) -> out
+ * (n,Ho,Wo,32), SiLU); op 1 SPPF's three chained MaxPool2d(3, 1, 1): in = out (n,h,w,4c), slices 1..3 of out (channels
+ * i c .. i c + c - 1) from slice 0, which comes back as given.
+ * cspreid_attention: LightSelfAttention of x (n,h,w,512), h w <= 256, params in blob order (fc.0 (512,64), fc.2
+ * (64,512) K-major, depthwise (9,512) with its BN scale folded, the BN shift (512), the spatial 1x1 (512)) -> out.
+ * cspreid_head: x (n,h,w,512), h >= 2, h w <= 256; params bn_global, bn_part0, bn_part1, each W (512,512) K-major with
+ * the BatchNorm1d folded and b (512) -> raw (n,1536), element 3 c + branch of [global | upper half | lower half] pool
+ * GEMVs, and out row rows[off + i] = raw_i / |raw_i|. */
+BOXMOT_B200_API int boxmot_b200_cspreid_conv(const float* in, int n, int off, int count, int h, int w, int c0,
+                                             int in_ld, int in_off, int k, int stride, const float* weight, int N,
+                                             const float* bias, const float* residual, int res_ld, int res_off,
+                                             float* out, int out_ld, int out_off);
+BOXMOT_B200_API int boxmot_b200_cspreid_map(int op, const float* in, int n, int off, int count, int h, int w, int c,
+                                            const float* weight, const float* bias, float* out);
+BOXMOT_B200_API int boxmot_b200_cspreid_attention(const float* x, int n, int off, int count, int h, int w,
+                                                  const float* params, float* out);
+BOXMOT_B200_API int boxmot_b200_cspreid_head(const float* x, int n, int off, int count, int h, int w,
+                                             const float* params, const int* rows, int out_rows, float* out,
+                                             float* raw);
 /* The float32 CUDA-core kernels of the OSNet family, MobileNetV2 and LMBN_n, one family per entry, launched as a loaded
  * model launches them, on host arrays (NHWC float32) over a crop window: the arrays hold n crops, the device crop count
  * is `count` and the window starts at crop `off`, so the kernels process crops 0 .. clamp(count - off, 0, n) - 1 of the
